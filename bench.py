@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""bench.py — BEV frames/s of the ST-P3 camera->BEV perception hot path on B200 (see DESIGN.md, Measurement).
+"""bench.py — BEV frames/s of the ST-P3 camera->BEV perception hot path on H100 (see DESIGN.md, Measurement).
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--workload perceive|lift_splat] [--batch b_per_gpu]
+                  [--dump-outputs DIR]
   python bench.py --impl reference ...     # the reference's CPU path (oracle port) on the host cores
 
 One "step" = one pass of the hot path over one batch of synthetic samples (6 cameras x 3 frames, 200x200 BEV);
@@ -66,11 +67,12 @@ def peaks():
         p = json.load(open(path))
         return {"hbm_gbs": p["hbm_gbs"], "bf16_tflops": p["bf16_tflops"],
                 "bf16_tflops_sustained": p.get("bf16_tflops_sustained", p["bf16_tflops"]), "source": "measured"}
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0, "source": "fallback"}
+    # H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 TFLOP/s dense BF16 -- not measured
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0, "source": "H100 SXM data sheet"}
 
 
 class ClockSampler:
-    """nvidia-smi sampled every 100 ms DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi sampled every 100 ms DURING the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -163,7 +165,7 @@ def build_model(device=None, lcfg=None):
 
 # ------------------------------------------------------------------------------------------------ reference arm
 def workload_config(args, cfg, world):
-    """`config` of the JSON line: identical for the B200 arm and the reference arm (it names the workload)."""
+    """`config` of the JSON line: identical for the CUDA arm and the reference arm (it names the workload)."""
     X, Y = cfg.bev_xy
     return {"workload": WORKLOADS[args.workload], "samples_per_gpu_per_step": args.batch,
             "global_batch": args.batch * world, "cameras": cfg.n_cameras, "frames": cfg.receptive_field, "bev": [X, Y],
@@ -175,7 +177,7 @@ def workload_config(args, cfg, world):
 
 class ReferenceArm:
     """The reference's own CPU implementation of the path on the host cores.  kind "reference": the UNMODIFIED
-    reference package (installed by oracle/build_ref.py into the git-ignored baseline/_ref/, or /root/reference in the
+    reference package (installed by oracle/build_ref.py into the git-ignored oracle/_ref/, or STP3_REFERENCE_ROOT in the
     build container) -- its STP3.get_geometry / projection_to_birds_eye_view, TemporalModel and Decoder -- imported
     through oracle/ref_loader.py; kind "port": the op-for-op CPU port under oracle/ when that install is absent."""
 
@@ -262,7 +264,7 @@ class ReferenceArm:
                 "sweep": {str(k): round(v, 3) for k, v in sweep.items()}}
 
     def describe(self, r, steps, warmup):
-        what = ("unmodified reference package (baseline/_ref or /root/reference via oracle/ref_loader.py): STP3.get_geometry + "
+        what = ("unmodified reference package (oracle/_ref via oracle/ref_loader.py): STP3.get_geometry + "
                 "projection_to_birds_eye_view" + (" + TemporalModel + Decoder" if self.workload in PERCEPTION else "")
                 if self.kind == "reference" else
                 "op-for-op CPU port of the reference (oracle/torch_port.py" + (" + oracle/torch_dense.py)" if self.workload in PERCEPTION else ")"))
@@ -275,7 +277,7 @@ def run_reference_arm(args, cfg):
     if int(os.environ.get("RANK", "0")) != 0:
         return
     world = int(os.environ.get("WORLD_SIZE", "1"))
-    steps, warmup = max(1, min(args.steps, 40)), min(args.warmup, 5)      # bounded: one sample takes seconds
+    steps, warmup = args.steps, args.warmup                 # one sample takes seconds on the CPU: choose --steps accordingly
     arm = ReferenceArm(args.workload, cfg)
     r = arm.time(steps, warmup)
     line = {
@@ -289,7 +291,7 @@ def run_reference_arm(args, cfg):
     print(json.dumps(line), flush=True)
 
 
-# ------------------------------------------------------------------------------------------------ B200 arm
+# ------------------------------------------------------------------------------------------------ CUDA arm
 OUR_KERNELS = ("conv_igemm", "aspp_fused", "block_fused", "lift_splat", "bev_finalize", "bev_discount", "pool_reduce", "pool_bias", "small_linear",
                "upsample2x", "col_sum_reduce", "hilo", "spatial_sum", "clear_bytes", "lift_splat_bwd")
 
@@ -349,7 +351,7 @@ def check_parity(res, cfg):
                          f"{worst_r:.2e} vs the reference (bar 1e-3) -- refusing to report a throughput for wrong results")
     return {"fixture": "tests/golden/e2e_perceive_level.npz (reference end to end at 200x200, sample seed 0)",
             "max_err_vs_fp64_oracle": worst_o, "max_err_vs_reference_fp32": worst_r, "bar": 1e-3,
-            "checked": "segmentation, pedestrian, hdmap logits of sample 0 of a replayed (graphed) step, 40k entries each"}
+            "checked": "segmentation, pedestrian, hdmap logits of sample 0 of a replayed (graphed) step, 12k entries each"}
 
 
 def main():
@@ -368,7 +370,12 @@ def main():
     ap.add_argument("--no-extras", action="store_true", help="skip the sustained run, the second rig and the latency mode")
     ap.add_argument("--profiler-range", action="store_true",
                     help="bracket the resident timed steps with cudaProfilerStart/Stop (ncu --profile-from-start off)")
+    ap.add_argument("--dump-outputs", metavar="DIR",
+                    help="write the outputs of the last timed step as DIR/<name>.npy (float32; a fixed, seeded sample of "
+                         "outputs above 64 MB in all) so that two builds can be compared on identical inputs")
     args = ap.parse_args()
+    if args.steps < 1 or args.warmup < 0:
+        ap.error("--steps must be >= 1 and --warmup >= 0")
     cfg = syn.CONFIGS["stress" if args.workload == "stress" else "perceive"]
     if os.environ.get("STP3_BENCH_DUMP_AFTER"):      # debugging aid: Python stacks of every thread after N seconds, then exit
         import faulthandler
@@ -410,7 +417,7 @@ def main():
     d_feat, d_depth = host["feat"].to(dev), host["depth_logits"].to(dev)
     d_mats = [m.to(dev) for m in host_mats]
     X, Y = cfg.bev_xy
-    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=dev)   # > 126 MB L2
+    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=dev)   # > 50 MB L2
     model = build_model(dev, cfg) if perceive else None
     graphed = None
     if perceive and not args.no_graph:
@@ -520,7 +527,13 @@ def main():
     if args.profiler_range:
         torch.cuda.cudart().cudaProfilerStart()
     _progress("timing resident steps")
-    total_ms = timed(step_resident, K)
+    last = {}
+
+    def step_kept():
+        last["out"] = step_resident()
+    total_ms = timed(step_kept, K)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(last["out"], args.dump_outputs)
     _progress("timing e2e")
     if args.profiler_range:
         torch.cuda.synchronize()
@@ -627,8 +640,6 @@ def main():
         roof_ls = {"bound": "hbm", "kernel": "lift-splat (scatter + finalize, one C-ABI call)",
                    "achieved": alg / (ls_ms * 1e-3) / 1e9, "peak": pk["hbm_gbs"], "unit": "GB/s",
                    "frac": alg / (ls_ms * 1e-3) / 1e9 / pk["hbm_gbs"], "peak_source": pk["source"],
-                   "traffic": TRAFFIC["lift_splat"]["bytes_per_sample"] * b if args.workload == "perceive" else None,
-                   "traffic_source": TRAFFIC["lift_splat"]["source"],
                    "algorithmic_bytes_per_step": alg, "ms": ls_ms, "rig": args.rig}
         for name, r in rigs.items():
             r["achieved"] = alg / (r["ms"] * 1e-3) / 1e9
@@ -649,15 +660,12 @@ def main():
                 if args.workload in ("perceive", "perceive_heads") else None
             ach = flops / (dense_ms * 1e-3) / 1e12 if flops and dense_ms > 0 else None
             line["stage_ms"] = stage_ms
-            line["roofline"] = {"bound": "tensor", "kernel": "conv_igemm_kernel<BN, PAIR, STACK> + aspp_fused_kernel + block_fused_kernel (temporal model + decoder)",
+            line["roofline"] = {"bound": "tensor", "kernel": "conv_igemm_kernel<BN, STACK> + aspp_fused_kernel + block_fused_kernel (temporal model + decoder)",
                                 "achieved": ach, "peak": pk["bf16_tflops_sustained"], "unit": "TFLOP/s",
                                 "frac": ach / pk["bf16_tflops_sustained"] if ach else None, "peak_source": pk["source"],
-                                "traffic": TRAFFIC["conv"]["bytes_per_sample"] * b if args.workload == "perceive" else None,
-                                "traffic_source": TRAFFIC["conv"]["source"],
                                 "algorithmic_flops_per_step": flops, "ms": dense_ms,
                                 "conv_kernel_ms_cupti": conv_ms_prof,
-                                "note": "algorithmic 2*MAC flops of the fp32 layers; the kernel issues 3 bf16 MMAs per product (hi*hi+hi*lo+lo*hi) to hold 1e-3 parity: "
-                                        "profiles/r02_precision_plan.txt shows every 2-MMA form missing the bar"}
+                                "note": "algorithmic 2*MAC flops of the fp32 layers; the kernel issues 3 bf16 MMAs per product (hi*hi+hi*lo+lo*hi) to hold 1e-3 parity"}
             line["roofline_lift_splat"] = roof_ls
         else:
             line["roofline"] = roof_ls
@@ -697,6 +705,25 @@ def main():
 
 
 _LINE = {}
+DUMP_LIMIT_BYTES = 64 * 1024 * 1024
+
+
+def dump_outputs(res, out_dir, limit=DUMP_LIMIT_BYTES, seed=0):
+    """res: {name: tensor or None} of one step -> out_dir/<name>.npy as float32 (None entries are heads the configuration
+    does not compute).  Above `limit` bytes in all, every output keeps the same seeded random subset of its flattened
+    entries (sorted indices), sized so that the files fit the limit; the subset is gathered where the tensor lives, so
+    only the sample crosses to the host."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    res = {k: t for k, t in res.items() if t is not None}
+    total = sum(t.numel() for t in res.values()) * 4
+    for name in sorted(res):
+        flat = res[name].detach().reshape(-1)
+        if total > limit:
+            n = int(flat.numel() * (limit / total))
+            idx = np.sort(np.random.default_rng(seed).choice(flat.numel(), size=n, replace=False))
+            flat = flat[torch.from_numpy(idx).to(flat.device)]
+        np.save(os.path.join(out_dir, f"{name}.npy"), flat.float().cpu().numpy().reshape(-1 if total > limit else res[name].shape))
 
 
 def extras_watchdog(limit_s, rank, exit_fn=os._exit, out=None):
@@ -712,14 +739,6 @@ def extras_watchdog(limit_s, rank, exit_fn=os._exit, out=None):
     dog.daemon = True
     dog.start()
     return dog
-
-# DRAM traffic (dram__bytes_read.sum + dram__bytes_write.sum) cannot be measured outside ncu: static values from the
-# committed `ncu --set full` captures, per sample
-TRAFFIC = {
-    "lift_splat": {"bytes_per_sample": int(263.6e6 / 4), "source": "static: profiles/r02_ncu_liftsplat_v2_summary.txt (scatter 108.7 MB + finalize 155.0 MB, B=4)"},
-    "conv": {"bytes_per_sample": int(2464e6 / 4), "source": "static: profiles/r02_ncu_conv_v3_summary.txt (the temporal model's 6 tensor-core launches incl. the four B2B launches + the first 10 decoder convs of 35, cold cache, B=4)"},
-}
-
 
 def _progress(msg):
     if os.environ.get("STP3_BENCH_PROGRESS"):

@@ -1,8 +1,8 @@
-/* stp3_b200 — C ABI of the B200-native (sm_100a) ST-P3 camera->BEV perception hot path.
+/* stp3_b200 — C ABI of the H100-native (sm_90a) ST-P3 camera->BEV perception hot path.
  *
  * The reference (OpenDriveLab/ST-P3) is 100 % Python/PyTorch and has no FFI of its own; the drop-in boundary is
  * the nn.Module surface (SURVEY.md §8b).  This header is the C boundary that sits directly underneath those
- * modules: each entry point names the reference interface it replaces (file:line under /root/reference).
+ * modules: each entry point names the reference interface it replaces (file:line in OpenDriveLab/ST-P3).
  *
  * Conventions
  *   - every pointer is a DEVICE pointer owned by the caller (PyTorch's caching allocator in practice), unless the
@@ -29,7 +29,7 @@ extern "C" {
 #define STP3_ECUDA (-3)    /* CUDA runtime / driver error (launch failure, no device) */
 #define STP3_EUNSUPPORTED (-4)
 
-/* Library / build identification ("sm_100a", ABI version). */
+/* Library / build identification ("sm_90a", ABI version). */
 int stp3_abi_version(void);
 const char* stp3_build_info(void);
 const char* stp3_last_error(void);
@@ -103,7 +103,7 @@ int stp3_lift_splat_bwd(const float* grad_out, const float* feat, const float* d
                         void* scratch, size_t scratch_bytes, float* grad_feat, float* grad_depth_logits, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------
- * Dense layers: implicit-GEMM convolution on tcgen05 tensor cores (TMEM accumulators, TMA-fed operands).
+ * Dense layers: implicit-GEMM convolution on the Hopper tensor cores (wgmma, register accumulators, TMA-fed operands).
  *
  * One entry point covers every convolution of the temporal block, the per-frame DeepLab head and the BEV decoder:
  *   CausalConv3d / conv_1x1x1_norm_activated / TemporalBlock   stp3/layers/temporal.py:252-273, 315-325, 426-489
@@ -144,7 +144,7 @@ typedef struct stp3_conv_desc {
   int res_cstride, res_coff;
   int n_valid;           /* real output channels written to y_f32 */
   int sigmoid;           /* apply a sigmoid to y_f32 (instance_center head, decoder.py:70) */
-  int tune_n_sub;        /* 0 = automatic; 1 / 2 = sub-tiles (8x16 pixels each) per CTA tile; 3 = 16x16 tile of a CTA pair (cta_group::2) */
+  int tune_n_sub;        /* accepted and ignored: the CTA tile is always 8x16 pixels */
   int tune_group;        /* 0 = automatic; 1 = never share an activation load between the dy taps of a 3x3; 3 = share;
                             +4 = stream the weights through the smem ring even if they would fit (more activation stages);
                             +8 = (bn 64) one stacked [W_hi; W_lo] operand: 2 MMAs per product instead of 3 */
@@ -222,7 +222,7 @@ int stp3_aspp_fused_fwd(const stp3_aspp_desc* desc, const void* x_hi, const void
  * Tail of a TemporalBlock (stp3/layers/temporal.py:426-489) as ONE back-to-back tensor-core kernel:
  *   out = relu(BN(aggregation 1x1x1 of [path 0 | path 1 | path 2 | pyramid pooling])) + (projection(x) | x)
  * with path 0 / 1 = the causal (2,3,3) / (1,3,3) convolutions of the entry convolutions' outputs `mid` and path 2 = a
- * 1x1x1 convolution of x.  Up to three MMA chains accumulate the paths side by side in TMEM, the activated concat is
+ * 1x1x1 convolution of x.  Up to three MMA chains accumulate the paths side by side (register accumulators), the activated concat is
  * converted to bf16 hi/lo in shared memory and multiplied with the aggregation weights; the 128-channel concat tensor
  * never exists.  Applicable when every path has <= 48 channels, x <= 64 spatial channels and the block <= 64 outputs.
  *   chain: src (0 = mid, 1 = x), cin_off (64-channel K block read), taps (dt, dy, dx), n_mma (MMA width, multiple of 16),
@@ -230,7 +230,7 @@ int stp3_aspp_fused_fwd(const stp3_aspp_desc* desc, const void* x_hi, const void
  *   piece_col[pp]: hidden-accumulator column of the 8-channel piece pp of the 128-channel operand P (-1 = zeros)
  *   w: bf16 rows of 64, blocks of [hi: 128 rows][lo: 128 rows]; one block per tap of chain 0, 1, 2, then two blocks of the
  *      aggregation weights (K blocks of P), then one of the projection; output channel n of an N-wide chain sits in row
- *      n (n < N/2) or 64 + n - N/2 (the two CTAs of a pair each load 64 rows)
+ *      n (n < N/2) or 64 + n - N/2
  *   hid_bias [B*T][128] (P order), img_bias [B*T][64] (aggregation bias + pooling branch), res_bias [B*T][64] or NULL
  *   col_sums optional (B*T, 64): per-image sums over pixels of the output; scratch: stp3_block_fused_scratch_bytes(B*T)
  */

@@ -5,16 +5,16 @@ import this file.  The product package (stp3_b200/) never does.
 
 Restates, in numpy with every fp32 rounding step written out explicitly:
 
-  * frustum axes                  /root/reference/stp3/models/stp3.py:111-130
-  * camera->ego geometry          /root/reference/stp3/models/stp3.py:186-201
-  * softmax(depth) (x) context    /root/reference/stp3/models/stp3.py:215-216
-  * sequential ego-motion warp    /root/reference/stp3/models/stp3.py:270-277
-  * voxel index (div + trunc)     /root/reference/stp3/models/stp3.py:287-289
-  * in-bounds mask and rank       /root/reference/stp3/models/stp3.py:239-255
-  * per-pillar sum                /root/reference/stp3/utils/geometry.py:299-318 (VoxelsSumming)
-  * discount recurrence + layout  /root/reference/stp3/models/stp3.py:292-299
-  * BEV grid parameters           /root/reference/stp3/utils/geometry.py:40-59
-  * 6-DoF pose -> 4x4             /root/reference/stp3/utils/geometry.py:124-172
+  * frustum axes                  stp3/models/stp3.py:111-130
+  * camera->ego geometry          stp3/models/stp3.py:186-201
+  * softmax(depth) (x) context    stp3/models/stp3.py:215-216
+  * sequential ego-motion warp    stp3/models/stp3.py:270-277
+  * voxel index (div + trunc)     stp3/models/stp3.py:287-289
+  * in-bounds mask and rank       stp3/models/stp3.py:239-255
+  * per-pillar sum                stp3/utils/geometry.py:299-318 (VoxelsSumming)
+  * discount recurrence + layout  stp3/models/stp3.py:292-299
+  * BEV grid parameters           stp3/utils/geometry.py:40-59
+  * 6-DoF pose -> 4x4             stp3/utils/geometry.py:124-172
 
 Parity pinning: the reference ships NO tests, golden vectors or fixtures for this path
 (SURVEY.md §4/§8c), so the oracle is pinned against outputs of the reference itself, run in the

@@ -1,5 +1,5 @@
 """Generates tests/golden/lift_splat_*.npz by running the UNMODIFIED reference (imported from
-/root/reference through oracle/ref_loader.py) on seeded synthetic inputs, on the CPU of the build
+the reference checkout through oracle/ref_loader.py) on seeded synthetic inputs, on the CPU of the build
 container.  Test infrastructure; run by hand:  python -m oracle.make_golden [case ...]
 
 The reference has no tests/fixtures of its own (SURVEY.md §4), so these files are what pins the

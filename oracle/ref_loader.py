@@ -1,10 +1,10 @@
 """TEST INFRASTRUCTURE — never imported by the product package.
 
-Imports the UNMODIFIED reference (OpenDriveLab/ST-P3 @ /root/reference) on CPU by
-stubbing the third-party packages that are absent from this image (SURVEY.md §8c).
-Only usable where /root/reference exists (the build container); the GPU box does
-not have it, so everything produced with this loader is shipped as fixtures under
-tests/golden/ (see oracle/make_golden.py).
+Imports the UNMODIFIED reference (OpenDriveLab/ST-P3; the install build() makes under
+oracle/_ref/, or STP3_REFERENCE_ROOT) on CPU by stubbing the third-party packages that
+are absent from this image (SURVEY.md §8c).  Tests must not depend on it: everything
+produced with this loader is stored as fixtures under tests/golden/ (see
+oracle/make_golden.py).
 
 Nothing from the reference is copied: the modules are imported from where they lie.
 """
@@ -14,10 +14,9 @@ import types
 from types import SimpleNamespace
 
 _REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-# the reference where it lies (build container), else its unmodified install under the git-ignored baseline/_ref/
-# (oracle/build_ref.py; that copy travels to the GPU box)
-_CANDIDATES = [os.environ.get("STP3_REFERENCE_ROOT"), "/root/reference", os.path.join(_REPO, "baseline", "_ref")]
-REFERENCE_ROOT = next((c for c in _CANDIDATES if c and os.path.isdir(os.path.join(c, "stp3"))), "/root/reference")
+# STP3_REFERENCE_ROOT when set, else the unmodified install under the git-ignored oracle/_ref/ (oracle/build_ref.py)
+_CANDIDATES = [os.environ.get("STP3_REFERENCE_ROOT"), os.path.join(_REPO, "oracle", "_ref")]
+REFERENCE_ROOT = next((c for c in _CANDIDATES if c and os.path.isdir(os.path.join(c, "stp3"))), _CANDIDATES[-1])
 
 
 def reference_available() -> bool:

@@ -7,12 +7,12 @@ imported through oracle/ref_loader.py in the build container, or the drop-in mod
 same names) and evaluates the reference semantics with torch.nn.functional ops in the dtype of the input (fp32 like
 the reference, or fp64 for a tighter oracle).  Nothing here calls the modules' own forward().
 
-  conv_1x1x1_norm_activated / CausalConv3d   /root/reference/stp3/layers/temporal.py:252-273, 315-325
-  PyramidSpatioTemporalPooling               /root/reference/stp3/layers/temporal.py:375-423
-  TemporalBlock                              /root/reference/stp3/layers/temporal.py:426-489
-  ASPP / DeepLabHead / UpsamplingAdd         /root/reference/stp3/layers/convolutions.py:204-280
-  TemporalModel                              /root/reference/stp3/models/temporal_model.py:50-60
-  Decoder (+ torchvision BasicBlock)         /root/reference/stp3/models/decoder.py:91-140
+  conv_1x1x1_norm_activated / CausalConv3d   stp3/layers/temporal.py:252-273, 315-325
+  PyramidSpatioTemporalPooling               stp3/layers/temporal.py:375-423
+  TemporalBlock                              stp3/layers/temporal.py:426-489
+  ASPP / DeepLabHead / UpsamplingAdd         stp3/layers/convolutions.py:204-280
+  TemporalModel                              stp3/models/temporal_model.py:50-60
+  Decoder (+ torchvision BasicBlock)         stp3/models/decoder.py:91-140
 
 Pinned by tests/test_dense_oracle.py: (a) in the build container against the reference modules' own forward on the
 same weights, (b) everywhere against tests/golden/dense_*.npz produced from the reference by oracle/make_golden.py.

@@ -2,15 +2,15 @@
 
 Only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline / `--impl reference` leg may import this.
 
-The reference is pure Python/PyTorch (SURVEY.md §0) and cannot travel to the GPU box (/root/reference does not
-exist there), so the "reference arm" of bench.py times THIS port: it issues the same ATen operator sequence, with
+The reference is pure Python/PyTorch (SURVEY.md §0) and is not part of this repository (it need not
+be present where bench.py runs), so the "reference arm" of bench.py times THIS port: it issues the same ATen operator sequence, with
 the same materialised intermediates (17 MB geometry, 371 MB outer product, boolean-mask index, argsort, cumsum
 trick, index_put, per-frame Python loops), as
 
-    STP3.get_geometry                    /root/reference/stp3/models/stp3.py:186-201
-    STP3.encoder_forward (softmax, (x))  /root/reference/stp3/models/stp3.py:214-221
-    STP3.projection_to_birds_eye_view    /root/reference/stp3/models/stp3.py:226-301
-    VoxelsSumming.forward                /root/reference/stp3/utils/geometry.py:299-318
+    STP3.get_geometry                    stp3/models/stp3.py:186-201
+    STP3.encoder_forward (softmax, (x))  stp3/models/stp3.py:214-221
+    STP3.projection_to_birds_eye_view    stp3/models/stp3.py:226-301
+    VoxelsSumming.forward                stp3/utils/geometry.py:299-318
 
 tests/test_torch_port.py checks it against the golden vectors made from the real reference (bitwise on ranks via
 the pooled output pattern, and to fp32 round-off on BEV values).  cpu_baseline.kind == "port".

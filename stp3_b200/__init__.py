@@ -1,4 +1,4 @@
-"""stp3_b200 — B200-native (sm_100a) implementation of ST-P3's camera->BEV perception hot path.
+"""stp3_b200 — H100-native (sm_90a) implementation of ST-P3's camera->BEV perception hot path.
 
 Host side: Python/PyTorch modules that keep the reference's nn.Module surfaces
 (stp3.models.encoder.Encoder, stp3.layers.temporal.TemporalBlock, stp3.models.temporal_model.TemporalModel,

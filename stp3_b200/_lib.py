@@ -1,8 +1,8 @@
 """ctypes loader for libstp3_b200.so (the C ABI declared in include/stp3_b200.h).
 
 There is NO fallback: if the library is missing or was not built, using an op raises.  The library is
-built in-tree (stp3_b200/csrc/Makefile, driven by __graft_entry__.build()) so that the .so travels with the
-repository snapshot to the GPU box.
+built in-tree (stp3_b200/csrc/Makefile, driven by __graft_entry__.build()), so the package is importable from the
+repository tree.
 """
 import ctypes
 import os
@@ -88,7 +88,7 @@ SIGNATURES = {
 
 
 def build(verbose: bool = False) -> str:
-    """Compile csrc/*.cu for sm_100a into stp3_b200/libstp3_b200.so (nvcc cross-compiles without a GPU)."""
+    """Compile csrc/*.cu for sm_90a into stp3_b200/libstp3_b200.so (nvcc cross-compiles without a GPU)."""
     cmd = ["make", "-C", os.path.join(_HERE, "csrc"), "-j8"]
     res = subprocess.run(cmd, capture_output=True, text=True)
     if verbose or res.returncode != 0:

@@ -1,45 +1,42 @@
-// ASPP branches + 1x1 projection as ONE back-to-back tcgen05 kernel (DeepLabHead of the temporal model,
+// ASPP branches + 1x1 projection as ONE back-to-back wgmma kernel (DeepLabHead of the temporal model,
 // stp3/layers/convolutions.py:242-270: four conv/BN/ReLU branches of the same input, concatenated, then project.0).
 //
 // The unfused form writes the 4 x 128-channel concat tensor to HBM (4 x 246 MB for a 4-sample step) and reads it back
-// (984 MB) -- the largest avoidable traffic of the dense path.  Here a CTA pair keeps a 16x16-pixel tile on chip:
+// (984 MB) -- the largest avoidable traffic of the dense path.  Here a CTA keeps an 8x16-pixel tile on chip:
 //
-//   for every branch b:   acc1  = sum_taps A(x, tap) . W_b[tap]            (tcgen05.mma cta_group::2, M = 256, N = 128)
-//                         P     = hi/lo split of relu(acc1 + bias_b)       (epilogue warps: TMEM -> registers -> SHARED memory,
-//                                                                           written in the 128B-swizzled K-major operand layout)
+//   for every branch b:   acc1  = sum_taps A(x, tap) . W_b[tap]            (wgmma, 64 rows per warpgroup, N = 128)
+//                         P     = hi/lo split of relu(acc1 + bias_b)       (registers -> SHARED memory, written in the
+//                                                                           128B-swizzled K-major operand layout)
 //                         acc2 += P . W_proj[:, b-th 128 input channels]   (second MMA chain, A operand = P)
 //   out = hi/lo split of relu(acc2 + per-image bias)                       (the global-pool branch is that bias)
 //
 // The same kernel runs the head's tail, 3x3 conv/BN/ReLU -> 1x1 classifier (convolutions.py:272-280), as a ONE-branch
 // instance (9 taps, two input K blocks, classifier rows padded to 128, no ReLU on the output).
 //
-// Same precision scheme as conv_tcgen05.cu (bf16 hi/lo planes, hi*hi + hi*lo + lo*hi, fp32 accumulation in TMEM), so the
-// result matches the unfused path to the last few bits of the split.
+// Same precision scheme as conv_igemm.cu (bf16 hi/lo planes, hi*hi + hi*lo + lo*hi, fp32 accumulation), so the result
+// matches the unfused path to the last few bits of the split.
 //
-//   warps : 0 = TMA producer (activation ring + weight ring, both CTAs), 1 = MMA issuer (leader CTA), 2..9 = epilogue
-//   MMA order: main(0), main(1), proj(0), main(2), proj(1), main(3), proj(2), main(0 of the next tile), proj(3), ... -- the
-//   projection of a (tile, branch) unit is issued after the main loop of the NEXT unit, so the tensor pipe works on that
-//   while the epilogue converts the finished one
-//   TMEM  : acc1 double-buffered (2 x 128 columns), acc2 128 columns
-//   smem  : 3 activation stages (32 KB) + 3 weight stages (16 KB) + P (2 K-blocks x hi/lo x 16 KB = 64 KB) = 208 KB
+//   warps : 0..7 = two warpgroups (rows 0..63 / 64..127 of the tile; each reads back only its own rows of P), 8 = TMA
+//           producer (activation ring + weight ring)
+//   smem  : 2 activation stages (64 KB) + 2 weight stages (64 KB) + P (2 K-blocks x hi/lo x 16 KB = 64 KB) = 192 KB
 #include <cuda_bf16.h>
 
 #include "common.cuh"
 #include "ptx.cuh"
+#include "wgmma.cuh"
 
 namespace stp3 {
 
-constexpr int kAsppThreads = 320;                 // 2 + 8 warps
+constexpr int kAsppThreads = 288;                 // 8 + 1 warps
 constexpr int kAsppMaxBranches = 4;
 constexpr int kAsppMaxTaps = 9 * kAsppMaxBranches;
-constexpr int kAsppNA = 3, kAsppNB = 3;
+constexpr int kAsppNA = 2, kAsppNB = 2;
 constexpr int kAStage = 2 * 8 * 16 * 128;         // hi + lo planes of 8 image rows x 16 pixels x 64 channels
-constexpr int kBStage = 2 * 64 * 128;             // hi + lo rows of this CTA's half (64) of the 128 weight rows
+constexpr int kBStage = 2 * 128 * 128;            // hi + lo planes of the 128 weight rows
 constexpr int kPPlane = 128 * 128;                // 128 pixel rows x 64 bf16
 constexpr int kAsppHidden = 128;
 
 struct AsppParams {
-  int early_trigger;       // debug switch: griddepcontrol.launch_dependents at the top of the kernel
   int n_img, T, T_total, H, W;
   int tiles_x, tiles_y, n_tiles;
   int kblocks;
@@ -56,7 +53,7 @@ struct AsppParams {
 };
 
 __device__ __forceinline__ bool aspp_tap_is_padding(const AsppParams& p, int t, int oy_tile, int ox0) {
-  const int ylo = oy_tile + p.tap[t][0], yhi = oy_tile + 15 + p.tap[t][0];
+  const int ylo = oy_tile + p.tap[t][0], yhi = oy_tile + 7 + p.tap[t][0];
   const int xlo = ox0 + p.tap[t][1], xhi = ox0 + 15 + p.tap[t][1];
   return yhi < 0 || ylo >= p.H || xhi < 0 || xlo >= p.W;
 }
@@ -64,75 +61,50 @@ __device__ __forceinline__ bool aspp_tap_is_padding(const AsppParams& p, int t, 
 __global__ void __launch_bounds__(kAsppThreads, 1)
 aspp_fused_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ CUtensorMap tm_a_lo,
                   const __grid_constant__ CUtensorMap tm_w, const AsppParams p) {
-  const uint32_t rank = ptx::cluster_ctarank();
-  const int cta = (int)(blockIdx.x >> 1), n_cta = (int)(gridDim.x >> 1);
+  const int cta = (int)blockIdx.x, n_cta = (int)gridDim.x;
   extern __shared__ unsigned char smem_raw[];
   unsigned char* smem = smem_raw + ((1024u - (ptx::smem_u32(smem_raw) & 1023u)) & 1023u);
   unsigned char* a_ring = smem;
   unsigned char* b_ring = a_ring + kAsppNA * kAStage;
   unsigned char* p_buf = b_ring + kAsppNB * kBStage;            // [kb2][hi | lo][128 rows x 128 B]
   float* s_bias = reinterpret_cast<float*>(p_buf + 4 * kPPlane);   // [n_br][128]
-  float* s_wb = s_bias + kAsppMaxBranches * kAsppHidden;           // [8 warps][64] per-image bias slices
-  uint64_t* bars = reinterpret_cast<uint64_t*>(s_wb + 8 * 64);
+  float* s_wb = s_bias + kAsppMaxBranches * kAsppHidden;           // [2 warpgroups][128] per-image bias
+  uint64_t* bars = reinterpret_cast<uint64_t*>(s_wb + 2 * kAsppHidden);
   uint64_t* a_full = bars;
   uint64_t* a_empty = a_full + kAsppNA;
   uint64_t* b_full = a_empty + kAsppNA;
   uint64_t* b_empty = b_full + kAsppNB;
-  uint64_t* acc1_full = b_empty + kAsppNB;        // [2]
-  uint64_t* acc1_empty = acc1_full + 2;           // [2]
-  uint64_t* p_full = acc1_empty + 2;              // [2] (per K block of P)
-  uint64_t* p_empty = p_full + 2;                 // [2]
-  uint64_t* acc2_full = p_empty + 2;
-  uint64_t* acc2_empty = acc2_full + 1;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc2_empty + 1);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (p.early_trigger) ptx::griddep_launch_dependents();
-  if (warp == 0 && lane == 0) {
+  if (warp == 8 && lane == 0) {
     ptx::prefetch_tmap(&tm_a_hi); ptx::prefetch_tmap(&tm_a_lo); ptx::prefetch_tmap(&tm_w);
-    for (int i = 0; i < kAsppNA; ++i) { ptx::mbar_init(&a_full[i], 2); ptx::mbar_init(&a_empty[i], 1); }
-    for (int i = 0; i < kAsppNB; ++i) { ptx::mbar_init(&b_full[i], 2); ptx::mbar_init(&b_empty[i], 1); }
-    for (int i = 0; i < 2; ++i) {
-      ptx::mbar_init(&acc1_full[i], 1);
-      ptx::mbar_init(&acc1_empty[i], 16);         // 8 epilogue warps of both CTAs
-      ptx::mbar_init(&p_full[i], 8);              // the 4 warps of one column half, both CTAs
-      ptx::mbar_init(&p_empty[i], 1);
-    }
-    ptx::mbar_init(acc2_full, 1);
-    ptx::mbar_init(acc2_empty, 16);
+    for (int i = 0; i < kAsppNA; ++i) { ptx::mbar_init(&a_full[i], 1); ptx::mbar_init(&a_empty[i], 2); }
+    for (int i = 0; i < kAsppNB; ++i) { ptx::mbar_init(&b_full[i], 1); ptx::mbar_init(&b_empty[i], 2); }
     ptx::fence_mbar_init();
   }
-  if (warp == 1) ptx::tmem_alloc_pair<512>(tmem_slot);
   for (int i = threadIdx.x; i < p.n_br * kAsppHidden; i += blockDim.x) s_bias[i] = p.br_bias[i];
-  ptx::tc_fence_before();
   __syncthreads();
-  ptx::cluster_sync();
-  ptx::tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   const int tiles_per_img = p.tiles_x * p.tiles_y;
   const int proj_blk0 = p.br_tap0[p.n_br] * p.kblocks;          // first projection block of the weight tensor
 
-  if (warp == 0) {
+  if (warp == 8) {
     // ===================== TMA producer =====================
     ptx::griddep_wait();
     int as = 0, bs = 0; uint32_t aph = 0, bph = 0;
-    auto load_b = [&](int blk) {                   // weight block `blk`: [hi 128 rows][lo 128 rows]; this CTA takes 64 of each
+    auto load_b = [&](int blk) {                   // weight block `blk`: [hi 128 rows][lo 128 rows]
       ptx::mbar_wait(&b_empty[bs], bph ^ 1);
       if (ptx::elect_one_sync()) {
-        const uint32_t bar = ptx::mapa(ptx::smem_u32(&b_full[bs]), 0);
         unsigned char* dst = b_ring + (size_t)bs * kBStage;
-        ptx::mbar_arrive_expect_tx_cluster(bar, (uint32_t)kBStage);
-        ptx::tma_load_2d_pair(dst, &tm_w, bar, 0, blk * 256 + (int)rank * 64);
-        ptx::tma_load_2d_pair(dst + 64 * 128, &tm_w, bar, 0, blk * 256 + 128 + (int)rank * 64);
+        ptx::mbar_arrive_expect_tx(&b_full[bs], (uint32_t)kBStage);
+        ptx::tma_load_2d(dst, &tm_w, &b_full[bs], 0, blk * 256);
+        ptx::tma_load_2d(dst + 128 * 128, &tm_w, &b_full[bs], 0, blk * 256 + 128);
       }
       __syncwarp();
       if (++bs == kAsppNB) { bs = 0; bph ^= 1; }
     };
-    int pend = -1;                                 // branch whose projection weights follow the next main loop's
     for (int tile = cta; tile < p.n_tiles; tile += n_cta) {
       const int img = tile / tiles_per_img, rem = tile % tiles_per_img;
-      const int oy_tile = (rem / p.tiles_x) * 16, ox0 = (rem % p.tiles_x) * 16;
-      const int oy0 = oy_tile + (int)rank * 8;
+      const int oy_tile = (rem / p.tiles_x) * 8, ox0 = (rem % p.tiles_x) * 16;
       const int bidx = img / p.T, tidx = img % p.T;
       for (int s = 0; s < p.n_br; ++s) {
         for (int t = p.br_tap0[s]; t < p.br_tap0[s + 1]; ++t) {
@@ -141,202 +113,133 @@ aspp_fused_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
             ptx::mbar_wait(&a_empty[as], aph ^ 1);
             if (ptx::elect_one_sync()) {
               unsigned char* sa = a_ring + (size_t)as * kAStage;
-              const uint32_t bar = ptx::mapa(ptx::smem_u32(&a_full[as]), 0);
-              ptx::mbar_arrive_expect_tx_cluster(bar, (uint32_t)kAStage);
-              ptx::tma_load_5d_pair(sa, &tm_a_hi, bar, kb * 64, ox0 + p.tap[t][1], oy0 + p.tap[t][0], tidx, bidx);
-              ptx::tma_load_5d_pair(sa + kAStage / 2, &tm_a_lo, bar, kb * 64, ox0 + p.tap[t][1], oy0 + p.tap[t][0], tidx, bidx);
+              ptx::mbar_arrive_expect_tx(&a_full[as], (uint32_t)kAStage);
+              ptx::tma_load_5d(sa, &tm_a_hi, &a_full[as], kb * 64, ox0 + p.tap[t][1], oy_tile + p.tap[t][0], tidx, bidx);
+              ptx::tma_load_5d(sa + kAStage / 2, &tm_a_lo, &a_full[as], kb * 64, ox0 + p.tap[t][1], oy_tile + p.tap[t][0], tidx, bidx);
             }
             __syncwarp();
             if (++as == kAsppNA) { as = 0; aph ^= 1; }
             load_b(t * p.kblocks + kb);
           }
         }
-        if (pend >= 0) { load_b(proj_blk0 + pend * 2); load_b(proj_blk0 + pend * 2 + 1); }   // projection weights of the previous unit
-        pend = s;
+        load_b(proj_blk0 + s * 2); load_b(proj_blk0 + s * 2 + 1);   // projection weights of this branch
       }
     }
-    if (pend >= 0) { load_b(proj_blk0 + pend * 2); load_b(proj_blk0 + pend * 2 + 1); }
-  } else if (warp == 1 && rank == 0) {
-    // ===================== MMA issuer (leader) =====================
-    const uint32_t idesc = ptx::umma_idesc_bf16(256, kAsppHidden);
+  } else {
+    // ===================== two warpgroups: branch MMAs, conversion to P, projection, output =====================
+    const int wg = warp >> 2, wq = warp & 3;
+    const int wtid = threadIdx.x & 127;
+    const bool wg_leader = wtid == 0;
+    const int row0 = wg * 64 + wq * 16 + (lane >> 2);       // accumulator rows of this thread: row0, row0 + 8
+    const int cq = 2 * (lane & 3);                           // first of its two columns in every 8-column group
+    float* wb = s_wb + wg * kAsppHidden;
     int as = 0, bs = 0; uint32_t aph = 0, bph = 0;
-    int buf1 = 0; uint32_t acc1_ph = 0, pph = 0, t2ph = 0;
-    auto issue = [&](uint32_t tmem_d, uint32_t a_hi, uint32_t a_lo, uint32_t b_hi, uint32_t b_lo, uint32_t accumulate) {
-      const uint64_t da_hi = ptx::umma_desc_k_sw128(a_hi), da_lo = ptx::umma_desc_k_sw128(a_lo);
-      const uint64_t db_hi = ptx::umma_desc_k_sw128(b_hi), db_lo = ptx::umma_desc_k_sw128(b_lo);
+    int pend_a = -1, pend_b = -1;               // ring slots read by the last committed wgmma group
+    auto release = [&]() {
+      if (wg_leader) {
+        if (pend_a >= 0) ptx::mbar_arrive(&a_empty[pend_a]);
+        if (pend_b >= 0) ptx::mbar_arrive(&b_empty[pend_b]);
+      }
+      pend_a = pend_b = -1;
+    };
+    auto issue = [&](float* acc, uint32_t a_hi, uint32_t a_lo, uint32_t b_hi, uint32_t b_lo, uint32_t accumulate,
+                     int slot_a, int slot_b) {
+      const uint64_t da_hi = wg::desc_k_sw128(a_hi), da_lo = wg::desc_k_sw128(a_lo);
+      const uint64_t db_hi = wg::desc_k_sw128(b_hi), db_lo = wg::desc_k_sw128(b_lo);
+      wg::fence();
 #pragma unroll
       for (int k = 0; k < 4; ++k) {
         const uint64_t koff = (uint64_t)((k * 32) >> 4);
-        ptx::umma_bf16_pair(tmem_d, da_hi + koff, db_hi + koff, idesc, accumulate | (uint32_t)k);
-        ptx::umma_bf16_pair(tmem_d, da_hi + koff, db_lo + koff, idesc, 1);
-        ptx::umma_bf16_pair(tmem_d, da_lo + koff, db_hi + koff, idesc, 1);
+        wg::mma_bf16<kAsppHidden>(acc, da_hi + koff, db_hi + koff, accumulate | (uint32_t)k);
+        wg::mma_bf16<kAsppHidden>(acc, da_hi + koff, db_lo + koff, 1);
+        wg::mma_bf16<kAsppHidden>(acc, da_lo + koff, db_hi + koff, 1);
       }
+      wg::commit();
+      wg::wait<1>();
+      release();
+      pend_a = slot_a; pend_b = slot_b;
     };
-    const uint32_t tmem_d2 = tmem_base + 2u * kAsppHidden;
-    // proj(j): acc2 (+)= P . W_proj[:, branch j]; issued one unit late (after the NEXT main loop, also across tiles), so the
-    // tensor pipe never waits for the epilogue's conversion of the unit it has just finished
-    auto proj = [&](int j) {
-      if (j == 0) {                                // the previous tile's output has left acc2
-        ptx::mbar_wait(acc2_empty, t2ph ^ 1);
-        ptx::tc_fence_after();
-      }
-      for (int kb2 = 0; kb2 < 2; ++kb2) {
-        ptx::mbar_wait(&p_full[kb2], pph);
-        ptx::mbar_wait(&b_full[bs], bph);
-        ptx::tc_fence_after();
-        if (ptx::elect_one_sync()) {
-          const uint32_t a_hi = ptx::smem_u32(p_buf + (size_t)kb2 * 2 * kPPlane);
-          const uint32_t b_hi = ptx::smem_u32(b_ring + (size_t)bs * kBStage);
-          issue(tmem_d2, a_hi, a_hi + kPPlane, b_hi, b_hi + 64 * 128, (j > 0 || kb2 > 0) ? 1u : 0u);
-          ptx::umma_commit_pair(&b_empty[bs]);
-          ptx::umma_commit_pair(&p_empty[kb2]);
-        }
-        __syncwarp();
-        if (++bs == kAsppNB) { bs = 0; bph ^= 1; }
-      }
-      pph ^= 1;
-      if (j == p.n_br - 1) {
-        if (ptx::elect_one_sync()) ptx::umma_commit_pair(acc2_full);
-        __syncwarp();
-        t2ph ^= 1;
-      }
-    };
-    int pend = -1;
+    ptx::griddep_wait();
     for (int tile = cta; tile < p.n_tiles; tile += n_cta) {
-      const int rem = tile % tiles_per_img;
-      const int oy_tile = (rem / p.tiles_x) * 16, ox0 = (rem % p.tiles_x) * 16;
+      const int img = tile / tiles_per_img, rem = tile % tiles_per_img;
+      const int oy_tile = (rem / p.tiles_x) * 8, ox0 = (rem % p.tiles_x) * 16;
+      ptx::bar_sync(1 + wg, 128);                // the previous tile's output has read the per-image bias
+      // written by the preceding (PDL-overlapped) pool_bias kernel: coherent loads
+      wb[wtid] = *(reinterpret_cast<const volatile float*>(p.img_bias) + (size_t)img * kAsppHidden + wtid);
+      float acc2[kAsppHidden / 2];
       for (int s = 0; s < p.n_br; ++s) {
-        // ---- main(s): acc1[buf1] = sum over the branch's taps
-        ptx::mbar_wait(&acc1_empty[buf1], acc1_ph ^ 1);
-        ptx::tc_fence_after();
-        const uint32_t tmem_d = tmem_base + (uint32_t)(buf1 * kAsppHidden);
+        // ---- main(s): acc1 = sum over the branch's taps
+        float acc1[kAsppHidden / 2];
         uint32_t accumulate = 0;
         for (int t = p.br_tap0[s]; t < p.br_tap0[s + 1]; ++t) {
           if (aspp_tap_is_padding(p, t, oy_tile, ox0)) continue;
           for (int kb = 0; kb < p.kblocks; ++kb) {
             ptx::mbar_wait(&a_full[as], aph);
             ptx::mbar_wait(&b_full[bs], bph);
-            ptx::tc_fence_after();
-            if (ptx::elect_one_sync()) {
-              const uint32_t a_hi = ptx::smem_u32(a_ring + (size_t)as * kAStage);
-              const uint32_t b_hi = ptx::smem_u32(b_ring + (size_t)bs * kBStage);
-              issue(tmem_d, a_hi, a_hi + kAStage / 2, b_hi, b_hi + 64 * 128, accumulate);
-              ptx::umma_commit_pair(&b_empty[bs]);
-              ptx::umma_commit_pair(&a_empty[as]);
-            }
-            __syncwarp();
+            const uint32_t a_hi = ptx::smem_u32(a_ring + (size_t)as * kAStage) + (uint32_t)(wg * 64 * 128);
+            const uint32_t b_hi = ptx::smem_u32(b_ring + (size_t)bs * kBStage);
+            issue(acc1, a_hi, a_hi + kAStage / 2, b_hi, b_hi + 128 * 128, accumulate, as, bs);
             accumulate = 1;
             if (++as == kAsppNA) { as = 0; aph ^= 1; }
             if (++bs == kAsppNB) { bs = 0; bph ^= 1; }
           }
         }
-        if (ptx::elect_one_sync()) ptx::umma_commit_pair(&acc1_full[buf1]);
-        __syncwarp();
-        if (++buf1 == 2) { buf1 = 0; acc1_ph ^= 1; }
-        if (pend >= 0) proj(pend);
-        pend = s;
-      }
-    }
-    if (pend >= 0) proj(pend);
-  } else if (warp >= 2) {
-    // ===================== epilogue =====================
-    const int e = warp - 2;
-    const int q = warp & 3;
-    const int half = e >> 2;                       // column half = K block of P this warp produces
-    const int r = q * 32 + lane;                   // accumulator row = pixel of this CTA's 8x16 sub-tile
-    const int col0 = half * 64;
-    int buf1 = 0; uint32_t acc1_ph = 0, pph = 0, t2ph = 0;
-    unsigned char* p_hi = p_buf + (size_t)half * 2 * kPPlane + (size_t)r * 128;
-    unsigned char* p_lo = p_hi + kPPlane;
-    const uint32_t sw = (uint32_t)(r & 7);
-    ptx::griddep_wait();
-    for (int tile = cta; tile < p.n_tiles; tile += n_cta) {
-      const int img = tile / tiles_per_img, rem = tile % tiles_per_img;
-      const int oy = (rem / p.tiles_x) * 16 + (int)rank * 8 + (r >> 4), ox = (rem % p.tiles_x) * 16 + (r & 15);
-      {                                            // this warp's slice of the per-image projection bias
-        const float* ib = p.img_bias + (size_t)img * kAsppHidden + col0;
-        float* wb = s_wb + e * 64;
-        __syncwarp();
-        const volatile float* ibv = ib;            // written by the preceding (PDL-overlapped) pool_bias kernel: coherent loads
-        wb[lane] = ibv[lane]; wb[lane + 32] = ibv[lane + 32];
-        __syncwarp();
-      }
-      for (int b = 0; b < p.n_br; ++b) {
-        ptx::mbar_wait(&acc1_full[buf1], acc1_ph);
-        ptx::mbar_wait(&p_empty[half], pph ^ 1);   // the projection of the previous branch has read P
-        ptx::tc_fence_after();
-        const uint32_t tmem_acc = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(buf1 * kAsppHidden + col0);
-        const float* bias = s_bias + b * kAsppHidden + col0;
-#pragma unroll 1
-        for (int j = 0; j < 4; ++j) {
-          uint32_t acc[16];
-          ptx::tmem_ld_32x32b_x16(tmem_acc + j * 16, acc);
-          ptx::tmem_ld_wait();
-          uint32_t hw[8], lw[8];
+        wg::wait<0>();                             // also: the previous branch's projection has read P
+        release();
+        // ---- P = hi/lo split of relu(acc1 + bias): column c -> K block c / 64, 16-byte chunk (c % 64) / 8 of the
+        // 128-byte row, XOR-swizzled with the row index (the layout TMA writes for a SWIZZLE_128B K-major operand)
+        const float* bias = s_bias + s * kAsppHidden;
 #pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            const float x0 = fmaxf(__uint_as_float(acc[2 * i]) + bias[j * 16 + 2 * i], 0.f);
-            const float x1 = fmaxf(__uint_as_float(acc[2 * i + 1]) + bias[j * 16 + 2 * i + 1], 0.f);
-            const uint32_t h = ptx::pack_bf16x2(x0, x1);
-            hw[i] = h;
-            lw[i] = ptx::pack_bf16x2(x0 - __uint_as_float(h << 16), x1 - __uint_as_float(h & 0xFFFF0000u));
+        for (int g8 = 0; g8 < 16; ++g8) {
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int row = row0 + 8 * h;
+            const float x0 = fmaxf(acc1[4 * g8 + 2 * h] + bias[8 * g8 + cq], 0.f);
+            const float x1 = fmaxf(acc1[4 * g8 + 2 * h + 1] + bias[8 * g8 + cq + 1], 0.f);
+            const uint32_t hw = ptx::pack_bf16x2(x0, x1);
+            const uint32_t lw = ptx::pack_bf16x2(x0 - __uint_as_float(hw << 16), x1 - __uint_as_float(hw & 0xFFFF0000u));
+            unsigned char* dst = p_buf + (size_t)(g8 >> 3) * 2 * kPPlane + (size_t)row * 128 +
+                                 ((((uint32_t)g8 & 7u) ^ (uint32_t)(row & 7)) << 4) + cq * 2;
+            *reinterpret_cast<uint32_t*>(dst) = hw;
+            *reinterpret_cast<uint32_t*>(dst + kPPlane) = lw;
           }
-          // channels [j*16, j*16+16) of the K block = 16-byte chunks 2j and 2j+1 of the 128-byte row, XOR-swizzled with
-          // the row index (the layout TMA writes and the UMMA descriptor of a SWIZZLE_128B K-major operand expects)
-          const uint32_t c0 = ((uint32_t)(2 * j) ^ sw) << 4, c1 = ((uint32_t)(2 * j + 1) ^ sw) << 4;
-          *reinterpret_cast<uint4*>(p_hi + c0) = make_uint4(hw[0], hw[1], hw[2], hw[3]);
-          *reinterpret_cast<uint4*>(p_hi + c1) = make_uint4(hw[4], hw[5], hw[6], hw[7]);
-          *reinterpret_cast<uint4*>(p_lo + c0) = make_uint4(lw[0], lw[1], lw[2], lw[3]);
-          *reinterpret_cast<uint4*>(p_lo + c1) = make_uint4(lw[4], lw[5], lw[6], lw[7]);
         }
-        ptx::tc_fence_before();
         ptx::fence_proxy_async();                  // the generic-proxy stores above are read by the tensor core (async proxy)
-        __syncwarp();
-        if (lane == 0) {
-          ptx::mbar_arrive_cluster(ptx::mapa(ptx::smem_u32(&acc1_empty[buf1]), 0));
-          ptx::mbar_arrive_cluster(ptx::mapa(ptx::smem_u32(&p_full[half]), 0));
+        ptx::bar_sync(1 + wg, 128);
+        // ---- proj(s): acc2 (+)= P . W_proj[:, branch s]
+        for (int kb2 = 0; kb2 < 2; ++kb2) {
+          ptx::mbar_wait(&b_full[bs], bph);
+          const uint32_t a_hi = ptx::smem_u32(p_buf + (size_t)kb2 * 2 * kPPlane) + (uint32_t)(wg * 64 * 128);
+          const uint32_t b_hi = ptx::smem_u32(b_ring + (size_t)bs * kBStage);
+          issue(acc2, a_hi, a_hi + kPPlane, b_hi, b_hi + 128 * 128, (s > 0 || kb2 > 0) ? 1u : 0u, -1, bs);
+          if (++bs == kAsppNB) { bs = 0; bph ^= 1; }
         }
-        pph ^= 1;
-        if (++buf1 == 2) { buf1 = 0; acc1_ph ^= 1; }
       }
+      wg::wait<0>();
+      release();
       // ---- output of the projection: relu(acc2 + per-image bias) -> hi/lo planes
-      ptx::mbar_wait(acc2_full, t2ph);
-      ptx::tc_fence_after();
-      t2ph ^= 1;
-      const bool valid = oy < p.H && ox < p.W;
-      const size_t pix = ((size_t)img * p.H + oy) * p.W + ox;
-      const uint32_t tmem_acc2 = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(2 * kAsppHidden + col0);
-      const float* wb = s_wb + e * 64;
-#pragma unroll 1
-      for (int j = 0; j < 4; ++j) {
-        uint32_t acc[16];
-        ptx::tmem_ld_32x32b_x16(tmem_acc2 + j * 16, acc);
-        ptx::tmem_ld_wait();
-        if (valid && col0 + j * 16 < p.n_store) {
-          uint32_t hw[8], lw[8];
 #pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            float x0 = __uint_as_float(acc[2 * i]) + wb[j * 16 + 2 * i];
-            float x1 = __uint_as_float(acc[2 * i + 1]) + wb[j * 16 + 2 * i + 1];
-            if (p.relu_out) { x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); }
-            const uint32_t h = ptx::pack_bf16x2(x0, x1);
-            hw[i] = h;
-            lw[i] = ptx::pack_bf16x2(x0 - __uint_as_float(h << 16), x1 - __uint_as_float(h & 0xFFFF0000u));
-          }
-          const size_t off = pix * p.out_cstride + p.out_coff + col0 + j * 16;
-          ptx::st_global_v8(p.out_hi + off, hw);
-          ptx::st_global_v8(p.out_lo + off, lw);
+      for (int h = 0; h < 2; ++h) {
+        const int row = row0 + 8 * h;
+        const int oy = oy_tile + (row >> 4), ox = ox0 + (row & 15);
+        if (oy >= p.H || ox >= p.W) continue;
+        const size_t pix = ((size_t)img * p.H + oy) * p.W + ox;
+#pragma unroll
+        for (int g8 = 0; g8 < 16; ++g8) {
+          const int c = 8 * g8 + cq;
+          if (c >= p.n_store) continue;
+          float x0 = acc2[4 * g8 + 2 * h] + wb[c];
+          float x1 = acc2[4 * g8 + 2 * h + 1] + wb[c + 1];
+          if (p.relu_out) { x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); }
+          const uint32_t hw = ptx::pack_bf16x2(x0, x1);
+          const uint32_t lw = ptx::pack_bf16x2(x0 - __uint_as_float(hw << 16), x1 - __uint_as_float(hw & 0xFFFF0000u));
+          const size_t off = pix * p.out_cstride + p.out_coff + c;
+          *reinterpret_cast<uint32_t*>(p.out_hi + off) = hw;
+          *reinterpret_cast<uint32_t*>(p.out_lo + off) = lw;
         }
       }
-      ptx::tc_fence_before();
-      __syncwarp();
-      if (lane == 0) ptx::mbar_arrive_cluster(ptx::mapa(ptx::smem_u32(acc2_empty), 0));
     }
   }
-  ptx::tc_fence_before();
-  __syncthreads();
-  ptx::cluster_sync();
-  if (warp == 1) ptx::tmem_dealloc_pair<512>(tmem_base);
 }
 
 typedef CUresult (*PFN_tmapEncodeTiledA)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
@@ -374,7 +277,7 @@ extern "C" int stp3_aspp_fused_fwd(const stp3_aspp_desc* d, const void* x_hi, co
   if (!enc) return set_error(STP3_ECUDA, "cuTensorMapEncodeTiled is not available from the driver");
   AsppParams p;
   p.n_img = d->B * d->T; p.T = d->T; p.T_total = d->T; p.H = d->H; p.W = d->W;
-  p.tiles_x = ceil_div(d->W, 16); p.tiles_y = ceil_div(d->H, 16);
+  p.tiles_x = ceil_div(d->W, 16); p.tiles_y = ceil_div(d->H, 8);
   const long long nt = (long long)p.n_img * p.tiles_x * p.tiles_y;
   STP3_CHECK_ARG(nt < (1ll << 31), "grid too large");
   p.n_tiles = (int)nt;
@@ -414,7 +317,7 @@ extern "C" int stp3_aspp_fused_fwd(const stp3_aspp_desc* d, const void* x_hi, co
     const int n_blocks = t * p.kblocks + 2 * d->n_br;
     const cuuint64_t wd[2] = {64, (cuuint64_t)n_blocks * 256};
     const cuuint64_t ws[1] = {128};
-    const cuuint32_t wb[2] = {64, 64};
+    const cuuint32_t wb[2] = {64, 128};
     const cuuint32_t we[2] = {1, 1};
     CUresult r3 = enc(&tm_w, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(w), wd, ws, wb, we,
                       CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
@@ -422,41 +325,25 @@ extern "C" int stp3_aspp_fused_fwd(const stp3_aspp_desc* d, const void* x_hi, co
     if (r3 != CUDA_SUCCESS) return set_error(STP3_ECUDA, "cuTensorMapEncodeTiled(weights) failed: %d", (int)r3);
   }
   const size_t smem_bytes = 1024 + (size_t)kAsppNA * kAStage + (size_t)kAsppNB * kBStage + 4 * (size_t)kPPlane +
-                            (kAsppMaxBranches * kAsppHidden + 8 * 64) * sizeof(float) + 32 * 8 + 16;
-  static thread_local int attr_dev = -1, occ_val = 0;           // once per device: these calls cost microseconds per eager launch
+                            (kAsppMaxBranches + 2) * kAsppHidden * sizeof(float) + 2 * (kAsppNA + kAsppNB) * 8;
+  static thread_local int attr_dev = -1;           // once per device: the attribute call costs microseconds per eager launch
   int cur_dev = 0;
   cudaGetDevice(&cur_dev);
-  const bool first_call = attr_dev != cur_dev;
-  if (first_call) STP3_CUDA_OK(cudaFuncSetAttribute(aspp_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes));
-  int num_sms = 148, dev = 0;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev);
+  if (attr_dev != cur_dev) {
+    STP3_CUDA_OK(cudaFuncSetAttribute(aspp_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes));
+    attr_dev = cur_dev;
+  }
+  int num_sms = 132;
+  cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, cur_dev);
   cudaLaunchConfig_t cfg = {};
-  unsigned pairs = (unsigned)(nt < num_sms / 2 ? nt : num_sms / 2);
-  cfg.gridDim = dim3(2 * pairs); cfg.blockDim = dim3(kAsppThreads);
+  cfg.gridDim = dim3((unsigned)(nt < num_sms ? nt : num_sms)); cfg.blockDim = dim3(kAsppThreads);
   cfg.dynamicSmemBytes = smem_bytes; cfg.stream = stream;
-  cudaLaunchAttribute attr[2];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr; cfg.numAttrs = 1;
-  int max_clusters = occ_val;
-  if (first_call) {
-    STP3_CUDA_OK(cudaOccupancyMaxActiveClusters(&max_clusters, aspp_fused_kernel, &cfg));
-    occ_val = max_clusters; attr_dev = cur_dev;
-  }
-  if (max_clusters < 1) return set_error(STP3_EUNSUPPORTED, "no CTA pair fits on this device");
-  if (cfg.gridDim.x > 2u * (unsigned)max_clusters) cfg.gridDim.x = 2u * (unsigned)max_clusters;
-  attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[1].val.programmaticStreamSerializationAllowed = 1;
-  cfg.numAttrs = stp3_pdl_enabled("STP3_FUSED_PDL") ? 2 : 1;
-  {
-    // No early griddepcontrol.launch_dependents from the back-to-back kernels: with it, a chain block_fused -> col_sum_reduce
-    // -> pool_bias -> aspp_fused in flight at once stopped making progress about once in 400 .. 2000 replayed steps
-    // (tools/hang_probe.py; 20000 replays are clean without it and with programmatic launch off altogether).  The
-    // dependents are released when the grid completes; this kernel itself still starts early behind its predecessor.
-    static const bool early = [] { const char* e = getenv("STP3_FUSED_EARLY_TRIGGER"); return e && atoi(e) != 0; }();
-    p.early_trigger = early ? 1 : 0;
-  }
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = attr; cfg.numAttrs = stp3_pdl_enabled("STP3_FUSED_PDL") ? 1 : 0;
+  // The kernel never executes griddepcontrol.launch_dependents: its dependents are released when the grid completes
+  // (see block_fused.cu); it still starts early behind its predecessor.
   STP3_CUDA_OK(cudaLaunchKernelEx(&cfg, aspp_fused_kernel, tm_hi, tm_lo, tm_w, p));
   STP3_CUDA_OK(cudaGetLastError());
   return STP3_OK;

@@ -1,6 +1,6 @@
 // Memory-bound helpers around the tensor-core path: layout / precision-split conversions, spatial sums, the tiny
 // dense layers of the spatially constant branches, and the bilinear x2 upsample + skip add of UpsamplingAdd.
-// All activations are channels-last bf16 hi/lo planes (see conv_tcgen05.cu).
+// All activations are channels-last bf16 hi/lo planes (see conv_igemm.cu).
 #include <cuda_bf16.h>
 
 #include "common.cuh"

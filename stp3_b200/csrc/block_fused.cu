@@ -1,42 +1,41 @@
-// Tail of a TemporalBlock as ONE back-to-back tcgen05 kernel (stp3/layers/temporal.py:426-489):
+// Tail of a TemporalBlock as ONE back-to-back wgmma kernel (stp3/layers/temporal.py:426-489):
 //
 //   path 0 = causal (2,3,3) conv/BN/ReLU of mid_0      path 1 = (1,3,3) conv/BN/ReLU of mid_1      path 2 = 1x1x1 conv/BN/ReLU of x
 //   out    = relu(BN(aggregation 1x1x1 of [path 0 | path 1 | path 2 | pyramid pooling])) + (projection(x) | x)
 //
 // (mid_0 / mid_1 = the paths' 1x1x1 entry convolutions, produced by a preceding stp3_conv_fwd launch).  The unfused form
 // writes the three paths into a 128-channel concat tensor and reads it back (2 x 246 MB per block and 4-sample step) and
-// needs one more pass over x for path 2 / the projection.  Here a CTA pair keeps a 16x16-pixel tile on chip:
+// needs one more pass over x for path 2 / the projection.  Here a CTA keeps an 8x16-pixel tile on chip:
 //
 //   (taps of one kernel column share ONE activation load: the box holds 8 + 2 image rows, tap j reads it shifted by j rows)
-//   main(u) : up to three MMA chains accumulate the paths side by side into ONE TMEM accumulator (chain c at column
-//             offset 48*c / 64: the concat happens in TMEM), each chain with its own input tensor, tap list, MMA width N
-//             and K-step range
-//   convert : epilogue warps read the accumulator in 8-channel pieces, add the (per-image) bias, ReLU, split to bf16 hi/lo
-//             and write the compacted 128-channel operand P into shared memory (128B-swizzled K-major)
-//   proj(u) : acc2 = P . W_agg  (N = 64);  acc3 = x_tile . W_projection (N = 64) when the block changes its width
+//   main    : the path chains one after the other, each into a register accumulator (its own input tensor, tap list,
+//             MMA width N and K-step range); chain c's columns are the hidden channels [tmem_col, tmem_col + N)
+//   convert : straight from the registers: add the (per-image) bias, ReLU, split to bf16 hi/lo and write the 8-channel
+//             pieces of the compacted 128-channel operand P into shared memory (128B-swizzled K-major)
+//   proj    : acc2 = P . W_agg  (N = 64);  acc3 = x_tile . W_projection (N = 64) when the block changes its width
 //   final   : out = relu(acc2 + per-image bias) + (acc3 + per-image bias | x), hi/lo planes, per-image column sums
 //
-// proj(u) is issued after main(u+1), like in aspp_fused.cu.  Same precision scheme (bf16 hi/lo planes, three MMAs per
-// product, fp32 accumulation in TMEM).
+// Two warpgroups own rows 0..63 / 64..127 of the tile (the A operand of P is a warpgroup's own rows, so P needs only a
+// warpgroup barrier); warp 8 is the TMA producer.  Same precision scheme as conv_igemm.cu (bf16 hi/lo planes, three
+// MMAs per product, fp32 accumulation).
 #include <cuda_bf16.h>
 
 #include "common.cuh"
 #include "ptx.cuh"
+#include "wgmma.cuh"
 
 namespace stp3 {
 
-constexpr int kBlkThreads = 320;
+constexpr int kBlkThreads = 288;                  // 2 warpgroups + the producer warp
 constexpr int kBlkMaxChains = 3;
 constexpr int kBlkMaxTaps = 32;                 // 18 + 9 + 1 path taps + the projection's
-constexpr int kBlkNA = 3, kBlkNB = 4;          // the kernel is TMA-latency bound: as many activation bytes in flight as fit
+constexpr int kBlkNA = 2, kBlkNB = 4;          // 200 KB of operand rings and P in 227 KB of shared memory
 constexpr int kBlkBoxRows = 10;                   // 8 image rows + 2: one activation load serves the three dy taps of a kernel column
 constexpr int kBlkAStage = 2 * kBlkBoxRows * 16 * 128;
 constexpr int kBlkMaxGroups = 16;
-constexpr int kBlkBRows = 32;                     // weight rows per CTA and plane: chains are at most 64 wide
+constexpr int kBlkBRows = 64;                     // weight rows per plane: chains are at most 64 wide
 constexpr int kBlkBStage = 2 * kBlkBRows * 128;
 constexpr int kBlkPPlane = 128 * 128;
-constexpr int kAcc1Stride = 160;                  // TMEM columns between the two hidden accumulators (144 used)
-constexpr int kAcc2Col = 320, kAcc3Col = 384;
 
 struct BlkChain {
   int src;                  // 0 = mid tensor, 1 = x tensor
@@ -44,13 +43,12 @@ struct BlkChain {
   int tap0, ntaps;
   int grp0, ngrp;           // tap groups: runs of <= 3 taps with the same (dt, dx) and consecutive dy share one activation load
   int n_mma;                // MMA width (multiple of 16)
-  int tmem_col;             // column offset inside the hidden accumulator
-  int ks_first, ks_end;     // UMMA_K = 16 steps that carry data
+  int tmem_col;             // first hidden column of the chain's outputs
+  int ks_first, ks_end;     // K = 16 steps that carry data
   int wblk0;                // first weight block (one per tap)
 };
 
 struct BlkParams {
-  int early_trigger;       // debug switch: griddepcontrol.launch_dependents at the top of the kernel
   int n_img, T, H, W;
   int tiles_x, tiles_y, n_tiles;
   int n_chain;
@@ -59,7 +57,7 @@ struct BlkParams {
   BlkChain res;
   signed char tap[kBlkMaxTaps][4];        // (dt, dy, dx)
   unsigned char gstart[kBlkMaxGroups], gsize[kBlkMaxGroups];   // first tap / number of taps of every group
-  int piece_col[16];        // TMEM column (inside the hidden accumulator) of the 8-channel piece pp of P, -1 = zeros
+  int piece_col[16];        // hidden column of the 8-channel piece pp of P, -1 = zeros
   const float* hid_bias;    // [n_img][128] bias of the hidden channels in P order
   const float* img_bias;    // [n_img][64]  aggregation bias (+ pyramid-pooling branch)
   const float* res_bias;    // [n_img][64]  projection bias (has_res_proj) or null
@@ -69,15 +67,15 @@ struct BlkParams {
   __nv_bfloat16* out_hi;
   __nv_bfloat16* out_lo;
   int out_cstride;
-  float* sum_part;          // [gridDim.x * 4][n_img][64] or null
+  float* sum_part;          // [gridDim.x * 8][n_img][64] or null
   int wagg_blk0;            // two weight blocks (K blocks of P) of the aggregation conv
 };
 
-// true if every input element the tap group touches for this (whole, 16x16) tile is zero padding
+// true if every input element the tap group touches for this 8x16 tile is zero padding
 __device__ __forceinline__ bool blk_group_is_padding(const BlkParams& p, int g, int tidx, int oy_tile, int ox0) {
   const int t0 = p.gstart[g];
   const int tt = tidx + p.tap[t0][0];
-  const int ylo = oy_tile + p.tap[t0][1], yhi = oy_tile + 15 + p.tap[t0][1] + p.gsize[g] - 1;
+  const int ylo = oy_tile + p.tap[t0][1], yhi = oy_tile + 7 + p.tap[t0][1] + p.gsize[g] - 1;
   const int xlo = ox0 + p.tap[t0][2], xhi = ox0 + 15 + p.tap[t0][2];
   return tt < 0 || tt >= p.T || yhi < 0 || ylo >= p.H || xhi < 0 || xlo >= p.W;
 }
@@ -86,54 +84,35 @@ __global__ void __launch_bounds__(kBlkThreads, 1)
 block_fused_kernel(const __grid_constant__ CUtensorMap tm_m_hi, const __grid_constant__ CUtensorMap tm_m_lo,
                    const __grid_constant__ CUtensorMap tm_x_hi, const __grid_constant__ CUtensorMap tm_x_lo,
                    const __grid_constant__ CUtensorMap tm_w, const BlkParams p) {
-  const uint32_t rank = ptx::cluster_ctarank();
-  const int cta = (int)(blockIdx.x >> 1), n_cta = (int)(gridDim.x >> 1);
+  const int cta = (int)blockIdx.x, n_cta = (int)gridDim.x;
   extern __shared__ unsigned char smem_raw[];
   unsigned char* smem = smem_raw + ((1024u - (ptx::smem_u32(smem_raw) & 1023u)) & 1023u);
   unsigned char* a_ring = smem;
   unsigned char* b_ring = a_ring + kBlkNA * kBlkAStage;
   unsigned char* p_buf = b_ring + kBlkNB * kBlkBStage;          // [kb2][hi | lo][128 rows x 128 B]
-  float* s_hb = reinterpret_cast<float*>(p_buf + 4 * kBlkPPlane);   // [4 converting warps][128] hidden bias of the image
-  float* s_wb = s_hb + 8 * 64;                                      // [4 finishing warps][128] img_bias (64) | res_bias (64)
-  uint64_t* bars = reinterpret_cast<uint64_t*>(s_wb + 8 * 64);
+  float* s_hb = reinterpret_cast<float*>(p_buf + 4 * kBlkPPlane);   // [2 warpgroups][128] hidden bias of the image
+  float* s_wb = s_hb + 2 * 128;                                     // [2 warpgroups][128] img_bias (64) | res_bias (64)
+  uint64_t* bars = reinterpret_cast<uint64_t*>(s_wb + 2 * 128);
   uint64_t* a_full = bars;
   uint64_t* a_empty = a_full + kBlkNA;
   uint64_t* b_full = a_empty + kBlkNA;
   uint64_t* b_empty = b_full + kBlkNB;
-  uint64_t* acc1_full = b_empty + kBlkNB;
-  uint64_t* acc1_empty = acc1_full + 2;
-  uint64_t* p_full = acc1_empty + 2;
-  uint64_t* p_empty = p_full + 2;
-  uint64_t* acc2_full = p_empty + 2;
-  uint64_t* acc2_empty = acc2_full + 1;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc2_empty + 1);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (p.early_trigger) ptx::griddep_launch_dependents();
-  if (warp == 0 && lane == 0) {
+  if (warp == 8 && lane == 0) {
     ptx::prefetch_tmap(&tm_m_hi); ptx::prefetch_tmap(&tm_m_lo); ptx::prefetch_tmap(&tm_x_hi); ptx::prefetch_tmap(&tm_x_lo);
     ptx::prefetch_tmap(&tm_w);
-    for (int i = 0; i < kBlkNA; ++i) { ptx::mbar_init(&a_full[i], 2); ptx::mbar_init(&a_empty[i], 1); }
-    for (int i = 0; i < kBlkNB; ++i) { ptx::mbar_init(&b_full[i], 2); ptx::mbar_init(&b_empty[i], 1); }
-    for (int i = 0; i < 2; ++i) {
-      ptx::mbar_init(&acc1_full[i], 1);
-      ptx::mbar_init(&acc1_empty[i], 8);          // the 4 converting warps of both CTAs
-      ptx::mbar_init(&p_full[i], 8);
-      ptx::mbar_init(&p_empty[i], 1);
-    }
-    ptx::mbar_init(acc2_full, 1);
-    ptx::mbar_init(acc2_empty, 8);                // the 4 finishing warps of both CTAs
+    for (int i = 0; i < kBlkNA; ++i) { ptx::mbar_init(&a_full[i], 1); ptx::mbar_init(&a_empty[i], 2); }
+    for (int i = 0; i < kBlkNB; ++i) { ptx::mbar_init(&b_full[i], 1); ptx::mbar_init(&b_empty[i], 2); }
     ptx::fence_mbar_init();
   }
-  if (warp == 1) ptx::tmem_alloc_pair<512>(tmem_slot);
-  ptx::tc_fence_before();
+  // P pieces without a hidden column stay zero for the kernel's lifetime
+  for (int i = threadIdx.x; i < 4 * kBlkPPlane / 16; i += blockDim.x) reinterpret_cast<uint4*>(p_buf)[i] = make_uint4(0u, 0u, 0u, 0u);
+  ptx::fence_proxy_async();
   __syncthreads();
-  ptx::cluster_sync();
-  ptx::tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   const int tiles_per_img = p.tiles_x * p.tiles_y;
 
-  if (warp == 0) {
+  if (warp == 8) {
     // ===================== TMA producer =====================
     ptx::griddep_wait();
     int as = 0, bs = 0; uint32_t aph = 0, bph = 0;
@@ -141,306 +120,217 @@ block_fused_kernel(const __grid_constant__ CUtensorMap tm_m_hi, const __grid_con
       ptx::mbar_wait(&a_empty[as], aph ^ 1);
       if (ptx::elect_one_sync()) {
         unsigned char* sa = a_ring + (size_t)as * kBlkAStage;
-        const uint32_t bar = ptx::mapa(ptx::smem_u32(&a_full[as]), 0);
-        ptx::mbar_arrive_expect_tx_cluster(bar, (uint32_t)kBlkAStage);
-        ptx::tma_load_5d_pair(sa, src ? &tm_x_hi : &tm_m_hi, bar, c, x, y, t, b);
-        ptx::tma_load_5d_pair(sa + kBlkAStage / 2, src ? &tm_x_lo : &tm_m_lo, bar, c, x, y, t, b);
+        ptx::mbar_arrive_expect_tx(&a_full[as], (uint32_t)kBlkAStage);
+        ptx::tma_load_5d(sa, src ? &tm_x_hi : &tm_m_hi, &a_full[as], c, x, y, t, b);
+        ptx::tma_load_5d(sa + kBlkAStage / 2, src ? &tm_x_lo : &tm_m_lo, &a_full[as], c, x, y, t, b);
       }
       __syncwarp();
       if (++as == kBlkNA) { as = 0; aph ^= 1; }
     };
-    // weight block `blk` = [hi 128 rows][lo 128 rows]; this CTA multiplies n_mma / 2 of its 64 rows: only those are fetched
-    // (boxes of 8 rows) -- with 28 taps per tile the weights, not the activations, were the larger L2 -> SM stream
+    // weight block `blk` = [hi 128 rows][lo 128 rows]; output column n of an N-wide chain is row n (n < N/2) or
+    // 64 + n - N/2 of each plane; only those rows are fetched (boxes of 8 rows)
     auto load_b = [&](int blk, int n_mma) {
       ptx::mbar_wait(&b_empty[bs], bph ^ 1);
       if (ptx::elect_one_sync()) {
-        const uint32_t bar = ptx::mapa(ptx::smem_u32(&b_full[bs]), 0);
         unsigned char* dst = b_ring + (size_t)bs * kBlkBStage;
         const int rows = n_mma / 2;
-        ptx::mbar_arrive_expect_tx_cluster(bar, (uint32_t)(2 * rows * 128));
+        ptx::mbar_arrive_expect_tx(&b_full[bs], (uint32_t)(2 * n_mma * 128));
         for (int r8 = 0; r8 < rows; r8 += 8) {
-          ptx::tma_load_2d_pair(dst + r8 * 128, &tm_w, bar, 0, blk * 256 + (int)rank * 64 + r8);
-          ptx::tma_load_2d_pair(dst + kBlkBRows * 128 + r8 * 128, &tm_w, bar, 0, blk * 256 + 128 + (int)rank * 64 + r8);
+          for (int h = 0; h < 2; ++h) {
+            ptx::tma_load_2d(dst + (h * rows + r8) * 128, &tm_w, &b_full[bs], 0, blk * 256 + h * 64 + r8);
+            ptx::tma_load_2d(dst + kBlkBRows * 128 + (h * rows + r8) * 128, &tm_w, &b_full[bs], 0, blk * 256 + 128 + h * 64 + r8);
+          }
         }
       }
       __syncwarp();
       if (++bs == kBlkNB) { bs = 0; bph ^= 1; }
     };
-    int pend_x = 0, pend_y = 0, pend_t = 0, pend_b = 0;
-    bool pend = false;
-    auto proj_loads = [&]() {
-      load_b(p.wagg_blk0, 64); load_b(p.wagg_blk0 + 1, 64);
-      if (p.has_res_proj) { load_a(1, p.res.cin_off, pend_x, pend_y, pend_t, pend_b); load_b(p.res.wblk0, 64); }
-    };
     for (int tile = cta; tile < p.n_tiles; tile += n_cta) {
       const int img = tile / tiles_per_img, rem = tile % tiles_per_img;
-      const int oy_tile = (rem / p.tiles_x) * 16, ox0 = (rem % p.tiles_x) * 16;
-      const int oy0 = oy_tile + (int)rank * 8;
+      const int oy_tile = (rem / p.tiles_x) * 8, ox0 = (rem % p.tiles_x) * 16;
       const int bidx = img / p.T, tidx = img % p.T;
       for (int c = 0; c < p.n_chain; ++c) {
         const BlkChain& ch = p.chain[c];
         for (int g = ch.grp0; g < ch.grp0 + ch.ngrp; ++g) {
           if (blk_group_is_padding(p, g, tidx, oy_tile, ox0)) continue;
           const int t0 = p.gstart[g];
-          load_a(ch.src, ch.cin_off, ox0 + p.tap[t0][2], oy0 + p.tap[t0][1], tidx + p.tap[t0][0], bidx);
+          load_a(ch.src, ch.cin_off, ox0 + p.tap[t0][2], oy_tile + p.tap[t0][1], tidx + p.tap[t0][0], bidx);
           for (int j = 0; j < p.gsize[g]; ++j) load_b(ch.wblk0 + (t0 + j - ch.tap0), ch.n_mma);
         }
       }
-      if (pend) proj_loads();
-      pend = true; pend_x = ox0; pend_y = oy0; pend_t = tidx; pend_b = bidx;
+      load_b(p.wagg_blk0, 64); load_b(p.wagg_blk0 + 1, 64);
+      if (p.has_res_proj) { load_a(1, p.res.cin_off, ox0, oy_tile, tidx, bidx); load_b(p.res.wblk0, 64); }
     }
-    if (pend) proj_loads();
-  } else if (warp == 1 && rank == 0) {
-    // ===================== MMA issuer (leader) =====================
+  } else {
+    // ===================== two warpgroups: MMA, convert, projection, output =====================
+    const int wg = warp >> 2, wq = warp & 3;
+    const int wtid = threadIdx.x & 127;
+    const bool wg_leader = wtid == 0;
+    const int row0 = wg * 64 + wq * 16 + (lane >> 2);       // accumulator rows of this thread: row0, row0 + 8
+    const int cq = 2 * (lane & 3);                           // first of its two columns in every 8-column group
+    float* hb = s_hb + wg * 128;
+    float* wb = s_wb + wg * 128;
     int as = 0, bs = 0; uint32_t aph = 0, bph = 0;
-    int buf1 = 0; uint32_t acc1_ph = 0, pph = 0, t2ph = 0;
-    auto issue = [&](uint32_t tmem_d, uint32_t a_hi, uint32_t a_lo, uint32_t b_hi, uint32_t b_lo, uint32_t idesc, int k0, int k1,
-                     uint32_t accumulate) {
-      const uint64_t da_hi = ptx::umma_desc_k_sw128(a_hi), da_lo = ptx::umma_desc_k_sw128(a_lo);
-      const uint64_t db_hi = ptx::umma_desc_k_sw128(b_hi), db_lo = ptx::umma_desc_k_sw128(b_lo);
+    int pend_a = -1, pend_b = -1;               // ring slots read by the last committed wgmma group
+    auto release = [&]() {
+      if (wg_leader) {
+        if (pend_a >= 0) ptx::mbar_arrive(&a_empty[pend_a]);
+        if (pend_b >= 0) ptx::mbar_arrive(&b_empty[pend_b]);
+      }
+      pend_a = pend_b = -1;
+    };
+    // acc (+)= A . B over k in [k0, k1) with hi*hi + hi*lo + lo*hi, then commit and release the previous group's slots
+    auto issue = [&](float* acc, int n, uint32_t a_hi, uint32_t a_lo, uint32_t b_hi, uint32_t b_lo, int k0, int k1,
+                     uint32_t accumulate, int slot_a, int slot_b) {
+      const uint64_t da_hi = wg::desc_k_sw128(a_hi), da_lo = wg::desc_k_sw128(a_lo);
+      const uint64_t db_hi = wg::desc_k_sw128(b_hi), db_lo = wg::desc_k_sw128(b_lo);
+      wg::fence();
 #pragma unroll
       for (int k = 0; k < 4; ++k) {
         if (k < k0 || k >= k1) continue;
         const uint64_t koff = (uint64_t)((k * 32) >> 4);
-        ptx::umma_bf16_pair(tmem_d, da_hi + koff, db_hi + koff, idesc, accumulate | (uint32_t)(k > k0));
-        ptx::umma_bf16_pair(tmem_d, da_hi + koff, db_lo + koff, idesc, 1);
-        ptx::umma_bf16_pair(tmem_d, da_lo + koff, db_hi + koff, idesc, 1);
+        wg::mma_bf16_n<64>(n, acc, da_hi + koff, db_hi + koff, accumulate | (uint32_t)(k > k0));
+        wg::mma_bf16_n<64>(n, acc, da_hi + koff, db_lo + koff, 1);
+        wg::mma_bf16_n<64>(n, acc, da_lo + koff, db_hi + koff, 1);
+      }
+      wg::commit();
+      wg::wait<1>();
+      release();
+      pend_a = slot_a; pend_b = slot_b;
+    };
+    float sacc[16];                              // column sums of this thread's columns (8 groups of 2)
+#pragma unroll
+    for (int i = 0; i < 16; ++i) sacc[i] = 0.f;
+    int sum_img = -1;
+    auto flush_sums = [&](int img_) {            // per column: sum over the 8 row pairs of the warp, once per image
+#pragma unroll
+      for (int i = 0; i < 16; ++i) {
+        float v = sacc[i];
+        v += __shfl_xor_sync(0xffffffffu, v, 4);
+        v += __shfl_xor_sync(0xffffffffu, v, 8);
+        v += __shfl_xor_sync(0xffffffffu, v, 16);
+        if (lane < 4) p.sum_part[(((size_t)blockIdx.x * 8 + warp) * p.n_img + img_) * 64 + 8 * (i >> 1) + cq + (i & 1)] = v;
+        sacc[i] = 0.f;
       }
     };
-    const uint32_t idesc64 = ptx::umma_idesc_bf16(256, 64);
-    auto proj = [&]() {
-      ptx::mbar_wait(acc2_empty, t2ph ^ 1);        // the previous unit's output has left acc2 / acc3
-      ptx::tc_fence_after();
-      for (int kb2 = 0; kb2 < 2; ++kb2) {
-        ptx::mbar_wait(&p_full[kb2], pph);
-        ptx::mbar_wait(&b_full[bs], bph);
-        ptx::tc_fence_after();
-        if (ptx::elect_one_sync()) {
-          const uint32_t a_hi = ptx::smem_u32(p_buf + (size_t)kb2 * 2 * kBlkPPlane);
-          const uint32_t b_hi = ptx::smem_u32(b_ring + (size_t)bs * kBlkBStage);
-          issue(tmem_base + kAcc2Col, a_hi, a_hi + kBlkPPlane, b_hi, b_hi + kBlkBRows * 128, idesc64, 0, 4, kb2 > 0 ? 1u : 0u);
-          ptx::umma_commit_pair(&b_empty[bs]);
-          ptx::umma_commit_pair(&p_empty[kb2]);
-        }
-        __syncwarp();
-        if (++bs == kBlkNB) { bs = 0; bph ^= 1; }
-      }
-      pph ^= 1;
-      if (p.has_res_proj) {
-        ptx::mbar_wait(&a_full[as], aph);
-        ptx::mbar_wait(&b_full[bs], bph);
-        ptx::tc_fence_after();
-        if (ptx::elect_one_sync()) {
-          const uint32_t a_hi = ptx::smem_u32(a_ring + (size_t)as * kBlkAStage);
-          const uint32_t b_hi = ptx::smem_u32(b_ring + (size_t)bs * kBlkBStage);
-          issue(tmem_base + kAcc3Col, a_hi, a_hi + kBlkAStage / 2, b_hi, b_hi + kBlkBRows * 128, idesc64, p.res.ks_first, p.res.ks_end, 0u);
-          ptx::umma_commit_pair(&b_empty[bs]);
-          ptx::umma_commit_pair(&a_empty[as]);
-        }
-        __syncwarp();
-        if (++as == kBlkNA) { as = 0; aph ^= 1; }
-        if (++bs == kBlkNB) { bs = 0; bph ^= 1; }
-      }
-      if (ptx::elect_one_sync()) ptx::umma_commit_pair(acc2_full);
-      __syncwarp();
-      t2ph ^= 1;
-    };
-    bool pend = false;
+    ptx::griddep_wait();
     for (int tile = cta; tile < p.n_tiles; tile += n_cta) {
       const int img = tile / tiles_per_img, rem = tile % tiles_per_img;
-      const int oy_tile = (rem / p.tiles_x) * 16, ox0 = (rem % p.tiles_x) * 16;
+      const int oy_tile = (rem / p.tiles_x) * 8, ox0 = (rem % p.tiles_x) * 16;
       const int tidx = img % p.T;
-      ptx::mbar_wait(&acc1_empty[buf1], acc1_ph ^ 1);
-      ptx::tc_fence_after();
+      if (p.sum_part && img != sum_img) {        // tiles come in image order
+        if (sum_img >= 0) flush_sums(sum_img);
+        sum_img = img;
+      }
+      ptx::bar_sync(1 + wg, 128);                // the previous tile is done with this warpgroup's bias rows
+      {                                          // bias rows of this image (written by a preceding small kernel)
+        const volatile float* hsrc = p.hid_bias + (size_t)img * 128;
+        hb[wtid] = hsrc[wtid];
+        const volatile float* isrc = p.img_bias + (size_t)img * 64;
+        if (wtid < 64) wb[wtid] = isrc[wtid];
+        else if (p.res_bias) wb[wtid] = *(reinterpret_cast<const volatile float*>(p.res_bias) + (size_t)img * 64 + wtid - 64);
+      }
+      ptx::bar_sync(1 + wg, 128);
+      // ---------- main: every chain into registers, converted into its pieces of P
       for (int c = 0; c < p.n_chain; ++c) {
         const BlkChain& ch = p.chain[c];
-        const uint32_t tmem_d = tmem_base + (uint32_t)(buf1 * kAcc1Stride + ch.tmem_col);
-        const uint32_t idesc = ptx::umma_idesc_bf16(256, ch.n_mma);
+        float acc[32];
         uint32_t accumulate = 0;
         for (int g = ch.grp0; g < ch.grp0 + ch.ngrp; ++g) {
           if (blk_group_is_padding(p, g, tidx, oy_tile, ox0)) continue;
           ptx::mbar_wait(&a_full[as], aph);
-          ptx::tc_fence_after();
-          const uint32_t a_hi0 = ptx::smem_u32(a_ring + (size_t)as * kBlkAStage);
+          const uint32_t a_hi0 = ptx::smem_u32(a_ring + (size_t)as * kBlkAStage) + (uint32_t)(wg * 64 * 128);
           for (int j = 0; j < p.gsize[g]; ++j) {
             ptx::mbar_wait(&b_full[bs], bph);
-            ptx::tc_fence_after();
-            if (ptx::elect_one_sync()) {
-              const uint32_t a_hi = a_hi0 + (uint32_t)(j * 16 * 128);          // tap j of the group: shifted by j image rows
-              const uint32_t b_hi = ptx::smem_u32(b_ring + (size_t)bs * kBlkBStage);
-              issue(tmem_d, a_hi, a_hi + kBlkAStage / 2, b_hi, b_hi + kBlkBRows * 128, idesc, ch.ks_first, ch.ks_end, accumulate);
-              ptx::umma_commit_pair(&b_empty[bs]);
-            }
-            __syncwarp();
+            const uint32_t a_hi = a_hi0 + (uint32_t)(j * 16 * 128);          // tap j of the group: shifted by j image rows
+            const uint32_t b_hi = ptx::smem_u32(b_ring + (size_t)bs * kBlkBStage);
+            issue(acc, ch.n_mma, a_hi, a_hi + kBlkAStage / 2, b_hi, b_hi + kBlkBRows * 128, ch.ks_first, ch.ks_end,
+                  accumulate, j + 1 == p.gsize[g] ? as : -1, bs);
             accumulate = 1;
             if (++bs == kBlkNB) { bs = 0; bph ^= 1; }
           }
-          if (ptx::elect_one_sync()) ptx::umma_commit_pair(&a_empty[as]);
-          __syncwarp();
           if (++as == kBlkNA) { as = 0; aph ^= 1; }
         }
-      }
-      if (ptx::elect_one_sync()) ptx::umma_commit_pair(&acc1_full[buf1]);
-      __syncwarp();
-      if (++buf1 == 2) { buf1 = 0; acc1_ph ^= 1; }
-      if (pend) proj();
-      pend = true;
-    }
-    if (pend) proj();
-  } else if (warp >= 2) {
-    // ===================== epilogue: two independent warp groups =====================
-    // warps 2..5 CONVERT (hidden accumulator -> operand P), warps 6..9 FINISH (acc2 / acc3 -> output): the conversion of
-    // tile u+1 overlaps the output of tile u instead of queueing behind it in the same warps.  Each group has one warp per
-    // TMEM lane quarter (warp id % 4).
-    const int e = warp - 2;
-    const int q = warp & 3;
-    const int r = q * 32 + lane;
-    ptx::griddep_wait();
-    if (e < 4) {
-      // ---------- convert: 16 pieces of 8 channels per thread (row r of both K blocks of P)
-      int buf1 = 0; uint32_t acc1_ph = 0, pph = 0;
-      const uint32_t sw = (uint32_t)(r & 7);
-      float* hb = s_hb + e * 128;
-      for (int tile = cta; tile < p.n_tiles; tile += n_cta) {
-        const int img = tile / tiles_per_img;
-        {                                          // hidden-bias row of this image (written by a preceding small kernel)
-          const volatile float* hsrc = p.hid_bias + (size_t)img * 128;
-          __syncwarp();
-#pragma unroll
-          for (int i = 0; i < 4; ++i) hb[lane + 32 * i] = hsrc[lane + 32 * i];
-          __syncwarp();
-        }
-        ptx::mbar_wait(&acc1_full[buf1], acc1_ph);
-        ptx::mbar_wait(&p_empty[0], pph ^ 1);      // the projection of the previous tile has read P
-        ptx::mbar_wait(&p_empty[1], pph ^ 1);
-        ptx::tc_fence_after();
-        const uint32_t tmem_acc = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(buf1 * kAcc1Stride);
-#pragma unroll 1
+        wg::wait<0>();
+        release();
+        // convert: piece pp of P holds hidden columns [piece_col[pp], +8) = 8-column group (piece_col - tmem_col) / 8
         for (int pp = 0; pp < 16; ++pp) {
-          const int col = p.piece_col[pp];
-          uint32_t hw[4] = {0u, 0u, 0u, 0u}, lw[4] = {0u, 0u, 0u, 0u};
-          if (col >= 0) {                          // warp-uniform
-            uint32_t acc[8];
-            ptx::tmem_ld_32x32b_x8(tmem_acc + col, acc);
-            ptx::tmem_ld_wait();
+          const int col = p.piece_col[pp] - ch.tmem_col;
+          if (p.piece_col[pp] < 0 || col < 0 || col >= ch.n_mma) continue;
+          const int grp8 = col >> 3;
 #pragma unroll
-            for (int i = 0; i < 4; ++i) {
-              const float x0 = fmaxf(__uint_as_float(acc[2 * i]) + hb[pp * 8 + 2 * i], 0.f);
-              const float x1 = fmaxf(__uint_as_float(acc[2 * i + 1]) + hb[pp * 8 + 2 * i + 1], 0.f);
-              const uint32_t h = ptx::pack_bf16x2(x0, x1);
-              hw[i] = h;
-              lw[i] = ptx::pack_bf16x2(x0 - __uint_as_float(h << 16), x1 - __uint_as_float(h & 0xFFFF0000u));
+          for (int g8 = 0; g8 < 8; ++g8) {               // chains are at most 64 wide: 8 groups of 8 columns
+            if (g8 != grp8) continue;
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              const int row = row0 + 8 * h;
+              const float x0 = fmaxf(acc[4 * g8 + 2 * h] + hb[pp * 8 + cq], 0.f);
+              const float x1 = fmaxf(acc[4 * g8 + 2 * h + 1] + hb[pp * 8 + cq + 1], 0.f);
+              const uint32_t hw = ptx::pack_bf16x2(x0, x1);
+              const uint32_t lw = ptx::pack_bf16x2(x0 - __uint_as_float(hw << 16), x1 - __uint_as_float(hw & 0xFFFF0000u));
+              unsigned char* dst = p_buf + (size_t)(pp >> 3) * 2 * kBlkPPlane + (size_t)row * 128 +
+                                   ((((uint32_t)pp & 7u) ^ (uint32_t)(row & 7)) << 4) + cq * 2;
+              *reinterpret_cast<uint32_t*>(dst) = hw;
+              *reinterpret_cast<uint32_t*>(dst + kBlkPPlane) = lw;
             }
           }
-          unsigned char* dst = p_buf + (size_t)(pp >> 3) * 2 * kBlkPPlane + (size_t)r * 128 + ((((uint32_t)pp & 7u) ^ sw) << 4);
-          *reinterpret_cast<uint4*>(dst) = make_uint4(hw[0], hw[1], hw[2], hw[3]);
-          *reinterpret_cast<uint4*>(dst + kBlkPPlane) = make_uint4(lw[0], lw[1], lw[2], lw[3]);
         }
-        ptx::tc_fence_before();
-        ptx::fence_proxy_async();
-        __syncwarp();
-        if (lane == 0) {
-          ptx::mbar_arrive_cluster(ptx::mapa(ptx::smem_u32(&acc1_empty[buf1]), 0));
-          ptx::mbar_arrive_cluster(ptx::mapa(ptx::smem_u32(&p_full[0]), 0));
-          ptx::mbar_arrive_cluster(ptx::mapa(ptx::smem_u32(&p_full[1]), 0));
-        }
-        pph ^= 1;
-        if (++buf1 == 2) { buf1 = 0; acc1_ph ^= 1; }
       }
-    } else {
-      // ---------- finish: out = relu(acc2 + bias) + residual, all 64 channels of row r, per-image column sums
-      uint32_t t2ph = 0;
-      float* wb = s_wb + (e - 4) * 128;            // img_bias (64) | res_bias (64)
-      float sacc[64];
+      ptx::fence_proxy_async();                  // the generic-proxy stores above are read by the tensor core (async proxy)
+      ptx::bar_sync(1 + wg, 128);
+      // ---------- projection: acc2 = P . W_agg, acc3 = x . W_projection
+      float acc2[32], acc3[32];
+      for (int kb2 = 0; kb2 < 2; ++kb2) {
+        ptx::mbar_wait(&b_full[bs], bph);
+        const uint32_t a_hi = ptx::smem_u32(p_buf + (size_t)kb2 * 2 * kBlkPPlane) + (uint32_t)(wg * 64 * 128);
+        const uint32_t b_hi = ptx::smem_u32(b_ring + (size_t)bs * kBlkBStage);
+        issue(acc2, 64, a_hi, a_hi + kBlkPPlane, b_hi, b_hi + kBlkBRows * 128, 0, 4, kb2 > 0 ? 1u : 0u, -1, bs);
+        if (++bs == kBlkNB) { bs = 0; bph ^= 1; }
+      }
+      if (p.has_res_proj) {
+        ptx::mbar_wait(&a_full[as], aph);
+        ptx::mbar_wait(&b_full[bs], bph);
+        const uint32_t a_hi = ptx::smem_u32(a_ring + (size_t)as * kBlkAStage) + (uint32_t)(wg * 64 * 128);
+        const uint32_t b_hi = ptx::smem_u32(b_ring + (size_t)bs * kBlkBStage);
+        issue(acc3, 64, a_hi, a_hi + kBlkAStage / 2, b_hi, b_hi + kBlkBRows * 128, p.res.ks_first, p.res.ks_end, 0u, as, bs);
+        if (++as == kBlkNA) { as = 0; aph ^= 1; }
+        if (++bs == kBlkNB) { bs = 0; bph ^= 1; }
+      }
+      wg::wait<0>();
+      release();
+      // ---------- output: relu(acc2 + bias) + residual, two channels per 8-column group and row
 #pragma unroll
-      for (int i = 0; i < 64; ++i) sacc[i] = 0.f;
-      int sum_img = -1;
-      auto flush_sums = [&](int img_) {            // per column: sum over the 32 lanes (once per image and warp)
-#pragma unroll
-        for (int i = 0; i < 64; ++i) {
-          float v = sacc[i];
-#pragma unroll
-          for (int off = 16; off > 0; off >>= 1) v += __shfl_xor_sync(0xffffffffu, v, off);
-          if (lane == (i & 31)) p.sum_part[(((size_t)blockIdx.x * 4 + q) * p.n_img + img_) * 64 + i] = v;
-          sacc[i] = 0.f;
-        }
-      };
-      for (int tile = cta; tile < p.n_tiles; tile += n_cta) {
-        const int img = tile / tiles_per_img, rem = tile % tiles_per_img;
-        const int oy = (rem / p.tiles_x) * 16 + (int)rank * 8 + (r >> 4), ox = (rem % p.tiles_x) * 16 + (r & 15);
-        if (p.sum_part && img != sum_img) {        // tiles come in image order
-          if (sum_img >= 0) flush_sums(sum_img);
-          sum_img = img;
-        }
-        {
-          const volatile float* isrc = p.img_bias + (size_t)img * 64;
-          __syncwarp();
-          wb[lane] = isrc[lane]; wb[lane + 32] = isrc[lane + 32];
-          if (p.res_bias) {
-            const volatile float* rsrc = p.res_bias + (size_t)img * 64;
-            wb[64 + lane] = rsrc[lane]; wb[96 + lane] = rsrc[lane + 32];
-          }
-          __syncwarp();
-        }
-        const bool valid = oy < p.H && ox < p.W;
+      for (int h = 0; h < 2; ++h) {
+        const int row = row0 + 8 * h;
+        const int oy = oy_tile + (row >> 4), ox = ox0 + (row & 15);
+        if (oy >= p.H || ox >= p.W) continue;
         const size_t pix = ((size_t)img * p.H + oy) * p.W + ox;
-        ptx::mbar_wait(acc2_full, t2ph);
-        ptx::tc_fence_after();
-        t2ph ^= 1;
-        const uint32_t tmem_2 = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)kAcc2Col;
-        const uint32_t tmem_3 = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)kAcc3Col;
 #pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          uint32_t acc[16], acc3[16], rh[8], rl[8];
-          if (!p.has_res_proj && valid) {          // identity residual: the block's input planes
-            const size_t off = pix * p.res_cstride + j * 16;
-            ptx::ld_global_v8(p.res_hi + off, rh);
-            ptx::ld_global_v8(p.res_lo + off, rl);
+        for (int g8 = 0; g8 < 8; ++g8) {
+          const int c = 8 * g8 + cq;
+          float v0 = fmaxf(acc2[4 * g8 + 2 * h] + wb[c], 0.f);
+          float v1 = fmaxf(acc2[4 * g8 + 2 * h + 1] + wb[c + 1], 0.f);
+          if (p.has_res_proj) {
+            v0 += acc3[4 * g8 + 2 * h] + wb[64 + c];
+            v1 += acc3[4 * g8 + 2 * h + 1] + wb[64 + c + 1];
+          } else {                               // identity residual: the block's input planes
+            const size_t off = pix * p.res_cstride + c;
+            const uint32_t rh = *reinterpret_cast<const volatile uint32_t*>(p.res_hi + off);
+            const uint32_t rl = *reinterpret_cast<const volatile uint32_t*>(p.res_lo + off);
+            v0 += __uint_as_float(rh << 16) + __uint_as_float(rl << 16);
+            v1 += __uint_as_float(rh & 0xFFFF0000u) + __uint_as_float(rl & 0xFFFF0000u);
           }
-          ptx::tmem_ld_32x32b_x16(tmem_2 + j * 16, acc);
-          if (p.has_res_proj) ptx::tmem_ld_32x32b_x16(tmem_3 + j * 16, acc3);
-          ptx::tmem_ld_wait();
-          if (valid) {
-            float v[16];
-#pragma unroll
-            for (int i = 0; i < 16; ++i) v[i] = fmaxf(__uint_as_float(acc[i]) + wb[j * 16 + i], 0.f);
-            if (p.has_res_proj) {
-#pragma unroll
-              for (int i = 0; i < 16; ++i) v[i] += __uint_as_float(acc3[i]) + wb[64 + j * 16 + i];
-            } else {
-#pragma unroll
-              for (int i = 0; i < 8; ++i) {
-                v[2 * i] += __uint_as_float(rh[i] << 16) + __uint_as_float(rl[i] << 16);
-                v[2 * i + 1] += __uint_as_float(rh[i] & 0xFFFF0000u) + __uint_as_float(rl[i] & 0xFFFF0000u);
-              }
-            }
-            uint32_t hw[8], lw[8];
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-              const uint32_t h = ptx::pack_bf16x2(v[2 * i], v[2 * i + 1]);
-              hw[i] = h;
-              lw[i] = ptx::pack_bf16x2(v[2 * i] - __uint_as_float(h << 16), v[2 * i + 1] - __uint_as_float(h & 0xFFFF0000u));
-            }
-            const size_t off = pix * p.out_cstride + j * 16;
-            ptx::st_global_v8(p.out_hi + off, hw);
-            ptx::st_global_v8(p.out_lo + off, lw);
-            if (p.sum_part) {
-#pragma unroll
-              for (int i = 0; i < 16; ++i) sacc[j * 16 + i] += v[i];
-            }
-          }
+          const uint32_t hw = ptx::pack_bf16x2(v0, v1);
+          const uint32_t lw = ptx::pack_bf16x2(v0 - __uint_as_float(hw << 16), v1 - __uint_as_float(hw & 0xFFFF0000u));
+          const size_t off = pix * p.out_cstride + c;
+          *reinterpret_cast<uint32_t*>(p.out_hi + off) = hw;
+          *reinterpret_cast<uint32_t*>(p.out_lo + off) = lw;
+          if (p.sum_part) { sacc[2 * g8] += v0; sacc[2 * g8 + 1] += v1; }
         }
-        ptx::tc_fence_before();
-        __syncwarp();
-        if (lane == 0) ptx::mbar_arrive_cluster(ptx::mapa(ptx::smem_u32(acc2_empty), 0));
       }
-      if (p.sum_part && sum_img >= 0) flush_sums(sum_img);
     }
+    if (p.sum_part && sum_img >= 0) flush_sums(sum_img);
   }
-  ptx::tc_fence_before();
-  __syncthreads();
-  ptx::cluster_sync();
-  if (warp == 1) ptx::tmem_dealloc_pair<512>(tmem_base);
 }
 
 typedef CUresult (*PFN_tmapEncodeTiledB)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
@@ -460,7 +350,7 @@ static PFN_tmapEncodeTiledB blk_encode_fn() {
 
 static int blk_num_sms() {
   static const int n = [] {
-    int dev = 0, v = 148;
+    int dev = 0, v = 132;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev);
     return v;
@@ -473,7 +363,7 @@ static int blk_num_sms() {
 using namespace stp3;
 
 extern "C" size_t stp3_block_fused_scratch_bytes(int n_img) {
-  return (size_t)blk_num_sms() * 4 * (size_t)(n_img > 0 ? n_img : 0) * 64 * sizeof(float);
+  return (size_t)blk_num_sms() * 8 * (size_t)(n_img > 0 ? n_img : 0) * 64 * sizeof(float);
 }
 
 extern "C" int stp3_block_fused_fwd(const stp3_block_desc* d, const void* mid_hi, const void* mid_lo, const void* x_hi,
@@ -495,7 +385,7 @@ extern "C" int stp3_block_fused_fwd(const stp3_block_desc* d, const void* mid_hi
 
   BlkParams p;
   p.n_img = d->B * d->T; p.T = d->T; p.H = d->H; p.W = d->W;
-  p.tiles_x = ceil_div(d->W, 16); p.tiles_y = ceil_div(d->H, 16);
+  p.tiles_x = ceil_div(d->W, 16); p.tiles_y = ceil_div(d->H, 8);
   const long long nt = (long long)p.n_img * p.tiles_x * p.tiles_y;
   STP3_CHECK_ARG(nt < (1ll << 31), "grid too large");
   p.n_tiles = (int)nt;
@@ -575,48 +465,35 @@ extern "C" int stp3_block_fused_fwd(const stp3_block_desc* d, const void* mid_hi
     if (r != CUDA_SUCCESS) return set_error(STP3_ECUDA, "cuTensorMapEncodeTiled(weights) failed: %d", (int)r);
   }
   const size_t smem_bytes = 1024 + (size_t)kBlkNA * kBlkAStage + (size_t)kBlkNB * kBlkBStage + 4 * (size_t)kBlkPPlane +
-                            2 * 8 * 64 * sizeof(float) + 32 * 8 + 16;
-  static thread_local int attr_dev = -1, occ_val = 0;           // once per device: these calls cost microseconds per eager launch
+                            4 * 128 * sizeof(float) + 2 * (kBlkNA + kBlkNB) * 8;
+  static thread_local int attr_dev = -1;           // once per device: the attribute call costs microseconds per eager launch
   int cur_dev = 0;
   cudaGetDevice(&cur_dev);
-  const bool first_call = attr_dev != cur_dev;
-  if (first_call) STP3_CUDA_OK(cudaFuncSetAttribute(block_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes));
+  if (attr_dev != cur_dev) {
+    STP3_CUDA_OK(cudaFuncSetAttribute(block_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes));
+    attr_dev = cur_dev;
+  }
   const int num_sms = blk_num_sms();
   cudaLaunchConfig_t cfg = {};
-  unsigned pairs = (unsigned)(nt < num_sms / 2 ? nt : num_sms / 2);
-  cfg.gridDim = dim3(2 * pairs); cfg.blockDim = dim3(kBlkThreads);
+  cfg.gridDim = dim3((unsigned)(nt < num_sms ? nt : num_sms)); cfg.blockDim = dim3(kBlkThreads);
   cfg.dynamicSmemBytes = smem_bytes; cfg.stream = stream;
-  cudaLaunchAttribute attr[2];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr; cfg.numAttrs = 1;
-  int max_clusters = occ_val;
-  if (first_call) {
-    STP3_CUDA_OK(cudaOccupancyMaxActiveClusters(&max_clusters, block_fused_kernel, &cfg));
-    occ_val = max_clusters; attr_dev = cur_dev;
-  }
-  if (max_clusters < 1) return set_error(STP3_EUNSUPPORTED, "no CTA pair fits on this device");
-  if (cfg.gridDim.x > 2u * (unsigned)max_clusters) cfg.gridDim.x = 2u * (unsigned)max_clusters;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = attr; cfg.numAttrs = stp3_pdl_enabled("STP3_FUSED_PDL") ? 1 : 0;
   p.sum_part = nullptr;
   if (col_sums) {
-    const size_t need = (size_t)cfg.gridDim.x * 4 * p.n_img * 64 * sizeof(float);
+    const size_t need = (size_t)cfg.gridDim.x * 8 * p.n_img * 64 * sizeof(float);
     STP3_CHECK_ARG(scratch && scratch_bytes >= need, "col_sums: scratch missing or smaller than stp3_block_fused_scratch_bytes()");
     p.sum_part = static_cast<float*>(scratch);
     STP3_CUDA_OK(cudaMemsetAsync(p.sum_part, 0, need, stream));
   }
-  attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[1].val.programmaticStreamSerializationAllowed = 1;
-  cfg.numAttrs = stp3_pdl_enabled("STP3_FUSED_PDL") ? 2 : 1;
-  {
-    // No early griddepcontrol.launch_dependents from the back-to-back kernels: with it, a chain block_fused -> col_sum_reduce
-    // -> pool_bias -> aspp_fused in flight at once stopped making progress about once in 400 .. 2000 replayed steps
-    // (tools/hang_probe.py; 20000 replays are clean without it and with programmatic launch off altogether).  The
-    // dependents are released when the grid completes; this kernel itself still starts early behind its predecessor.
-    static const bool early = [] { const char* e = getenv("STP3_FUSED_EARLY_TRIGGER"); return e && atoi(e) != 0; }();
-    p.early_trigger = early ? 1 : 0;
-  }
+  // The back-to-back kernels never execute griddepcontrol.launch_dependents, so their dependents start only when the
+  // grid has completed.  Each of them needs a whole SM; an early trigger would let a chain block_fused -> col_sum_reduce
+  // -> pool_bias -> aspp_fused be resident at once, and such a chain was seen to stop making progress.  The kernel itself
+  // still starts early behind its predecessor (griddepcontrol.wait before it reads what that predecessor wrote).
   STP3_CUDA_OK(cudaLaunchKernelEx(&cfg, block_fused_kernel, tm[0], tm[1], tm[2], tm[3], tm_w, p));
   STP3_CUDA_OK(cudaGetLastError());
-  if (col_sums) return launch_col_sum_reduce(p.sum_part, (int)cfg.gridDim.x * 4, p.n_img, col_sums, stream);
+  if (col_sums) return launch_col_sum_reduce(p.sum_part, (int)cfg.gridDim.x * 8, p.n_img, col_sums, stream);
   return STP3_OK;
 }

@@ -1,4 +1,4 @@
-// Shared helpers for libstp3_b200.so (sm_100a only).
+// Shared helpers for libstp3_b200.so (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cstdarg>
@@ -28,7 +28,7 @@ int set_error(int code, const char* fmt, ...);
 
 inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
 
-// col_sums[img][c] = fixed-order sum of the (n_part, n_img, 64) partial rows an epilogue wrote (conv_tcgen05.cu)
+// col_sums[img][c] = fixed-order sum of the (n_part, n_img, 64) partial rows an epilogue wrote (conv_igemm.cu)
 int launch_col_sum_reduce(const float* part, int n_part, int n_img, float* out, cudaStream_t stream);
 
 }  // namespace stp3

@@ -21,7 +21,7 @@ int set_error(int code, const char* fmt, ...) {
 extern "C" int stp3_abi_version(void) { return 3; }
 
 extern "C" const char* stp3_build_info(void) {
-  return "stp3_b200 abi 3; sm_100a; nvcc " __DATE__ " " __TIME__;
+  return "stp3_b200 abi 3; sm_90a; nvcc " __DATE__ " " __TIME__;
 }
 
 extern "C" const char* stp3_last_error(void) { return stp3::error_buffer(); }

@@ -1,4 +1,6 @@
-// Fused lift-splat for sm_100a.
+// Fused lift-splat for sm_90a.  This file is compiled with ptxas -O1 (csrc/Makefile): the -O2/-O3 code ptxas 12.9 emits
+// for lift_splat_scatter_tma_kernel faults with an illegal address in its pooling phase on the H100, while the same
+// source at -O1 / -O0 runs clean and bit-exact (DESIGN.md §3.1).
 //
 //   K1  lift_splat_scatter_kernel : one CTA per (b, t, camera, tile of TW image columns)
 //         phase A  depth logits and context features of the tile -> shared memory (coalesced tile loads),
@@ -16,7 +18,7 @@
 //         Reads (and re-zeroes) only the occupied pillars, so the scatter grid is left clean for the next call
 //         and never needs a memset.
 //
-// Reference semantics: /root/reference/stp3/models/stp3.py:186-301, stp3/utils/geometry.py:299-318.
+// Reference semantics: stp3/models/stp3.py:186-301, stp3/utils/geometry.py:299-318.
 #include <cuda_bf16.h>
 
 #include <cmath>
@@ -825,8 +827,8 @@ bev_finalize_kernel(float* __restrict__ grid, unsigned char* __restrict__ occ, f
 }
 
 // Channels-last outputs (fp32 NHWC, or the bf16 hi/lo planes the tensor-core layers read): one thread = one pillar x
-// 16 channels, LPP = C/16 neighbouring lanes cover a pillar.  Every global access is a full 32-byte sector per lane
-// (LDG.256 / STG.256) and the lanes of a pillar touch one contiguous row -- the lane-per-pillar mapping of the kernel
+// 16 channels, LPP = C/16 neighbouring lanes cover a pillar.  Every lane moves a full 32-byte sector per access
+// (two 128-bit instructions) and the lanes of a pillar touch one contiguous row -- the lane-per-pillar mapping of the kernel
 // above would write half sectors 128 bytes apart here.  Same arithmetic, same workspace-cleaning contract; the CTA
 // clears the occupancy bytes itself because it covers all channels of its pillars.
 // PeerOut (frame-sharded mode, fused with the all-gather): instead of one local tensor the fp32 channels-last rows of

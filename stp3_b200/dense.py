@@ -138,24 +138,22 @@ def pack_conv(weight: torch.Tensor, bias: torch.Tensor, *, stride: int = 1, dila
 
 
 # ------------------------------------------------------------------------------------------------ autotuner
-# The conv kernel has two tiling knobs (sub-tiles per CTA tile -- or a 16x16 tile shared by a CTA pair through
-# tcgen05.mma.cta_group::2, n_sub = 3 -- and sharing one activation load between the dy taps of a 3x3).  Which combination wins depends on the layer (K depth, N width, image size, whether the weights are
-# smem-resident), so the first eager call of every (layer, shape) times the candidates back to back and the winner is
-# cached; CUDA-graph capture then records the tuned launches.  STP3_CONV_AUTOTUNE=0 disables it (kernel heuristics).
+# The conv kernel has tiling knobs (sharing one activation load between the dy taps of a 3x3, streaming the weights
+# through the ring instead of keeping them resident, the stacked hi/lo weight operand).  Which combination wins depends
+# on the layer (K depth, N width, image size, whether the weights are smem-resident), so the first eager call of every
+# (layer, shape) times the candidates back to back and the winner is cached; CUDA-graph capture then records the tuned
+# launches.  STP3_CONV_AUTOTUNE=0 disables it (kernel heuristics).
 import os as _os
 
 _TUNED = {}
 _AUTOTUNE = _os.environ.get("STP3_CONV_AUTOTUNE", "1") != "0"
-_TUNE_PAIR = _os.environ.get("STP3_CONV_PAIR", "1") != "0"
 TUNE_LOG = []      # (description, {config: ms}) for reports
 
 
 def _tune(key, desc, launch, groupable, ntaps=1, bn=0):
-    cands = [(1, 1), (2, 1)] + ([(1, 3), (2, 3)] if groupable else [])
-    if _TUNE_PAIR:
-        cands += [(3, 1)] + ([(3, 3)] if groupable else [])
+    cands = [(1, 1)] + ([(1, 3)] if groupable else [])
     if ntaps > 1:       # weights streamed through the ring instead of resident: more activation stages in flight
-        cands += [(ns, g + 4) for ns, g in cands if ns != 1]
+        cands += [(ns, g + 4) for ns, g in cands]
     if bn == 64:        # stacked [W_hi; W_lo] operand: two MMAs per product instead of three
         cands += [(ns, g + 8) for ns, g in cands]
     times = {}
@@ -186,8 +184,8 @@ def conv(x: HL, pc: PackedConv, *, cin_off: int = 0, out: Optional[HL] = None, o
     out2 (bn = 128 layers, n_store <= 64): output columns [64, 64+n_store2) go to out2[..., out2_coff:...] with activation
     relu2 -- two 64-column convolutions of the same input in one launch.
     col_sums (B*T, 64) fp32 (bn = 64 layers): receives the per-image sums over pixels of the activated output.
-    tune = (n_sub, group) forces a tiling (n_sub 3 = CTA pair; group +4 = streamed weights, +8 = stacked hi/lo weight
-    operand) instead of the autotuned one."""
+    tune = (n_sub, group) forces a tiling (n_sub is ignored: the tile is 8x16 pixels; group +4 = streamed weights,
+    +8 = stacked hi/lo weight operand) instead of the autotuned one."""
     B, T_total, H, W, cs = x.hi.shape
     t0, T = frames if frames is not None else (0, T_total)      # process frames [t0, t0+T) of every sample
     Ho, Wo = out_hw if out_hw is not None else ((H + pc.stride - 1) // pc.stride, (W + pc.stride - 1) // pc.stride)

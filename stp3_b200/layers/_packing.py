@@ -30,5 +30,5 @@ class PackedModule(nn.Module):
     def _require_eval(self):
         if self.training:
             raise NotImplementedError(
-                f"{type(self).__name__}: the sm_100a path implements the inference forward (eval-mode BatchNorm "
+                f"{type(self).__name__}: the sm_90a path implements the inference forward (eval-mode BatchNorm "
                 "folded into the tensor-core kernels); call .eval() -- training through this module is SURVEY.md row f2")

@@ -1,5 +1,5 @@
 """2-D building blocks of the BEV path with the reference's constructor signatures and parameter names
-(stp3/layers/convolutions.py:183-280) so checkpoints load unchanged; forward() runs on the tcgen05 kernels.
+(stp3/layers/convolutions.py:183-280) so checkpoints load unchanged; forward() runs on the wgmma kernels.
 
   UpsamplingAdd  : bilinear x2 -> 1x1 conv -> BN, + skip.   Executed as 1x1 conv + folded BN at LOW resolution and a
                    fused upsample+add kernel (the interpolation weights sum to one, so the affine map commutes).

@@ -1,5 +1,5 @@
 """3-D spatio-temporal block with the reference's constructor signatures and parameter names
-(stp3/layers/temporal.py:252-273, 315-325, 375-489); forward() runs on the tcgen05 implicit-GEMM kernels.
+(stp3/layers/temporal.py:252-273, 315-325, 375-489); forward() runs on the wgmma implicit-GEMM kernels.
 
 TemporalBlock data flow on the device (channels-last hi/lo planes, o = half rounded up to 8):
     x --1x1x1 (paths 0,1 fused, N=128)--> mid[0:half | 64:64+half]

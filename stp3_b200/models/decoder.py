@@ -1,5 +1,5 @@
 """BEV decoder with the reference's constructor/forward surface and parameter names (stp3/models/decoder.py:8-140):
-ResNet-18 stages 1-3 as a U-Net over the BEV grid and 3x3 -> 1x1 heads, executed on the tcgen05 kernels."""
+ResNet-18 stages 1-3 as a U-Net over the BEV grid and 3x3 -> 1x1 heads, executed on the wgmma kernels."""
 import torch
 import torch.nn as nn
 from torchvision.models.resnet import resnet18

@@ -4,7 +4,7 @@ heads (context features, depth logits) at 1/8 resolution.
 The trunk is third-party (efficientnet-pytorch 0.7.0, not vendored by the reference and absent from this image;
 SURVEY.md §8c): it is taken from `efficientnet_pytorch` when importable, or injected (`backbone=`: any module that
 maps (M,3,H,W) -> (reduction_3 (M,c3,H/8,W/8), reduction_4 (M,c4,H/16,W/16))).  The heads -- DeepLabHead +
-UpsamplingConcat, the layers this repository owns -- run on the tcgen05 kernels."""
+UpsamplingConcat, the layers this repository owns -- run on the wgmma kernels."""
 import math
 
 import torch

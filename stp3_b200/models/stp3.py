@@ -1,12 +1,12 @@
 """STP3 perception model with the reference's constructor / forward surface (stp3/models/stp3.py:15-184) for the
 perception configuration (N_FUTURE_FRAMES = 0, PLANNING disabled): Encoder -> lift-splat -> TemporalModel -> Decoder,
-every stage on hand-written sm_100a kernels behind the C ABI.
+every stage on hand-written sm_90a kernels behind the C ABI.
 
 Device data flow of forward():
-    Encoder heads (tcgen05)  -> feature / depth-logit tensors
+    Encoder heads (wgmma)  -> feature / depth-logit tensors
     stp3_lift_splat_fwd      -> BEV grid directly as channels-last bf16 hi/lo planes + per-(b,t,c) spatial sums
-    TemporalModel (tcgen05)  -> ego-motion channels and pooling branches enter as per-image biases
-    Decoder (tcgen05)        -> fp32 logits in the reference's (B,S,k,X,Y) layout
+    TemporalModel (wgmma)  -> ego-motion channels and pooling branches enter as per-image biases
+    Decoder (wgmma)        -> fp32 logits in the reference's (B,S,k,X,Y) layout
 Prediction (N_FUTURE_FRAMES > 0) and planning are outside the hot path (SURVEY.md §2) and are refused loudly.
 """
 import torch
@@ -141,7 +141,7 @@ class STP3(nn.Module):
 
     def forward_trunk_features(self, r_lo, r_hi, intrinsics, extrinsics, future_egomotion):
         """forward() entering after the (third-party) EfficientNet trunk: r_lo (B,S,N,c3,H/8,W/8), r_hi
-        (B,S,N,c4,H/16,W/16) -- the encoder heads (encoder.py:88-95) run on the tcgen05 kernels and hand their context
+        (B,S,N,c4,H/16,W/16) -- the encoder heads (encoder.py:88-95) run on the wgmma kernels and hand their context
         features to the lift-splat channels-last."""
         S = self.receptive_field
         dev = r_lo.device
@@ -287,7 +287,7 @@ class STP3(nn.Module):
 
 class GraphedPerception:
     """STP3.forward_features for a fixed batch size replayed as ONE CUDA graph: the ~70 kernel launches of a step
-    (lift-splat, tcgen05 convolutions, helpers) are captured once -- tensor maps and kernel arguments are baked in, all
+    (lift-splat, wgmma convolutions, helpers) are captured once -- tensor maps and kernel arguments are baked in, all
     buffers are static -- so a step costs one graph launch instead of ~70 Python/ctypes launches.
 
         g = GraphedPerception(model, batch)

@@ -41,7 +41,7 @@ def load_e2e_case(name):
 
 def e2e_errors(g, key, tensor):
     """(error vs the fp64 oracle, error vs the reference's fp32 output), both as a fraction of max |value|, on the
-    fixture's 40k-entry sample of output `key`; tensor = this implementation's full output for ONE sample."""
+    fixture's 12k-entry sample of output `key`; tensor = this implementation's full output for ONE sample."""
     flat = np.asarray(tensor, dtype=np.float64).reshape(-1)
     got = flat[g[f"{key}_index"]]
     m = float(g[f"{key}_max"])

@@ -1,5 +1,5 @@
 """bench.py contract checks that need no GPU: the reference arm (CPU port of the reference's path) prints ONE JSON line
-with the keys the driver reads, and the B200 arm refuses to run without a CUDA device (no CPU fallback)."""
+with the keys a caller reads, and the CUDA arm refuses to run without a CUDA device (no CPU fallback)."""
 import json
 import os
 import subprocess
@@ -22,7 +22,7 @@ def test_reference_arm_prints_one_json_line():
     d = json.loads(lines[0])
     assert d["impl"] == "reference" and d["metric"] == "bev_frames_per_sec" and d["unit"] == "frames/s"
     assert d["higher_is_better"] is True and d["value"] > 0 and d["vs_baseline"] is None
-    # "reference" = the unmodified reference package (baseline/_ref or /root/reference); "port" only where neither exists
+    # "reference" = the unmodified reference package (oracle/_ref); "port" only where it does not exist
     assert d["cpu_baseline"]["kind"] in ("reference", "port")
     assert d["cpu_baseline"]["cores"] >= 1 and d["cpu_baseline"]["value"] == d["value"]
     assert d["e2e"] == {"value": d["value"], "unit": "frames/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0}
@@ -30,7 +30,7 @@ def test_reference_arm_prints_one_json_line():
 
 
 def test_reference_arm_uses_the_installed_reference_when_present():
-    """baseline/_ref (oracle/build_ref.py) or /root/reference present -> the arm times the reference's own modules."""
+    """oracle/_ref (oracle/build_ref.py) present -> the arm times the reference's own modules."""
     sys.path.insert(0, ROOT)
     from oracle import ref_loader
     if not ref_loader.reference_available():

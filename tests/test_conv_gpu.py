@@ -1,4 +1,4 @@
-"""GPU parity of the tcgen05 implicit-GEMM convolution (through the C ABI) against a float64 PyTorch convolution of
+"""GPU parity of the wgmma implicit-GEMM convolution (through the C ABI) against a float64 PyTorch convolution of
 the same op (this is a floating-point kernel, so a torch reference is the oracle; tolerance stated per test)."""
 import pytest
 import torch
@@ -81,9 +81,8 @@ def test_conv2d_matches_fp64(cin, cout, k, stride, dil, hw):
     (64, 256, 3, 2, (33, 33)),        # dilation 2, BN = 256 (two launches)
 ])
 def test_every_tiling_matches_fp64(tune, cin, cout, k, dil, hw):
-    """Every tiling the autotuner may pick -- 8x16 / 16x16 tiles per CTA, the 16x16 tile of a CTA pair
-    (tcgen05.mma.cta_group::2, n_sub = 3), with and without the shared dy-tap activation load -- gives the same
-    result."""
+    """Every tiling the autotuner may pick -- with and without the shared dy-tap activation load, for every accepted
+    n_sub value -- gives the same result."""
     if tune[1] == 3 and (k != 3 or dil != 1):
         pytest.skip("taps are not groupable")
     H, W = hw

@@ -1,6 +1,6 @@
 """CPU: pins oracle/torch_dense.py (the plain-PyTorch restatement used as the dense oracle on the GPU box) to
 (a) the golden outputs produced from the unmodified reference modules, using the drop-in modules purely as parameter
-containers, and (b) when /root/reference is present, the reference modules' own forward."""
+containers, and (b) when the reference install (oracle/_ref) is present, the reference modules' own forward."""
 import os
 
 import numpy as np
@@ -64,7 +64,7 @@ def test_decoder_restatement_matches_reference_output(name, gates):
 def test_state_dict_keys_match_reference_when_available():
     from oracle.ref_loader import load_reference, reference_available
     if not reference_available():
-        pytest.skip("/root/reference not present (GPU box)")
+        pytest.skip("reference install (oracle/_ref) not present")
     ref = load_reference()
     a = TemporalModel(70, 3, (20, 20)).state_dict()
     b = ref.temporal_model.TemporalModel(70, 3, (20, 20)).state_dict()

@@ -1,8 +1,8 @@
 """Host logic of the two back-to-back kernels, checked without a GPU: the packed weight blocks, tap tables, chain
 descriptors, piece map and bias tables that `DeepLabHead._pack` / `TemporalBlock._pack` hand to stp3_aspp_fused_fwd /
 stp3_block_fused_fwd are run through a plain fp64 emulation of what the kernels do with them (the indexing documented in
-include/stp3_b200.h and stp3_b200/csrc/{aspp,block}_fused.cu: block order, rows of a CTA pair, K-step ranges, TMEM
-columns, pieces of P) and compared with the fp64 oracle of the same module.  A packing / table mistake shows up here as
+include/stp3_b200.h and stp3_b200/csrc/{aspp,block}_fused.cu: block order, weight rows of an N-wide chain, K-step ranges,
+hidden-accumulator columns, pieces of P) and compared with the fp64 oracle of the same module.  A packing / table mistake shows up here as
 an O(1) error; the bf16 hi+lo split of the weights leaves ~1e-5.
 """
 import os

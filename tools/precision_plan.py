@@ -1,6 +1,6 @@
 """Oracle-driven precision plan for the dense path (test / analysis tool; runs on the CPU, imports oracle/).
 
-The tcgen05 convolutions carry fp32 tensors as 16-bit planes.  This script evaluates, at the HEADLINE size (one perceive
+The tensor-core convolutions carry fp32 tensors as 16-bit planes.  This script evaluates, at the HEADLINE size (one perceive
 sample: 3 frames x 200x200x64 BEV, ASPP dilations 12/24/36 live), what each storage format of the activations costs
 in logit error against the fp64 oracle, by re-running the oracle's own functional graph with every STORED tensor
 rounded the way the kernels would store it:
@@ -12,7 +12,7 @@ rounded the way the kernels would store it:
 weights stay hi+lo (exact to 2^-22) unless --w1 (single fp16 plane: 1 MMA per product).
 
     python tools/precision_plan.py [--hw 200] [--plans all-f16 ...]
-Prints max |err| / max |logit| per head for every plan; profiles/r02_precision_plan.txt is its output.
+Prints max |err| / max |logit| per head for every plan.
 """
 import argparse
 import copy
