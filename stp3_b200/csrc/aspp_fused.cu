@@ -5,9 +5,9 @@
 // (984 MB) -- the largest avoidable traffic of the dense path.  Here a CTA keeps an 8x16-pixel tile on chip:
 //
 //   for every branch b:   acc1  = sum_taps A(x, tap) . W_b[tap]            (wgmma, 64 rows per warpgroup, N = 128)
-//                         P     = hi/lo split of relu(acc1 + bias_b)       (registers -> SHARED memory, written in the
-//                                                                           128B-swizzled K-major operand layout)
-//                         acc2 += P . W_proj[:, b-th 128 input channels]   (second MMA chain, A operand = P)
+//                         P     = hi/lo split of relu(acc1 + bias_b)       (in registers: the accumulator fragment,
+//                                                                           packed to bf16x2, is the wgmma A fragment)
+//                         acc2 += P . W_proj[:, b-th 128 input channels]   (second MMA chain, A operand = P from registers)
 //   out = hi/lo split of relu(acc2 + per-image bias)                       (the global-pool branch is that bias)
 //
 // The same kernel runs the head's tail, 3x3 conv/BN/ReLU -> 1x1 classifier (convolutions.py:272-280), as a ONE-branch
@@ -16,9 +16,12 @@
 // Same precision scheme as conv_igemm.cu (bf16 hi/lo planes, hi*hi + hi*lo + lo*hi, fp32 accumulation), so the result
 // matches the unfused path to the last few bits of the split.
 //
-//   warps : 0..7 = two warpgroups (rows 0..63 / 64..127 of the tile; each reads back only its own rows of P), 8 = TMA
-//           producer (activation ring + weight ring)
-//   smem  : 2 activation stages (64 KB) + 2 weight stages (64 KB) + P (2 K-blocks x hi/lo x 16 KB = 64 KB) = 192 KB
+//   warps : 0..7 = two warpgroups (rows 0..63 / 64..127 of the tile), 8 = TMA producer (activation ring + weight ring),
+//           9..11 idle.  The producer warpgroup hands its registers to the MMA warpgroups (setmaxnreg 40 / 232): acc1,
+//           acc2 and P live at once do not fit the 168 registers per thread of an even split
+//   smem  : 3 activation stages (96 KB) + 3 weight stages (96 KB) = 192 KB.  P never touches shared memory, so both rings
+//           are three deep: a step's operands are requested two MMA steps before they are used (with two stages, one
+//           step of MMAs had to cover the whole TMA latency)
 #include <cuda_bf16.h>
 
 #include "common.cuh"
@@ -27,13 +30,12 @@
 
 namespace stp3 {
 
-constexpr int kAsppThreads = 288;                 // 8 + 1 warps
+constexpr int kAsppThreads = 384;                 // 8 + 4 warps
 constexpr int kAsppMaxBranches = 4;
 constexpr int kAsppMaxTaps = 9 * kAsppMaxBranches;
-constexpr int kAsppNA = 2, kAsppNB = 2;
+constexpr int kAsppNA = 3, kAsppNB = 3;
 constexpr int kAStage = 2 * 8 * 16 * 128;         // hi + lo planes of 8 image rows x 16 pixels x 64 channels
 constexpr int kBStage = 2 * 128 * 128;            // hi + lo planes of the 128 weight rows
-constexpr int kPPlane = 128 * 128;                // 128 pixel rows x 64 bf16
 constexpr int kAsppHidden = 128;
 
 struct AsppParams {
@@ -66,8 +68,7 @@ aspp_fused_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
   unsigned char* smem = smem_raw + ((1024u - (ptx::smem_u32(smem_raw) & 1023u)) & 1023u);
   unsigned char* a_ring = smem;
   unsigned char* b_ring = a_ring + kAsppNA * kAStage;
-  unsigned char* p_buf = b_ring + kAsppNB * kBStage;            // [kb2][hi | lo][128 rows x 128 B]
-  float* s_bias = reinterpret_cast<float*>(p_buf + 4 * kPPlane);   // [n_br][128]
+  float* s_bias = reinterpret_cast<float*>(b_ring + kAsppNB * kBStage);   // [n_br][128]
   float* s_wb = s_bias + kAsppMaxBranches * kAsppHidden;           // [2 warpgroups][128] per-image bias
   uint64_t* bars = reinterpret_cast<uint64_t*>(s_wb + 2 * kAsppHidden);
   uint64_t* a_full = bars;
@@ -87,7 +88,9 @@ aspp_fused_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
   const int tiles_per_img = p.tiles_x * p.tiles_y;
   const int proj_blk0 = p.br_tap0[p.n_br] * p.kblocks;          // first projection block of the weight tensor
 
-  if (warp == 8) {
+  if (warp >= 8) {
+    ptx::setmaxnreg_dec<40>();
+    if (warp != 8) return;
     // ===================== TMA producer =====================
     ptx::griddep_wait();
     int as = 0, bs = 0; uint32_t aph = 0, bph = 0;
@@ -126,6 +129,7 @@ aspp_fused_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
       }
     }
   } else {
+    ptx::setmaxnreg_inc<232>();
     // ===================== two warpgroups: branch MMAs, conversion to P, projection, output =====================
     const int wg = warp >> 2, wq = warp & 3;
     const int wtid = threadIdx.x & 127;
@@ -184,34 +188,45 @@ aspp_fused_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
             if (++bs == kAsppNB) { bs = 0; bph ^= 1; }
           }
         }
-        wg::wait<0>();                             // also: the previous branch's projection has read P
+        wg::wait<0>();                             // also: the previous branch's projection has read P's registers
         release();
-        // ---- P = hi/lo split of relu(acc1 + bias): column c -> K block c / 64, 16-byte chunk (c % 64) / 8 of the
-        // 128-byte row, XOR-swizzled with the row index (the layout TMA writes for a SWIZZLE_128B K-major operand)
+        // ---- P = hi/lo split of relu(acc1 + bias), kept in registers, and proj(s): acc2 (+)= P . W_proj[:, branch s],
+        // one 64-column K block kb2 at a time.  Accumulator entries (4 g8 + 2 h, +1) -- row row0 + 8 h, columns
+        // 8 g8 + cq, +1 -- become bf16x2 register 2 (g8 % 8) + h, and registers 4 k .. 4 k + 3 are the A fragment of the
+        // block's columns 16 k .. 16 k + 15 (wgmma.cuh, mma_bf16_rs128).  Converting per block lets each half of acc1
+        // die as its half of P is made: acc1, acc2 and all of P would exceed the 168 registers a thread of this
+        // 288-thread kernel gets, and ptxas would serialise every wgmma.
         const float* bias = s_bias + s * kAsppHidden;
 #pragma unroll
-        for (int g8 = 0; g8 < 16; ++g8) {
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            const int row = row0 + 8 * h;
-            const float x0 = fmaxf(acc1[4 * g8 + 2 * h] + bias[8 * g8 + cq], 0.f);
-            const float x1 = fmaxf(acc1[4 * g8 + 2 * h + 1] + bias[8 * g8 + cq + 1], 0.f);
-            const uint32_t hw = ptx::pack_bf16x2(x0, x1);
-            const uint32_t lw = ptx::pack_bf16x2(x0 - __uint_as_float(hw << 16), x1 - __uint_as_float(hw & 0xFFFF0000u));
-            unsigned char* dst = p_buf + (size_t)(g8 >> 3) * 2 * kPPlane + (size_t)row * 128 +
-                                 ((((uint32_t)g8 & 7u) ^ (uint32_t)(row & 7)) << 4) + cq * 2;
-            *reinterpret_cast<uint32_t*>(dst) = hw;
-            *reinterpret_cast<uint32_t*>(dst + kPPlane) = lw;
-          }
-        }
-        ptx::fence_proxy_async();                  // the generic-proxy stores above are read by the tensor core (async proxy)
-        ptx::bar_sync(1 + wg, 128);
-        // ---- proj(s): acc2 (+)= P . W_proj[:, branch s]
         for (int kb2 = 0; kb2 < 2; ++kb2) {
+          uint32_t p_hi[16], p_lo[16];
+#pragma unroll
+          for (int g = 0; g < 8; ++g) {
+            const int g8 = 8 * kb2 + g;
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              const float x0 = fmaxf(acc1[4 * g8 + 2 * h] + bias[8 * g8 + cq], 0.f);
+              const float x1 = fmaxf(acc1[4 * g8 + 2 * h + 1] + bias[8 * g8 + cq + 1], 0.f);
+              const uint32_t hw = ptx::pack_bf16x2(x0, x1);
+              p_hi[2 * g + h] = hw;
+              p_lo[2 * g + h] = ptx::pack_bf16x2(x0 - __uint_as_float(hw << 16), x1 - __uint_as_float(hw & 0xFFFF0000u));
+            }
+          }
           ptx::mbar_wait(&b_full[bs], bph);
-          const uint32_t a_hi = ptx::smem_u32(p_buf + (size_t)kb2 * 2 * kPPlane) + (uint32_t)(wg * 64 * 128);
           const uint32_t b_hi = ptx::smem_u32(b_ring + (size_t)bs * kBStage);
-          issue(acc2, a_hi, a_hi + kPPlane, b_hi, b_hi + 128 * 128, (s > 0 || kb2 > 0) ? 1u : 0u, -1, bs);
+          const uint64_t db_hi = wg::desc_k_sw128(b_hi), db_lo = wg::desc_k_sw128(b_hi + 128 * 128);
+          wg::fence();
+#pragma unroll
+          for (int k = 0; k < 4; ++k) {
+            const uint64_t koff = (uint64_t)((k * 32) >> 4);
+            wg::mma_bf16_rs128(acc2, &p_hi[4 * k], db_hi + koff, (s > 0 || kb2 > 0 || k > 0) ? 1u : 0u);
+            wg::mma_bf16_rs128(acc2, &p_hi[4 * k], db_lo + koff, 1);
+            wg::mma_bf16_rs128(acc2, &p_lo[4 * k], db_hi + koff, 1);
+          }
+          wg::commit();
+          wg::wait<0>();                           // P's registers are read until the group completes
+          release();
+          pend_b = bs;
           if (++bs == kAsppNB) { bs = 0; bph ^= 1; }
         }
       }
@@ -324,7 +339,7 @@ extern "C" int stp3_aspp_fused_fwd(const stp3_aspp_desc* d, const void* x_hi, co
                       CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r3 != CUDA_SUCCESS) return set_error(STP3_ECUDA, "cuTensorMapEncodeTiled(weights) failed: %d", (int)r3);
   }
-  const size_t smem_bytes = 1024 + (size_t)kAsppNA * kAStage + (size_t)kAsppNB * kBStage + 4 * (size_t)kPPlane +
+  const size_t smem_bytes = 1024 + (size_t)kAsppNA * kAStage + (size_t)kAsppNB * kBStage +
                             (kAsppMaxBranches + 2) * kAsppHidden * sizeof(float) + 2 * (kAsppNA + kAsppNB) * 8;
   static thread_local int attr_dev = -1;           // once per device: the attribute call costs microseconds per eager launch
   int cur_dev = 0;

@@ -1,4 +1,4 @@
-// Thin inline-PTX wrappers for sm_90a: mbarrier, TMA (cp.async.bulk.tensor), programmatic dependent launch.
+// Thin inline-PTX wrappers for sm_90a: mbarrier, TMA (cp.async.bulk.tensor), programmatic dependent launch, setmaxnreg.
 #pragma once
 #include <cstdint>
 #include <cuda.h>  // CUtensorMap (types only; the encode entry point is fetched at run time)
@@ -117,6 +117,13 @@ __device__ __forceinline__ void tma_load_5d(void* dst, const CUtensorMap* m, uin
       "l"(m), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
       : "memory");
 }
+
+// warpgroup register reallocation (every warp of the warpgroup executes it): lower / raise this warpgroup's per-thread
+// register count to N
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
 
 // named barrier over `count` threads (a multiple of 32) of the CTA
 __device__ __forceinline__ void bar_sync(int id, int count) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory"); }
