@@ -10,14 +10,25 @@
 //   (taps of one kernel column share ONE activation load: the box holds 8 + 2 image rows, tap j reads it shifted by j rows)
 //   main    : the path chains one after the other, each into a register accumulator (its own input tensor, tap list,
 //             MMA width N and K-step range); chain c's columns are the hidden channels [tmem_col, tmem_col + N)
-//   convert : straight from the registers: add the (per-image) bias, ReLU, split to bf16 hi/lo and write the 8-channel
-//             pieces of the compacted 128-channel operand P into shared memory (128B-swizzled K-major)
-//   proj    : acc2 = P . W_agg  (N = 64);  acc3 = x_tile . W_projection (N = 64) when the block changes its width
+//   convert : straight from the registers: add the (per-image) bias, ReLU and split to bf16 hi/lo.  The packed fp32
+//             accumulator fragment of two 8-column groups is the wgmma A fragment of 16 channels of the compacted
+//             128-channel operand P, so P never leaves the registers
+//   agg     : acc2 += P_k . W_agg[k] (register-A wgmma, N = 64) for every K = 16 step of P as soon as both of its
+//             8-channel pieces exist; a step that straddles two chains keeps the first chain's half until the next one
+//             completes it.  The steps are issued in increasing k, so acc2 sums exactly as the shared-memory P did
+//   proj    : acc3 = x_tile . W_projection (N = 64) when the block changes its width, on the activation stage that
+//             path 2 (the 1x1x1 chain of x, always the last chain) has loaded
 //   final   : out = relu(acc2 + per-image bias) + (acc3 + per-image bias | x), hi/lo planes, per-image column sums
 //
-// Two warpgroups own rows 0..63 / 64..127 of the tile (the A operand of P is a warpgroup's own rows, so P needs only a
-// warpgroup barrier); warp 8 is the TMA producer.  Same precision scheme as conv_igemm.cu (bf16 hi/lo planes, three
-// MMAs per product, fp32 accumulation).
+// Two warpgroups own rows 0..63 / 64..127 of the tile; warp 8 is the TMA producer, and its warpgroup hands its registers
+// to the MMA warpgroups (setmaxnreg 40 / 232: a chain accumulator, acc2, acc3 and the P fragments live at once do not
+// fit the 168 registers per thread of an even split, and ptxas would serialise the wgmma).  Same precision scheme as
+// conv_igemm.cu (bf16 hi/lo planes, three MMAs per product, fp32 accumulation).  Every chain's MMA width, K-step count
+// and place in P select compile-time issue sequences once per chain, so no wgmma sits behind a run-time width or
+// K-skip branch.
+//
+//   smem : 3 activation stages (120 KB) + 4 weight stages (64 KB) + the aggregation weights, resident for the kernel's
+//          lifetime (32 KB; they are the same for every tile)
 #include <cuda_bf16.h>
 
 #include "common.cuh"
@@ -26,16 +37,24 @@
 
 namespace stp3 {
 
-constexpr int kBlkThreads = 288;                  // 2 warpgroups + the producer warp
+constexpr int kBlkThreads = 384;                  // 2 MMA warpgroups + the producer warpgroup
 constexpr int kBlkMaxChains = 3;
 constexpr int kBlkMaxTaps = 32;                 // 18 + 9 + 1 path taps + the projection's
-constexpr int kBlkNA = 2, kBlkNB = 4;          // 200 KB of operand rings and P in 227 KB of shared memory
+constexpr int kBlkNA = 3, kBlkNB = 4;
 constexpr int kBlkBoxRows = 10;                   // 8 image rows + 2: one activation load serves the three dy taps of a kernel column
 constexpr int kBlkAStage = 2 * kBlkBoxRows * 16 * 128;
 constexpr int kBlkMaxGroups = 16;
 constexpr int kBlkBRows = 64;                     // weight rows per plane: chains are at most 64 wide
 constexpr int kBlkBStage = 2 * kBlkBRows * 128;
-constexpr int kBlkPPlane = 128 * 128;
+
+// The two chain layouts the kernel is compiled for, i.e. the two TemporalBlock packs.  Per chain: MMA width N, the
+// 8-channel pieces of P it produces (its column groups 0 .. npc - 1), the first of them:
+//   kBlkThreePaths: three 33..40-channel paths at N = 48, pieces 0-4 | 5-9 | 10-14 (piece 15 is zero)
+//   kBlkDiagPair  : the block-diagonal chain of both mid paths at N = 64, pieces 0-7, then path 2 at N = 32, pieces 8-11
+// Chain 0 of the first layout ends in the middle of a K = 16 step of P; chain 1 completes that step.  Chain 2 issues its
+// last half step with a zero second half.  K steps with no piece at all (the second layout's steps 6 and 7) are not
+// issued: they would add exact zeros to acc2.
+enum BlkLayout { kBlkThreePaths = 0, kBlkDiagPair = 1 };
 
 struct BlkChain {
   int src;                  // 0 = mid tensor, 1 = x tensor
@@ -46,6 +65,7 @@ struct BlkChain {
   int tmem_col;             // first hidden column of the chain's outputs
   int ks_first, ks_end;     // K = 16 steps that carry data
   int wblk0;                // first weight block (one per tap)
+  int pc0;                  // first 8-channel piece of P this chain produces
 };
 
 struct BlkParams {
@@ -53,11 +73,10 @@ struct BlkParams {
   int tiles_x, tiles_y, n_tiles;
   int n_chain;
   BlkChain chain[kBlkMaxChains];
-  int has_res_proj;         // acc3 = x . W_projection
+  int has_res_proj;         // acc3 = x . W_projection, on the last chain's activation stage
   BlkChain res;
   signed char tap[kBlkMaxTaps][4];        // (dt, dy, dx)
   unsigned char gstart[kBlkMaxGroups], gsize[kBlkMaxGroups];   // first tap / number of taps of every group
-  int piece_col[16];        // hidden column of the 8-channel piece pp of P, -1 = zeros
   const float* hid_bias;    // [n_img][128] bias of the hidden channels in P order
   const float* img_bias;    // [n_img][64]  aggregation bias (+ pyramid-pooling branch)
   const float* res_bias;    // [n_img][64]  projection bias (has_res_proj) or null
@@ -71,6 +90,9 @@ struct BlkParams {
   int wagg_blk0;            // two weight blocks (K blocks of P) of the aggregation conv
 };
 
+template <int V>
+struct BlkC { static constexpr int value = V; };
+
 // true if every input element the tap group touches for this 8x16 tile is zero padding
 __device__ __forceinline__ bool blk_group_is_padding(const BlkParams& p, int g, int tidx, int oy_tile, int ox0) {
   const int t0 = p.gstart[g];
@@ -80,6 +102,7 @@ __device__ __forceinline__ bool blk_group_is_padding(const BlkParams& p, int g, 
   return tt < 0 || tt >= p.T || yhi < 0 || ylo >= p.H || xhi < 0 || xlo >= p.W;
 }
 
+template <int LAYOUT>
 __global__ void __launch_bounds__(kBlkThreads, 1)
 block_fused_kernel(const __grid_constant__ CUtensorMap tm_m_hi, const __grid_constant__ CUtensorMap tm_m_lo,
                    const __grid_constant__ CUtensorMap tm_x_hi, const __grid_constant__ CUtensorMap tm_x_lo,
@@ -89,14 +112,15 @@ block_fused_kernel(const __grid_constant__ CUtensorMap tm_m_hi, const __grid_con
   unsigned char* smem = smem_raw + ((1024u - (ptx::smem_u32(smem_raw) & 1023u)) & 1023u);
   unsigned char* a_ring = smem;
   unsigned char* b_ring = a_ring + kBlkNA * kBlkAStage;
-  unsigned char* p_buf = b_ring + kBlkNB * kBlkBStage;          // [kb2][hi | lo][128 rows x 128 B]
-  float* s_hb = reinterpret_cast<float*>(p_buf + 4 * kBlkPPlane);   // [2 warpgroups][128] hidden bias of the image
+  unsigned char* w_agg = b_ring + kBlkNB * kBlkBStage;             // the two aggregation blocks, as two weight stages
+  float* s_hb = reinterpret_cast<float*>(w_agg + 2 * kBlkBStage);   // [2 warpgroups][128] hidden bias of the image
   float* s_wb = s_hb + 2 * 128;                                     // [2 warpgroups][128] img_bias (64) | res_bias (64)
   uint64_t* bars = reinterpret_cast<uint64_t*>(s_wb + 2 * 128);
   uint64_t* a_full = bars;
   uint64_t* a_empty = a_full + kBlkNA;
   uint64_t* b_full = a_empty + kBlkNA;
   uint64_t* b_empty = b_full + kBlkNB;
+  uint64_t* w_agg_full = b_empty + kBlkNB;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (warp == 8 && lane == 0) {
@@ -104,16 +128,34 @@ block_fused_kernel(const __grid_constant__ CUtensorMap tm_m_hi, const __grid_con
     ptx::prefetch_tmap(&tm_w);
     for (int i = 0; i < kBlkNA; ++i) { ptx::mbar_init(&a_full[i], 1); ptx::mbar_init(&a_empty[i], 2); }
     for (int i = 0; i < kBlkNB; ++i) { ptx::mbar_init(&b_full[i], 1); ptx::mbar_init(&b_empty[i], 2); }
+    ptx::mbar_init(w_agg_full, 2);               // one arrive.expect_tx per aggregation block
     ptx::fence_mbar_init();
   }
-  // P pieces without a hidden column stay zero for the kernel's lifetime
-  for (int i = threadIdx.x; i < 4 * kBlkPPlane / 16; i += blockDim.x) reinterpret_cast<uint4*>(p_buf)[i] = make_uint4(0u, 0u, 0u, 0u);
-  ptx::fence_proxy_async();
   __syncthreads();
   const int tiles_per_img = p.tiles_x * p.tiles_y;
 
-  if (warp == 8) {
+  if (warp >= 8) {
+    ptx::setmaxnreg_dec<40>();
+    if (warp != 8) return;
     // ===================== TMA producer =====================
+    // weight block `blk` = [hi 128 rows][lo 128 rows]; output column n of an N-wide chain is row n (n < N/2) or
+    // 64 + n - N/2 of each plane; only those rows are fetched (boxes of 8 rows)
+    auto fetch_b = [&](unsigned char* dst, uint64_t* bar, int blk, int n_mma) {
+      const int rows = n_mma / 2;
+      ptx::mbar_arrive_expect_tx(bar, (uint32_t)(2 * n_mma * 128));
+      for (int r8 = 0; r8 < rows; r8 += 8) {
+        for (int h = 0; h < 2; ++h) {
+          ptx::tma_load_2d(dst + (h * rows + r8) * 128, &tm_w, bar, 0, blk * 256 + h * 64 + r8);
+          ptx::tma_load_2d(dst + kBlkBRows * 128 + (h * rows + r8) * 128, &tm_w, bar, 0, blk * 256 + 128 + h * 64 + r8);
+        }
+      }
+    };
+    // module weights, not written by the predecessor: fetched before the dependency wait
+    if (ptx::elect_one_sync()) {
+      fetch_b(w_agg, w_agg_full, p.wagg_blk0, 64);
+      fetch_b(w_agg + kBlkBStage, w_agg_full, p.wagg_blk0 + 1, 64);
+    }
+    __syncwarp();
     ptx::griddep_wait();
     int as = 0, bs = 0; uint32_t aph = 0, bph = 0;
     auto load_a = [&](int src, int c, int x, int y, int t, int b) {
@@ -127,21 +169,9 @@ block_fused_kernel(const __grid_constant__ CUtensorMap tm_m_hi, const __grid_con
       __syncwarp();
       if (++as == kBlkNA) { as = 0; aph ^= 1; }
     };
-    // weight block `blk` = [hi 128 rows][lo 128 rows]; output column n of an N-wide chain is row n (n < N/2) or
-    // 64 + n - N/2 of each plane; only those rows are fetched (boxes of 8 rows)
     auto load_b = [&](int blk, int n_mma) {
       ptx::mbar_wait(&b_empty[bs], bph ^ 1);
-      if (ptx::elect_one_sync()) {
-        unsigned char* dst = b_ring + (size_t)bs * kBlkBStage;
-        const int rows = n_mma / 2;
-        ptx::mbar_arrive_expect_tx(&b_full[bs], (uint32_t)(2 * n_mma * 128));
-        for (int r8 = 0; r8 < rows; r8 += 8) {
-          for (int h = 0; h < 2; ++h) {
-            ptx::tma_load_2d(dst + (h * rows + r8) * 128, &tm_w, &b_full[bs], 0, blk * 256 + h * 64 + r8);
-            ptx::tma_load_2d(dst + kBlkBRows * 128 + (h * rows + r8) * 128, &tm_w, &b_full[bs], 0, blk * 256 + 128 + h * 64 + r8);
-          }
-        }
-      }
+      if (ptx::elect_one_sync()) fetch_b(b_ring + (size_t)bs * kBlkBStage, &b_full[bs], blk, n_mma);
       __syncwarp();
       if (++bs == kBlkNB) { bs = 0; bph ^= 1; }
     };
@@ -158,11 +188,11 @@ block_fused_kernel(const __grid_constant__ CUtensorMap tm_m_hi, const __grid_con
           for (int j = 0; j < p.gsize[g]; ++j) load_b(ch.wblk0 + (t0 + j - ch.tap0), ch.n_mma);
         }
       }
-      load_b(p.wagg_blk0, 64); load_b(p.wagg_blk0 + 1, 64);
-      if (p.has_res_proj) { load_a(1, p.res.cin_off, ox0, oy_tile, tidx, bidx); load_b(p.res.wblk0, 64); }
+      if (p.has_res_proj) load_b(p.res.wblk0, 64);          // its activations: the last chain's stage
     }
   } else {
-    // ===================== two warpgroups: MMA, convert, projection, output =====================
+    ptx::setmaxnreg_inc<232>();
+    // ===================== two warpgroups: chains, conversion to P, aggregation, projection, output =====================
     const int wg = warp >> 2, wq = warp & 3;
     const int wtid = threadIdx.x & 127;
     const bool wg_leader = wtid == 0;
@@ -170,6 +200,7 @@ block_fused_kernel(const __grid_constant__ CUtensorMap tm_m_hi, const __grid_con
     const int cq = 2 * (lane & 3);                           // first of its two columns in every 8-column group
     float* hb = s_hb + wg * 128;
     float* wb = s_wb + wg * 128;
+    const uint32_t w_agg_u32 = ptx::smem_u32(w_agg);
     int as = 0, bs = 0; uint32_t aph = 0, bph = 0;
     int pend_a = -1, pend_b = -1;               // ring slots read by the last committed wgmma group
     auto release = [&]() {
@@ -179,25 +210,113 @@ block_fused_kernel(const __grid_constant__ CUtensorMap tm_m_hi, const __grid_con
       }
       pend_a = pend_b = -1;
     };
-    // acc (+)= A . B over k in [k0, k1) with hi*hi + hi*lo + lo*hi, then commit and release the previous group's slots
-    auto issue = [&](float* acc, int n, uint32_t a_hi, uint32_t a_lo, uint32_t b_hi, uint32_t b_lo, int k0, int k1,
-                     uint32_t accumulate, int slot_a, int slot_b) {
-      const uint64_t da_hi = wg::desc_k_sw128(a_hi), da_lo = wg::desc_k_sw128(a_lo);
-      const uint64_t db_hi = wg::desc_k_sw128(b_hi), db_lo = wg::desc_k_sw128(b_lo);
+    // acc (+)= A . B over KS K steps from k0 with hi*hi + hi*lo + lo*hi, then commit and release the previous group's slots
+    auto issue = [&](auto n_c, auto ks_c, float* acc, uint32_t a_hi, uint32_t b_hi, int k0, uint32_t accumulate,
+                     int slot_a, int slot_b) {
+      constexpr int N = decltype(n_c)::value, KS = decltype(ks_c)::value;
+      const uint64_t da_hi = wg::desc_k_sw128(a_hi) + (uint64_t)(2 * k0), da_lo = wg::desc_k_sw128(a_hi + kBlkAStage / 2) + (uint64_t)(2 * k0);
+      const uint64_t db_hi = wg::desc_k_sw128(b_hi) + (uint64_t)(2 * k0), db_lo = wg::desc_k_sw128(b_hi + kBlkBRows * 128) + (uint64_t)(2 * k0);
       wg::fence();
 #pragma unroll
-      for (int k = 0; k < 4; ++k) {
-        if (k < k0 || k >= k1) continue;
-        const uint64_t koff = (uint64_t)((k * 32) >> 4);
-        wg::mma_bf16_n<64>(n, acc, da_hi + koff, db_hi + koff, accumulate | (uint32_t)(k > k0));
-        wg::mma_bf16_n<64>(n, acc, da_hi + koff, db_lo + koff, 1);
-        wg::mma_bf16_n<64>(n, acc, da_lo + koff, db_hi + koff, 1);
+      for (int k = 0; k < KS; ++k) {
+        wg::mma_bf16<N>(acc, da_hi + 2 * k, db_hi + 2 * k, k == 0 ? accumulate : 1u);
+        wg::mma_bf16<N>(acc, da_hi + 2 * k, db_lo + 2 * k, 1);
+        wg::mma_bf16<N>(acc, da_lo + 2 * k, db_hi + 2 * k, 1);
       }
       wg::commit();
       wg::wait<1>();
       release();
       pend_a = slot_a; pend_b = slot_b;
     };
+    // one K = 16 step of the aggregation: acc2 (+)= P_s . W_agg[s], P_s from registers (hi / lo A fragments)
+    float acc2[32], acc3[32];
+    auto agg_step = [&](int s, const uint32_t* f_hi, const uint32_t* f_lo) {
+      const uint32_t b_hi = w_agg_u32 + (uint32_t)((s >> 2) * kBlkBStage);
+      const uint64_t koff = (uint64_t)(2 * (s & 3));
+      const uint64_t db_hi = wg::desc_k_sw128(b_hi) + koff, db_lo = wg::desc_k_sw128(b_hi + kBlkBRows * 128) + koff;
+      wg::mma_bf16_rs64(acc2, f_hi, db_hi, s > 0 ? 1u : 0u);
+      wg::mma_bf16_rs64(acc2, f_hi, db_lo, 1);
+      wg::mma_bf16_rs64(acc2, f_lo, db_hi, 1);
+    };
+    uint32_t carry_hi[2] = {0u, 0u}, carry_lo[2] = {0u, 0u};   // the first half of a K step that straddles two chains
+    int agg_next = 0;                           // next K step of the aggregation
+
+    // one chain of one tile: its taps (and the projection on the same activation stage), then its pieces of P into acc2
+    auto run_chain = [&](auto n_c, auto npc_c, auto odd_c, auto close_c, const BlkChain& ch, int tidx, int oy_tile, int ox0,
+                         bool with_proj) {
+      constexpr int N = decltype(n_c)::value, NPC = decltype(npc_c)::value, ODD = decltype(odd_c)::value;
+      constexpr bool OPEN = ((NPC - ODD) & 1) != 0, CLOSE = decltype(close_c)::value != 0;
+      float acc[N / 2];
+      auto taps = [&](auto ks_c) {
+        uint32_t accumulate = 0;
+        for (int g = ch.grp0; g < ch.grp0 + ch.ngrp; ++g) {
+          if (blk_group_is_padding(p, g, tidx, oy_tile, ox0)) continue;
+          ptx::mbar_wait(&a_full[as], aph);
+          const uint32_t a_hi0 = ptx::smem_u32(a_ring + (size_t)as * kBlkAStage) + (uint32_t)(wg * 64 * 128);
+          for (int j = 0; j < p.gsize[g]; ++j) {
+            ptx::mbar_wait(&b_full[bs], bph);
+            const bool last = j + 1 == p.gsize[g];
+            const uint32_t b_hi = ptx::smem_u32(b_ring + (size_t)bs * kBlkBStage);
+            // tap j of the group: shifted by j image rows
+            issue(n_c, ks_c, acc, a_hi0 + (uint32_t)(j * 16 * 128), b_hi, ch.ks_first, accumulate,
+                  last && !with_proj ? as : -1, bs);
+            accumulate = 1;
+            if (++bs == kBlkNB) { bs = 0; bph ^= 1; }
+          }
+          if (with_proj) {                       // the 1x1 projection of x reads the same stage (one group, centre tap)
+            ptx::mbar_wait(&b_full[bs], bph);
+            issue(BlkC<64>{}, ks_c, acc3, a_hi0, ptx::smem_u32(b_ring + (size_t)bs * kBlkBStage), p.res.ks_first, 0u, as, bs);
+            if (++bs == kBlkNB) { bs = 0; bph ^= 1; }
+          }
+          if (++as == kBlkNA) { as = 0; aph ^= 1; }
+        }
+      };
+      switch (ch.ks_end - ch.ks_first) {
+        case 1: taps(BlkC<1>{}); break;
+        case 2: taps(BlkC<2>{}); break;
+        case 3: taps(BlkC<3>{}); break;
+        default: taps(BlkC<4>{}); break;
+      }
+      wg::wait<0>();                             // also: the previous chain's aggregation has read its P registers
+      release();
+      // piece k of the chain = its 8-column group k = P piece pc0 + k: relu(acc + bias) split to bf16 hi / lo.
+      // Accumulator entries (4 k + 2 h, +1) -- row row0 + 8 h, columns 8 k + cq, +1 -- are bf16x2 register h of the piece
+      uint32_t f_hi[NPC][2], f_lo[NPC][2];
+#pragma unroll
+      for (int k = 0; k < NPC; ++k) {
+        const float* bias = hb + (ch.pc0 + k) * 8 + cq;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const float x0 = fmaxf(acc[4 * k + 2 * h] + bias[0], 0.f);
+          const float x1 = fmaxf(acc[4 * k + 2 * h + 1] + bias[1], 0.f);
+          const uint32_t hw = ptx::pack_bf16x2(x0, x1);
+          f_hi[k][h] = hw;
+          f_lo[k][h] = ptx::pack_bf16x2(x0 - __uint_as_float(hw << 16), x1 - __uint_as_float(hw & 0xFFFF0000u));
+        }
+      }
+      wg::fence();
+      if constexpr (ODD) {                       // complete the step the previous chain began
+        const uint32_t a_hi[4] = {carry_hi[0], carry_hi[1], f_hi[0][0], f_hi[0][1]};
+        const uint32_t a_lo[4] = {carry_lo[0], carry_lo[1], f_lo[0][0], f_lo[0][1]};
+        agg_step(agg_next++, a_hi, a_lo);
+      }
+#pragma unroll
+      for (int k = ODD; k + 1 < NPC; k += 2) {
+        const uint32_t a_hi[4] = {f_hi[k][0], f_hi[k][1], f_hi[k + 1][0], f_hi[k + 1][1]};
+        const uint32_t a_lo[4] = {f_lo[k][0], f_lo[k][1], f_lo[k + 1][0], f_lo[k + 1][1]};
+        agg_step(agg_next++, a_hi, a_lo);
+      }
+      if constexpr (OPEN && CLOSE) {             // the last piece of P: the other half of its step is zero
+        const uint32_t a_hi[4] = {f_hi[NPC - 1][0], f_hi[NPC - 1][1], 0u, 0u};
+        const uint32_t a_lo[4] = {f_lo[NPC - 1][0], f_lo[NPC - 1][1], 0u, 0u};
+        agg_step(agg_next++, a_hi, a_lo);
+      } else if constexpr (OPEN) {
+        carry_hi[0] = f_hi[NPC - 1][0]; carry_hi[1] = f_hi[NPC - 1][1];
+        carry_lo[0] = f_lo[NPC - 1][0]; carry_lo[1] = f_lo[NPC - 1][1];
+      }
+      wg::commit();
+    };
+
     float sacc[16];                              // column sums of this thread's columns (8 groups of 2)
 #pragma unroll
     for (int i = 0; i < 16; ++i) sacc[i] = 0.f;
@@ -213,6 +332,7 @@ block_fused_kernel(const __grid_constant__ CUtensorMap tm_m_hi, const __grid_con
         sacc[i] = 0.f;
       }
     };
+    ptx::mbar_wait(w_agg_full, 0);
     ptx::griddep_wait();
     for (int tile = cta; tile < p.n_tiles; tile += n_cta) {
       const int img = tile / tiles_per_img, rem = tile % tiles_per_img;
@@ -231,70 +351,15 @@ block_fused_kernel(const __grid_constant__ CUtensorMap tm_m_hi, const __grid_con
         else if (p.res_bias) wb[wtid] = *(reinterpret_cast<const volatile float*>(p.res_bias) + (size_t)img * 64 + wtid - 64);
       }
       ptx::bar_sync(1 + wg, 128);
-      // ---------- main: every chain into registers, converted into its pieces of P
-      for (int c = 0; c < p.n_chain; ++c) {
-        const BlkChain& ch = p.chain[c];
-        float acc[32];
-        uint32_t accumulate = 0;
-        for (int g = ch.grp0; g < ch.grp0 + ch.ngrp; ++g) {
-          if (blk_group_is_padding(p, g, tidx, oy_tile, ox0)) continue;
-          ptx::mbar_wait(&a_full[as], aph);
-          const uint32_t a_hi0 = ptx::smem_u32(a_ring + (size_t)as * kBlkAStage) + (uint32_t)(wg * 64 * 128);
-          for (int j = 0; j < p.gsize[g]; ++j) {
-            ptx::mbar_wait(&b_full[bs], bph);
-            const uint32_t a_hi = a_hi0 + (uint32_t)(j * 16 * 128);          // tap j of the group: shifted by j image rows
-            const uint32_t b_hi = ptx::smem_u32(b_ring + (size_t)bs * kBlkBStage);
-            issue(acc, ch.n_mma, a_hi, a_hi + kBlkAStage / 2, b_hi, b_hi + kBlkBRows * 128, ch.ks_first, ch.ks_end,
-                  accumulate, j + 1 == p.gsize[g] ? as : -1, bs);
-            accumulate = 1;
-            if (++bs == kBlkNB) { bs = 0; bph ^= 1; }
-          }
-          if (++as == kBlkNA) { as = 0; aph ^= 1; }
-        }
-        wg::wait<0>();
-        release();
-        // convert: piece pp of P holds hidden columns [piece_col[pp], +8) = 8-column group (piece_col - tmem_col) / 8
-        for (int pp = 0; pp < 16; ++pp) {
-          const int col = p.piece_col[pp] - ch.tmem_col;
-          if (p.piece_col[pp] < 0 || col < 0 || col >= ch.n_mma) continue;
-          const int grp8 = col >> 3;
-#pragma unroll
-          for (int g8 = 0; g8 < 8; ++g8) {               // chains are at most 64 wide: 8 groups of 8 columns
-            if (g8 != grp8) continue;
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-              const int row = row0 + 8 * h;
-              const float x0 = fmaxf(acc[4 * g8 + 2 * h] + hb[pp * 8 + cq], 0.f);
-              const float x1 = fmaxf(acc[4 * g8 + 2 * h + 1] + hb[pp * 8 + cq + 1], 0.f);
-              const uint32_t hw = ptx::pack_bf16x2(x0, x1);
-              const uint32_t lw = ptx::pack_bf16x2(x0 - __uint_as_float(hw << 16), x1 - __uint_as_float(hw & 0xFFFF0000u));
-              unsigned char* dst = p_buf + (size_t)(pp >> 3) * 2 * kBlkPPlane + (size_t)row * 128 +
-                                   ((((uint32_t)pp & 7u) ^ (uint32_t)(row & 7)) << 4) + cq * 2;
-              *reinterpret_cast<uint32_t*>(dst) = hw;
-              *reinterpret_cast<uint32_t*>(dst + kBlkPPlane) = lw;
-            }
-          }
-        }
-      }
-      ptx::fence_proxy_async();                  // the generic-proxy stores above are read by the tensor core (async proxy)
-      ptx::bar_sync(1 + wg, 128);
-      // ---------- projection: acc2 = P . W_agg, acc3 = x . W_projection
-      float acc2[32], acc3[32];
-      for (int kb2 = 0; kb2 < 2; ++kb2) {
-        ptx::mbar_wait(&b_full[bs], bph);
-        const uint32_t a_hi = ptx::smem_u32(p_buf + (size_t)kb2 * 2 * kBlkPPlane) + (uint32_t)(wg * 64 * 128);
-        const uint32_t b_hi = ptx::smem_u32(b_ring + (size_t)bs * kBlkBStage);
-        issue(acc2, 64, a_hi, a_hi + kBlkPPlane, b_hi, b_hi + kBlkBRows * 128, 0, 4, kb2 > 0 ? 1u : 0u, -1, bs);
-        if (++bs == kBlkNB) { bs = 0; bph ^= 1; }
-      }
-      if (p.has_res_proj) {
-        ptx::mbar_wait(&a_full[as], aph);
-        ptx::mbar_wait(&b_full[bs], bph);
-        const uint32_t a_hi = ptx::smem_u32(a_ring + (size_t)as * kBlkAStage) + (uint32_t)(wg * 64 * 128);
-        const uint32_t b_hi = ptx::smem_u32(b_ring + (size_t)bs * kBlkBStage);
-        issue(acc3, 64, a_hi, a_hi + kBlkAStage / 2, b_hi, b_hi + kBlkBRows * 128, p.res.ks_first, p.res.ks_end, 0u, as, bs);
-        if (++as == kBlkNA) { as = 0; aph ^= 1; }
-        if (++bs == kBlkNB) { bs = 0; bph ^= 1; }
+      // ---------- the chains, each followed by the aggregation steps its pieces of P complete
+      agg_next = 0;
+      if constexpr (LAYOUT == kBlkThreePaths) {
+        run_chain(BlkC<48>{}, BlkC<5>{}, BlkC<0>{}, BlkC<0>{}, p.chain[0], tidx, oy_tile, ox0, false);
+        run_chain(BlkC<48>{}, BlkC<5>{}, BlkC<1>{}, BlkC<0>{}, p.chain[1], tidx, oy_tile, ox0, false);
+        run_chain(BlkC<48>{}, BlkC<5>{}, BlkC<0>{}, BlkC<1>{}, p.chain[2], tidx, oy_tile, ox0, p.has_res_proj != 0);
+      } else {
+        run_chain(BlkC<64>{}, BlkC<8>{}, BlkC<0>{}, BlkC<0>{}, p.chain[0], tidx, oy_tile, ox0, false);
+        run_chain(BlkC<32>{}, BlkC<4>{}, BlkC<0>{}, BlkC<0>{}, p.chain[1], tidx, oy_tile, ox0, p.has_res_proj != 0);
       }
       wg::wait<0>();
       release();
@@ -332,7 +397,6 @@ block_fused_kernel(const __grid_constant__ CUtensorMap tm_m_hi, const __grid_con
     if (p.sum_part && sum_img >= 0) flush_sums(sum_img);
   }
 }
-
 typedef CUresult (*PFN_tmapEncodeTiledB)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                          const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
                                          CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
@@ -428,13 +492,26 @@ extern "C" int stp3_block_fused_fwd(const stp3_block_desc* d, const void* mid_hi
     stp3_block_chain rs = d->res;
     STP3_CHECK_ARG(rs.n_taps == 1 && rs.src == 1 && rs.n_mma == 64, "the projection chain is a 1x1 on x with 64 outputs");
     const int rc = fill(p.res, rs); if (rc) return rc;
+    const BlkChain& last = p.chain[p.n_chain - 1];
+    STP3_CHECK_ARG(last.src == 1 && last.ntaps == 1 && last.cin_off == p.res.cin_off &&
+                   last.ks_first == p.res.ks_first && last.ks_end == p.res.ks_end,
+                   "the projection shares the last chain's activations: that chain is the 1x1 of x over the same channels");
   } else {
     p.res = p.chain[0];
   }
-  for (int i = 0; i < 16; ++i) {
-    STP3_CHECK_ARG(d->piece_col[i] < 0 || (d->piece_col[i] % 8 == 0 && d->piece_col[i] + 8 <= 144), "bad piece column");
-    p.piece_col[i] = d->piece_col[i];
+  // P: chain c produces pieces pc0 .. pc0 + npc - 1 (its 8-column groups 0 .. npc - 1), in chain order; zeros after
+  static const int kShapes[2][kBlkMaxChains][2] = {{{48, 5}, {48, 5}, {48, 5}}, {{64, 8}, {32, 4}, {0, 0}}};
+  const int layout = p.n_chain == 3 ? kBlkThreePaths : kBlkDiagPair;
+  int pp = 0;
+  for (int c = 0; c < p.n_chain; ++c) {
+    BlkChain& ch = p.chain[c];
+    ch.pc0 = pp;
+    int npc = 0;
+    while (pp < 16 && d->piece_col[pp] >= 0 && d->piece_col[pp] == ch.tmem_col + 8 * npc && 8 * npc < ch.n_mma) { ++pp; ++npc; }
+    STP3_CHECK_ARG(p.n_chain >= 2 && ch.n_mma == kShapes[layout][c][0] && npc == kShapes[layout][c][1],
+                   "chain %d of %d: (N, pieces of P) = (%d, %d) is not a compiled chain layout", c, p.n_chain, ch.n_mma, npc);
   }
+  for (; pp < 16; ++pp) STP3_CHECK_ARG(d->piece_col[pp] < 0, "piece %d of P: the chains' pieces are consecutive, zeros follow", pp);
   p.hid_bias = hid_bias; p.img_bias = img_bias; p.res_bias = res_bias;
   p.res_hi = static_cast<const __nv_bfloat16*>(x_hi); p.res_lo = static_cast<const __nv_bfloat16*>(x_lo);
   p.res_cstride = d->x_cstride;
@@ -464,13 +541,14 @@ extern "C" int stp3_block_fused_fwd(const stp3_block_desc* d, const void* mid_hi
                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) return set_error(STP3_ECUDA, "cuTensorMapEncodeTiled(weights) failed: %d", (int)r);
   }
-  const size_t smem_bytes = 1024 + (size_t)kBlkNA * kBlkAStage + (size_t)kBlkNB * kBlkBStage + 4 * (size_t)kBlkPPlane +
-                            4 * 128 * sizeof(float) + 2 * (kBlkNA + kBlkNB) * 8;
+  const size_t smem_bytes = 1024 + (size_t)kBlkNA * kBlkAStage + (size_t)(kBlkNB + 2) * kBlkBStage +
+                            4 * 128 * sizeof(float) + (2 * (kBlkNA + kBlkNB) + 1) * 8;
   static thread_local int attr_dev = -1;           // once per device: the attribute call costs microseconds per eager launch
   int cur_dev = 0;
   cudaGetDevice(&cur_dev);
   if (attr_dev != cur_dev) {
-    STP3_CUDA_OK(cudaFuncSetAttribute(block_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes));
+    STP3_CUDA_OK(cudaFuncSetAttribute(block_fused_kernel<kBlkThreePaths>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes));
+    STP3_CUDA_OK(cudaFuncSetAttribute(block_fused_kernel<kBlkDiagPair>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes));
     attr_dev = cur_dev;
   }
   const int num_sms = blk_num_sms();
@@ -492,7 +570,10 @@ extern "C" int stp3_block_fused_fwd(const stp3_block_desc* d, const void* mid_hi
   // grid has completed.  Each of them needs a whole SM; an early trigger would let a chain block_fused -> col_sum_reduce
   // -> pool_bias -> aspp_fused be resident at once, and such a chain was seen to stop making progress.  The kernel itself
   // still starts early behind its predecessor (griddepcontrol.wait before it reads what that predecessor wrote).
-  STP3_CUDA_OK(cudaLaunchKernelEx(&cfg, block_fused_kernel, tm[0], tm[1], tm[2], tm[3], tm_w, p));
+  if (layout == kBlkThreePaths)
+    STP3_CUDA_OK(cudaLaunchKernelEx(&cfg, block_fused_kernel<kBlkThreePaths>, tm[0], tm[1], tm[2], tm[3], tm_w, p));
+  else
+    STP3_CUDA_OK(cudaLaunchKernelEx(&cfg, block_fused_kernel<kBlkDiagPair>, tm[0], tm[1], tm[2], tm[3], tm_w, p));
   STP3_CUDA_OK(cudaGetLastError());
   if (col_sums) return launch_col_sum_reduce(p.sum_part, (int)cfg.gridDim.x * 8, p.n_img, col_sums, stream);
   return STP3_OK;
