@@ -25,6 +25,7 @@
 #include <cuda_bf16.h>
 
 #include "common.cuh"
+#include "pipeline.cuh"
 #include "ptx.cuh"
 #include "wgmma.cuh"
 
@@ -37,6 +38,16 @@ constexpr int kAsppNA = 3, kAsppNB = 3;
 constexpr int kAStage = 2 * 8 * 16 * 128;         // hi + lo planes of 8 image rows x 16 pixels x 64 channels
 constexpr int kBStage = 2 * 128 * 128;            // hi + lo planes of the 128 weight rows
 constexpr int kAsppHidden = 128;
+
+// shared memory, from the 1024-byte aligned base (the kernel carves it, the host sizes the launch from `bytes`)
+struct AsppSmem {
+  static constexpr int a_ring = 0;                                          // kAsppNA activation stages
+  static constexpr int b_ring = a_ring + kAsppNA * kAStage;                 // kAsppNB weight stages
+  static constexpr int bias = b_ring + kAsppNB * kBStage;                   // fp32 [kAsppMaxBranches][128] branch biases
+  static constexpr int wb = bias + kAsppMaxBranches * kAsppHidden * 4;      // fp32 [2 warpgroups][128] per-image bias
+  static constexpr int bars = wb + 2 * kAsppHidden * 4;                     // full / empty barriers of both rings
+  static constexpr size_t bytes = 1024 + bars + 2 * (kAsppNA + kAsppNB) * 8;   // + the alignment slack
+};
 
 struct AsppParams {
   int n_img, T, T_total, H, W;
@@ -66,21 +77,18 @@ aspp_fused_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
   const int cta = (int)blockIdx.x, n_cta = (int)gridDim.x;
   extern __shared__ unsigned char smem_raw[];
   unsigned char* smem = smem_raw + ((1024u - (ptx::smem_u32(smem_raw) & 1023u)) & 1023u);
-  unsigned char* a_ring = smem;
-  unsigned char* b_ring = a_ring + kAsppNA * kAStage;
-  float* s_bias = reinterpret_cast<float*>(b_ring + kAsppNB * kBStage);   // [n_br][128]
-  float* s_wb = s_bias + kAsppMaxBranches * kAsppHidden;           // [2 warpgroups][128] per-image bias
-  uint64_t* bars = reinterpret_cast<uint64_t*>(s_wb + 2 * kAsppHidden);
-  uint64_t* a_full = bars;
-  uint64_t* a_empty = a_full + kAsppNA;
-  uint64_t* b_full = a_empty + kAsppNA;
-  uint64_t* b_empty = b_full + kAsppNB;
+  unsigned char* a_ring = smem + AsppSmem::a_ring;
+  unsigned char* b_ring = smem + AsppSmem::b_ring;
+  float* s_bias = reinterpret_cast<float*>(smem + AsppSmem::bias);
+  float* s_wb = reinterpret_cast<float*>(smem + AsppSmem::wb);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + AsppSmem::bars);
+  Ring ra{bars, bars + kAsppNA, kAsppNA};
+  Ring rb{bars + 2 * kAsppNA, bars + 2 * kAsppNA + kAsppNB, kAsppNB};
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (warp == 8 && lane == 0) {
     ptx::prefetch_tmap(&tm_a_hi); ptx::prefetch_tmap(&tm_a_lo); ptx::prefetch_tmap(&tm_w);
-    for (int i = 0; i < kAsppNA; ++i) { ptx::mbar_init(&a_full[i], 1); ptx::mbar_init(&a_empty[i], 2); }
-    for (int i = 0; i < kAsppNB; ++i) { ptx::mbar_init(&b_full[i], 1); ptx::mbar_init(&b_empty[i], 2); }
+    ra.init(2); rb.init(2);
     ptx::fence_mbar_init();
   }
   for (int i = threadIdx.x; i < p.n_br * kAsppHidden; i += blockDim.x) s_bias[i] = p.br_bias[i];
@@ -93,17 +101,12 @@ aspp_fused_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
     if (warp != 8) return;
     // ===================== TMA producer =====================
     ptx::griddep_wait();
-    int as = 0, bs = 0; uint32_t aph = 0, bph = 0;
     auto load_b = [&](int blk) {                   // weight block `blk`: [hi 128 rows][lo 128 rows]
-      ptx::mbar_wait(&b_empty[bs], bph ^ 1);
-      if (ptx::elect_one_sync()) {
-        unsigned char* dst = b_ring + (size_t)bs * kBStage;
-        ptx::mbar_arrive_expect_tx(&b_full[bs], (uint32_t)kBStage);
-        ptx::tma_load_2d(dst, &tm_w, &b_full[bs], 0, blk * 256);
-        ptx::tma_load_2d(dst + 128 * 128, &tm_w, &b_full[bs], 0, blk * 256 + 128);
-      }
-      __syncwarp();
-      if (++bs == kAsppNB) { bs = 0; bph ^= 1; }
+      rb.produce(kBStage, [&](int s, uint64_t* bar) {
+        unsigned char* dst = b_ring + (size_t)s * kBStage;
+        ptx::tma_load_2d(dst, &tm_w, bar, 0, blk * 256);
+        ptx::tma_load_2d(dst + 128 * 128, &tm_w, bar, 0, blk * 256 + 128);
+      });
     };
     for (int tile = cta; tile < p.n_tiles; tile += n_cta) {
       const int img = tile / tiles_per_img, rem = tile % tiles_per_img;
@@ -113,15 +116,11 @@ aspp_fused_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
         for (int t = p.br_tap0[s]; t < p.br_tap0[s + 1]; ++t) {
           if (aspp_tap_is_padding(p, t, oy_tile, ox0)) continue;
           for (int kb = 0; kb < p.kblocks; ++kb) {
-            ptx::mbar_wait(&a_empty[as], aph ^ 1);
-            if (ptx::elect_one_sync()) {
-              unsigned char* sa = a_ring + (size_t)as * kAStage;
-              ptx::mbar_arrive_expect_tx(&a_full[as], (uint32_t)kAStage);
-              ptx::tma_load_5d(sa, &tm_a_hi, &a_full[as], kb * 64, ox0 + p.tap[t][1], oy_tile + p.tap[t][0], tidx, bidx);
-              ptx::tma_load_5d(sa + kAStage / 2, &tm_a_lo, &a_full[as], kb * 64, ox0 + p.tap[t][1], oy_tile + p.tap[t][0], tidx, bidx);
-            }
-            __syncwarp();
-            if (++as == kAsppNA) { as = 0; aph ^= 1; }
+            ra.produce(kAStage, [&](int s, uint64_t* bar) {
+              unsigned char* sa = a_ring + (size_t)s * kAStage;
+              ptx::tma_load_5d(sa, &tm_a_hi, bar, kb * 64, ox0 + p.tap[t][1], oy_tile + p.tap[t][0], tidx, bidx);
+              ptx::tma_load_5d(sa + kAStage / 2, &tm_a_lo, bar, kb * 64, ox0 + p.tap[t][1], oy_tile + p.tap[t][0], tidx, bidx);
+            });
             load_b(t * p.kblocks + kb);
           }
         }
@@ -133,19 +132,10 @@ aspp_fused_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
     // ===================== two warpgroups: branch MMAs, conversion to P, projection, output =====================
     const int wg = warp >> 2, wq = warp & 3;
     const int wtid = threadIdx.x & 127;
-    const bool wg_leader = wtid == 0;
     const int row0 = wg * 64 + wq * 16 + (lane >> 2);       // accumulator rows of this thread: row0, row0 + 8
     const int cq = 2 * (lane & 3);                           // first of its two columns in every 8-column group
     float* wb = s_wb + wg * kAsppHidden;
-    int as = 0, bs = 0; uint32_t aph = 0, bph = 0;
-    int pend_a = -1, pend_b = -1;               // ring slots read by the last committed wgmma group
-    auto release = [&]() {
-      if (wg_leader) {
-        if (pend_a >= 0) ptx::mbar_arrive(&a_empty[pend_a]);
-        if (pend_b >= 0) ptx::mbar_arrive(&b_empty[pend_b]);
-      }
-      pend_a = pend_b = -1;
-    };
+    PendingSlots pend{ra.empty, rb.empty, wtid == 0};
     auto issue = [&](float* acc, uint32_t a_hi, uint32_t a_lo, uint32_t b_hi, uint32_t b_lo, uint32_t accumulate,
                      int slot_a, int slot_b) {
       const uint64_t da_hi = wg::desc_k_sw128(a_hi), da_lo = wg::desc_k_sw128(a_lo);
@@ -154,14 +144,11 @@ aspp_fused_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
 #pragma unroll
       for (int k = 0; k < 4; ++k) {
         const uint64_t koff = (uint64_t)((k * 32) >> 4);
-        wg::mma_bf16<kAsppHidden>(acc, da_hi + koff, db_hi + koff, accumulate | (uint32_t)k);
-        wg::mma_bf16<kAsppHidden>(acc, da_hi + koff, db_lo + koff, 1);
-        wg::mma_bf16<kAsppHidden>(acc, da_lo + koff, db_hi + koff, 1);
+        wg::mma_hilo<kAsppHidden>(acc, da_hi + koff, da_lo + koff, db_hi + koff, db_lo + koff, accumulate | (uint32_t)k);
       }
       wg::commit();
       wg::wait<1>();
-      release();
-      pend_a = slot_a; pend_b = slot_b;
+      pend.release_and_defer(slot_a, slot_b);
     };
     ptx::griddep_wait();
     for (int tile = cta; tile < p.n_tiles; tile += n_cta) {
@@ -178,18 +165,18 @@ aspp_fused_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
         for (int t = p.br_tap0[s]; t < p.br_tap0[s + 1]; ++t) {
           if (aspp_tap_is_padding(p, t, oy_tile, ox0)) continue;
           for (int kb = 0; kb < p.kblocks; ++kb) {
-            ptx::mbar_wait(&a_full[as], aph);
-            ptx::mbar_wait(&b_full[bs], bph);
-            const uint32_t a_hi = ptx::smem_u32(a_ring + (size_t)as * kAStage) + (uint32_t)(wg * 64 * 128);
-            const uint32_t b_hi = ptx::smem_u32(b_ring + (size_t)bs * kBStage);
-            issue(acc1, a_hi, a_hi + kAStage / 2, b_hi, b_hi + 128 * 128, accumulate, as, bs);
+            ra.wait_full();
+            rb.wait_full();
+            const uint32_t a_hi = ptx::smem_u32(a_ring + (size_t)ra.slot * kAStage) + (uint32_t)(wg * 64 * 128);
+            const uint32_t b_hi = ptx::smem_u32(b_ring + (size_t)rb.slot * kBStage);
+            issue(acc1, a_hi, a_hi + kAStage / 2, b_hi, b_hi + 128 * 128, accumulate, ra.slot, rb.slot);
             accumulate = 1;
-            if (++as == kAsppNA) { as = 0; aph ^= 1; }
-            if (++bs == kAsppNB) { bs = 0; bph ^= 1; }
+            ra.advance();
+            rb.advance();
           }
         }
         wg::wait<0>();                             // also: the previous branch's projection has read P's registers
-        release();
+        pend.release();
         // ---- P = hi/lo split of relu(acc1 + bias), kept in registers, and proj(s): acc2 (+)= P . W_proj[:, branch s],
         // one 64-column K block kb2 at a time.  Accumulator entries (4 g8 + 2 h, +1) -- row row0 + 8 h, columns
         // 8 g8 + cq, +1 -- become bf16x2 register 2 (g8 % 8) + h, and registers 4 k .. 4 k + 3 are the A fragment of the
@@ -207,31 +194,27 @@ aspp_fused_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
             for (int h = 0; h < 2; ++h) {
               const float x0 = fmaxf(acc1[4 * g8 + 2 * h] + bias[8 * g8 + cq], 0.f);
               const float x1 = fmaxf(acc1[4 * g8 + 2 * h + 1] + bias[8 * g8 + cq + 1], 0.f);
-              const uint32_t hw = ptx::pack_bf16x2(x0, x1);
-              p_hi[2 * g + h] = hw;
-              p_lo[2 * g + h] = ptx::pack_bf16x2(x0 - __uint_as_float(hw << 16), x1 - __uint_as_float(hw & 0xFFFF0000u));
+              ptx::split_hilo(x0, x1, p_hi[2 * g + h], p_lo[2 * g + h]);
             }
           }
-          ptx::mbar_wait(&b_full[bs], bph);
-          const uint32_t b_hi = ptx::smem_u32(b_ring + (size_t)bs * kBStage);
+          rb.wait_full();
+          const uint32_t b_hi = ptx::smem_u32(b_ring + (size_t)rb.slot * kBStage);
           const uint64_t db_hi = wg::desc_k_sw128(b_hi), db_lo = wg::desc_k_sw128(b_hi + 128 * 128);
           wg::fence();
 #pragma unroll
           for (int k = 0; k < 4; ++k) {
             const uint64_t koff = (uint64_t)((k * 32) >> 4);
-            wg::mma_bf16_rs128(acc2, &p_hi[4 * k], db_hi + koff, (s > 0 || kb2 > 0 || k > 0) ? 1u : 0u);
-            wg::mma_bf16_rs128(acc2, &p_hi[4 * k], db_lo + koff, 1);
-            wg::mma_bf16_rs128(acc2, &p_lo[4 * k], db_hi + koff, 1);
+            wg::mma_hilo_rs<kAsppHidden>(acc2, &p_hi[4 * k], &p_lo[4 * k], db_hi + koff, db_lo + koff,
+                                         (s > 0 || kb2 > 0 || k > 0) ? 1u : 0u);
           }
           wg::commit();
           wg::wait<0>();                           // P's registers are read until the group completes
-          release();
-          pend_b = bs;
-          if (++bs == kAsppNB) { bs = 0; bph ^= 1; }
+          pend.release_and_defer(-1, rb.slot);
+          rb.advance();
         }
       }
       wg::wait<0>();
-      release();
+      pend.release();
       // ---- output of the projection: relu(acc2 + per-image bias) -> hi/lo planes
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
@@ -246,8 +229,8 @@ aspp_fused_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
           float x0 = acc2[4 * g8 + 2 * h] + wb[c];
           float x1 = acc2[4 * g8 + 2 * h + 1] + wb[c + 1];
           if (p.relu_out) { x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); }
-          const uint32_t hw = ptx::pack_bf16x2(x0, x1);
-          const uint32_t lw = ptx::pack_bf16x2(x0 - __uint_as_float(hw << 16), x1 - __uint_as_float(hw & 0xFFFF0000u));
+          uint32_t hw, lw;
+          ptx::split_hilo(x0, x1, hw, lw);
           const size_t off = pix * p.out_cstride + p.out_coff + c;
           *reinterpret_cast<uint32_t*>(p.out_hi + off) = hw;
           *reinterpret_cast<uint32_t*>(p.out_lo + off) = lw;
@@ -255,21 +238,6 @@ aspp_fused_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
       }
     }
   }
-}
-
-typedef CUresult (*PFN_tmapEncodeTiledA)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                         const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                         CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static PFN_tmapEncodeTiledA aspp_encode_fn() {
-  static PFN_tmapEncodeTiledA fn = nullptr;
-  if (!fn) {
-    void* ptr = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &qres) == cudaSuccess &&
-        qres == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<PFN_tmapEncodeTiledA>(ptr);
-  }
-  return fn;
 }
 
 }  // namespace stp3
@@ -288,8 +256,7 @@ extern "C" int stp3_aspp_fused_fwd(const stp3_aspp_desc* d, const void* x_hi, co
   STP3_CHECK_ARG(d->out_cstride % 16 == 0 && d->out_coff % 16 == 0 && d->out_coff + n_store <= d->out_cstride &&
                  (reinterpret_cast<uintptr_t>(y_hi) & 31) == 0 && (reinterpret_cast<uintptr_t>(y_lo) & 31) == 0,
                  "output planes: n_store channels at a 16-channel aligned offset, 32-byte aligned");
-  PFN_tmapEncodeTiledA enc = aspp_encode_fn();
-  if (!enc) return set_error(STP3_ECUDA, "cuTensorMapEncodeTiled is not available from the driver");
+  if (!tmap_encode_fn()) return set_error(STP3_ECUDA, "cuTensorMapEncodeTiled is not available from the driver");
   AsppParams p;
   p.n_img = d->B * d->T; p.T = d->T; p.T_total = d->T; p.H = d->H; p.W = d->W;
   p.tiles_x = ceil_div(d->W, 16); p.tiles_y = ceil_div(d->H, 8);
@@ -316,50 +283,19 @@ extern "C" int stp3_aspp_fused_fwd(const stp3_aspp_desc* d, const void* x_hi, co
 
   CUtensorMap tm_hi, tm_lo, tm_w;
   {
-    const cuuint64_t dims[5] = {(cuuint64_t)d->in_cstride, (cuuint64_t)d->W, (cuuint64_t)d->H, (cuuint64_t)d->T, (cuuint64_t)d->B};
-    const cuuint64_t strides[4] = {(cuuint64_t)d->in_cstride * 2, (cuuint64_t)d->W * d->in_cstride * 2,
-                                   (cuuint64_t)d->H * d->W * d->in_cstride * 2, (cuuint64_t)d->T * d->H * d->W * d->in_cstride * 2};
-    const cuuint32_t box[5] = {64, 16, 8, 1, 1};
-    const cuuint32_t es[5] = {1, 1, 1, 1, 1};
-    CUresult r1 = enc(&tm_hi, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 5, const_cast<void*>(x_hi), dims, strides, box, es,
-                      CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    CUresult r2 = enc(&tm_lo, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 5, const_cast<void*>(x_lo), dims, strides, box, es,
-                      CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    const CUresult r1 = encode_act_5d(&tm_hi, x_hi, d->in_cstride, d->W, d->H, d->T, d->B, 16, 8, 1);
+    const CUresult r2 = encode_act_5d(&tm_lo, x_lo, d->in_cstride, d->W, d->H, d->T, d->B, 16, 8, 1);
     if (r1 != CUDA_SUCCESS || r2 != CUDA_SUCCESS)
       return set_error(STP3_ECUDA, "cuTensorMapEncodeTiled(activation) failed: %d %d", (int)r1, (int)r2);
-    const int n_blocks = t * p.kblocks + 2 * d->n_br;
-    const cuuint64_t wd[2] = {64, (cuuint64_t)n_blocks * 256};
-    const cuuint64_t ws[1] = {128};
-    const cuuint32_t wb[2] = {64, 128};
-    const cuuint32_t we[2] = {1, 1};
-    CUresult r3 = enc(&tm_w, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(w), wd, ws, wb, we,
-                      CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    const CUresult r3 = encode_rows_2d(&tm_w, w, (long long)(t * p.kblocks + 2 * d->n_br) * 256, 128);
     if (r3 != CUDA_SUCCESS) return set_error(STP3_ECUDA, "cuTensorMapEncodeTiled(weights) failed: %d", (int)r3);
   }
-  const size_t smem_bytes = 1024 + (size_t)kAsppNA * kAStage + (size_t)kAsppNB * kBStage +
-                            (kAsppMaxBranches + 2) * kAsppHidden * sizeof(float) + 2 * (kAsppNA + kAsppNB) * 8;
-  static thread_local int attr_dev = -1;           // once per device: the attribute call costs microseconds per eager launch
-  int cur_dev = 0;
-  cudaGetDevice(&cur_dev);
-  if (attr_dev != cur_dev) {
-    STP3_CUDA_OK(cudaFuncSetAttribute(aspp_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes));
-    attr_dev = cur_dev;
-  }
-  int num_sms = 132;
-  cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, cur_dev);
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3((unsigned)(nt < num_sms ? nt : num_sms)); cfg.blockDim = dim3(kAsppThreads);
-  cfg.dynamicSmemBytes = smem_bytes; cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr; cfg.numAttrs = stp3_pdl_enabled("STP3_FUSED_PDL") ? 1 : 0;
+  STP3_CUDA_OK(set_max_dynamic_smem<aspp_fused_kernel>((int)AsppSmem::bytes));
+  const int n_sm = num_sms();
   // The kernel never executes griddepcontrol.launch_dependents: its dependents are released when the grid completes
   // (see block_fused.cu); it still starts early behind its predecessor.
-  STP3_CUDA_OK(cudaLaunchKernelEx(&cfg, aspp_fused_kernel, tm_hi, tm_lo, tm_w, p));
+  STP3_CUDA_OK(launch_pdl(kPdlFused, aspp_fused_kernel, dim3((unsigned)(nt < n_sm ? nt : n_sm)), dim3(kAsppThreads),
+                          AsppSmem::bytes, stream, tm_hi, tm_lo, tm_w, p));
   STP3_CUDA_OK(cudaGetLastError());
   return STP3_OK;
 }

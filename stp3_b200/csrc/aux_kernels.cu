@@ -8,10 +8,6 @@
 
 namespace stp3 {
 
-__device__ __forceinline__ void split_bf16(float x, __nv_bfloat16& h, __nv_bfloat16& l) {
-  h = __float2bfloat16_rn(x);
-  l = __float2bfloat16_rn(x - __bfloat162float(h));
-}
 __device__ __forceinline__ float join_bf16(__nv_bfloat16 h, __nv_bfloat16 l) {
   return __bfloat162float(h) + __bfloat162float(l);
 }
@@ -44,7 +40,7 @@ f32_to_hilo_kernel(const float* __restrict__ x, int channels_last, int C, int HW
     const int px = p0 + ty + 8 * k, c = c0 + tx;
     if (px < HW && c < cp) {
       __nv_bfloat16 h, l;
-      split_bf16(tile[tx][ty + 8 * k], h, l);
+      ptx::split_hilo(tile[tx][ty + 8 * k], h, l);
       hi[((size_t)img * HW + px) * cp + c] = h;
       lo[((size_t)img * HW + px) * cp + c] = l;
     }
@@ -216,8 +212,9 @@ upsample2x_add_kernel(const __nv_bfloat16* __restrict__ xh, const __nv_bfloat16*
       const float wt = wys[a] * wxs[b];
 #pragma unroll
       for (int e = 0; e < 4; ++e) {
-        acc[2 * e] = fmaf(wt, __uint_as_float(hw[e] << 16) + __uint_as_float(lw[e] << 16), acc[2 * e]);
-        acc[2 * e + 1] = fmaf(wt, __uint_as_float(hw[e] & 0xFFFF0000u) + __uint_as_float(lw[e] & 0xFFFF0000u), acc[2 * e + 1]);
+        const float2 x = ptx::join_hilo(hw[e], lw[e]);
+        acc[2 * e] = fmaf(wt, x.x, acc[2 * e]);
+        acc[2 * e + 1] = fmaf(wt, x.y, acc[2 * e + 1]);
       }
     }
   const size_t opix = (img * H2 + oy) * W2 + ox;
@@ -227,19 +224,14 @@ upsample2x_add_kernel(const __nv_bfloat16* __restrict__ xh, const __nv_bfloat16*
     const uint32_t hw[4] = {hv.x, hv.y, hv.z, hv.w}, lw[4] = {lv.x, lv.y, lv.z, lv.w};
 #pragma unroll
     for (int e = 0; e < 4; ++e) {
-      acc[2 * e] += __uint_as_float(hw[e] << 16) + __uint_as_float(lw[e] << 16);
-      acc[2 * e + 1] += __uint_as_float(hw[e] & 0xFFFF0000u) + __uint_as_float(lw[e] & 0xFFFF0000u);
+      const float2 x = ptx::join_hilo(hw[e], lw[e]);
+      acc[2 * e] += x.x;
+      acc[2 * e + 1] += x.y;
     }
   }
   uint32_t oh[4], ol[4];
 #pragma unroll
-  for (int e = 0; e < 4; ++e) {
-    __nv_bfloat16 h0, l0, h1, l1;
-    split_bf16(acc[2 * e], h0, l0);
-    split_bf16(acc[2 * e + 1], h1, l1);
-    oh[e] = (uint32_t)__bfloat16_as_ushort(h0) | ((uint32_t)__bfloat16_as_ushort(h1) << 16);
-    ol[e] = (uint32_t)__bfloat16_as_ushort(l0) | ((uint32_t)__bfloat16_as_ushort(l1) << 16);
-  }
+  for (int e = 0; e < 4; ++e) ptx::split_hilo(acc[2 * e], acc[2 * e + 1], oh[e], ol[e]);
   *reinterpret_cast<uint4*>(yh + opix * ys + y_off + g * 8) = make_uint4(oh[0], oh[1], oh[2], oh[3]);
   *reinterpret_cast<uint4*>(yl + opix * ys + y_off + g * 8) = make_uint4(ol[0], ol[1], ol[2], ol[3]);
 }
@@ -286,7 +278,7 @@ extern "C" int stp3_pool_bias(const float* sums, int sums_stride, int n_img, int
   STP3_CHECK_ARG(sums && W1 && b1 && W2 && out && n_img > 0 && T > 0 && C > 0 && R > 0 && CO > 0 && n_const >= 0 &&
                  n_const < C && C - n_const <= sums_stride && CO <= co_stride && (n_const == 0 || const_vals),
                  "stp3_pool_bias: bad argument");
-  STP3_CUDA_OK(launch_pdl(pool_bias_kernel, dim3(n_img, CO >= 64 ? 4 : 1), dim3(256), (size_t)(C + R) * sizeof(float), (cudaStream_t)stream,
+  STP3_CUDA_OK(launch_pdl(kPdlAux, pool_bias_kernel, dim3(n_img, CO >= 64 ? 4 : 1), dim3(256), (size_t)(C + R) * sizeof(float), (cudaStream_t)stream,
                           sums, sums_stride, T, C, inv_hw, temporal, const_vals, n_const, W1, b1, R, W2, CO, bias, out,
                           co_stride, accumulate));
   return STP3_OK;
@@ -295,7 +287,7 @@ extern "C" int stp3_pool_bias(const float* sums, int sums_stride, int n_img, int
 extern "C" int stp3_small_linear(const float* x, const float* W, int n, int ci, int co, const float* bias, float* y,
                                  int co_stride, int accumulate, void* stream) {
   STP3_CHECK_ARG(x && W && y && n > 0 && ci > 0 && co > 0 && co <= co_stride, "stp3_small_linear: bad argument");
-  STP3_CUDA_OK(launch_pdl(small_linear_kernel, dim3(n), dim3(128), 0, (cudaStream_t)stream, x, W, ci, co, bias, y,
+  STP3_CUDA_OK(launch_pdl(kPdlAux, small_linear_kernel, dim3(n), dim3(128), 0, (cudaStream_t)stream, x, W, ci, co, bias, y,
                           co_stride, accumulate));
   return STP3_OK;
 }
@@ -310,7 +302,7 @@ extern "C" int stp3_upsample2x_add(const void* x_hi, const void* x_lo, int n_img
                  y_coff % 8 == 0 && y_coff + C <= y_cstride && x_cstride % 8 == 0 && s_cstride % 8 == 0 &&
                  y_cstride % 8 == 0, "stp3_upsample2x_add: channel windows must be multiples of 8");
   const size_t total = (size_t)n_img * (2 * h) * (2 * w) * (C / 8);
-    STP3_CUDA_OK(launch_pdl(upsample2x_add_kernel, dim3((unsigned)((total + 255) / 256)), dim3(256), 0, (cudaStream_t)stream,
+    STP3_CUDA_OK(launch_pdl(kPdlAux, upsample2x_add_kernel, dim3((unsigned)((total + 255) / 256)), dim3(256), 0, (cudaStream_t)stream,
       (const bf16*)x_hi, (const bf16*)x_lo, h, w, x_cstride, (const bf16*)s_hi, (const bf16*)s_lo, s_cstride, s_coff,
       (bf16*)y_hi, (bf16*)y_lo, y_cstride, y_coff, C / 8, total));
   return STP3_OK;

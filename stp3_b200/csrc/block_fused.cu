@@ -32,6 +32,7 @@
 #include <cuda_bf16.h>
 
 #include "common.cuh"
+#include "pipeline.cuh"
 #include "ptx.cuh"
 #include "wgmma.cuh"
 
@@ -46,6 +47,17 @@ constexpr int kBlkAStage = 2 * kBlkBoxRows * 16 * 128;
 constexpr int kBlkMaxGroups = 16;
 constexpr int kBlkBRows = 64;                     // weight rows per plane: chains are at most 64 wide
 constexpr int kBlkBStage = 2 * kBlkBRows * 128;
+
+// shared memory, from the 1024-byte aligned base (the kernel carves it, the host sizes the launch from `bytes`)
+struct BlkSmem {
+  static constexpr int a_ring = 0;                                // kBlkNA activation stages
+  static constexpr int b_ring = a_ring + kBlkNA * kBlkAStage;     // kBlkNB weight stages
+  static constexpr int w_agg = b_ring + kBlkNB * kBlkBStage;      // the two aggregation blocks, as two weight stages
+  static constexpr int hb = w_agg + 2 * kBlkBStage;               // fp32 [2 warpgroups][128] hidden bias of the image
+  static constexpr int wb = hb + 2 * 128 * 4;                     // fp32 [2 warpgroups][128] img_bias (64) | res_bias (64)
+  static constexpr int bars = wb + 2 * 128 * 4;                   // full / empty barriers of both rings, w_agg_full
+  static constexpr size_t bytes = 1024 + bars + (2 * (kBlkNA + kBlkNB) + 1) * 8;   // + the alignment slack
+};
 
 // The two chain layouts the kernel is compiled for, i.e. the two TemporalBlock packs.  Per chain: MMA width N, the
 // 8-channel pieces of P it produces (its column groups 0 .. npc - 1), the first of them:
@@ -110,24 +122,21 @@ block_fused_kernel(const __grid_constant__ CUtensorMap tm_m_hi, const __grid_con
   const int cta = (int)blockIdx.x, n_cta = (int)gridDim.x;
   extern __shared__ unsigned char smem_raw[];
   unsigned char* smem = smem_raw + ((1024u - (ptx::smem_u32(smem_raw) & 1023u)) & 1023u);
-  unsigned char* a_ring = smem;
-  unsigned char* b_ring = a_ring + kBlkNA * kBlkAStage;
-  unsigned char* w_agg = b_ring + kBlkNB * kBlkBStage;             // the two aggregation blocks, as two weight stages
-  float* s_hb = reinterpret_cast<float*>(w_agg + 2 * kBlkBStage);   // [2 warpgroups][128] hidden bias of the image
-  float* s_wb = s_hb + 2 * 128;                                     // [2 warpgroups][128] img_bias (64) | res_bias (64)
-  uint64_t* bars = reinterpret_cast<uint64_t*>(s_wb + 2 * 128);
-  uint64_t* a_full = bars;
-  uint64_t* a_empty = a_full + kBlkNA;
-  uint64_t* b_full = a_empty + kBlkNA;
-  uint64_t* b_empty = b_full + kBlkNB;
-  uint64_t* w_agg_full = b_empty + kBlkNB;
+  unsigned char* a_ring = smem + BlkSmem::a_ring;
+  unsigned char* b_ring = smem + BlkSmem::b_ring;
+  unsigned char* w_agg = smem + BlkSmem::w_agg;
+  float* s_hb = reinterpret_cast<float*>(smem + BlkSmem::hb);
+  float* s_wb = reinterpret_cast<float*>(smem + BlkSmem::wb);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + BlkSmem::bars);
+  Ring ra{bars, bars + kBlkNA, kBlkNA};
+  Ring rb{bars + 2 * kBlkNA, bars + 2 * kBlkNA + kBlkNB, kBlkNB};
+  uint64_t* w_agg_full = bars + 2 * (kBlkNA + kBlkNB);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (warp == 8 && lane == 0) {
     ptx::prefetch_tmap(&tm_m_hi); ptx::prefetch_tmap(&tm_m_lo); ptx::prefetch_tmap(&tm_x_hi); ptx::prefetch_tmap(&tm_x_lo);
     ptx::prefetch_tmap(&tm_w);
-    for (int i = 0; i < kBlkNA; ++i) { ptx::mbar_init(&a_full[i], 1); ptx::mbar_init(&a_empty[i], 2); }
-    for (int i = 0; i < kBlkNB; ++i) { ptx::mbar_init(&b_full[i], 1); ptx::mbar_init(&b_empty[i], 2); }
+    ra.init(2); rb.init(2);
     ptx::mbar_init(w_agg_full, 2);               // one arrive.expect_tx per aggregation block
     ptx::fence_mbar_init();
   }
@@ -142,7 +151,6 @@ block_fused_kernel(const __grid_constant__ CUtensorMap tm_m_hi, const __grid_con
     // 64 + n - N/2 of each plane; only those rows are fetched (boxes of 8 rows)
     auto fetch_b = [&](unsigned char* dst, uint64_t* bar, int blk, int n_mma) {
       const int rows = n_mma / 2;
-      ptx::mbar_arrive_expect_tx(bar, (uint32_t)(2 * n_mma * 128));
       for (int r8 = 0; r8 < rows; r8 += 8) {
         for (int h = 0; h < 2; ++h) {
           ptx::tma_load_2d(dst + (h * rows + r8) * 128, &tm_w, bar, 0, blk * 256 + h * 64 + r8);
@@ -152,28 +160,22 @@ block_fused_kernel(const __grid_constant__ CUtensorMap tm_m_hi, const __grid_con
     };
     // module weights, not written by the predecessor: fetched before the dependency wait
     if (ptx::elect_one_sync()) {
+      ptx::mbar_arrive_expect_tx(w_agg_full, 2 * 64 * 128);
       fetch_b(w_agg, w_agg_full, p.wagg_blk0, 64);
+      ptx::mbar_arrive_expect_tx(w_agg_full, 2 * 64 * 128);
       fetch_b(w_agg + kBlkBStage, w_agg_full, p.wagg_blk0 + 1, 64);
     }
     __syncwarp();
     ptx::griddep_wait();
-    int as = 0, bs = 0; uint32_t aph = 0, bph = 0;
     auto load_a = [&](int src, int c, int x, int y, int t, int b) {
-      ptx::mbar_wait(&a_empty[as], aph ^ 1);
-      if (ptx::elect_one_sync()) {
-        unsigned char* sa = a_ring + (size_t)as * kBlkAStage;
-        ptx::mbar_arrive_expect_tx(&a_full[as], (uint32_t)kBlkAStage);
-        ptx::tma_load_5d(sa, src ? &tm_x_hi : &tm_m_hi, &a_full[as], c, x, y, t, b);
-        ptx::tma_load_5d(sa + kBlkAStage / 2, src ? &tm_x_lo : &tm_m_lo, &a_full[as], c, x, y, t, b);
-      }
-      __syncwarp();
-      if (++as == kBlkNA) { as = 0; aph ^= 1; }
+      ra.produce(kBlkAStage, [&](int s, uint64_t* bar) {
+        unsigned char* sa = a_ring + (size_t)s * kBlkAStage;
+        ptx::tma_load_5d(sa, src ? &tm_x_hi : &tm_m_hi, bar, c, x, y, t, b);
+        ptx::tma_load_5d(sa + kBlkAStage / 2, src ? &tm_x_lo : &tm_m_lo, bar, c, x, y, t, b);
+      });
     };
     auto load_b = [&](int blk, int n_mma) {
-      ptx::mbar_wait(&b_empty[bs], bph ^ 1);
-      if (ptx::elect_one_sync()) fetch_b(b_ring + (size_t)bs * kBlkBStage, &b_full[bs], blk, n_mma);
-      __syncwarp();
-      if (++bs == kBlkNB) { bs = 0; bph ^= 1; }
+      rb.produce(2 * n_mma * 128, [&](int s, uint64_t* bar) { fetch_b(b_ring + (size_t)s * kBlkBStage, bar, blk, n_mma); });
     };
     for (int tile = cta; tile < p.n_tiles; tile += n_cta) {
       const int img = tile / tiles_per_img, rem = tile % tiles_per_img;
@@ -195,21 +197,12 @@ block_fused_kernel(const __grid_constant__ CUtensorMap tm_m_hi, const __grid_con
     // ===================== two warpgroups: chains, conversion to P, aggregation, projection, output =====================
     const int wg = warp >> 2, wq = warp & 3;
     const int wtid = threadIdx.x & 127;
-    const bool wg_leader = wtid == 0;
     const int row0 = wg * 64 + wq * 16 + (lane >> 2);       // accumulator rows of this thread: row0, row0 + 8
     const int cq = 2 * (lane & 3);                           // first of its two columns in every 8-column group
     float* hb = s_hb + wg * 128;
     float* wb = s_wb + wg * 128;
     const uint32_t w_agg_u32 = ptx::smem_u32(w_agg);
-    int as = 0, bs = 0; uint32_t aph = 0, bph = 0;
-    int pend_a = -1, pend_b = -1;               // ring slots read by the last committed wgmma group
-    auto release = [&]() {
-      if (wg_leader) {
-        if (pend_a >= 0) ptx::mbar_arrive(&a_empty[pend_a]);
-        if (pend_b >= 0) ptx::mbar_arrive(&b_empty[pend_b]);
-      }
-      pend_a = pend_b = -1;
-    };
+    PendingSlots pend{ra.empty, rb.empty, wtid == 0};
     // acc (+)= A . B over KS K steps from k0 with hi*hi + hi*lo + lo*hi, then commit and release the previous group's slots
     auto issue = [&](auto n_c, auto ks_c, float* acc, uint32_t a_hi, uint32_t b_hi, int k0, uint32_t accumulate,
                      int slot_a, int slot_b) {
@@ -218,15 +211,11 @@ block_fused_kernel(const __grid_constant__ CUtensorMap tm_m_hi, const __grid_con
       const uint64_t db_hi = wg::desc_k_sw128(b_hi) + (uint64_t)(2 * k0), db_lo = wg::desc_k_sw128(b_hi + kBlkBRows * 128) + (uint64_t)(2 * k0);
       wg::fence();
 #pragma unroll
-      for (int k = 0; k < KS; ++k) {
-        wg::mma_bf16<N>(acc, da_hi + 2 * k, db_hi + 2 * k, k == 0 ? accumulate : 1u);
-        wg::mma_bf16<N>(acc, da_hi + 2 * k, db_lo + 2 * k, 1);
-        wg::mma_bf16<N>(acc, da_lo + 2 * k, db_hi + 2 * k, 1);
-      }
+      for (int k = 0; k < KS; ++k)
+        wg::mma_hilo<N>(acc, da_hi + 2 * k, da_lo + 2 * k, db_hi + 2 * k, db_lo + 2 * k, k == 0 ? accumulate : 1u);
       wg::commit();
       wg::wait<1>();
-      release();
-      pend_a = slot_a; pend_b = slot_b;
+      pend.release_and_defer(slot_a, slot_b);
     };
     // one K = 16 step of the aggregation: acc2 (+)= P_s . W_agg[s], P_s from registers (hi / lo A fragments)
     float acc2[32], acc3[32];
@@ -234,9 +223,7 @@ block_fused_kernel(const __grid_constant__ CUtensorMap tm_m_hi, const __grid_con
       const uint32_t b_hi = w_agg_u32 + (uint32_t)((s >> 2) * kBlkBStage);
       const uint64_t koff = (uint64_t)(2 * (s & 3));
       const uint64_t db_hi = wg::desc_k_sw128(b_hi) + koff, db_lo = wg::desc_k_sw128(b_hi + kBlkBRows * 128) + koff;
-      wg::mma_bf16_rs64(acc2, f_hi, db_hi, s > 0 ? 1u : 0u);
-      wg::mma_bf16_rs64(acc2, f_hi, db_lo, 1);
-      wg::mma_bf16_rs64(acc2, f_lo, db_hi, 1);
+      wg::mma_hilo_rs<64>(acc2, f_hi, f_lo, db_hi, db_lo, s > 0 ? 1u : 0u);
     };
     uint32_t carry_hi[2] = {0u, 0u}, carry_lo[2] = {0u, 0u};   // the first half of a K step that straddles two chains
     int agg_next = 0;                           // next K step of the aggregation
@@ -251,24 +238,25 @@ block_fused_kernel(const __grid_constant__ CUtensorMap tm_m_hi, const __grid_con
         uint32_t accumulate = 0;
         for (int g = ch.grp0; g < ch.grp0 + ch.ngrp; ++g) {
           if (blk_group_is_padding(p, g, tidx, oy_tile, ox0)) continue;
-          ptx::mbar_wait(&a_full[as], aph);
-          const uint32_t a_hi0 = ptx::smem_u32(a_ring + (size_t)as * kBlkAStage) + (uint32_t)(wg * 64 * 128);
+          ra.wait_full();
+          const uint32_t a_hi0 = ptx::smem_u32(a_ring + (size_t)ra.slot * kBlkAStage) + (uint32_t)(wg * 64 * 128);
           for (int j = 0; j < p.gsize[g]; ++j) {
-            ptx::mbar_wait(&b_full[bs], bph);
+            rb.wait_full();
             const bool last = j + 1 == p.gsize[g];
-            const uint32_t b_hi = ptx::smem_u32(b_ring + (size_t)bs * kBlkBStage);
+            const uint32_t b_hi = ptx::smem_u32(b_ring + (size_t)rb.slot * kBlkBStage);
             // tap j of the group: shifted by j image rows
             issue(n_c, ks_c, acc, a_hi0 + (uint32_t)(j * 16 * 128), b_hi, ch.ks_first, accumulate,
-                  last && !with_proj ? as : -1, bs);
+                  last && !with_proj ? ra.slot : -1, rb.slot);
             accumulate = 1;
-            if (++bs == kBlkNB) { bs = 0; bph ^= 1; }
+            rb.advance();
           }
           if (with_proj) {                       // the 1x1 projection of x reads the same stage (one group, centre tap)
-            ptx::mbar_wait(&b_full[bs], bph);
-            issue(BlkC<64>{}, ks_c, acc3, a_hi0, ptx::smem_u32(b_ring + (size_t)bs * kBlkBStage), p.res.ks_first, 0u, as, bs);
-            if (++bs == kBlkNB) { bs = 0; bph ^= 1; }
+            rb.wait_full();
+            issue(BlkC<64>{}, ks_c, acc3, a_hi0, ptx::smem_u32(b_ring + (size_t)rb.slot * kBlkBStage), p.res.ks_first, 0u,
+                  ra.slot, rb.slot);
+            rb.advance();
           }
-          if (++as == kBlkNA) { as = 0; aph ^= 1; }
+          ra.advance();
         }
       };
       switch (ch.ks_end - ch.ks_first) {
@@ -278,7 +266,7 @@ block_fused_kernel(const __grid_constant__ CUtensorMap tm_m_hi, const __grid_con
         default: taps(BlkC<4>{}); break;
       }
       wg::wait<0>();                             // also: the previous chain's aggregation has read its P registers
-      release();
+      pend.release();
       // piece k of the chain = its 8-column group k = P piece pc0 + k: relu(acc + bias) split to bf16 hi / lo.
       // Accumulator entries (4 k + 2 h, +1) -- row row0 + 8 h, columns 8 k + cq, +1 -- are bf16x2 register h of the piece
       uint32_t f_hi[NPC][2], f_lo[NPC][2];
@@ -289,9 +277,7 @@ block_fused_kernel(const __grid_constant__ CUtensorMap tm_m_hi, const __grid_con
         for (int h = 0; h < 2; ++h) {
           const float x0 = fmaxf(acc[4 * k + 2 * h] + bias[0], 0.f);
           const float x1 = fmaxf(acc[4 * k + 2 * h + 1] + bias[1], 0.f);
-          const uint32_t hw = ptx::pack_bf16x2(x0, x1);
-          f_hi[k][h] = hw;
-          f_lo[k][h] = ptx::pack_bf16x2(x0 - __uint_as_float(hw << 16), x1 - __uint_as_float(hw & 0xFFFF0000u));
+          ptx::split_hilo(x0, x1, f_hi[k][h], f_lo[k][h]);
         }
       }
       wg::fence();
@@ -362,7 +348,7 @@ block_fused_kernel(const __grid_constant__ CUtensorMap tm_m_hi, const __grid_con
         run_chain(BlkC<32>{}, BlkC<4>{}, BlkC<0>{}, BlkC<0>{}, p.chain[1], tidx, oy_tile, ox0, p.has_res_proj != 0);
       }
       wg::wait<0>();
-      release();
+      pend.release();
       // ---------- output: relu(acc2 + bias) + residual, two channels per 8-column group and row
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
@@ -380,13 +366,13 @@ block_fused_kernel(const __grid_constant__ CUtensorMap tm_m_hi, const __grid_con
             v1 += acc3[4 * g8 + 2 * h + 1] + wb[64 + c + 1];
           } else {                               // identity residual: the block's input planes
             const size_t off = pix * p.res_cstride + c;
-            const uint32_t rh = *reinterpret_cast<const volatile uint32_t*>(p.res_hi + off);
-            const uint32_t rl = *reinterpret_cast<const volatile uint32_t*>(p.res_lo + off);
-            v0 += __uint_as_float(rh << 16) + __uint_as_float(rl << 16);
-            v1 += __uint_as_float(rh & 0xFFFF0000u) + __uint_as_float(rl & 0xFFFF0000u);
+            const float2 r = ptx::join_hilo(*reinterpret_cast<const volatile uint32_t*>(p.res_hi + off),
+                                            *reinterpret_cast<const volatile uint32_t*>(p.res_lo + off));
+            v0 += r.x;
+            v1 += r.y;
           }
-          const uint32_t hw = ptx::pack_bf16x2(v0, v1);
-          const uint32_t lw = ptx::pack_bf16x2(v0 - __uint_as_float(hw << 16), v1 - __uint_as_float(hw & 0xFFFF0000u));
+          uint32_t hw, lw;
+          ptx::split_hilo(v0, v1, hw, lw);
           const size_t off = pix * p.out_cstride + c;
           *reinterpret_cast<uint32_t*>(p.out_hi + off) = hw;
           *reinterpret_cast<uint32_t*>(p.out_lo + off) = lw;
@@ -397,37 +383,12 @@ block_fused_kernel(const __grid_constant__ CUtensorMap tm_m_hi, const __grid_con
     if (p.sum_part && sum_img >= 0) flush_sums(sum_img);
   }
 }
-typedef CUresult (*PFN_tmapEncodeTiledB)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                         const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                         CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static PFN_tmapEncodeTiledB blk_encode_fn() {
-  static PFN_tmapEncodeTiledB fn = nullptr;
-  if (!fn) {
-    void* ptr = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &qres) == cudaSuccess &&
-        qres == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<PFN_tmapEncodeTiledB>(ptr);
-  }
-  return fn;
-}
-
-static int blk_num_sms() {
-  static const int n = [] {
-    int dev = 0, v = 132;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev);
-    return v;
-  }();
-  return n;
-}
-
 }  // namespace stp3
 
 using namespace stp3;
 
 extern "C" size_t stp3_block_fused_scratch_bytes(int n_img) {
-  return (size_t)blk_num_sms() * 8 * (size_t)(n_img > 0 ? n_img : 0) * 64 * sizeof(float);
+  return (size_t)num_sms() * 8 * (size_t)(n_img > 0 ? n_img : 0) * 64 * sizeof(float);
 }
 
 extern "C" int stp3_block_fused_fwd(const stp3_block_desc* d, const void* mid_hi, const void* mid_lo, const void* x_hi,
@@ -444,8 +405,7 @@ extern "C" int stp3_block_fused_fwd(const stp3_block_desc* d, const void* mid_hi
   STP3_CHECK_ARG((d->has_res_proj != 0) == (res_bias != nullptr), "res_bias is given exactly when the block has a projection");
   auto al32 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 31) == 0; };
   STP3_CHECK_ARG(al32(y_hi) && al32(y_lo) && al32(x_hi) && al32(x_lo), "planes must be 32-byte aligned");
-  PFN_tmapEncodeTiledB enc = blk_encode_fn();
-  if (!enc) return set_error(STP3_ECUDA, "cuTensorMapEncodeTiled is not available from the driver");
+  if (!tmap_encode_fn()) return set_error(STP3_ECUDA, "cuTensorMapEncodeTiled is not available from the driver");
 
   BlkParams p;
   p.n_img = d->B * d->T; p.T = d->T; p.H = d->H; p.W = d->W;
@@ -520,48 +480,22 @@ extern "C" int stp3_block_fused_fwd(const stp3_block_desc* d, const void* mid_hi
   CUtensorMap tm[4], tm_w;
   const void* planes[4] = {mid_hi, mid_lo, x_hi, x_lo};
   for (int i = 0; i < 4; ++i) {
-    const int cs = i < 2 ? d->mid_cstride : d->x_cstride;
-    const cuuint64_t dims[5] = {(cuuint64_t)cs, (cuuint64_t)d->W, (cuuint64_t)d->H, (cuuint64_t)d->T, (cuuint64_t)d->B};
-    const cuuint64_t strides[4] = {(cuuint64_t)cs * 2, (cuuint64_t)d->W * cs * 2, (cuuint64_t)d->H * d->W * cs * 2,
-                                   (cuuint64_t)d->T * d->H * d->W * cs * 2};
-    const cuuint32_t box[5] = {64, 16, (cuuint32_t)kBlkBoxRows, 1, 1};
-    const cuuint32_t es[5] = {1, 1, 1, 1, 1};
-    CUresult r = enc(&tm[i], CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 5, const_cast<void*>(planes[i]), dims, strides, box, es,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    const CUresult r = encode_act_5d(&tm[i], planes[i], i < 2 ? d->mid_cstride : d->x_cstride, d->W, d->H, d->T, d->B,
+                                     16, kBlkBoxRows, 1);
     if (r != CUDA_SUCCESS) return set_error(STP3_ECUDA, "cuTensorMapEncodeTiled(activation %d) failed: %d", i, (int)r);
   }
   {
-    const cuuint64_t wd[2] = {64, (cuuint64_t)blk * 256};
-    const cuuint64_t ws[1] = {128};
-    const cuuint32_t wb[2] = {64, 8};
-    const cuuint32_t we[2] = {1, 1};
-    CUresult r = enc(&tm_w, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(w), wd, ws, wb, we,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    const CUresult r = encode_rows_2d(&tm_w, w, (long long)blk * 256, 8);
     if (r != CUDA_SUCCESS) return set_error(STP3_ECUDA, "cuTensorMapEncodeTiled(weights) failed: %d", (int)r);
   }
-  const size_t smem_bytes = 1024 + (size_t)kBlkNA * kBlkAStage + (size_t)(kBlkNB + 2) * kBlkBStage +
-                            4 * 128 * sizeof(float) + (2 * (kBlkNA + kBlkNB) + 1) * 8;
-  static thread_local int attr_dev = -1;           // once per device: the attribute call costs microseconds per eager launch
-  int cur_dev = 0;
-  cudaGetDevice(&cur_dev);
-  if (attr_dev != cur_dev) {
-    STP3_CUDA_OK(cudaFuncSetAttribute(block_fused_kernel<kBlkThreePaths>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes));
-    STP3_CUDA_OK(cudaFuncSetAttribute(block_fused_kernel<kBlkDiagPair>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes));
-    attr_dev = cur_dev;
-  }
-  const int num_sms = blk_num_sms();
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3((unsigned)(nt < num_sms ? nt : num_sms)); cfg.blockDim = dim3(kBlkThreads);
-  cfg.dynamicSmemBytes = smem_bytes; cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr; cfg.numAttrs = stp3_pdl_enabled("STP3_FUSED_PDL") ? 1 : 0;
+  auto kern = layout == kBlkThreePaths ? block_fused_kernel<kBlkThreePaths> : block_fused_kernel<kBlkDiagPair>;
+  STP3_CUDA_OK(layout == kBlkThreePaths ? set_max_dynamic_smem<block_fused_kernel<kBlkThreePaths>>((int)BlkSmem::bytes)
+                                        : set_max_dynamic_smem<block_fused_kernel<kBlkDiagPair>>((int)BlkSmem::bytes));
+  const int n_sm = num_sms();
+  const unsigned grid = (unsigned)(nt < n_sm ? nt : n_sm);
   p.sum_part = nullptr;
   if (col_sums) {
-    const size_t need = (size_t)cfg.gridDim.x * 8 * p.n_img * 64 * sizeof(float);
+    const size_t need = (size_t)grid * 8 * p.n_img * 64 * sizeof(float);
     STP3_CHECK_ARG(scratch && scratch_bytes >= need, "col_sums: scratch missing or smaller than stp3_block_fused_scratch_bytes()");
     p.sum_part = static_cast<float*>(scratch);
     STP3_CUDA_OK(cudaMemsetAsync(p.sum_part, 0, need, stream));
@@ -570,11 +504,9 @@ extern "C" int stp3_block_fused_fwd(const stp3_block_desc* d, const void* mid_hi
   // grid has completed.  Each of them needs a whole SM; an early trigger would let a chain block_fused -> col_sum_reduce
   // -> pool_bias -> aspp_fused be resident at once, and such a chain was seen to stop making progress.  The kernel itself
   // still starts early behind its predecessor (griddepcontrol.wait before it reads what that predecessor wrote).
-  if (layout == kBlkThreePaths)
-    STP3_CUDA_OK(cudaLaunchKernelEx(&cfg, block_fused_kernel<kBlkThreePaths>, tm[0], tm[1], tm[2], tm[3], tm_w, p));
-  else
-    STP3_CUDA_OK(cudaLaunchKernelEx(&cfg, block_fused_kernel<kBlkDiagPair>, tm[0], tm[1], tm[2], tm[3], tm_w, p));
+  STP3_CUDA_OK(launch_pdl(kPdlFused, kern, dim3(grid), dim3(kBlkThreads), BlkSmem::bytes, stream, tm[0], tm[1], tm[2],
+                          tm[3], tm_w, p));
   STP3_CUDA_OK(cudaGetLastError());
-  if (col_sums) return launch_col_sum_reduce(p.sum_part, (int)cfg.gridDim.x * 8, p.n_img, col_sums, stream);
+  if (col_sums) return launch_col_sum_reduce(p.sum_part, (int)grid * 8, p.n_img, col_sums, stream);
   return STP3_OK;
 }

@@ -26,6 +26,7 @@
 #include <cstdlib>
 
 #include "common.cuh"
+#include "pipeline.cuh"
 #include "ptx.cuh"
 #include "wgmma.cuh"
 
@@ -111,10 +112,14 @@ template <int BN, bool STACK = false>
 struct ConvSmem {
   static constexpr int kAccCols = STACK ? 2 * BN : BN;                 // accumulator columns
   static constexpr int kAccStride = kAccCols + 4;                      // floats per row of the shared accumulator tile
-  static constexpr size_t tail_bytes() {
-    return (1 + kMaxHeadOut) * BN * sizeof(float) + kMaxHeadOut * 128 * sizeof(float) + kEpiWarps * 64 * sizeof(float) +
-           (size_t)128 * kAccStride * sizeof(float) + (2 * kMaxAStages + 2 * kMaxBStages + 8) * 8;
-  }
+  // the tail behind the operand rings (or the resident weights), byte offsets from its start
+  static constexpr int bias = 0;                                       // fp32 [BN]
+  static constexpr int head = bias + BN * 4;                           // fp32 [kMaxHeadOut][BN] fused head weights
+  static constexpr int hx = head + kMaxHeadOut * BN * 4;               // fp32 [kMaxHeadOut][128] head partials handed between column halves
+  static constexpr int wb = hx + kMaxHeadOut * 128 * 4;                // fp32 [kEpiWarps][64] per-image bias slice of each epilogue warp
+  static constexpr int acc = wb + kEpiWarps * 64 * 4;                  // fp32 [128][kAccStride] accumulator tile
+  static constexpr int bars = acc + 128 * kAccStride * 4;              // A ring, B ring, resident-weights barrier
+  static constexpr size_t tail_bytes() { return bars + (2 * kMaxAStages + 2 * kMaxBStages + 8) * 8; }
 };
 
 // true if every input element the tap group touches for this tile is zero padding (same answer in the producer and
@@ -166,17 +171,22 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
   const int a_stage_bytes = 2 * p.a_plane_bytes;
   unsigned char* a_ring = smem;
   unsigned char* b_ring = a_ring + (size_t)p.na_stages * a_stage_bytes;            // ring, or the resident weights
-  float* s_bias = reinterpret_cast<float*>(b_ring + (size_t)(resident ? k_iters : p.nb_stages) * p.b_tile_bytes);
-  float* s_head = s_bias + BN;                    // [kMaxHeadOut][BN]
-  float* s_hx = s_head + kMaxHeadOut * BN;        // [kMaxHeadOut][128] head partials handed between column halves
-  float* s_wb = s_hx + kMaxHeadOut * 128;         // [kEpiWarps][64] per-image bias slice of each epilogue warp
-  float* s_acc = s_wb + kEpiWarps * 64;           // [128][kAccStride] accumulator tile
-  uint64_t* bars = reinterpret_cast<uint64_t*>(s_acc + 128 * S::kAccStride);
-  uint64_t* a_full = bars;
-  uint64_t* a_empty = a_full + kMaxAStages;
-  uint64_t* b_full = a_empty + kMaxAStages;
-  uint64_t* b_empty = b_full + kMaxBStages;
-  uint64_t* bres_bar = b_empty + kMaxBStages;
+  unsigned char* tail = b_ring + (size_t)(resident ? k_iters : p.nb_stages) * p.b_tile_bytes;
+  float* s_bias = reinterpret_cast<float*>(tail + S::bias);
+  float* s_head = reinterpret_cast<float*>(tail + S::head);
+  float* s_hx = reinterpret_cast<float*>(tail + S::hx);
+  float* s_wb = reinterpret_cast<float*>(tail + S::wb);
+  float* s_acc = reinterpret_cast<float*>(tail + S::acc);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(tail + S::bars);
+  Ring ra{bars, bars + kMaxAStages, p.na_stages};
+  Ring rb{bars + 2 * kMaxAStages, bars + 2 * kMaxAStages + kMaxBStages, p.nb_stages};   // no slots: resident weights
+  uint64_t* bres_bar = bars + 2 * (kMaxAStages + kMaxBStages);
+  // The MMA warpgroups walk both rings with counters of their own: the same walk through a Ring makes ptxas spill more
+  // in four of the six instantiations
+  uint64_t* const a_full = ra.full;
+  uint64_t* const a_empty = ra.empty;
+  uint64_t* const b_full = rb.full;
+  uint64_t* const b_empty = rb.empty;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
@@ -186,8 +196,7 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
   ptx::griddep_launch_dependents();
   if (warp == kEpiWarps && lane == 0) {
     ptx::prefetch_tmap(&tm_a_hi); ptx::prefetch_tmap(&tm_a_lo); ptx::prefetch_tmap(&tm_w);
-    for (int i = 0; i < p.na_stages; ++i) { ptx::mbar_init(&a_full[i], 1); ptx::mbar_init(&a_empty[i], 2); }
-    for (int i = 0; i < p.nb_stages; ++i) { ptx::mbar_init(&b_full[i], 1); ptx::mbar_init(&b_empty[i], 2); }
+    ra.init(2); rb.init(2);
     ptx::mbar_init(bres_bar, 1);
     ptx::fence_mbar_init();
   }
@@ -212,7 +221,6 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
     }
     __syncwarp();
     ptx::griddep_wait();                        // activations come from the preceding kernel
-    int as = 0, bs = 0; uint32_t aph = 0, bph = 0;
     for (int tile = cta; tile < p.n_tiles; tile += n_cta) {
       const int img = tile / tiles_per_img, rem = tile % tiles_per_img;
       const int oy0 = (rem / p.tiles_x) * tile_h, ox0 = (rem % p.tiles_x) * kTileW;
@@ -224,26 +232,17 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
         const int t = tidx + p.tap[tap0][0];
         if (p.skip_t && group_is_padding(p, grp, tidx, oy0, ox0, tile_h)) continue;
         for (int kb = 0; kb < p.kblocks; ++kb) {
-          ptx::mbar_wait(&a_empty[as], aph ^ 1);
-          if (ptx::elect_one_sync()) {
-            unsigned char* sa = a_ring + (size_t)as * a_stage_bytes;
+          ra.produce((uint32_t)a_stage_bytes, [&](int s, uint64_t* bar) {
+            unsigned char* sa = a_ring + (size_t)s * a_stage_bytes;
             const int c = p.cin_off + kb * kBK;
-            ptx::mbar_arrive_expect_tx(&a_full[as], (uint32_t)a_stage_bytes);
-            ptx::tma_load_5d(sa, &tm_a_hi, &a_full[as], c, x, y, t, bidx);
-            ptx::tma_load_5d(sa + p.a_plane_bytes, &tm_a_lo, &a_full[as], c, x, y, t, bidx);
-          }
-          __syncwarp();
-          if (++as == p.na_stages) { as = 0; aph ^= 1; }
+            ptx::tma_load_5d(sa, &tm_a_hi, bar, c, x, y, t, bidx);
+            ptx::tma_load_5d(sa + p.a_plane_bytes, &tm_a_lo, bar, c, x, y, t, bidx);
+          });
           if (!resident) {
             for (int j = 0; j < gsz; ++j) {
               const int it = (tap0 + j) * p.kblocks + kb;          // [tap][kb][plane][rows] blocks of 64-wide rows
-              ptx::mbar_wait(&b_empty[bs], bph ^ 1);
-              if (ptx::elect_one_sync()) {
-                ptx::mbar_arrive_expect_tx(&b_full[bs], (uint32_t)p.b_load_bytes);
-                load_b(b_ring + (size_t)bs * p.b_tile_bytes, it, &b_full[bs]);
-              }
-              __syncwarp();
-              if (++bs == p.nb_stages) { bs = 0; bph ^= 1; }
+              rb.produce((uint32_t)p.b_load_bytes,
+                         [&](int s, uint64_t* bar) { load_b(b_ring + (size_t)s * p.b_tile_bytes, it, bar); });
             }
           }
         }
@@ -262,14 +261,7 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
       const int rem_m = tile % tiles_per_img;
       const int oy_m = (rem_m / p.tiles_x) * tile_h, ox_m = (rem_m % p.tiles_x) * kTileW;
       uint32_t accumulate = 0;
-      int pend_a = -1, pend_b = -1;              // ring slots read by the last committed wgmma group
-      auto release = [&]() {
-        if (wg_leader) {
-          if (pend_a >= 0) ptx::mbar_arrive(&a_empty[pend_a]);
-          if (pend_b >= 0) ptx::mbar_arrive(&b_empty[pend_b]);
-        }
-        pend_a = pend_b = -1;
-      };
+      PendingSlots pend{a_empty, b_empty, wg_leader};
       for (int grp = 0; grp < n_groups; ++grp) {
         if (p.skip_t && group_is_padding(p, grp, tidx, oy_m, ox_m, tile_h)) continue;
         const int tap0 = p.gstart[grp], gsz = p.gsize[grp];
@@ -302,9 +294,7 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
                   wg::mma_bf16<2 * BN>(accr, da_hi + koff, db_hi + koff, acc0);                // A_hi x [W_hi; W_lo]
                   wg::mma_bf16<BN>(accr, da_lo + koff, db_lo + koff, 1);                       // A_lo x W_hi
                 } else {
-                  wg::mma_bf16<BN>(accr, da_hi + koff, db_hi + koff, acc0);
-                  wg::mma_bf16<BN>(accr, da_hi + koff, db_lo + koff, 1);
-                  wg::mma_bf16<BN>(accr, da_lo + koff, db_hi + koff, 1);
+                  wg::mma_hilo<BN>(accr, da_hi + koff, da_lo + koff, db_hi + koff, db_lo + koff, acc0);
                 }
               }
             } else {
@@ -325,9 +315,9 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
             }
             wg::commit();
             wg::wait<1>();                         // the previous group has read its operands
-            release();
-            pend_b = resident ? -1 : bs;
-            if (j + 1 == gsz) pend_a = as;
+            pend.release();
+            pend.b = resident ? -1 : bs;
+            if (j + 1 == gsz) pend.a = as;
             accumulate = 1;
             if (!resident) { if (++bs == p.nb_stages) { bs = 0; bph ^= 1; } }
           }
@@ -335,7 +325,7 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
         }
       }
       wg::wait<0>();
-      release();
+      pend.release();
       // registers -> s_acc (columns the MMAs computed)
       const int ncols = STACK ? 2 * kBRows : kBRows;
       const int row0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
@@ -480,11 +470,10 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
             if (p.res_mode) {
 #pragma unroll
               for (int e2 = 0; e2 < 8; ++e2) {
-                const float r0 = __uint_as_float(rhw[e2] << 16) + __uint_as_float(rlw[e2] << 16);
-                const float r1 = __uint_as_float(rhw[e2] & 0xFFFF0000u) + __uint_as_float(rlw[e2] & 0xFFFF0000u);
+                const float2 r = ptx::join_hilo(rhw[e2], rlw[e2]);
                 float& a0 = v[e2 * 2], &a1 = v[e2 * 2 + 1];
-                if (p.res_mode == 1) { a0 += r0; a1 += r1; if (d_relu) { a0 = fmaxf(a0, 0.f); a1 = fmaxf(a1, 0.f); } }
-                else { if (d_relu) { a0 = fmaxf(a0, 0.f); a1 = fmaxf(a1, 0.f); } a0 += r0; a1 += r1; }
+                if (p.res_mode == 1) { a0 += r.x; a1 += r.y; if (d_relu) { a0 = fmaxf(a0, 0.f); a1 = fmaxf(a1, 0.f); } }
+                else { if (d_relu) { a0 = fmaxf(a0, 0.f); a1 = fmaxf(a1, 0.f); } a0 += r.x; a1 += r.y; }
               }
             } else if (d_relu) {
 #pragma unroll
@@ -495,13 +484,7 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
               __nv_bfloat16* olp = d_lo + pix * d_cstride + d_coff + cb;
               uint32_t hw[8], lw[8];
 #pragma unroll
-              for (int e2 = 0; e2 < 8; ++e2) {
-                const float x0 = v[e2 * 2], x1 = v[e2 * 2 + 1];
-                const uint32_t h = ptx::pack_bf16x2(x0, x1);                   // one cvt.rn.bf16x2.f32
-                const float r0 = x0 - __uint_as_float(h << 16), r1 = x1 - __uint_as_float(h & 0xFFFF0000u);
-                hw[e2] = h;
-                lw[e2] = ptx::pack_bf16x2(r0, r1);
-              }
+              for (int e2 = 0; e2 < 8; ++e2) ptx::split_hilo(v[e2 * 2], v[e2 * 2 + 1], hw[e2], lw[e2]);
               if (d_vec && cb + 16 <= d_nstore) {               // one full 32-byte sector per plane and lane
                 ptx::st_global_v8(ohp, hw);
                 ptx::st_global_v8(olp, lw);
@@ -617,24 +600,44 @@ __global__ void col_sum_reduce_kernel(const float* __restrict__ part, int n_part
 }
 
 // ------------------------------------------------------------------------------------------------ host side
-typedef CUresult (*PFN_tmapEncodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                        const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                        CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-static PFN_tmapEncodeTiled encode_fn() {
-  static PFN_tmapEncodeTiled fn = nullptr;
-  if (!fn) {
-    void* ptr = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &qres) == cudaSuccess &&
-        qres == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<PFN_tmapEncodeTiled>(ptr);
-  }
-  return fn;
+int launch_col_sum_reduce(const float* part, int n_part, int n_img, float* out, cudaStream_t stream) {
+  STP3_CUDA_OK(launch_pdl(kPdlAux, col_sum_reduce_kernel, dim3(n_img), dim3(64, 16), 0, stream, part, n_part, n_img, 64, out));
+  return STP3_OK;
 }
 
-int launch_col_sum_reduce(const float* part, int n_part, int n_img, float* out, cudaStream_t stream) {
-  STP3_CUDA_OK(launch_pdl(col_sum_reduce_kernel, dim3(n_img), dim3(64, 16), 0, stream, part, n_part, n_img, 64, out));
+// Ring depths for this instantiation's shared-memory tail, then the launch.  p.a_plane_bytes is set.
+template <int BN, bool STACK, bool FULLK>
+static int launch_conv(ConvParams& p, const CUtensorMap& tm_hi, const CUtensorMap& tm_lo, const CUtensorMap& tm_w,
+                       int n_mma, int k_iters, bool stream_weights, unsigned grid, cudaStream_t stream) {
+  using SM = ConvSmem<BN, STACK>;
+  const size_t smem_cap = 227 * 1024;
+  const size_t a_stage = 2 * (size_t)p.a_plane_bytes;
+  p.b_rows = FULLK ? BN : n_mma;
+  p.b_tile_bytes = 2 * p.b_rows * kBK * 2;
+  p.b_load_bytes = 2 * n_mma * kBK * 2;
+  const size_t avail = smem_cap - 1024 - SM::tail_bytes();
+  const size_t wbytes = (size_t)k_iters * (size_t)p.b_tile_bytes;
+  // small weight tensors stay resident in smem next to >= 2 activation stages
+  const bool res = !stream_weights && wbytes + 2 * a_stage <= avail;
+  int na, nb;
+  if (res) {
+    na = (int)((avail - wbytes) / a_stage); nb = 0;
+  } else {
+    // as many activation stages as fit beside two weight slots, then fill up with weight slots (a slot is released
+    // one wgmma group after its last reader, so two slots keep a tap group of any size moving)
+    na = (int)((avail - 2 * (size_t)p.b_tile_bytes) / a_stage);
+    if (na > kMaxAStages) na = kMaxAStages;
+    if (na < 2 || (size_t)na * a_stage + 2 * (size_t)p.b_tile_bytes > avail)
+      return set_error(STP3_EUNSUPPORTED, "convolution does not fit in shared memory");
+    nb = (int)((avail - (size_t)na * a_stage) / (size_t)p.b_tile_bytes);
+  }
+  if (na > kMaxAStages) na = kMaxAStages;
+  if (nb > kMaxBStages) nb = kMaxBStages;
+  p.na_stages = na; p.nb_stages = nb; p.b_resident = res ? 1 : 0;
+  const size_t smem_bytes = 1024 + na * a_stage + (res ? wbytes : (size_t)nb * (size_t)p.b_tile_bytes) + SM::tail_bytes();
+  constexpr auto kern = conv_igemm_kernel<BN, STACK, FULLK>;
+  STP3_CUDA_OK(set_max_dynamic_smem<kern>((int)smem_cap));
+  STP3_CUDA_OK(launch_pdl(kPdlConv, kern, dim3(grid), dim3(kConvThreads), smem_bytes, stream, tm_hi, tm_lo, tm_w, p));
   return STP3_OK;
 }
 
@@ -642,18 +645,8 @@ int launch_col_sum_reduce(const float* part, int n_part, int n_img, float* out, 
 
 using namespace stp3;
 
-static int conv_num_sms() {
-  static const int n = [] {
-    int dev = 0, v = 132;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev);
-    return v;
-  }();
-  return n;
-}
-
 extern "C" size_t stp3_conv_col_sums_scratch_bytes(int n_img, int bn) {
-  return (size_t)conv_num_sms() * 4 * (size_t)(n_img > 0 ? n_img : 0) * (size_t)(bn > 0 ? bn : 0) * sizeof(float);
+  return (size_t)num_sms() * 4 * (size_t)(n_img > 0 ? n_img : 0) * (size_t)(bn > 0 ? bn : 0) * sizeof(float);
 }
 
 extern "C" int stp3_conv_fwd(const stp3_conv_desc* d, const void* x_hi, const void* x_lo, const void* w,
@@ -682,15 +675,13 @@ extern "C" int stp3_conv_fwd(const stp3_conv_desc* d, const void* x_hi, const vo
   if (d->res_mode) STP3_CHECK_ARG(res_hi && res_lo && d->res_cstride % 8 == 0 && d->res_coff % 8 == 0 &&
                                   d->res_coff + d->bn <= d->res_cstride, "bad residual tensor");
   if (y_f32) STP3_CHECK_ARG(d->n_valid > 0 && d->n_valid <= d->bn, "n_valid out of range");
-  PFN_tmapEncodeTiled enc = encode_fn();
-  if (!enc) return set_error(STP3_ECUDA, "cuTensorMapEncodeTiled is not available from the driver");
+  if (!tmap_encode_fn()) return set_error(STP3_ECUDA, "cuTensorMapEncodeTiled is not available from the driver");
 
   // tuning knobs (0 = automatic): desc->tune_group, or the STP3_CONV_GROUP environment variable.  tune_n_sub is
   // accepted for ABI compatibility; the tile is always 8 x 16 pixels.
   static const int env_group = [] { const char* e = getenv("STP3_CONV_GROUP"); return e ? atoi(e) : 0; }();
   const int want_group_raw = d->tune_group ? d->tune_group : env_group;
   const int want_group = want_group_raw & 3;
-  static const bool use_pdl = stp3_pdl_enabled("STP3_CONV_PDL");
   const bool stream_weights = (want_group_raw & 4) != 0;    // +4: keep the weights in the ring even if they would fit
   // +8: stacked [W_hi; W_lo] operand (bn = 64 only).  Untuned (tune_group == 0) multi-tap 64-column layers use it: it
   // reads the activation tile twice instead of three times
@@ -715,20 +706,9 @@ extern "C" int stp3_conv_fwd(const stp3_conv_desc* d, const void* x_hi, const vo
 
   CUtensorMap tm_hi, tm_lo, tm_w;
   {
-    const cuuint64_t dims[5] = {(cuuint64_t)d->in_cstride, (cuuint64_t)d->W, (cuuint64_t)d->H, (cuuint64_t)T_total,
-                                (cuuint64_t)d->B};
-    const cuuint64_t strides[4] = {(cuuint64_t)d->in_cstride * 2, (cuuint64_t)d->W * d->in_cstride * 2,
-                                   (cuuint64_t)d->H * d->W * d->in_cstride * 2,
-                                   (cuuint64_t)T_total * d->H * d->W * d->in_cstride * 2};
-    const cuuint32_t box[5] = {(cuuint32_t)kBK, (cuuint32_t)((kTileW - 1) * d->stride + 1),
-                               (cuuint32_t)((box_h - 1) * d->stride + 1), 1, 1};
-    const cuuint32_t estr[5] = {1, (cuuint32_t)d->stride, (cuuint32_t)d->stride, 1, 1};
-    CUresult r1 = enc(&tm_hi, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 5, const_cast<void*>(x_hi), dims, strides, box, estr,
-                      CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    CUresult r2 = enc(&tm_lo, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 5, const_cast<void*>(x_lo), dims, strides, box, estr,
-                      CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    const int box_w = (kTileW - 1) * d->stride + 1, box_rows = (box_h - 1) * d->stride + 1;
+    const CUresult r1 = encode_act_5d(&tm_hi, x_hi, d->in_cstride, d->W, d->H, T_total, d->B, box_w, box_rows, d->stride);
+    const CUresult r2 = encode_act_5d(&tm_lo, x_lo, d->in_cstride, d->W, d->H, T_total, d->B, box_w, box_rows, d->stride);
     if (r1 != CUDA_SUCCESS || r2 != CUDA_SUCCESS)
       return set_error(STP3_ECUDA, "cuTensorMapEncodeTiled(activation) failed: %d %d", (int)r1, (int)r2);
   }
@@ -737,13 +717,7 @@ extern "C" int stp3_conv_fwd(const stp3_conv_desc* d, const void* x_hi, const vo
   // the MMAs cover only the columns that carry weights (n_cols, rounded up to a multiple of 16)
   const int n_mma = d->bn <= 128 && d->n_cols > 0 && d->n_cols < d->bn ? ((d->n_cols + 15) / 16) * 16 : bn_launch;
   {
-    const cuuint64_t dims[2] = {(cuuint64_t)kBK, (cuuint64_t)d->ntaps * kblocks * 2 * d->bn};
-    const cuuint64_t strides[1] = {(cuuint64_t)kBK * 2};
-    const cuuint32_t box[2] = {(cuuint32_t)kBK, (cuuint32_t)n_mma};
-    const cuuint32_t estr[2] = {1, 1};
-    CUresult r = enc(&tm_w, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(w), dims, strides, box, estr,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    const CUresult r = encode_rows_2d(&tm_w, w, (long long)d->ntaps * kblocks * 2 * d->bn, n_mma);
     if (r != CUDA_SUCCESS) return set_error(STP3_ECUDA, "cuTensorMapEncodeTiled(weights) failed: %d", (int)r);
   }
 
@@ -797,12 +771,8 @@ extern "C" int stp3_conv_fwd(const stp3_conv_desc* d, const void* x_hi, const vo
   const long long nblk = (long long)p.n_img * p.tiles_x * p.tiles_y;
   STP3_CHECK_ARG(nblk > 0 && nblk < (1ll << 31), "grid too large");
   p.n_tiles = (int)nblk;
-  const int num_sms = conv_num_sms();
-  unsigned grid = (unsigned)(nblk < num_sms ? nblk : num_sms);           // persistent: one CTA per SM
-  const size_t smem_cap = 227 * 1024;
-  const size_t a_stage = 2 * (size_t)p.a_plane_bytes;
-
-  int launched_grid = (int)grid;
+  const int n_sm = num_sms();
+  const unsigned grid = (unsigned)(nblk < n_sm ? nblk : n_sm);           // persistent: one CTA per SM
   p.sum_part = nullptr;
   if (d->col_sums) {
     STP3_CHECK_ARG(d->bn == 64, "col_sums: 64-column convolutions only");
@@ -826,62 +796,22 @@ extern "C" int stp3_conv_fwd(const stp3_conv_desc* d, const void* x_hi, const vo
     p.vec256 = (y_hi && d->out_cstride % 16 == 0 && p.out_coff % 16 == 0 && al32(y_hi) && al32(y_lo) ? 1 : 0) |
                (d->res_mode && d->res_cstride % 16 == 0 && p.res_coff % 16 == 0 && al32(res_hi) && al32(res_lo) ? 2 : 0) |
                (d->y2_hi && d->out2_cstride % 16 == 0 && d->out2_coff % 16 == 0 && al32(d->y2_hi) && al32(d->y2_lo) ? 4 : 0);
-#define STP3_LAUNCH_CONV(BN_, STACK_, FULLK_)                                                                     \
-    do {                                                                                                          \
-      using SM = ConvSmem<BN_, STACK_>;                                                                           \
-      p.b_rows = FULLK_ ? BN_ : n_mma;                                                                            \
-      p.b_tile_bytes = 2 * p.b_rows * kBK * 2;                                                                    \
-      p.b_load_bytes = 2 * n_mma * kBK * 2;                                                                       \
-      const size_t avail = smem_cap - 1024 - SM::tail_bytes();                                                    \
-      const size_t wbytes = (size_t)k_iters * (size_t)p.b_tile_bytes;                                             \
-      /* small weight tensors stay resident in smem next to >= 2 activation stages */                            \
-      const bool res = !stream_weights && wbytes + 2 * a_stage <= avail;                                          \
-      int na, nb;                                                                                                 \
-      if (res) {                                                                                                  \
-        na = (int)((avail - wbytes) / a_stage); nb = 0;                                                           \
-      } else {                                                                                                    \
-        /* as many activation stages as fit beside two weight slots, then fill up with weight slots (a slot is  */ \
-        /* released one wgmma group after its last reader, so two slots keep a tap group of any size moving)    */ \
-        na = (int)((avail - 2 * (size_t)p.b_tile_bytes) / a_stage);                                               \
-        if (na > kMaxAStages) na = kMaxAStages;                                                                   \
-        if (na < 2 || (size_t)na * a_stage + 2 * (size_t)p.b_tile_bytes > avail)                                  \
-          return set_error(STP3_EUNSUPPORTED, "convolution does not fit in shared memory");                       \
-        nb = (int)((avail - (size_t)na * a_stage) / (size_t)p.b_tile_bytes);                                      \
-      }                                                                                                           \
-      if (na > kMaxAStages) na = kMaxAStages;                                                                     \
-      if (nb > kMaxBStages) nb = kMaxBStages;                                                                     \
-      p.na_stages = na; p.nb_stages = nb; p.b_resident = res ? 1 : 0;                                             \
-      const size_t smem_bytes = 1024 + na * a_stage + (res ? wbytes : (size_t)nb * (size_t)p.b_tile_bytes) + SM::tail_bytes(); \
-      auto kern = conv_igemm_kernel<BN_, STACK_, FULLK_>;                                                         \
-      /* once per kernel instantiation and device: the attribute call costs microseconds on every eager launch */ \
-      static thread_local int attr_dev = -1;                                                                      \
-      int cur_dev = 0; cudaGetDevice(&cur_dev);                                                                   \
-      if (attr_dev != cur_dev) {                                                                                  \
-        STP3_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_cap));     \
-        attr_dev = cur_dev;                                                                                       \
-      }                                                                                                           \
-      cudaLaunchConfig_t cfg = {};                                                                                \
-      cfg.gridDim = dim3(grid); cfg.blockDim = dim3(kConvThreads);                                                \
-      cfg.dynamicSmemBytes = smem_bytes; cfg.stream = stream;                                                     \
-      cudaLaunchAttribute attr[1];                                                                                \
-      attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;                                            \
-      attr[0].val.programmaticStreamSerializationAllowed = 1;                                                     \
-      cfg.attrs = attr; cfg.numAttrs = use_pdl ? 1 : 0;                                                           \
-      launched_grid = (int)cfg.gridDim.x;                                                                         \
-      STP3_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, tm_hi, tm_lo, tm_w, p));                                        \
-    } while (0)
-    if (bn_launch == 64) {
-      if (stack) { if (full_k) STP3_LAUNCH_CONV(64, true, true); else STP3_LAUNCH_CONV(64, true, false); }
-      else { if (full_k) STP3_LAUNCH_CONV(64, false, true); else STP3_LAUNCH_CONV(64, false, false); }
-    } else {
-      if (full_k) STP3_LAUNCH_CONV(128, false, true); else STP3_LAUNCH_CONV(128, false, false);
-    }
-#undef STP3_LAUNCH_CONV
+    int rc;
+    if (bn_launch == 64 && stack)
+      rc = full_k ? launch_conv<64, true, true>(p, tm_hi, tm_lo, tm_w, n_mma, k_iters, stream_weights, grid, stream)
+                  : launch_conv<64, true, false>(p, tm_hi, tm_lo, tm_w, n_mma, k_iters, stream_weights, grid, stream);
+    else if (bn_launch == 64)
+      rc = full_k ? launch_conv<64, false, true>(p, tm_hi, tm_lo, tm_w, n_mma, k_iters, stream_weights, grid, stream)
+                  : launch_conv<64, false, false>(p, tm_hi, tm_lo, tm_w, n_mma, k_iters, stream_weights, grid, stream);
+    else
+      rc = full_k ? launch_conv<128, false, true>(p, tm_hi, tm_lo, tm_w, n_mma, k_iters, stream_weights, grid, stream)
+                  : launch_conv<128, false, false>(p, tm_hi, tm_lo, tm_w, n_mma, k_iters, stream_weights, grid, stream);
+    if (rc) return rc;
     STP3_CUDA_OK(cudaGetLastError());
   }
   if (p.sum_part) {
-    STP3_CUDA_OK(launch_pdl(col_sum_reduce_kernel, dim3(p.n_img), dim3(64, 16), 0, stream, (const float*)p.sum_part,
-                            launched_grid * 4, p.n_img, 64, static_cast<float*>(d->col_sums)));
+    STP3_CUDA_OK(launch_pdl(kPdlAux, col_sum_reduce_kernel, dim3(p.n_img), dim3(64, 16), 0, stream,
+                            (const float*)p.sum_part, (int)grid * 4, p.n_img, 64, static_cast<float*>(d->col_sums)));
   }
   return STP3_OK;
 }

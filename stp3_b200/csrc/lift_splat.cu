@@ -89,10 +89,6 @@ __device__ __forceinline__ void flush_segment(float* gbase, unsigned char* obase
 // hi + lo and the three products hi*hi + hi*lo + lo*hi, i.e. ~16 significand bits per operand like the hi/lo planes the
 // BEV grid is stored in downstream.  A pair whose points fall into several pillars takes one more pass per pillar with
 // the operand masked to it (up to kSegPasses); anything beyond that is left to a scalar segmented walk.
-__device__ __forceinline__ void split_bf16x2(float x0, float x1, uint32_t& hi, uint32_t& lo) {
-  hi = ptx::pack_bf16x2(x0, x1);
-  lo = ptx::pack_bf16x2(x0 - __uint_as_float(hi << 16), x1 - __uint_as_float(hi & 0xFFFF0000u));
-}
 __device__ __forceinline__ void mma_bf16_m16n8k16(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
   asm volatile(
       "mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
@@ -576,7 +572,7 @@ lift_splat_scatter_tma_kernel(const __grid_constant__ LiftSplatTmaMaps maps, con
   }
   __syncthreads();
 
-  // ---- phase C: pooling on the tensor cores (see split_bf16x2 / mma_bf16_m16n8k16 above).
+  // ---- phase C: pooling on the tensor cores (ptx::split_hilo, mma_bf16_m16n8k16 below).
   // warp = (image column wl, half of the 64 channels); per m-tile of 16 depth bins: A = probabilities masked to the
   // pass's pillar (16 x Hf), B = the column's features (Hf x 32 channels, fragments loaded once per channel chunk),
   // accumulators flushed with one red.global.add.v2.f32 per lane and (depth bin, 8-channel group).
@@ -613,7 +609,7 @@ lift_splat_scatter_tma_kernel(const __grid_constant__ LiftSplatTmaMaps maps, con
               if (h < Hf) x0 = s_feat[cl * fstride + h * TW + wl];
               if (h + 1 < Hf) x1 = s_feat[cl * fstride + (h + 1) * TW + wl];
             }
-            split_bf16x2(x0, x1, bh[nt][ks][r], bl[nt][ks][r]);
+            ptx::split_hilo(x0, x1, bh[nt][ks][r], bl[nt][ks][r]);
           }
         }
       }
@@ -641,7 +637,7 @@ lift_splat_scatter_tma_kernel(const __grid_constant__ LiftSplatTmaMaps maps, con
                 x0 = rk.x == sg ? q.x : 0.f;
                 x1 = rk.y == sg ? q.y : 0.f;
               }
-              split_bf16x2(x0, x1, ah[ks][r], al[ks][r]);
+              ptx::split_hilo(x0, x1, ah[ks][r], al[ks][r]);
             }
           }
 #pragma unroll
@@ -1020,21 +1016,6 @@ __global__ void clear_bytes_kernel(unsigned char* __restrict__ p, size_t n) {
 
 using namespace stp3;
 
-typedef CUresult (*PFN_tmapEncode)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static PFN_tmapEncode tmap_encode_fn() {
-  static PFN_tmapEncode fn = nullptr;
-  if (!fn) {
-    void* ptr = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &qres) == cudaSuccess &&
-        qres == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<PFN_tmapEncode>(ptr);
-  }
-  return fn;
-}
-
 static size_t grid_bytes(int B, int S, int C, int nx, int ny) {
   const size_t g = (size_t)B * S * nx * ny * C * sizeof(float);
   return (g + 255) & ~(size_t)255;
@@ -1138,7 +1119,7 @@ static int lift_splat_impl(const float* feat, int feat_layout, const float* dept
   int rc = STP3_OK;
   bool used_tma = false;
   if (tma_ok) {
-    PFN_tmapEncode enc = tmap_encode_fn();
+    const TmapEncodeFn enc = tmap_encode_fn();
     if (enc) {
       LiftSplatTmaMaps maps;
       const long long n_img = (long long)B * S * N;

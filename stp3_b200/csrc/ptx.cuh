@@ -2,6 +2,7 @@
 #pragma once
 #include <cstdint>
 #include <cuda.h>  // CUtensorMap (types only; the encode entry point is fetched at run time)
+#include <cuda_bf16.h>
 
 namespace stp3 {
 namespace ptx {
@@ -13,6 +14,23 @@ __device__ __forceinline__ uint32_t pack_bf16x2(float a, float b) {
   uint32_t r;
   asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(b), "f"(a));
   return r;
+}
+
+// The hi/lo plane format of every fp32 tensor: hi = bf16(x), lo = bf16(x - hi), both rounded to nearest even.
+// A pair (x0, x1) -> packed bf16x2 words, x0 in the low halves.
+__device__ __forceinline__ void split_hilo(float x0, float x1, uint32_t& hi, uint32_t& lo) {
+  hi = pack_bf16x2(x0, x1);
+  lo = pack_bf16x2(x0 - __uint_as_float(hi << 16), x1 - __uint_as_float(hi & 0xFFFF0000u));
+}
+// one element (the same rounding as the pair form)
+__device__ __forceinline__ void split_hilo(float x, __nv_bfloat16& hi, __nv_bfloat16& lo) {
+  hi = __float2bfloat16_rn(x);
+  lo = __float2bfloat16_rn(x - __bfloat162float(hi));
+}
+// hi + lo of the low and the high halves of a packed pair
+__device__ __forceinline__ float2 join_hilo(uint32_t hi, uint32_t lo) {
+  return make_float2(__uint_as_float(hi << 16) + __uint_as_float(lo << 16),
+                     __uint_as_float(hi & 0xFFFF0000u) + __uint_as_float(lo & 0xFFFF0000u));
 }
 
 // 32-byte global accesses (8 x 32 bit) as two 128-bit instructions: Hopper has no 256-bit load / store.  16-byte aligned.

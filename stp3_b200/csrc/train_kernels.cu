@@ -53,13 +53,7 @@ __device__ __forceinline__ void load8_split(const float* row, int c0, int C, boo
   }
   uint32_t h[4], l[4];
 #pragma unroll
-  for (int e = 0; e < 4; ++e) {
-    const __nv_bfloat16 h0 = __float2bfloat16_rn(v[2 * e]), h1 = __float2bfloat16_rn(v[2 * e + 1]);
-    const __nv_bfloat16 l0 = __float2bfloat16_rn(v[2 * e] - __bfloat162float(h0));
-    const __nv_bfloat16 l1 = __float2bfloat16_rn(v[2 * e + 1] - __bfloat162float(h1));
-    h[e] = (uint32_t)__bfloat16_as_ushort(h0) | ((uint32_t)__bfloat16_as_ushort(h1) << 16);
-    l[e] = (uint32_t)__bfloat16_as_ushort(l0) | ((uint32_t)__bfloat16_as_ushort(l1) << 16);
-  }
+  for (int e = 0; e < 4; ++e) ptx::split_hilo(v[2 * e], v[2 * e + 1], h[e], l[e]);
   hi = make_uint4(h[0], h[1], h[2], h[3]);
   lo = make_uint4(l[0], l[1], l[2], l[3]);
 }
@@ -248,11 +242,6 @@ __global__ void sums_finalize_kernel(const double* __restrict__ part, int n_part
 }
 
 // ------------------------------------------------------------------------------------------------ elementwise
-__device__ __forceinline__ void split_bf16(float v, __nv_bfloat16& h, __nv_bfloat16& l) {
-  h = __float2bfloat16_rn(v);
-  l = __float2bfloat16_rn(v - __bfloat162float(h));
-}
-
 // y = relu?((x - mean) * invstd * gamma + beta (+ res)); one thread = one pixel x 8 channels (two 128-bit loads);
 // groups of 8 channels in [C, y_cs) of the bf16 planes are written as zeros (padding of the next conv's K blocks)
 __global__ void __launch_bounds__(256)
@@ -294,13 +283,7 @@ bn_apply_kernel(const float* __restrict__ x, int x_cs, const float* __restrict__
   if (yh && c0 < hl_cs) {
     uint32_t oh[4], ol[4];
 #pragma unroll
-    for (int e = 0; e < 4; ++e) {
-      __nv_bfloat16 h0, l0, h1, l1;
-      split_bf16(v[2 * e], h0, l0);
-      split_bf16(v[2 * e + 1], h1, l1);
-      oh[e] = (uint32_t)__bfloat16_as_ushort(h0) | ((uint32_t)__bfloat16_as_ushort(h1) << 16);
-      ol[e] = (uint32_t)__bfloat16_as_ushort(l0) | ((uint32_t)__bfloat16_as_ushort(l1) << 16);
-    }
+    for (int e = 0; e < 4; ++e) ptx::split_hilo(v[2 * e], v[2 * e + 1], oh[e], ol[e]);
     *reinterpret_cast<uint4*>(yh + p * hl_cs + c0) = make_uint4(oh[0], oh[1], oh[2], oh[3]);
     *reinterpret_cast<uint4*>(yl + p * hl_cs + c0) = make_uint4(ol[0], ol[1], ol[2], ol[3]);
   }

@@ -110,6 +110,31 @@ __device__ __forceinline__ void mma_bf16_rs64(float* d, const uint32_t* a, uint6
       : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(accumulate));
 }
 
+// One K = 16 step of a product of two operands stored as bf16 hi / lo planes: hi*hi + hi*lo + lo*hi, in that order
+// (fp32 accumulation; lo*lo is below the fp32 round-off of the sum)
+template <int N>
+__device__ __forceinline__ void mma_hilo(float* d, uint64_t da_hi, uint64_t da_lo, uint64_t db_hi, uint64_t db_lo,
+                                         uint32_t accumulate) {
+  mma_bf16<N>(d, da_hi, db_hi, accumulate);
+  mma_bf16<N>(d, da_hi, db_lo, 1);
+  mma_bf16<N>(d, da_lo, db_hi, 1);
+}
+// the same with the A planes in registers (mma_bf16_rs64 / mma_bf16_rs128 fragments)
+template <int N>
+__device__ __forceinline__ void mma_hilo_rs(float* d, const uint32_t* a_hi, const uint32_t* a_lo, uint64_t db_hi,
+                                            uint64_t db_lo, uint32_t accumulate) {
+  static_assert(N == 64 || N == 128, "register-A MMA: N = 64 or 128");
+  if constexpr (N == 64) {
+    mma_bf16_rs64(d, a_hi, db_hi, accumulate);
+    mma_bf16_rs64(d, a_hi, db_lo, 1);
+    mma_bf16_rs64(d, a_lo, db_hi, 1);
+  } else {
+    mma_bf16_rs128(d, a_hi, db_hi, accumulate);
+    mma_bf16_rs128(d, a_hi, db_lo, 1);
+    mma_bf16_rs128(d, a_lo, db_hi, 1);
+  }
+}
+
 // MN-major operand tile (the transpose bit set): for every K index one row of 64 bf16 (128 B) holding 64 consecutive
 // M (or N) entries, 128-byte swizzled as TMA writes it, 8 K rows per 1024-byte atom.  SBO = 1024 B between groups of
 // 8 K rows; LBO = bytes between 64-wide M / N blocks (unused when the operand is 64 wide, as in stp3_conv_wgrad).
