@@ -44,6 +44,9 @@ const char* stp3_last_error(void);
  *                                                                          discount recurrence, (C,X,Y) layout)
  *   VoxelsSumming.forward                  stp3/utils/geometry.py:299-318
  *
+ * stp3_lift_splat_desc describes the call: the camera / ego-motion / frustum geometry, the BEV grid, the shapes and the
+ * frame range.  The forward and the backward take the same descriptor and their tensors as arguments.
+ *
  * Layouts (all fp32 unless noted)
  *   feat          feat_layout==0: (B,S,N,C,Hf,Wf)  [the reference Encoder's NCHW output]
  *                 feat_layout==1: (B,S,N,Hf,Wf,C)  [channels-last, produced by this library's conv kernels]
@@ -52,8 +55,8 @@ const char* stp3_last_error(void);
  *   cam_t         (B,S,N,3)
  *   ego_R, ego_t  (B,S,3,3), (B,S,3)  from pose_vec2mat(future_egomotion)  (geometry.py:158-172)
  *   xs, ys, ds    (Wf), (Hf), (D): the three axes of STP3.create_frustum (stp3.py:111-130)
- *   bev_off       HOST float[3] = (bev_start_position - bev_resolution/2) as evaluated in fp32 by torch (stp3.py:288)
- *   bev_res       HOST float[3]
+ *   bev_off       (bev_start_position - bev_resolution/2) as evaluated in fp32 by torch (stp3.py:288)
+ *   bev_res       bev_resolution; nx, ny, nz = bev_dimension
  *   ranks_out     optional (B,S,N,D,Hf,Wf) int32: pillar rank ix*(ny*nz)+iy*nz+iz of every lifted point after the
  *                 ego warp, -1 where the reference's mask (stp3.py:239-246) drops it.  Bit-exact with the CPU
  *                 reference; used by the parity tests.
@@ -63,26 +66,53 @@ const char* stp3_last_error(void);
  *                                of the tensor-core path, consumed directly by stp3_conv_fwd
  *   pool_sum      optional (B,S,C) fp32: sum over the nx*ny cells of out[b,t,c] (feeds the pyramid-pooling branch
  *                 of TemporalBlock, temporal.py:408-423); fully overwritten by the call.
- *   workspace     >= stp3_lift_splat_workspace_bytes(...) bytes, 256-byte aligned.  It holds the channels-last
+ *   workspace     >= stp3_lift_splat_workspace_bytes(desc) bytes, 256-byte aligned.  It holds the channels-last
  *                 fp32 scatter grid (B,S,nx*ny,C) and a per-pillar occupancy map.  It must be ALL ZERO on entry:
  *                 clear it once with stp3_lift_splat_workspace_init() after allocating it; every successful
  *                 stp3_lift_splat_fwd leaves it zero again (the finalize kernel re-zeroes exactly the pillars it
  *                 read), so no per-call memset is needed.  After a failed call, re-initialise it.
  * nz must be 1 (the reference's squeeze(0) at stp3.py:298 assumes it).
+ *
+ * Frame-sharded mode (f_count > 0; latency mode, SURVEY.md §8e): when the global batch is smaller than the number of
+ * GPUs the B*S camera frames are split across ranks.  Each rank splats its flat frames f_begin + [0, f_count)
+ * (f = b*S + t, the ego-motion chain of frame t still uses the poses t..S-2 of its sample) and writes them RAW -- no
+ * discount recurrence, `discount` is ignored -- as channels-last fp32 grids (f_count, nx, ny, C): out_layout must be 1
+ * and ranks_out and pool_sum NULL.  The workspace is sized for the f_count frames.
+ *   n_peers == 0  the frames go to `out`; after ONE all-gather of those grids (ncclAllGather over NVLink;
+ *                 stp3_b200/parallel.py) every rank holds (B, S, nx, ny, C) and stp3_bev_discount applies
+ *                 out[t] = out[t-1]*discount + raw[t] (stp3.py:296) and emits the bf16 hi/lo planes the temporal block
+ *                 consumes.
+ *   n_peers > 0   FUSED WITH THE ALL-GATHER (needs C in {32, 64, 128}; `out` is ignored): the finalize epilogue stores
+ *                 every finished BEV row of flat frame f straight into slot f of all n_peers gathered buffers
+ *                 peer_out[r] (each (B*S, nx, ny, C) fp32, 32-byte aligned; peer-mapped device pointers of every rank's
+ *                 buffer including this rank's own, e.g. from CUDA IPC / torch symmetric memory) over NVLink -- no
+ *                 separate collective launch.  The caller brackets the call with a cross-rank barrier on both sides
+ *                 (buffers free / stores landed) and then runs stp3_bev_discount on its own buffer.  peer_out is a HOST
+ *                 array of n_peers <= 8 pointers.
  */
-size_t stp3_lift_splat_workspace_bytes(int B, int S, int C, int nx, int ny);
-int stp3_lift_splat_workspace_init(void* workspace, size_t workspace_bytes, void* stream);
+typedef struct stp3_lift_splat_desc {
+  const float* cam_M;
+  const float* cam_t;
+  const float* ego_R;
+  const float* ego_t;
+  const float* xs;
+  const float* ys;
+  const float* ds;
+  float bev_off[3];
+  float bev_res[3];
+  int nx, ny, nz;
+  float discount;
+  int B, S, N, D, Hf, Wf, C;
+  int feat_layout;
+  int use_depth_distribution;
+  int f_begin, f_count;  /* 0, 0: every frame, with the discount recurrence; f_count > 0: frame-sharded mode */
+} stp3_lift_splat_desc;
 
-int stp3_lift_splat_fwd(const float* feat, int feat_layout, const float* depth_logits,
-                        const float* cam_M, const float* cam_t, const float* ego_R, const float* ego_t,
-                        const float* xs, const float* ys, const float* ds,
-                        const float* bev_off /*host[3]*/, const float* bev_res /*host[3]*/,
-                        int nx, int ny, int nz, float discount,
-                        int B, int S, int N, int D, int Hf, int Wf, int C,
-                        int use_depth_distribution,
-                        int32_t* ranks_out, float* pool_sum,
-                        void* workspace, size_t workspace_bytes,
-                        float* out, int out_layout, void* stream);
+size_t stp3_lift_splat_workspace_bytes(const stp3_lift_splat_desc* desc);
+int stp3_lift_splat_workspace_init(void* workspace, size_t workspace_bytes, void* stream);
+int stp3_lift_splat_fwd(const stp3_lift_splat_desc* desc, const float* feat, const float* depth_logits,
+                        int32_t* ranks_out, float* pool_sum, void* workspace, size_t workspace_bytes,
+                        float* out, int out_layout, int n_peers, void* const* peer_out, void* stream);
 
 /* Backward of stp3_lift_splat_fwd (training through the drop-in, SURVEY.md row f2): given grad_out = dLoss/d out
  * (B,S,C,nx,ny) fp32 it returns grad_feat (B,S,N,C,Hf,Wf) and grad_depth_logits (B,S,N,D,Hf,Wf; may be NULL, and is not
@@ -91,16 +121,12 @@ int stp3_lift_splat_fwd(const float* feat, int feat_layout, const float* depth_l
  *   projection_to_birds_eye_view           stp3/models/stp3.py:239-296     (mask, index_put, bev = bev*discount + tmp)
  *   outer product + softmax over depth     stp3/models/stp3.py:214-216
  * Voxel indices are recomputed with the forward's exact arithmetic (not differentiable, like the reference's .long()).
- * feat is NCHW (feat_layout 0).  scratch: stp3_lift_splat_bwd_scratch_bytes() bytes of device memory (no invariant).
- * Gathers only, no atomics: deterministic. */
-size_t stp3_lift_splat_bwd_scratch_bytes(int B, int S, int C, int nx, int ny);
-int stp3_lift_splat_bwd(const float* grad_out, const float* feat, const float* depth_logits,
-                        const float* cam_M, const float* cam_t, const float* ego_R, const float* ego_t,
-                        const float* xs, const float* ys, const float* ds,
-                        const float* bev_off /*host[3]*/, const float* bev_res /*host[3]*/,
-                        int nx, int ny, int nz, float discount,
-                        int B, int S, int N, int D, int Hf, int Wf, int C, int use_depth_distribution,
-                        void* scratch, size_t scratch_bytes, float* grad_feat, float* grad_depth_logits, void* stream);
+ * feat is NCHW (desc->feat_layout 0) and every frame is processed (desc->f_count 0).  scratch:
+ * stp3_lift_splat_bwd_scratch_bytes(desc) bytes of device memory (no invariant).  Gathers only, no atomics: deterministic. */
+size_t stp3_lift_splat_bwd_scratch_bytes(const stp3_lift_splat_desc* desc);
+int stp3_lift_splat_bwd(const stp3_lift_splat_desc* desc, const float* grad_out, const float* feat,
+                        const float* depth_logits, void* scratch, size_t scratch_bytes, float* grad_feat,
+                        float* grad_depth_logits, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------
  * Dense layers: implicit-GEMM convolution on the Hopper tensor cores (wgmma, register accumulators, TMA-fed operands).
@@ -336,35 +362,7 @@ int stp3_phase_interleave(const float* p00, const float* p01, const float* p10, 
 int stp3_sigmoid_bwd(const float* g, const float* s, long long n, float* dz, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------
- * Frame-sharded lift-splat (latency mode, SURVEY.md §8e): when the global batch is smaller than the number of GPUs the
- * B*S camera frames are split across ranks.  Each rank splats its flat frames f_begin + [0, f_count) (f = b*S + t, the
- * ego-motion chain of frame t still uses the poses t..S-2 of its sample) and writes them RAW -- no discount
- * recurrence -- as channels-last fp32 grids out_raw (f_count, nx, ny, C).  After ONE all-gather of those grids
- * (ncclAllGather over NVLink; stp3_b200/parallel.py) every rank holds (B, S, nx, ny, C) and stp3_bev_discount applies
- * out[t] = out[t-1]*discount + raw[t] (stp3.py:296) and emits the bf16 hi/lo planes the temporal block consumes.
- * workspace: stp3_lift_splat_workspace_bytes(f_count, 1, C, nx, ny) bytes, all-zero on entry (same invariant). */
-int stp3_lift_splat_frames_fwd(const float* feat, int feat_layout, const float* depth_logits,
-                               const float* cam_M, const float* cam_t, const float* ego_R, const float* ego_t,
-                               const float* xs, const float* ys, const float* ds,
-                               const float* bev_off /*host[3]*/, const float* bev_res /*host[3]*/,
-                               int nx, int ny, int nz,
-                               int B, int S, int N, int D, int Hf, int Wf, int C,
-                               int use_depth_distribution, int f_begin, int f_count,
-                               void* workspace, size_t workspace_bytes, float* out_raw, void* stream);
-/* The same, FUSED WITH THE ALL-GATHER: the finalize epilogue stores every finished BEV row of flat frame f straight into
- * slot f of all n_peers gathered buffers peer_out[r] (each (B*S, nx, ny, C) fp32; peer-mapped device pointers of every
- * rank's buffer including this rank's own, e.g. from CUDA IPC / torch symmetric memory) over NVLink -- no separate
- * collective launch.  The caller brackets the call with a cross-rank barrier on both sides (buffers free / stores
- * landed) and then runs stp3_bev_discount on its own buffer.  peer_out is a HOST array of n_peers <= 8 pointers. */
-int stp3_lift_splat_frames_allgather_fwd(const float* feat, int feat_layout, const float* depth_logits,
-                                         const float* cam_M, const float* cam_t, const float* ego_R, const float* ego_t,
-                                         const float* xs, const float* ys, const float* ds,
-                                         const float* bev_off /*host[3]*/, const float* bev_res /*host[3]*/,
-                                         int nx, int ny, int nz,
-                                         int B, int S, int N, int D, int Hf, int Wf, int C,
-                                         int use_depth_distribution, int f_begin, int f_count,
-                                         void* workspace, size_t workspace_bytes,
-                                         int n_peers, void* const* peer_out, void* stream);
+ * Discount recurrence of the frame-sharded lift-splat (stp3_lift_splat_fwd with f_count > 0), after the all-gather */
 int stp3_bev_discount(const float* raw /*(B,S,nx,ny,C) fp32*/, int B, int S, int nx, int ny, int C, float discount,
                       void* out_hi, void* out_lo /*(B,S,nx,ny,C) bf16 each*/, void* stream);
 

@@ -19,7 +19,19 @@ _I = ctypes.c_int
 _F = ctypes.c_float
 _SZ = ctypes.c_size_t
 _LL = ctypes.c_longlong
-_FP = ctypes.POINTER(ctypes.c_float)
+
+
+class LiftSplatDesc(ctypes.Structure):
+    """Mirror of stp3_lift_splat_desc (include/stp3_b200.h)."""
+    _fields_ = [("cam_M", _V), ("cam_t", _V), ("ego_R", _V), ("ego_t", _V), ("xs", _V), ("ys", _V), ("ds", _V),
+                ("bev_off", _F * 3), ("bev_res", _F * 3), ("nx", _I), ("ny", _I), ("nz", _I), ("discount", _F),
+                ("B", _I), ("S", _I), ("N", _I), ("D", _I), ("Hf", _I), ("Wf", _I), ("C", _I),
+                ("feat_layout", _I), ("use_depth_distribution", _I), ("f_begin", _I), ("f_count", _I)]
+
+
+_LSD = ctypes.POINTER(LiftSplatDesc)
+
+
 class ConvDesc(ctypes.Structure):
     """Mirror of stp3_conv_desc (include/stp3_b200.h)."""
     _fields_ = [("B", _I), ("T", _I), ("H", _I), ("W", _I), ("T_total", _I), ("t0", _I), ("in_cstride", _I), ("cin_off", _I), ("cin", _I),
@@ -61,7 +73,7 @@ SIGNATURES = {
     "stp3_conv_col_sums_scratch_bytes": (_SZ, [_I, _I]),
     "stp3_build_info": (ctypes.c_char_p, []),
     "stp3_last_error": (ctypes.c_char_p, []),
-    "stp3_lift_splat_workspace_bytes": (_SZ, [_I, _I, _I, _I, _I]),
+    "stp3_lift_splat_workspace_bytes": (_SZ, [_LSD]),
     "stp3_lift_splat_workspace_init": (_I, [_V, _SZ, _V]),
     "stp3_f32_to_hilo": (_I, [_V, _I, _I, _I, _I, _I, _I, _V, _V, _V]),
     "stp3_hilo_to_f32": (_I, [_V, _V, _I, _I, _I, _I, _I, _I, _V, _V]),
@@ -69,22 +81,14 @@ SIGNATURES = {
     "stp3_pool_bias": (_I, [_V, _I, _I, _I, _I, _F, _I, _V, _I, _V, _V, _I, _V, _I, _V, _V, _I, _I, _V]),
     "stp3_small_linear": (_I, [_V, _V, _I, _I, _I, _V, _V, _I, _I, _V]),
     "stp3_upsample2x_add": (_I, [_V, _V, _I, _I, _I, _I, _V, _V, _I, _I, _V, _V, _I, _I, _I, _V]),
-    "stp3_lift_splat_frames_fwd": (_I, [_V, _I, _V, _V, _V, _V, _V, _V, _V, _V, _FP, _FP, _I, _I, _I,
-                                        _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _V, _SZ, _V, _V]),
     "stp3_block_fused_scratch_bytes": (_SZ, [_I]),
     "stp3_block_fused_fwd": (_I, [ctypes.POINTER(BlockDesc), _V, _V, _V, _V, _V, _V, _V, _V, _V, _V, _V, _V, _SZ, _V]),
     "stp3_aspp_fused_fwd": (_I, [ctypes.POINTER(AsppDesc), _V, _V, _V, _V, _V, _V, _V, _V]),
-    "stp3_lift_splat_bwd_scratch_bytes": (_SZ, [_I, _I, _I, _I, _I]),
-    "stp3_lift_splat_bwd": (_I, [_V, _V, _V, _V, _V, _V, _V, _V, _V, _V, _FP, _FP, _I, _I, _I, _F,
-                                 _I, _I, _I, _I, _I, _I, _I, _I, _V, _SZ, _V, _V, _V]),
-    "stp3_lift_splat_frames_allgather_fwd": (_I, [_V, _I, _V, _V, _V, _V, _V, _V, _V, _V, _FP, _FP, _I, _I, _I,
-                                                  _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _V, _SZ, _I,
-                                                  ctypes.POINTER(ctypes.c_void_p), _V]),
+    "stp3_lift_splat_bwd_scratch_bytes": (_SZ, [_LSD]),
+    "stp3_lift_splat_bwd": (_I, [_LSD, _V, _V, _V, _V, _SZ, _V, _V, _V]),
     "stp3_bev_discount": (_I, [_V, _I, _I, _I, _I, _I, _F, _V, _V, _V]),
     "stp3_conv_fwd": (_I, [ctypes.POINTER(ConvDesc), _V, _V, _V, _V, _V, _V, _V, _V, _V, _V, ctypes.POINTER(ConvHead), _V]),
-    "stp3_lift_splat_fwd": (_I, [_V, _I, _V, _V, _V, _V, _V, _V, _V, _V, _FP, _FP,
-                                 _I, _I, _I, _F, _I, _I, _I, _I, _I, _I, _I, _I,
-                                 _V, _V, _V, _SZ, _V, _I, _V]),
+    "stp3_lift_splat_fwd": (_I, [_LSD, _V, _V, _V, _V, _V, _SZ, _V, _I, _I, ctypes.POINTER(_V), _V]),
     # train mode of the decoder
     "stp3_conv_wgrad_scratch_bytes": (_SZ, [_I, _I, _I, _I, _I, _I, _I]),
     "stp3_conv_wgrad": (_I, [_V, _I, _I, _I, _I, _I, _V, _I, _I, _I, _I, _I, _I, _I, _I, _V, _SZ, _V, _V]),

@@ -32,6 +32,13 @@ inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
 // col_sums[img][c] = fixed-order sum of the (n_part, n_img, 64) partial rows an epilogue wrote (conv_igemm.cu)
 int launch_col_sum_reduce(const float* part, int n_part, int n_img, float* out, cudaStream_t stream);
 
+// The checks the lift-splat forward and backward share (lift_splat.cu): the descriptor with feat and depth_logits, at
+// most max_frames frames per sample.  Fills the BEV quantisation constants (lift_geom.cuh) and returns STP3_OK, or an
+// STP3_E* code with the message set; `fn` names the entry point in the null-pointer message.
+struct BevQuant;
+int check_lift_splat_desc(const char* fn, const stp3_lift_splat_desc* d, const float* feat, const float* depth_logits,
+                          int max_frames, BevQuant& q);
+
 // ---------------------------------------------------------------- launch plumbing (launch.cu)
 using TmapEncodeFn = CUresult (*)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,

@@ -1023,10 +1023,17 @@ static size_t grid_bytes(int B, int S, int C, int nx, int ny) {
 
 static size_t occ_bytes(int B, int S, int nx, int ny) { return ((size_t)B * S * nx * ny + 255) & ~(size_t)255; }
 
-extern "C" size_t stp3_lift_splat_workspace_bytes(int B, int S, int C, int nx, int ny) {
+static size_t workspace_bytes_for(int B, int S, int C, int nx, int ny) {
   if (B <= 0 || S <= 0 || C <= 0 || nx <= 0 || ny <= 0) return 0;
   const size_t part = (((size_t)B * ceil_div(nx * ny, 32) * S * C * sizeof(float)) + 255) & ~(size_t)255;
   return grid_bytes(B, S, C, nx, ny) + occ_bytes(B, S, nx, ny) + part;   // scatter grid | occupancy | pool partials
+}
+
+// frame mode lays its f_count raw frames out as f_count samples of one frame
+extern "C" size_t stp3_lift_splat_workspace_bytes(const stp3_lift_splat_desc* desc) {
+  if (!desc || desc->f_count < 0) return 0;
+  const bool raw = desc->f_count > 0;
+  return workspace_bytes_for(raw ? desc->f_count : desc->B, raw ? 1 : desc->S, desc->C, desc->nx, desc->ny);
 }
 
 extern "C" int stp3_lift_splat_workspace_init(void* workspace, size_t workspace_bytes, void* stream) {
@@ -1035,54 +1042,70 @@ extern "C" int stp3_lift_splat_workspace_init(void* workspace, size_t workspace_
   return STP3_OK;
 }
 
-// Shared implementation.  f_count < 0: the normal call (all B*S frames, discount recurrence over each sample's S
-// frames).  f_count >= 0: frame-sharded call -- only the flat frames f_begin + [0, f_count) are splatted and written
-// RAW (no recurrence), one (nx, ny, C) grid per frame; the caller all-gathers them and applies stp3_bev_discount.
-static int lift_splat_impl(const float* feat, int feat_layout, const float* depth_logits,
-                           const float* cam_M, const float* cam_t, const float* ego_R, const float* ego_t,
-                           const float* xs, const float* ys, const float* ds,
-                           const float* bev_off, const float* bev_res,
-                           int nx, int ny, int nz, float discount,
-                           int B, int S, int N, int D, int Hf, int Wf, int C,
-                           int use_depth_distribution,
-                           int32_t* ranks_out, float* pool_sum,
-                           void* workspace, size_t workspace_bytes,
-                           float* out, int out_layout, int f_begin, int f_count, void* stream_,
-                           const PeerOut* peers = nullptr) {
+int stp3::check_lift_splat_desc(const char* fn, const stp3_lift_splat_desc* d, const float* feat,
+                                const float* depth_logits, int max_frames, BevQuant& q) {
+  STP3_CHECK_ARG(d && feat && d->cam_M && d->cam_t && d->ego_R && d->ego_t && d->xs && d->ys && d->ds,
+                 "%s: null pointer argument", fn);
+  STP3_CHECK_ARG(d->use_depth_distribution == 0 || depth_logits, "depth_logits is NULL but use_depth_distribution=1");
+  STP3_CHECK_ARG(d->B > 0 && d->S > 0 && d->N > 0 && d->D > 0 && d->Hf > 0 && d->Wf > 0 && d->C > 0, "non-positive dimension");
+  STP3_CHECK_ARG(d->S <= max_frames, "receptive field S=%d exceeds the supported %d", d->S, max_frames);
+  STP3_CHECK_ARG(d->nx > 0 && d->ny > 0, "empty BEV grid");
+  STP3_CHECK_ARG(d->nz == 1, "nz=%d: the reference (stp3.py:298) and this kernel support a single height bin", d->nz);
+  STP3_CHECK_ARG((long long)d->nx * d->ny * d->nz < (1ll << 31), "BEV grid too large for int32 ranks");
+  STP3_CHECK_ARG(d->feat_layout == 0 || d->feat_layout == 1, "feat_layout must be 0 (NCHW) or 1 (NHWC)");
+  STP3_CHECK_ARG(d->f_count == 0 ? d->f_begin == 0
+                                 : d->f_begin >= 0 && d->f_count > 0 && (long long)d->f_begin + d->f_count <= (long long)d->B * d->S,
+                 "frame range outside [0, B*S)");
+  for (int i = 0; i < 3; ++i) {
+    q.off[i] = d->bev_off[i]; q.res[i] = d->bev_res[i];
+    int e = 0;
+    const float m = frexpf(d->bev_res[i], &e);       // res = m * 2^e ; power of two <=> m == 0.5
+    q.inv_ok[i] = (m == 0.5f && e > -100 && e < 100) ? 1 : 0;
+    q.inv[i] = q.inv_ok[i] ? ldexpf(1.0f, 1 - e) : 0.f;
+  }
+  q.nx = d->nx; q.ny = d->ny; q.nz = d->nz;
+  return STP3_OK;
+}
+
+// f_count == 0: all B*S frames, discount recurrence over each sample's S frames.  f_count > 0: frame-sharded call --
+// only the flat frames f_begin + [0, f_count) are splatted and written RAW (no recurrence), one (nx, ny, C) grid per
+// frame, to `out` or to every peer's gathered buffer; the caller all-gathers them and applies stp3_bev_discount.
+extern "C" int stp3_lift_splat_fwd(const stp3_lift_splat_desc* desc, const float* feat, const float* depth_logits,
+                                   int32_t* ranks_out, float* pool_sum, void* workspace, size_t workspace_bytes,
+                                   float* out, int out_layout, int n_peers, void* const* peer_out, void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  const bool raw = f_count >= 0;
-  PeerOut po;
-  po.n = 0; po.first_slot = 0;
-  for (int i = 0; i < kMaxPeers; ++i) po.ptr[i] = nullptr;
-  if (peers) po = *peers;
-  if (raw) STP3_CHECK_ARG(f_begin >= 0 && f_count > 0 && f_begin + f_count <= B * S, "frame range outside [0, B*S)");
-  const int Bw = raw ? f_count : B, Sw = raw ? 1 : S;      // shape of the scatter grid / finalize launch
-  STP3_CHECK_ARG(feat && cam_M && cam_t && ego_R && ego_t && xs && ys && ds && bev_off && bev_res && (out || po.n > 0) && workspace,
-                 "stp3_lift_splat_fwd: null pointer argument");
-  STP3_CHECK_ARG(use_depth_distribution == 0 || depth_logits, "depth_logits is NULL but use_depth_distribution=1");
-  STP3_CHECK_ARG(B > 0 && S > 0 && N > 0 && D > 0 && Hf > 0 && Wf > 0 && C > 0, "non-positive dimension");
-  STP3_CHECK_ARG(S <= kMaxFrames, "receptive field S=%d exceeds the supported %d", S, kMaxFrames);
-  STP3_CHECK_ARG(nx > 0 && ny > 0, "empty BEV grid");
-  STP3_CHECK_ARG(nz == 1, "nz=%d: the reference (stp3.py:298) and this kernel support a single height bin", nz);
-  STP3_CHECK_ARG((long long)nx * ny * nz < (1ll << 31), "BEV grid too large for int32 ranks");
-  STP3_CHECK_ARG(feat_layout == 0 || feat_layout == 1, "feat_layout must be 0 (NCHW) or 1 (NHWC)");
+  BevQuant q;
+  if (const int rc = check_lift_splat_desc("stp3_lift_splat_fwd", desc, feat, depth_logits, kMaxFrames, q)) return rc;
+  const int nx = desc->nx, ny = desc->ny, nz = desc->nz;
+  const int B = desc->B, S = desc->S, N = desc->N, D = desc->D, Hf = desc->Hf, Wf = desc->Wf, C = desc->C;
+  const int feat_layout = desc->feat_layout, use_depth_distribution = desc->use_depth_distribution;
+  const bool raw = desc->f_count > 0;
+  const float discount = raw ? 0.f : desc->discount;
+  const int Bw = raw ? desc->f_count : B, Sw = raw ? 1 : S;     // shape of the scatter grid / finalize launch
+  STP3_CHECK_ARG(n_peers >= 0 && n_peers <= kMaxPeers && (n_peers == 0 || peer_out),
+                 "n_peers must be in [0, %d], with peer_out when it is not 0", kMaxPeers);
+  STP3_CHECK_ARG((out || n_peers > 0) && workspace, "stp3_lift_splat_fwd: null pointer argument");
+  STP3_CHECK_ARG(raw || n_peers == 0, "peer outputs need frame mode (f_count > 0)");
+  STP3_CHECK_ARG(!raw || (!ranks_out && !pool_sum), "frame mode writes no ranks_out or pool_sum");
   STP3_CHECK_ARG(out_layout >= 0 && out_layout <= 2, "out_layout must be 0 (C,X,Y), 1 (X,Y,C) or 2 (bf16 hi/lo X,Y,C)");
+  STP3_CHECK_ARG(!raw || out_layout == 1, "frame mode writes fp32 channels-last frames (out_layout 1)");
+  STP3_CHECK_ARG(n_peers == 0 || C == 32 || C == 64 || C == 128,
+                 "peer outputs need C in {32, 64, 128} (channels-last finalize kernel)");
   STP3_CHECK_ARG(out_layout != 2 || C % 8 == 0, "out_layout 2 needs C %% 8 == 0");
+  PeerOut po;
+  po.n = n_peers; po.first_slot = desc->f_begin;
+  for (int i = 0; i < kMaxPeers; ++i) po.ptr[i] = i < n_peers ? static_cast<float*>(peer_out[i]) : nullptr;
+  for (int i = 0; i < n_peers; ++i)
+    STP3_CHECK_ARG(po.ptr[i] && (reinterpret_cast<uintptr_t>(po.ptr[i]) & 31) == 0, "peer buffer %d is null or not 32-byte aligned", i);
   STP3_CHECK_ARG((reinterpret_cast<uintptr_t>(workspace) & 255) == 0, "workspace must be 256-byte aligned");
-  const size_t need = stp3_lift_splat_workspace_bytes(Bw, Sw, C, nx, ny);
+  const size_t need = stp3_lift_splat_workspace_bytes(desc);
   if (workspace_bytes < need) return set_error(STP3_ENOSPC, "workspace too small: %zu < %zu", workspace_bytes, need);
 
   LiftSplatParams p;
-  p.f_begin = raw ? f_begin : 0;
-  p.feat = feat; p.depth = depth_logits; p.cam_M = cam_M; p.cam_t = cam_t; p.ego_R = ego_R; p.ego_t = ego_t;
-  p.xs = xs; p.ys = ys; p.ds = ds;
-  for (int i = 0; i < 3; ++i) {
-    p.off[i] = bev_off[i]; p.res[i] = bev_res[i];
-    int e = 0;
-    const float m = frexpf(bev_res[i], &e);          // res = m * 2^e ; power of two <=> m == 0.5
-    p.inv_ok[i] = (m == 0.5f && e > -100 && e < 100) ? 1 : 0;
-    p.inv[i] = p.inv_ok[i] ? ldexpf(1.0f, 1 - e) : 0.f;
-  }
+  p.f_begin = desc->f_begin;
+  p.feat = feat; p.depth = depth_logits; p.cam_M = desc->cam_M; p.cam_t = desc->cam_t; p.ego_R = desc->ego_R;
+  p.ego_t = desc->ego_t; p.xs = desc->xs; p.ys = desc->ys; p.ds = desc->ds;
+  for (int i = 0; i < 3; ++i) { p.off[i] = q.off[i]; p.res[i] = q.res[i]; p.inv[i] = q.inv[i]; p.inv_ok[i] = q.inv_ok[i]; }
   p.nx = nx; p.ny = ny; p.nz = nz;
   p.B = B; p.S = S; p.N = N; p.D = D; p.Hf = Hf; p.Wf = Wf; p.C = C;
   p.feat_nhwc = feat_layout; p.use_depth = use_depth_distribution;
@@ -1187,14 +1210,12 @@ static int lift_splat_impl(const float* feat, int feat_layout, const float* dept
 #define STP3_FIN_CL(LPP_, PEERS_) \
     bev_finalize_cl_kernel<LPP_, 4, PEERS_><<<cgrid, 256, 0, stream>>>(p.grid, p.occ, out, pool_part, Sw, nvox, discount, out_layout, po)
     if (po.n > 0) {
-      STP3_CHECK_ARG(out_layout == 1, "peer outputs are fp32 channels-last");
       if (C == 32) STP3_FIN_CL(2, true); else if (C == 64) STP3_FIN_CL(4, true); else STP3_FIN_CL(8, true);
     } else {
       if (C == 32) STP3_FIN_CL(2, false); else if (C == 64) STP3_FIN_CL(4, false); else STP3_FIN_CL(8, false);
     }
 #undef STP3_FIN_CL
   } else {
-    STP3_CHECK_ARG(po.n == 0, "peer outputs need C in {32, 64, 128} (channels-last finalize kernel)");
 #define STP3_FINALIZE(VEC, SMAX) \
   bev_finalize_kernel<VEC, SMAX><<<fgrid, fblock, 0, stream>>>(p.grid, p.occ, out, pool_part, Sw, C, nvox, discount, out_layout)
   if (C % 8 == 0) { if (Sw <= 4) STP3_FINALIZE(true, 4); else STP3_FINALIZE(true, 8); }
@@ -1215,56 +1236,6 @@ static int lift_splat_impl(const float* feat, int feat_layout, const float* dept
   return STP3_OK;
 }
 
-
-extern "C" int stp3_lift_splat_fwd(const float* feat, int feat_layout, const float* depth_logits,
-                                   const float* cam_M, const float* cam_t, const float* ego_R, const float* ego_t,
-                                   const float* xs, const float* ys, const float* ds,
-                                   const float* bev_off, const float* bev_res,
-                                   int nx, int ny, int nz, float discount,
-                                   int B, int S, int N, int D, int Hf, int Wf, int C,
-                                   int use_depth_distribution,
-                                   int32_t* ranks_out, float* pool_sum,
-                                   void* workspace, size_t workspace_bytes,
-                                   float* out, int out_layout, void* stream) {
-  return lift_splat_impl(feat, feat_layout, depth_logits, cam_M, cam_t, ego_R, ego_t, xs, ys, ds, bev_off, bev_res, nx, ny,
-                         nz, discount, B, S, N, D, Hf, Wf, C, use_depth_distribution, ranks_out, pool_sum, workspace,
-                         workspace_bytes, out, out_layout, 0, -1, stream);
-}
-
-extern "C" int stp3_lift_splat_frames_fwd(const float* feat, int feat_layout, const float* depth_logits,
-                                          const float* cam_M, const float* cam_t, const float* ego_R, const float* ego_t,
-                                          const float* xs, const float* ys, const float* ds,
-                                          const float* bev_off, const float* bev_res,
-                                          int nx, int ny, int nz,
-                                          int B, int S, int N, int D, int Hf, int Wf, int C,
-                                          int use_depth_distribution, int f_begin, int f_count,
-                                          void* workspace, size_t workspace_bytes, float* out_raw, void* stream) {
-  STP3_CHECK_ARG(f_count > 0, "stp3_lift_splat_frames_fwd: empty frame range");
-  return lift_splat_impl(feat, feat_layout, depth_logits, cam_M, cam_t, ego_R, ego_t, xs, ys, ds, bev_off, bev_res, nx, ny,
-                         nz, 0.f, B, S, N, D, Hf, Wf, C, use_depth_distribution, nullptr, nullptr, workspace,
-                         workspace_bytes, out_raw, 1, f_begin, f_count, stream);
-}
-
-extern "C" int stp3_lift_splat_frames_allgather_fwd(const float* feat, int feat_layout, const float* depth_logits,
-                                                    const float* cam_M, const float* cam_t, const float* ego_R, const float* ego_t,
-                                                    const float* xs, const float* ys, const float* ds,
-                                                    const float* bev_off, const float* bev_res,
-                                                    int nx, int ny, int nz,
-                                                    int B, int S, int N, int D, int Hf, int Wf, int C,
-                                                    int use_depth_distribution, int f_begin, int f_count,
-                                                    void* workspace, size_t workspace_bytes,
-                                                    int n_peers, void* const* peer_out, void* stream) {
-  STP3_CHECK_ARG(f_count > 0, "stp3_lift_splat_frames_allgather_fwd: empty frame range");
-  STP3_CHECK_ARG(n_peers >= 1 && n_peers <= kMaxPeers && peer_out, "n_peers must be in [1, %d]", kMaxPeers);
-  PeerOut po;
-  po.n = n_peers; po.first_slot = f_begin;
-  for (int i = 0; i < kMaxPeers; ++i) po.ptr[i] = i < n_peers ? static_cast<float*>(peer_out[i]) : nullptr;
-  for (int i = 0; i < n_peers; ++i)
-    STP3_CHECK_ARG(po.ptr[i] && (reinterpret_cast<uintptr_t>(po.ptr[i]) & 31) == 0, "peer buffer %d is null or not 32-byte aligned", i);
-  return lift_splat_impl(feat, feat_layout, depth_logits, cam_M, cam_t, ego_R, ego_t, xs, ys, ds, bev_off, bev_res, nx, ny,
-                         nz, 0.f, B, S, N, D, Hf, Wf, C, use_depth_distribution, nullptr, nullptr, workspace,
-                         workspace_bytes, nullptr, 1, f_begin, f_count, stream, &po);
-}
 
 namespace stp3 {
 // out[b,t] = out[b,t-1]*discount + raw[b,t] over channels-last fp32 raw splats, written as bf16 hi/lo planes

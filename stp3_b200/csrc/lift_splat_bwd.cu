@@ -245,46 +245,34 @@ lift_splat_bwd_kernel(const LiftBwdParams p) {
 
 using namespace stp3;
 
-extern "C" size_t stp3_lift_splat_bwd_scratch_bytes(int B, int S, int C, int nx, int ny) {
-  if (B <= 0 || S <= 0 || C <= 0 || nx <= 0 || ny <= 0) return 0;
-  return (size_t)B * S * nx * ny * C * sizeof(float);
+extern "C" size_t stp3_lift_splat_bwd_scratch_bytes(const stp3_lift_splat_desc* d) {
+  if (!d || d->B <= 0 || d->S <= 0 || d->C <= 0 || d->nx <= 0 || d->ny <= 0) return 0;
+  return (size_t)d->B * d->S * d->nx * d->ny * d->C * sizeof(float);
 }
 
-extern "C" int stp3_lift_splat_bwd(const float* grad_out, const float* feat, const float* depth_logits,
-                                   const float* cam_M, const float* cam_t, const float* ego_R, const float* ego_t,
-                                   const float* xs, const float* ys, const float* ds,
-                                   const float* bev_off, const float* bev_res, int nx, int ny, int nz, float discount,
-                                   int B, int S, int N, int D, int Hf, int Wf, int C, int use_depth_distribution,
-                                   void* scratch, size_t scratch_bytes, float* grad_feat, float* grad_depth_logits,
-                                   void* stream_) {
+extern "C" int stp3_lift_splat_bwd(const stp3_lift_splat_desc* desc, const float* grad_out, const float* feat,
+                                   const float* depth_logits, void* scratch, size_t scratch_bytes, float* grad_feat,
+                                   float* grad_depth_logits, void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  STP3_CHECK_ARG(grad_out && feat && cam_M && cam_t && ego_R && ego_t && xs && ys && ds && bev_off && bev_res && scratch &&
-                 grad_feat, "stp3_lift_splat_bwd: null pointer argument");
-  STP3_CHECK_ARG(use_depth_distribution == 0 || depth_logits, "depth_logits is NULL but use_depth_distribution=1");
-  STP3_CHECK_ARG(B > 0 && S > 0 && N > 0 && D > 0 && Hf > 0 && Wf > 0 && C > 0 && nx > 0 && ny > 0, "non-positive dimension");
-  STP3_CHECK_ARG(S <= kBwdMaxFrames, "receptive field S=%d exceeds the supported %d", S, kBwdMaxFrames);
-  STP3_CHECK_ARG(nz == 1, "nz=%d: a single height bin is supported (stp3.py:298)", nz);
-  const size_t need = stp3_lift_splat_bwd_scratch_bytes(B, S, C, nx, ny);
+  LiftBwdParams p;
+  if (const int rc = check_lift_splat_desc("stp3_lift_splat_bwd", desc, feat, depth_logits, kBwdMaxFrames, p.q)) return rc;
+  STP3_CHECK_ARG(grad_out && scratch && grad_feat, "stp3_lift_splat_bwd: null pointer argument");
+  STP3_CHECK_ARG(desc->feat_layout == 0, "stp3_lift_splat_bwd: feat must be NCHW (feat_layout 0)");
+  STP3_CHECK_ARG(desc->f_count == 0, "stp3_lift_splat_bwd: every frame is processed (f_count 0)");
+  const int B = desc->B, S = desc->S, N = desc->N, D = desc->D, Hf = desc->Hf, Wf = desc->Wf, C = desc->C;
+  const size_t need = stp3_lift_splat_bwd_scratch_bytes(desc);
   if (scratch_bytes < need) return set_error(STP3_ENOSPC, "scratch too small: %zu < %zu", scratch_bytes, need);
-  const int nvox = nx * ny * nz;
+  const int nvox = desc->nx * desc->ny * desc->nz;
 
   dim3 g1(ceil_div(nvox, 32), ceil_div(C, 32), B);
-  bev_grad_to_grid_kernel<<<g1, dim3(32, 8), 0, stream>>>(grad_out, static_cast<float*>(scratch), S, C, nvox, discount);
+  bev_grad_to_grid_kernel<<<g1, dim3(32, 8), 0, stream>>>(grad_out, static_cast<float*>(scratch), S, C, nvox,
+                                                          desc->discount);
   STP3_CUDA_OK(cudaGetLastError());
 
-  LiftBwdParams p;
-  p.feat = feat; p.depth = depth_logits; p.cam_M = cam_M; p.cam_t = cam_t; p.ego_R = ego_R; p.ego_t = ego_t;
-  p.xs = xs; p.ys = ys; p.ds = ds;
-  for (int i = 0; i < 3; ++i) {
-    p.q.off[i] = bev_off[i]; p.q.res[i] = bev_res[i];
-    int e = 0;
-    const float m = frexpf(bev_res[i], &e);
-    p.q.inv_ok[i] = (m == 0.5f && e > -100 && e < 100) ? 1 : 0;
-    p.q.inv[i] = p.q.inv_ok[i] ? ldexpf(1.0f, 1 - e) : 0.f;
-  }
-  p.q.nx = nx; p.q.ny = ny; p.q.nz = nz;
+  p.feat = feat; p.depth = depth_logits; p.cam_M = desc->cam_M; p.cam_t = desc->cam_t; p.ego_R = desc->ego_R;
+  p.ego_t = desc->ego_t; p.xs = desc->xs; p.ys = desc->ys; p.ds = desc->ds;
   p.B = B; p.S = S; p.N = N; p.D = D; p.Hf = Hf; p.Wf = Wf; p.C = C;
-  p.use_depth = use_depth_distribution;
+  p.use_depth = desc->use_depth_distribution;
   p.tiles_w = ceil_div(Wf, kBwdTW);
   p.ggrid = static_cast<const float*>(scratch);
   p.gfeat = grad_feat; p.gdepth = grad_depth_logits;

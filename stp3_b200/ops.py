@@ -46,6 +46,56 @@ class Workspace:
 _default_ws = Workspace()
 
 
+def _ptr(t: Optional[torch.Tensor]):
+    return t.data_ptr() if t is not None else None
+
+
+def _lift_desc(feat, depth_logits, cam_M, cam_t, ego_R, ego_t, xs, ys, ds, bev_off, bev_res, bev_dim, discount=0.0,
+               feat_channels_last=False, use_depth_distribution=True, f_begin=0, f_count=0):
+    """What every lift-splat call shares: the shapes, fp32 contiguous inputs on feat's device, the shape checks and the
+    stp3_lift_splat_desc (include/stp3_b200.h).  Returns (desc, feat, depth_logits); desc.keep holds the geometry
+    tensors the descriptor points into, so they live as long as it does."""
+    _require_cuda(feat, depth_logits)
+    dev = feat.device
+    if feat_channels_last:
+        B, S, N, Hf, Wf, C = feat.shape
+    else:
+        B, S, N, C, Hf, Wf = feat.shape
+    D = ds.numel()
+    nx, ny, nz = (int(v) for v in bev_dim)
+    feat = _f32c(feat)
+    depth_logits = _f32c(depth_logits) if depth_logits is not None else None
+    if use_depth_distribution:
+        assert depth_logits is not None and tuple(depth_logits.shape) == (B, S, N, D, Hf, Wf), "depth_logits shape"
+    geom = [_f32c(t.to(dev)) for t in (cam_M, cam_t, ego_R, ego_t, xs, ys, ds)]
+    cam_M, cam_t, ego_R, ego_t, xs, ys, _ = geom
+    assert cam_M.shape == (B, S, N, 3, 3) and cam_t.shape == (B, S, N, 3)
+    assert ego_R.shape == (B, S, 3, 3) and ego_t.shape == (B, S, 3)
+    assert xs.numel() == Wf and ys.numel() == Hf
+    desc = _lib.LiftSplatDesc(*(t.data_ptr() for t in geom), _host3(bev_off), _host3(bev_res), nx, ny, nz,
+                              float(discount), B, S, N, D, Hf, Wf, C, int(feat_channels_last),
+                              int(use_depth_distribution), int(f_begin), int(f_count))
+    desc.keep = geom
+    return desc, feat, depth_logits
+
+
+def _lift_fwd(desc, feat, depth_logits, workspace: Optional[Workspace], out, out_layout: int, ranks=None, psum=None,
+              peer_ptrs=None):
+    """stp3_lift_splat_fwd on the current stream; the workspace is re-initialised when the call fails."""
+    L = _lib.lib()
+    dev = feat.device
+    workspace = workspace or _default_ws
+    ws = workspace.get(L.stp3_lift_splat_workspace_bytes(desc), dev)
+    peers = (ctypes.c_void_p * len(peer_ptrs))(*[int(x) for x in peer_ptrs]) if peer_ptrs is not None else None
+    with torch.cuda.device(dev):
+        code = L.stp3_lift_splat_fwd(desc, feat.data_ptr(), _ptr(depth_logits), _ptr(ranks), _ptr(psum), ws.data_ptr(),
+                                     ws.numel(), _ptr(out), out_layout, len(peer_ptrs or ()), peers,
+                                     torch.cuda.current_stream(dev).cuda_stream)
+    if code != 0:
+        workspace.reset()
+    _lib.check(code, "stp3_lift_splat_fwd")
+
+
 def lift_splat(feat, depth_logits, cam_M, cam_t, ego_R, ego_t, xs, ys, ds, bev_off, bev_res, bev_dim,
                discount: float, *, feat_channels_last: bool = False, out_channels_last: bool = False,
                use_depth_distribution: bool = True, return_ranks: bool = False, pool_sum: bool = False,
@@ -59,26 +109,10 @@ def lift_splat(feat, depth_logits, cam_M, cam_t, ego_R, ego_t, xs, ys, ds, bev_o
       bev_off, bev_res (3,) float (host values); bev_dim (3,) int
     Returns out (B,S,C,X,Y) [or (B,S,X,Y,C)], and optionally ranks (B,S,N,D,Hf,Wf) int32 and pool sums (B,S,C).
     Semantics: stp3/models/stp3.py:186-301 of the reference."""
-    _require_cuda(feat, depth_logits)
+    desc, feat, depth_logits = _lift_desc(feat, depth_logits, cam_M, cam_t, ego_R, ego_t, xs, ys, ds, bev_off, bev_res,
+                                          bev_dim, discount, feat_channels_last, use_depth_distribution)
     dev = feat.device
-    if feat_channels_last:
-        B, S, N, Hf, Wf, C = feat.shape
-    else:
-        B, S, N, C, Hf, Wf = feat.shape
-    D = ds.numel()
-    nx, ny, nz = (int(v) for v in bev_dim)
-    feat = _f32c(feat)
-    depth_logits = _f32c(depth_logits) if depth_logits is not None else None
-    if use_depth_distribution:
-        assert depth_logits is not None and tuple(depth_logits.shape) == (B, S, N, D, Hf, Wf), "depth_logits shape"
-    cam_M, cam_t, ego_R, ego_t = (_f32c(t.to(dev)) for t in (cam_M, cam_t, ego_R, ego_t))
-    xs, ys, ds = (_f32c(t.to(dev)) for t in (xs, ys, ds))
-    assert cam_M.shape == (B, S, N, 3, 3) and cam_t.shape == (B, S, N, 3)
-    assert ego_R.shape == (B, S, 3, 3) and ego_t.shape == (B, S, 3)
-    assert xs.numel() == Wf and ys.numel() == Hf
-    L = _lib.lib()
-    need = L.stp3_lift_splat_workspace_bytes(B, S, C, nx, ny)
-    ws = (workspace or _default_ws).get(need, dev)
+    B, S, C, nx, ny = desc.B, desc.S, desc.C, desc.nx, desc.ny
     oshape = (B, S, nx, ny, C) if out_channels_last else (B, S, C, nx, ny)
     layout = int(out_channels_last)
     if out_hilo is not None:      # two bf16 planes (2,B,S,nx,ny,C): the activation format of the tensor-core path
@@ -88,20 +122,9 @@ def lift_splat(feat, depth_logits, cam_M, cam_t, ego_R, ego_t, xs, ys, ds, bev_o
         out = torch.empty(oshape, dtype=torch.float32, device=dev)
     else:
         assert tuple(out.shape) == oshape and out.is_contiguous() and out.dtype == torch.float32
-    ranks = torch.empty((B, S, N, D, Hf, Wf), dtype=torch.int32, device=dev) if return_ranks else None
+    ranks = torch.empty((B, S, desc.N, desc.D, desc.Hf, desc.Wf), dtype=torch.int32, device=dev) if return_ranks else None
     psum = torch.zeros((B, S, C), dtype=torch.float32, device=dev) if pool_sum else None
-    stream = torch.cuda.current_stream(dev).cuda_stream
-    with torch.cuda.device(dev):
-        code = L.stp3_lift_splat_fwd(
-            feat.data_ptr(), int(feat_channels_last), depth_logits.data_ptr() if depth_logits is not None else None,
-            cam_M.data_ptr(), cam_t.data_ptr(), ego_R.data_ptr(), ego_t.data_ptr(),
-            xs.data_ptr(), ys.data_ptr(), ds.data_ptr(), _host3(bev_off), _host3(bev_res),
-            nx, ny, nz, float(discount), B, S, N, D, Hf, Wf, C, int(use_depth_distribution),
-            ranks.data_ptr() if ranks is not None else None, psum.data_ptr() if psum is not None else None,
-            ws.data_ptr(), ws.numel(), out.data_ptr(), layout, stream)
-    if code != 0:
-        (workspace or _default_ws).reset()
-    _lib.check(code, "stp3_lift_splat_fwd")
+    _lift_fwd(desc, feat, depth_logits, workspace, out, layout, ranks=ranks, psum=psum)
     res = (out,)
     if return_ranks:
         res += (ranks,)
@@ -114,29 +137,19 @@ def lift_splat_backward(grad_out, feat, depth_logits, cam_M, cam_t, ego_R, ego_t
                         discount: float, *, use_depth_distribution: bool = True):
     """Gradients of lift_splat()'s (B,S,C,X,Y) output w.r.t. feat (B,S,N,C,Hf,Wf) and depth_logits (B,S,N,D,Hf,Wf):
     stp3_lift_splat_bwd (include/stp3_b200.h).  Returns (grad_feat, grad_depth_logits or None)."""
-    _require_cuda(feat, depth_logits)
+    desc, feat, depth_logits = _lift_desc(feat, depth_logits, cam_M, cam_t, ego_R, ego_t, xs, ys, ds, bev_off, bev_res,
+                                          bev_dim, discount, use_depth_distribution=use_depth_distribution)
     dev = feat.device
-    B, S, N, C, Hf, Wf = feat.shape
-    D = ds.numel()
-    nx, ny, nz = (int(v) for v in bev_dim)
     grad_out = _f32c(grad_out)
-    assert tuple(grad_out.shape) == (B, S, C, nx, ny)
-    feat = _f32c(feat)
-    depth_logits = _f32c(depth_logits) if depth_logits is not None else None
-    cam_M, cam_t, ego_R, ego_t = (_f32c(t.to(dev)) for t in (cam_M, cam_t, ego_R, ego_t))
-    xs, ys, ds = (_f32c(t.to(dev)) for t in (xs, ys, ds))
+    assert tuple(grad_out.shape) == (desc.B, desc.S, desc.C, desc.nx, desc.ny)
     L = _lib.lib()
-    nbytes = L.stp3_lift_splat_bwd_scratch_bytes(B, S, C, nx, ny)
+    nbytes = L.stp3_lift_splat_bwd_scratch_bytes(desc)
     scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
     g_feat = torch.empty_like(feat)
     g_depth = torch.empty_like(depth_logits) if (use_depth_distribution and depth_logits is not None) else None
     with torch.cuda.device(dev):
-        code = L.stp3_lift_splat_bwd(
-            grad_out.data_ptr(), feat.data_ptr(), depth_logits.data_ptr() if depth_logits is not None else None,
-            cam_M.data_ptr(), cam_t.data_ptr(), ego_R.data_ptr(), ego_t.data_ptr(), xs.data_ptr(), ys.data_ptr(),
-            ds.data_ptr(), _host3(bev_off), _host3(bev_res), nx, ny, nz, float(discount), B, S, N, D, Hf, Wf, C,
-            int(use_depth_distribution), scratch.data_ptr(), nbytes, g_feat.data_ptr(),
-            g_depth.data_ptr() if g_depth is not None else None, torch.cuda.current_stream(dev).cuda_stream)
+        code = L.stp3_lift_splat_bwd(desc, grad_out.data_ptr(), feat.data_ptr(), _ptr(depth_logits), scratch.data_ptr(),
+                                     nbytes, g_feat.data_ptr(), _ptr(g_depth), torch.cuda.current_stream(dev).cuda_stream)
     _lib.check(code, "stp3_lift_splat_bwd")
     return g_feat, g_depth
 
@@ -178,48 +191,17 @@ def lift_splat_frames(feat, depth_logits, cam_M, cam_t, ego_R, ego_t, xs, ys, ds
                       use_depth_distribution: bool = True, workspace: Optional[Workspace] = None,
                       peer_ptrs=None) -> Optional[torch.Tensor]:
     """Frame-sharded lift-splat: RAW (no discount recurrence) channels-last splats (f_count, X, Y, C) fp32 of the flat
-    frames f_begin + [0, f_count), f = b*S + t.  See stp3_lift_splat_frames_fwd in include/stp3_b200.h.
-    peer_ptrs (list of device pointers, one (B*S, X, Y, C) fp32 buffer per rank): the finalize epilogue stores the frames
-    into slot f of every rank's buffer instead (stp3_lift_splat_frames_allgather_fwd); returns None."""
-    _require_cuda(feat, depth_logits)
-    dev = feat.device
-    if feat_channels_last:
-        B, S, N, Hf, Wf, C = feat.shape
-    else:
-        B, S, N, C, Hf, Wf = feat.shape
-    D = ds.numel()
-    nx, ny, nz = (int(v) for v in bev_dim)
-    feat = _f32c(feat)
-    depth_logits = _f32c(depth_logits) if depth_logits is not None else None
-    cam_M, cam_t, ego_R, ego_t = (_f32c(t.to(dev)) for t in (cam_M, cam_t, ego_R, ego_t))
-    xs, ys, ds = (_f32c(t.to(dev)) for t in (xs, ys, ds))
-    L = _lib.lib()
-    need = L.stp3_lift_splat_workspace_bytes(f_count, 1, C, nx, ny)
-    ws = (workspace or _default_ws).get(need, dev)
-    if peer_ptrs is not None:
-        arr = (ctypes.c_void_p * len(peer_ptrs))(*[int(x) for x in peer_ptrs])
-        with torch.cuda.device(dev):
-            code = L.stp3_lift_splat_frames_allgather_fwd(
-                feat.data_ptr(), int(feat_channels_last), depth_logits.data_ptr() if depth_logits is not None else None,
-                cam_M.data_ptr(), cam_t.data_ptr(), ego_R.data_ptr(), ego_t.data_ptr(), xs.data_ptr(), ys.data_ptr(),
-                ds.data_ptr(), _host3(bev_off), _host3(bev_res), nx, ny, nz, B, S, N, D, Hf, Wf, C,
-                int(use_depth_distribution), int(f_begin), int(f_count), ws.data_ptr(), ws.numel(), len(peer_ptrs), arr,
-                torch.cuda.current_stream(dev).cuda_stream)
-        if code != 0:
-            (workspace or _default_ws).reset()
-        _lib.check(code, "stp3_lift_splat_frames_allgather_fwd")
-        return None
-    out = torch.empty((f_count, nx, ny, C), dtype=torch.float32, device=dev)
-    with torch.cuda.device(dev):
-        code = L.stp3_lift_splat_frames_fwd(
-            feat.data_ptr(), int(feat_channels_last), depth_logits.data_ptr() if depth_logits is not None else None,
-            cam_M.data_ptr(), cam_t.data_ptr(), ego_R.data_ptr(), ego_t.data_ptr(), xs.data_ptr(), ys.data_ptr(),
-            ds.data_ptr(), _host3(bev_off), _host3(bev_res), nx, ny, nz, B, S, N, D, Hf, Wf, C,
-            int(use_depth_distribution), int(f_begin), int(f_count), ws.data_ptr(), ws.numel(), out.data_ptr(),
-            torch.cuda.current_stream(dev).cuda_stream)
-    if code != 0:
-        (workspace or _default_ws).reset()
-    _lib.check(code, "stp3_lift_splat_frames_fwd")
+    frames f_begin + [0, f_count), f = b*S + t.  See the frame-sharded mode of stp3_lift_splat_fwd in
+    include/stp3_b200.h.  peer_ptrs (list of device pointers, one (B*S, X, Y, C) fp32 buffer per rank): the finalize
+    epilogue stores the frames into slot f of every rank's buffer instead; returns None."""
+    if f_count <= 0:        # f_count == 0 would describe the unsharded call
+        raise RuntimeError(f"lift_splat_frames: empty frame range (f_count={f_count})")
+    desc, feat, depth_logits = _lift_desc(feat, depth_logits, cam_M, cam_t, ego_R, ego_t, xs, ys, ds, bev_off, bev_res,
+                                          bev_dim, 0.0, feat_channels_last, use_depth_distribution, f_begin, f_count)
+    out = None
+    if peer_ptrs is None:
+        out = torch.empty((f_count, desc.nx, desc.ny, desc.C), dtype=torch.float32, device=feat.device)
+    _lift_fwd(desc, feat, depth_logits, workspace, out, 1, peer_ptrs=peer_ptrs)
     return out
 
 

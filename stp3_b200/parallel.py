@@ -82,7 +82,7 @@ def all_gather_frames(local: torch.Tensor, n_frames: int) -> torch.Tensor:
 class PeerFrameBuffer:
     """Every rank's (n_frames, X, Y, C) fp32 gather buffer in symmetric memory (torch.distributed._symmetric_memory: CUDA
     peer mappings over NVLink), so that the frame-sharded lift-splat can store its frames into all ranks' buffers from
-    its own epilogue (stp3_lift_splat_frames_allgather_fwd) instead of running a separate all-gather.
+    its own epilogue (stp3_lift_splat_fwd with n_peers > 0) instead of running a separate all-gather.
     barrier() = device-side cross-rank barrier on the current stream (signal pads of the symmetric allocation)."""
 
     def __init__(self, n_frames: int, X: int, Y: int, C: int, device, group=None):

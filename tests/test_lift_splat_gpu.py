@@ -209,3 +209,25 @@ def test_frame_sharded_raw_splats_plus_discount_equal_fused_path():
     planes = ops.bev_discount(rawp, cfg.discount)
     got = (planes[0].float() + planes[1].float())[..., :C]
     assert (got - ref).abs().max() <= 2e-5 * ref.abs().max()
+
+
+def test_frame_sharded_peer_stores_land_in_their_slots():
+    """The all-gather fused into the finalize epilogue (peer_ptrs), with this device's own buffer as the only peer: the
+    frames f_begin + [0, f_count) of each of two 'ranks' land in their slots and equal the raw splats of the same range."""
+    from stp3_b200 import parallel
+    dev = torch.device("cuda:0")
+    lcfg = syn.LiftSplatConfig(x_bound=(-8.0, 8.0, 0.5), y_bound=(-8.0, 8.0, 0.5), d_bound=(2.0, 10.0, 1.0),
+                               final_dim=(32, 48), out_channels=64, n_cameras=2, receptive_field=3)
+    inp = syn.lift_inputs(lcfg, 2, seed=7, random_pose=True)
+    mats = G.lift_matrices(inp["intrinsics"], inp["extrinsics"], inp["future_egomotion"])
+    res, start, dim = G.calculate_birds_eye_view_parameters(lcfg.x_bound, lcfg.y_bound, lcfg.z_bound)
+    args = (inp["feat"].to(dev), inp["depth_logits"].to(dev), *mats,
+            *G.frustum_axes(lcfg.final_dim, lcfg.downsample, lcfg.d_bound), G.bev_offset(start, res), res, dim)
+    B, S, C = inp["feat"].shape[0], inp["feat"].shape[1], inp["feat"].shape[3]
+    gathered = torch.full((B * S, int(dim[0]), int(dim[1]), C), float("nan"), device=dev)
+    for r in range(2):
+        f0, fc = parallel.shard_batch(B * S, r, 2)
+        assert ops.lift_splat_frames(*args, f0, fc, peer_ptrs=[gathered.data_ptr()]) is None
+        raw = ops.lift_splat_frames(*args, f0, fc)
+        assert torch.allclose(gathered[f0:f0 + fc], raw, rtol=1e-5, atol=1e-6 * float(raw.abs().max()))
+    assert not gathered.isnan().any()
