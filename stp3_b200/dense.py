@@ -150,12 +150,20 @@ _AUTOTUNE = _os.environ.get("STP3_CONV_AUTOTUNE", "1") != "0"
 TUNE_LOG = []      # (description, {config: ms}) for reports
 
 
-def _tune(key, desc, launch, groupable, ntaps=1, bn=0):
+def tune_candidates(pc: PackedConv) -> List[Tuple[int, int]]:
+    """The (n_sub, group) tilings the autotuner times for this packed convolution."""
+    taps = pc.taps
+    groupable = any(taps[i + 1][0] == taps[i][0] and taps[i + 1][2] == taps[i][2] and
+                    taps[i + 1][1] == taps[i][1] + pc.stride for i in range(len(taps) - 1))
     cands = [(1, 1)] + ([(1, 3)] if groupable else [])
-    if ntaps > 1:       # weights streamed through the ring instead of resident: more activation stages in flight
+    if len(taps) > 1:   # weights streamed through the ring instead of resident: more activation stages in flight
         cands += [(ns, g + 4) for ns, g in cands]
-    if bn == 64:        # stacked [W_hi; W_lo] operand: two MMAs per product instead of three
+    if pc.bn == 64:     # stacked [W_hi; W_lo] operand: two MMAs per product instead of three
         cands += [(ns, g + 8) for ns, g in cands]
+    return cands
+
+
+def _tune(key, desc, launch, cands):
     times = {}
     for ns, g in cands:
         launch(ns, g)                                   # warm (descriptor / attribute setup)
@@ -253,15 +261,12 @@ def conv(x: HL, pc: PackedConv, *, cin_off: int = 0, out: Optional[HL] = None, o
            hd is not None, out2 is not None)
     cfg = tune if tune is not None else _TUNED.get(key)
     if cfg is None and _AUTOTUNE and not torch.cuda.is_current_stream_capturing():
-        taps = pc.taps
-        groupable = any(taps[i + 1][0] == taps[i][0] and taps[i + 1][2] == taps[i][2] and
-                        taps[i + 1][1] == taps[i][1] + pc.stride for i in range(len(taps) - 1))
-        desc = f"{len(taps)}tap cin{pc.cin_p} bn{pc.bn} s{pc.stride} {B * T}x{Ho}x{Wo}"
+        desc = f"{len(pc.taps)}tap cin{pc.cin_p} bn{pc.bn} s{pc.stride} {B * T}x{Ho}x{Wo}"
         # the tuner launches the layer many times: an output that aliases an input would be corrupted silently
         ins = {x.hi.data_ptr(), x.lo.data_ptr()} | ({residual.hi.data_ptr(), residual.lo.data_ptr()} if residual is not None else set())
         outs = {t.data_ptr() for t in ((out.hi, out.lo) if out is not None else ()) + ((out2.hi, out2.lo) if out2 is not None else ())}
         assert not (ins & outs), "stp3_b200.dense.conv: output aliases an input (in-place convolution is not supported)"
-        cfg = _tune(key, desc, launch, groupable, len(taps), pc.bn)
+        cfg = _tune(key, desc, launch, tune_candidates(pc))
     launch(*(cfg or (0, 0)))
     return out
 
