@@ -195,6 +195,11 @@ typedef struct stp3_conv_desc {
   int f32_layout;        /* layout of y_f32: 0 = (B*T, n_valid, Ho, Wo) like the reference, 1 = channels-last (B*T, Ho, Wo,
                             n_valid) -- what stp3_lift_splat_fwd(feat_layout = 1) fetches as ONE TMA box per tile (the encoder
                             heads hand their context features over this way, encoder.py:88-95 -> stp3.py:216) */
+  int swish;             /* apply swish x * sigmoid(x) to y_hi / y_lo instead of ReLU (EfficientNet expand convolutions);
+                            not with relu or a second destination */
+  long long w_img_stride; /* 0: one weight tensor for every image; > 0: image i's weights start at w + i * w_img_stride
+                            (bf16 elements, a multiple of 64) -- the squeeze-excite gated projections (stp3_se_gate).  Such
+                            weights are streamed through the shared-memory ring, never resident */
 } stp3_conv_desc;
 
 /* Optional fused 1x1 "head" evaluated on the activated output tile while it is still in registers:
@@ -360,6 +365,40 @@ int stp3_phase_interleave(const float* p00, const float* p01, const float* p10, 
                           int C, float* out, void* stream);
 /* dz = g * s * (1 - s), s = sigmoid(z) the forward output (instance_center head, decoder.py:70) */
 int stp3_sigmoid_bwd(const float* g, const float* s, long long n, float* dz, void* stream);
+
+/* ---------------------------------------------------------------------------------------------------------
+ * EfficientNet trunk (efficientnet-pytorch 0.7.0, truncated like stp3/models/encoder.py:39-55).  The 1x1 expand and
+ * projection convolutions of an MBConv block are stp3_conv_fwd calls (swish, per-image weights); these are the rest.
+ * Static "same" padding: pad_t / pad_l are the top / left pads computed for the model's nominal image size; inputs
+ * outside the image read as zero, which is the bottom / right pad.  BatchNorm (eps 1e-3) is folded by the caller.
+ *
+ * Stem: fp32 NCHW images (n_img, 3, H, W) -> 3x3 stride-2 conv (w [cout][3][3][3], bias [cout]) + swish -> hi/lo planes
+ * (n_img, Ho, Wo, out_cstride); channels [cout, out_cstride) are written as zeros.  cout <= 64. */
+int stp3_effnet_stem(const float* x, int n_img, int H, int W, int Ho, int Wo, int pad_t, int pad_l, const float* w,
+                     const float* bias, int cout, int out_cstride, void* y_hi, void* y_lo, void* stream);
+/* Depthwise k x k convolution (k 3 or 5, stride 1 or 2) + folded BN + swish on hi/lo planes, channels [0, C) of
+ * x (n_img, H, W, in_cstride) -> y (n_img, Ho, Wo, out_cstride); other channels of y are not touched.  w [k*k][C] fp32,
+ * bias [C].  sums (optional, (n_img, C) fp32): per-(image, channel) sums of the activated output -- the squeeze-excite
+ * means -- through stp3_dw_sums_scratch_bytes(desc) bytes of scratch and a fixed-order reduction (bitwise repeatable). */
+typedef struct stp3_dw_desc {
+  int n_img, H, W, Ho, Wo;
+  int k, stride, pad_t, pad_l;
+  int C;                 /* multiple of 8; padding channels with zero weights and bias come out zero */
+  int in_cstride, out_cstride;   /* multiples of 64 */
+} stp3_dw_desc;
+size_t stp3_dw_sums_scratch_bytes(const stp3_dw_desc* desc);
+int stp3_dw_fwd(const stp3_dw_desc* desc, const void* x_hi, const void* x_lo, const float* w, const float* bias,
+                void* y_hi, void* y_lo, float* sums, void* scratch, size_t scratch_bytes, void* stream);
+/* Squeeze-excite gate of every image, gate = sigmoid(w_e . swish(w_r . (sums * inv_hw) + b_r) + b_e) (w_r [R][C],
+ * w_e [C][R]), folded into per-image projection weights w_img = W_proj . diag(gate) (w_proj [cout][C] fp32, BN folded)
+ * in the packed hi/lo layout of stp3_conv_fwd: per image stp3_se_proj_weight_elems(C, cout) bf16 elements holding column
+ * chunks of 128 output channels (the last one 64 or 128 rows wide, zero padded), chunk j at the offset of the chunks
+ * before it, each [C/64 rounded up][2][bn_j][64].  gate (n_img, C) fp32 receives the gate (computed once per image by a
+ * first kernel; a second one scales the weights). */
+long long stp3_se_proj_weight_elems(int cin, int cout);
+int stp3_se_gate(const float* sums, int sums_stride, int n_img, int C, float inv_hw, const float* w_r, const float* b_r,
+                 int R, const float* w_e, const float* b_e, const float* w_proj, int cout, float* gate, void* w_img,
+                 void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------
  * Discount recurrence of the frame-sharded lift-splat (stp3_lift_splat_fwd with f_count > 0), after the all-gather */

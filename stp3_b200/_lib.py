@@ -40,7 +40,13 @@ class ConvDesc(ctypes.Structure):
                 ("res_cstride", _I), ("res_coff", _I), ("n_valid", _I), ("sigmoid", _I), ("tune_n_sub", _I), ("tune_group", _I),
                 ("n_cols", _I), ("col_sums", _V), ("col_sums_scratch", _V), ("col_sums_scratch_bytes", _SZ),
                 ("y2_hi", _V), ("y2_lo", _V), ("out2_cstride", _I), ("out2_coff", _I), ("n_store2", _I), ("relu2", _I),
-                ("k_lo", _I), ("k_hi", _I), ("f32_layout", _I)]
+                ("k_lo", _I), ("k_hi", _I), ("f32_layout", _I), ("swish", _I), ("w_img_stride", _LL)]
+
+
+class DwDesc(ctypes.Structure):
+    """Mirror of stp3_dw_desc (include/stp3_b200.h)."""
+    _fields_ = [("n_img", _I), ("H", _I), ("W", _I), ("Ho", _I), ("Wo", _I), ("k", _I), ("stride", _I), ("pad_t", _I),
+                ("pad_l", _I), ("C", _I), ("in_cstride", _I), ("out_cstride", _I)]
 
 
 class AsppDesc(ctypes.Structure):
@@ -101,6 +107,12 @@ SIGNATURES = {
     "stp3_upsample2x_bwd": (_I, [_V, _I, _I, _I, _I, _V, _V]),
     "stp3_phase_interleave": (_I, [_V, _V, _V, _V, _I, _I, _I, _I, _V, _V]),
     "stp3_sigmoid_bwd": (_I, [_V, _V, _LL, _V, _V]),
+    # EfficientNet trunk
+    "stp3_effnet_stem": (_I, [_V, _I, _I, _I, _I, _I, _I, _I, _V, _V, _I, _I, _V, _V, _V]),
+    "stp3_dw_sums_scratch_bytes": (_SZ, [ctypes.POINTER(DwDesc)]),
+    "stp3_dw_fwd": (_I, [ctypes.POINTER(DwDesc), _V, _V, _V, _V, _V, _V, _V, _V, _SZ, _V]),
+    "stp3_se_proj_weight_elems": (_LL, [_I, _I]),
+    "stp3_se_gate": (_I, [_V, _I, _I, _I, _F, _V, _V, _I, _V, _V, _V, _I, _V, _V, _V]),
 }
 
 

@@ -102,6 +102,8 @@ struct ConvParams {
   // warp keeps running sums of its pixels in registers and writes one partial row per (CTA, row quarter, image) --
   // plain stores, fixed order: deterministic.  BN = 64 only.  sum_part: [gridDim.x][4][n_img][BN], zeroed by the host.
   float* sum_part;
+  int swish;                // swish instead of ReLU on the primary destination (EfficientNet expand convolutions)
+  long long w_img_rows;     // > 0: per-image weights, image i's blocks start w_img_rows rows further (streamed only)
 };
 
 // STACK (BN = 64 only): the hi and lo weight planes of a K step form ONE B operand of 2*BN rows, so a product is two
@@ -210,14 +212,14 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
   if (warp == kEpiWarps) {
     // ===================== TMA producer (whole warp walks the loops; one elected lane issues) =====================
     // load_b: the weight tile of K step `it` into `dst` (called by the elected lane; transaction bytes on `bar`)
-    auto load_b = [&](unsigned char* dst, int it, uint64_t* bar) {
-      const int row_hi = (it * 2) * p.w_rows + p.w_row_off, row_lo = row_hi + p.w_rows;
+    auto load_b = [&](unsigned char* dst, int it, uint64_t* bar, int img_w) {
+      const int row_hi = (int)((it * 2) * p.w_rows + p.w_row_off + img_w * p.w_img_rows), row_lo = row_hi + p.w_rows;
       ptx::tma_load_2d(dst, &tm_w, bar, 0, row_hi);                       // [W_hi; W_lo], also the stacked operand
       ptx::tma_load_2d(dst + kBRows * kBK * 2, &tm_w, bar, 0, row_lo);
     };
     if (resident && ptx::elect_one_sync()) {
       ptx::mbar_arrive_expect_tx(bres_bar, (uint32_t)(k_iters * p.b_load_bytes));
-      for (int it = 0; it < k_iters; ++it) load_b(b_ring + (size_t)it * p.b_tile_bytes, it, bres_bar);
+      for (int it = 0; it < k_iters; ++it) load_b(b_ring + (size_t)it * p.b_tile_bytes, it, bres_bar, 0);
     }
     __syncwarp();
     ptx::griddep_wait();                        // activations come from the preceding kernel
@@ -242,7 +244,7 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
             for (int j = 0; j < gsz; ++j) {
               const int it = (tap0 + j) * p.kblocks + kb;          // [tap][kb][plane][rows] blocks of 64-wide rows
               rb.produce((uint32_t)p.b_load_bytes,
-                         [&](int s, uint64_t* bar) { load_b(b_ring + (size_t)s * p.b_tile_bytes, it, bar); });
+                         [&](int s, uint64_t* bar) { load_b(b_ring + (size_t)s * p.b_tile_bytes, it, bar, img); });
             }
           }
         }
@@ -354,6 +356,7 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
     const int d_coff = second ? p.out2_coff - 64 : p.out_coff;          // d_coff + column = channel in the destination
     const int d_nstore = second ? 64 + p.n_store2 : p.n_store;
     const bool d_relu = (second ? p.relu2 : p.relu) != 0;
+    const bool d_swish = !second && p.swish != 0;
     const bool d_vec = ((p.vec256 >> (second ? 2 : 0)) & 1) != 0;
     constexpr bool kSums = BN == 64;              // column sums need kColsPerWarp (= 32) accumulators per thread
     float sacc[kSums ? 32 : 1];
@@ -478,6 +481,10 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
             } else if (d_relu) {
 #pragma unroll
               for (int i = 0; i < 16; ++i) v[i] = fmaxf(v[i], 0.f);
+            }
+            if (d_swish) {                         // after a res_mode 1 residual, like ReLU; swish launches take no res_mode 2
+#pragma unroll
+              for (int i = 0; i < 16; ++i) v[i] = v[i] / (1.f + __expf(-v[i]));
             }
             if (d_hi && cb < d_nstore) {
               __nv_bfloat16* ohp = d_hi + pix * d_cstride + d_coff + cb;
@@ -675,6 +682,11 @@ extern "C" int stp3_conv_fwd(const stp3_conv_desc* d, const void* x_hi, const vo
   if (d->res_mode) STP3_CHECK_ARG(res_hi && res_lo && d->res_cstride % 8 == 0 && d->res_coff % 8 == 0 &&
                                   d->res_coff + d->bn <= d->res_cstride, "bad residual tensor");
   if (y_f32) STP3_CHECK_ARG(d->n_valid > 0 && d->n_valid <= d->bn, "n_valid out of range");
+  STP3_CHECK_ARG(!d->swish || (!d->relu && d->res_mode != 2 && !d->y2_hi), "swish: not with relu, res_mode 2 or a second destination");
+  if (d->w_img_stride)
+    STP3_CHECK_ARG(d->w_img_stride > 0 && d->w_img_stride % 64 == 0 &&
+                   d->w_img_stride >= (long long)d->ntaps * (d->cin / 64) * 2 * d->bn * 64,
+                   "w_img_stride: a multiple of 64 elements, at least one image's weight blocks");
   if (!tmap_encode_fn()) return set_error(STP3_ECUDA, "cuTensorMapEncodeTiled is not available from the driver");
 
   // tuning knobs (0 = automatic): desc->tune_group, or the STP3_CONV_GROUP environment variable.  tune_n_sub is
@@ -682,7 +694,8 @@ extern "C" int stp3_conv_fwd(const stp3_conv_desc* d, const void* x_hi, const vo
   static const int env_group = [] { const char* e = getenv("STP3_CONV_GROUP"); return e ? atoi(e) : 0; }();
   const int want_group_raw = d->tune_group ? d->tune_group : env_group;
   const int want_group = want_group_raw & 3;
-  const bool stream_weights = (want_group_raw & 4) != 0;    // +4: keep the weights in the ring even if they would fit
+  // +4: keep the weights in the ring even if they would fit; per-image weights always stream
+  const bool stream_weights = (want_group_raw & 4) != 0 || d->w_img_stride != 0;
   // +8: stacked [W_hi; W_lo] operand (bn = 64 only).  Untuned (tune_group == 0) multi-tap 64-column layers use it: it
   // reads the activation tile twice instead of three times
   const bool stack = d->bn == 64 && ((want_group_raw & 8) != 0 || (want_group_raw == 0 && d->ntaps > 1));
@@ -717,7 +730,9 @@ extern "C" int stp3_conv_fwd(const stp3_conv_desc* d, const void* x_hi, const vo
   // the MMAs cover only the columns that carry weights (n_cols, rounded up to a multiple of 16)
   const int n_mma = d->bn <= 128 && d->n_cols > 0 && d->n_cols < d->bn ? ((d->n_cols + 15) / 16) * 16 : bn_launch;
   {
-    const CUresult r = encode_rows_2d(&tm_w, w, (long long)d->ntaps * kblocks * 2 * d->bn, n_mma);
+    const long long rows = d->w_img_stride ? (long long)(d->B * d->T - 1) * (d->w_img_stride / 64) + (long long)d->ntaps * kblocks * 2 * d->bn
+                                           : (long long)d->ntaps * kblocks * 2 * d->bn;
+    const CUresult r = encode_rows_2d(&tm_w, w, rows, n_mma);
     if (r != CUDA_SUCCESS) return set_error(STP3_ECUDA, "cuTensorMapEncodeTiled(weights) failed: %d", (int)r);
   }
 
@@ -739,6 +754,7 @@ extern "C" int stp3_conv_fwd(const stp3_conv_desc* d, const void* x_hi, const vo
   p.a_plane_bytes = box_h * kTileW * kBK * 2; p.w_rows = d->bn; p.n_mma = n_mma;
   for (int i = 0; i < d->ntaps; ++i) { p.tap[i][0] = d->taps[i][0]; p.tap[i][1] = d->taps[i][1]; p.tap[i][2] = d->taps[i][2]; p.tap[i][3] = 0; }
   p.relu = d->relu; p.res_mode = d->res_mode;
+  p.swish = d->swish; p.w_img_rows = d->w_img_stride / 64;
   p.res_hi = static_cast<const __nv_bfloat16*>(res_hi); p.res_lo = static_cast<const __nv_bfloat16*>(res_lo);
   p.res_cstride = d->res_cstride;
   p.out_hi = static_cast<__nv_bfloat16*>(y_hi); p.out_lo = static_cast<__nv_bfloat16*>(y_lo);

@@ -150,13 +150,16 @@ _AUTOTUNE = _os.environ.get("STP3_CONV_AUTOTUNE", "1") != "0"
 TUNE_LOG = []      # (description, {config: ms}) for reports
 
 
-def tune_candidates(pc: PackedConv) -> List[Tuple[int, int]]:
-    """The (n_sub, group) tilings the autotuner times for this packed convolution."""
+def tune_candidates(pc: PackedConv, per_image: bool = False) -> List[Tuple[int, int]]:
+    """The (n_sub, group) tilings the autotuner times for this packed convolution.  Per-image weights are never
+    resident: only the streamed (+4) tilings are offered for them."""
     taps = pc.taps
     groupable = any(taps[i + 1][0] == taps[i][0] and taps[i + 1][2] == taps[i][2] and
                     taps[i + 1][1] == taps[i][1] + pc.stride for i in range(len(taps) - 1))
     cands = [(1, 1)] + ([(1, 3)] if groupable else [])
-    if len(taps) > 1:   # weights streamed through the ring instead of resident: more activation stages in flight
+    if per_image:
+        cands = [(ns, g + 4) for ns, g in cands]
+    elif len(taps) > 1:   # weights streamed through the ring instead of resident: more activation stages in flight
         cands += [(ns, g + 4) for ns, g in cands]
     if pc.bn == 64:     # stacked [W_hi; W_lo] operand: two MMAs per product instead of three
         cands += [(ns, g + 8) for ns, g in cands]
@@ -186,14 +189,16 @@ def conv(x: HL, pc: PackedConv, *, cin_off: int = 0, out: Optional[HL] = None, o
          out_hw: Optional[Tuple[int, int]] = None, n_store: int = 0, frames: Optional[Tuple[int, int]] = None,
          head: Optional[dict] = None, store: bool = True, tune: Optional[Tuple[int, int]] = None,
          col_sums: Optional[torch.Tensor] = None, out2: Optional[HL] = None, out2_coff: int = 0, n_store2: int = 0,
-         relu2: bool = False, out_f32_nhwc: bool = False) -> Optional[HL]:
+         relu2: bool = False, out_f32_nhwc: bool = False, swish: bool = False, w_img_stride: int = 0) -> Optional[HL]:
     """y = act(conv(x[..., cin_off:cin_off+cin]) + bias [+ residual]) written into out[..., out_coff:...]; when
     img_bias (n_img, bn) is given it REPLACES the convolution's bias vector (build it with bias_table()).
     out2 (bn = 128 layers, n_store <= 64): output columns [64, 64+n_store2) go to out2[..., out2_coff:...] with activation
     relu2 -- two 64-column convolutions of the same input in one launch.
     col_sums (B*T, 64) fp32 (bn = 64 layers): receives the per-image sums over pixels of the activated output.
     tune = (n_sub, group) forces a tiling (n_sub is ignored: the tile is 8x16 pixels; group +4 = streamed weights,
-    +8 = stacked hi/lo weight operand) instead of the autotuned one."""
+    +8 = stacked hi/lo weight operand) instead of the autotuned one.
+    swish: x * sigmoid(x) instead of ReLU.  w_img_stride > 0: pc.w holds image 0's weights and image i's start
+    w_img_stride bf16 elements further (squeeze-excite gated projections, se_gate())."""
     B, T_total, H, W, cs = x.hi.shape
     t0, T = frames if frames is not None else (0, T_total)      # process frames [t0, t0+T) of every sample
     Ho, Wo = out_hw if out_hw is not None else ((H + pc.stride - 1) // pc.stride, (W + pc.stride - 1) // pc.stride)
@@ -226,6 +231,7 @@ def conv(x: HL, pc: PackedConv, *, cin_off: int = 0, out: Optional[HL] = None, o
         assert out.hi.shape[:4] == (B, T, Ho, Wo), (out.hi.shape, (B, T, Ho, Wo))
         d.out_cstride, d.out_coff, d.n_store = out.hi.shape[-1], out_coff, n_store
     d.relu = int(relu)
+    d.swish, d.w_img_stride = int(swish), int(w_img_stride)
     if residual is not None:
         d.res_mode = 2 if res_after_act else 1
         d.res_cstride, d.res_coff = residual.hi.shape[-1], res_coff
@@ -258,7 +264,7 @@ def conv(x: HL, pc: PackedConv, *, cin_off: int = 0, out: Optional[HL] = None, o
         _lib.check(code, "stp3_conv_fwd")
 
     key = (pc.uid, B, T, H, W, cs, cin_off, Ho, Wo, t0, int(relu), residual is not None, out_f32 is not None,
-           hd is not None, out2 is not None)
+           hd is not None, out2 is not None, int(swish), int(w_img_stride))
     cfg = tune if tune is not None else _TUNED.get(key)
     if cfg is None and _AUTOTUNE and not torch.cuda.is_current_stream_capturing():
         desc = f"{len(pc.taps)}tap cin{pc.cin_p} bn{pc.bn} s{pc.stride} {B * T}x{Ho}x{Wo}"
@@ -266,7 +272,7 @@ def conv(x: HL, pc: PackedConv, *, cin_off: int = 0, out: Optional[HL] = None, o
         ins = {x.hi.data_ptr(), x.lo.data_ptr()} | ({residual.hi.data_ptr(), residual.lo.data_ptr()} if residual is not None else set())
         outs = {t.data_ptr() for t in ((out.hi, out.lo) if out is not None else ()) + ((out2.hi, out2.lo) if out2 is not None else ())}
         assert not (ins & outs), "stp3_b200.dense.conv: output aliases an input (in-place convolution is not supported)"
-        cfg = _tune(key, desc, launch, tune_candidates(pc))
+        cfg = _tune(key, desc, launch, tune_candidates(pc, per_image=w_img_stride > 0))
     launch(*(cfg or (0, 0)))
     return out
 
@@ -536,3 +542,80 @@ def upsample2x_add(x: HL, skip: Optional[HL], c: int, skip_coff: int = 0, out: O
             out.lo.data_ptr(), out.hi.shape[-1], out_coff, c, _stream(x.hi.device))
     _lib.check(code, "stp3_upsample2x_add")
     return out
+
+
+# ------------------------------------------------------------------------------------------------ EfficientNet trunk
+def effnet_stem(x: torch.Tensor, w: torch.Tensor, b: torch.Tensor, out_hw: Tuple[int, int], pad: Tuple[int, int],
+                cp: int = KB) -> HL:
+    """x (M, 3, H, W) fp32 NCHW images -> HL (M, 1, Ho, Wo, cp): 3x3 stride-2 conv (w (cout, 3, 3, 3) and b BN-folded)
+    + swish; pad = (top, left) static pads."""
+    if not x.is_cuda:
+        raise RuntimeError("stp3_b200 dense ops run on CUDA tensors only (there is no CPU path)")
+    x = x.detach().float().contiguous()
+    M, C, H, W = x.shape
+    assert C == 3 and w.shape[1:] == (3, 3, 3) and w.is_contiguous() and b.is_contiguous()
+    Ho, Wo = out_hw
+    out = HL.empty(M, 1, Ho, Wo, w.shape[0], x.device, cp=cp)
+    with torch.cuda.device(x.device):
+        code = _lib.lib().stp3_effnet_stem(x.data_ptr(), M, H, W, Ho, Wo, pad[0], pad[1], w.data_ptr(), b.data_ptr(),
+                                           w.shape[0], cp, out.hi.data_ptr(), out.lo.data_ptr(), _stream(x.device))
+    _lib.check(code, "stp3_effnet_stem")
+    return out
+
+
+def dw_conv(x: HL, w: torch.Tensor, b: torch.Tensor, k: int, stride: int, pad: Tuple[int, int], out_hw: Tuple[int, int],
+            out: Optional[HL] = None, sums: Optional[torch.Tensor] = None) -> HL:
+    """Depthwise k x k conv + folded BN + swish of channels [0, C) (w (k*k, C) fp32, b (C), C = len(b)) -> HL
+    (B, T, Ho, Wo, .); sums (B*T, C) fp32 receives the per-image sums of the output (stp3_dw_fwd)."""
+    B, T, H, W, cs = x.hi.shape
+    C = b.numel()
+    Ho, Wo = out_hw
+    if out is None:
+        out = HL.empty(B, T, Ho, Wo, x.c, x.hi.device, cp=pad_to(C))
+    assert out.hi.shape[:4] == (B, T, Ho, Wo) and w.shape == (k * k, C) and w.is_contiguous() and b.is_contiguous()
+    d = _lib.DwDesc(n_img=B * T, H=H, W=W, Ho=Ho, Wo=Wo, k=k, stride=stride, pad_t=pad[0], pad_l=pad[1], C=C,
+                    in_cstride=cs, out_cstride=out.hi.shape[-1])
+    scratch, nbytes = None, 0
+    if sums is not None:
+        assert sums.shape == (B * T, C) and sums.dtype == torch.float32 and sums.is_contiguous()
+        nbytes = _lib.lib().stp3_dw_sums_scratch_bytes(ctypes.byref(d))
+        scratch = torch.empty(nbytes, dtype=torch.uint8, device=x.hi.device)
+    ptr = lambda t: t.data_ptr() if t is not None else None
+    with torch.cuda.device(x.hi.device):
+        code = _lib.lib().stp3_dw_fwd(ctypes.byref(d), x.hi.data_ptr(), x.lo.data_ptr(), w.data_ptr(), b.data_ptr(),
+                                      out.hi.data_ptr(), out.lo.data_ptr(), ptr(sums), ptr(scratch), nbytes,
+                                      _stream(x.hi.device))
+    _lib.check(code, "stp3_dw_fwd")
+    return out
+
+
+def se_proj_weight_elems(cin: int, cout: int) -> int:
+    return int(_lib.lib().stp3_se_proj_weight_elems(cin, cout))
+
+
+def se_chunks(cout: int) -> List[Tuple[int, int, int]]:
+    """(first output channel, channels, bn) of the 128-column chunks a projection runs as (stp3_se_gate's layout)."""
+    return [(n0, min(128, cout - n0), 128 if cout - n0 > 64 else 64) for n0 in range(0, cout, 128)]
+
+
+def se_gate(sums: torch.Tensor, hw: int, C: int, w_r, b_r, w_e, b_e, w_proj: torch.Tensor,
+            gate: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """Squeeze-excite gate of every image folded into per-image projection weights: returns (n_img,
+    se_proj_weight_elems(C, cout)) bf16 -- W_proj . diag(gate_img), packed hi/lo in se_chunks(cout) column chunks.
+    gate: optional (n_img, C) fp32 destination of the gate itself (allocated when not given)."""
+    n_img = sums.shape[0]
+    R, cout = w_r.shape[0], w_proj.shape[0]
+    assert w_r.shape == (R, C) and w_e.shape == (C, R) and w_proj.shape == (cout, C) and sums.shape[1] >= C
+    for t in (sums, w_r, b_r, w_e, b_e, w_proj) + ((gate,) if gate is not None else ()):
+        assert t.dtype == torch.float32 and t.is_contiguous() and t.is_cuda
+    if gate is None:
+        gate = torch.empty((n_img, C), dtype=torch.float32, device=sums.device)
+    assert gate.shape == (n_img, C)
+    w_img = torch.empty((n_img, se_proj_weight_elems(C, cout)), dtype=torch.bfloat16, device=sums.device)
+    with torch.cuda.device(sums.device):
+        code = _lib.lib().stp3_se_gate(sums.data_ptr(), sums.shape[1], n_img, C, 1.0 / hw, w_r.data_ptr(),
+                                       b_r.data_ptr(), R, w_e.data_ptr(), b_e.data_ptr(), w_proj.data_ptr(), cout,
+                                       gate.data_ptr(), w_img.data_ptr(),
+                                       _stream(sums.device))
+    _lib.check(code, "stp3_se_gate")
+    return w_img

@@ -190,7 +190,29 @@ class UpsamplingConcat(PackedModule):
             P[key] = dense.pack_conv(P["c0"][0], P["c0"][1], in_layout=[(0, cf, 0), (cf, cc, cf)])
         cat = dense.from_f32(fine_f32.unsqueeze(1), cp=dense.pad_to(cf + cc))
         dense.upsample2x_add(coarse, None, cc, out=cat, out_coff=cf)
-        y = dense.conv(cat, P[key], relu=True)
+        return self._convs(cat, P[key], out_f32, out_f32_nhwc)
+
+    def forward_cat(self, coarse: dense.HL, cat: dense.HL, cf: int, out_f32: Optional[torch.Tensor] = None,
+                    out_f32_nhwc: bool = False):
+        """forward_hl with the fine map already in channels [0, cf) of `cat` (B, 1, 2h, 2w, pad_to(cf + coarse.c)) hi/lo,
+        where its producer wrote it: the upsampled coarse map goes into the channels behind it, so the fine map makes no
+        fp32 round trip.  The other channels of `cat` need not be initialised."""
+        self._require_eval()
+        P = self.packed()
+        cc = coarse.c
+        assert cf + cc == self.in_channels and cf % 8 == 0 and cat.hi.shape[-1] == dense.pad_to(cf + cc)
+        key = ("c0p", cf, cc)
+        if key not in P:
+            P[key] = dense.pack_conv(P["c0"][0], P["c0"][1], in_layout=[(0, cf, 0), (cf, cc, cf)])
+        # the first convolution reads channels up to k_hi: the coarse map's zero padding channels fill the gap
+        n_up = (P[key].k_hi or cat.hi.shape[-1]) - cf
+        assert n_up <= coarse.hi.shape[-1]
+        dense.upsample2x_add(coarse, None, n_up, out=cat, out_coff=cf)
+        return self._convs(cat, P[key], out_f32, out_f32_nhwc)
+
+    def _convs(self, cat: dense.HL, pc0: dense.PackedConv, out_f32, out_f32_nhwc):
+        P = self.packed()
+        y = dense.conv(cat, pc0, relu=True)
         if out_f32 is None:
             return dense.conv(y, P["c1"], relu=True)
         B = y.hi.shape[0]

@@ -1,10 +1,12 @@
 """Image encoder with the reference's surface (stp3/models/encoder.py:9-108): a truncated EfficientNet trunk and two
 heads (context features, depth logits) at 1/8 resolution.
 
-The trunk is third-party (efficientnet-pytorch 0.7.0, not vendored by the reference and absent from this image;
-SURVEY.md §8c): it is taken from `efficientnet_pytorch` when importable, or injected (`backbone=`: any module that
-maps (M,3,H,W) -> (reduction_3 (M,c3,H/8,W/8), reduction_4 (M,c4,H/16,W/16))).  The heads -- DeepLabHead +
-UpsamplingConcat, the layers this repository owns -- run on the wgmma kernels."""
+The trunk (efficientnet-pytorch 0.7.0, not vendored by the reference; SURVEY.md §8c) is chosen by `backbone=`:
+  "native"      the sm_90a trunk of this package (models/efficientnet.py, same state-dict keys);
+  None          efficientnet_pytorch's pretrained model when the package is importable, else the native trunk;
+  a module      injected: maps (M,3,H,W) -> (reduction_3 (M,c3,H/8,W/8), reduction_4 (M,c4,H/16,W/16)).
+The heads -- DeepLabHead + UpsamplingConcat -- run on the wgmma kernels.  With the native trunk the endpoints reach the
+heads as hi/lo planes: block 9 writes reduction_3 straight into the heads' concat tensor."""
 import math
 
 import torch
@@ -12,6 +14,7 @@ import torch.nn as nn
 
 from .. import dense
 from ..layers.convolutions import DeepLabHead, UpsamplingConcat
+from .efficientnet import EfficientNetTrunk
 
 
 class Encoder(nn.Module):
@@ -30,11 +33,15 @@ class Encoder(nn.Module):
         if backbone is None:
             try:
                 from efficientnet_pytorch import EfficientNet
-            except ImportError as e:
-                raise RuntimeError("efficientnet_pytorch is not installed: pass backbone=<module returning "
-                                   "(reduction_3, reduction_4)> to Encoder / STP3") from e
-            backbone = EfficientNet.from_pretrained(cfg.NAME)
-        if hasattr(backbone, "_conv_stem"):        # an efficientnet_pytorch model: truncate it like encoder.py:39-55
+                backbone = EfficientNet.from_pretrained(cfg.NAME)
+            except ImportError:
+                backbone = "native"
+        if isinstance(backbone, str):
+            if backbone != "native":
+                raise ValueError(f"backbone={backbone!r}: pass 'native', None or a module")
+            backbone = EfficientNetTrunk(self.version, self.downsample)
+        if hasattr(backbone, "_conv_stem") and not isinstance(backbone, EfficientNetTrunk):
+            # an efficientnet_pytorch model: truncate it like encoder.py:39-55 (the native trunk is built truncated)
             _truncate_efficientnet(backbone, self.version, self.downsample)
         self.backbone = backbone
         index = int(math.log2(self.downsample))
@@ -69,13 +76,41 @@ class Encoder(nn.Module):
             self.depth_layer_2.forward_hl(self.depth_layer_1.forward_hl(x), r_lo, out_f32=depth)
         return feat, depth
 
+    @property
+    def native(self) -> bool:
+        return isinstance(self.backbone, EfficientNetTrunk)
+
+    def features_native(self, x: torch.Tensor, channels_last: bool = False):
+        """(M,3,H,W) fp32 images -> heads_f32's outputs through the native trunk, hi/lo from the stem to the heads."""
+        M, _, H, W = x.shape
+        ds = self.downsample
+        index = int(math.log2(ds))
+        c_hi, c_lo = self.reduction_channel[index + 1], self.reduction_channel[index]
+        cat = dense.HL.empty(M, 1, H // ds, W // ds, c_lo + c_hi, x.device)
+        r_lo, r_hi = self.backbone.forward_hl(x, r3_out=cat)
+        assert r_lo is cat and r_hi.hi.shape[2:4] == (H // (2 * ds), W // (2 * ds)), "image size must be a multiple of 16"
+        Hf, Wf = H // ds, W // ds
+        feat = torch.empty((M, Hf, Wf, self.C) if channels_last else (M, self.C, Hf, Wf), dtype=torch.float32,
+                           device=x.device)
+        self.feature_layer_2.forward_cat(self.feature_layer_1.forward_hl(r_hi), cat, c_lo, out_f32=feat,
+                                         out_f32_nhwc=channels_last)
+        depth = None
+        if self.use_depth_distribution:
+            depth = torch.empty((M, self.D, Hf, Wf), dtype=torch.float32, device=x.device)
+            self.depth_layer_2.forward_cat(self.depth_layer_1.forward_hl(r_hi), cat, c_lo, out_f32=depth)
+        return feat, depth
+
     def trunk(self, x):
         """(M,3,H,W) images -> (reduction_3 (M,c3,H/8,W/8), reduction_4 (M,c4,H/16,W/16)) (encoder.py:57-86)."""
+        if self.native:
+            return self.backbone(x.float().contiguous())
         if hasattr(self.backbone, "_conv_stem"):
             return _efficientnet_endpoints(self.backbone, x)
         return self.backbone(x)
 
     def get_features_depth(self, x, channels_last: bool = False):
+        if self.native:
+            return self.features_native(x.float().contiguous(), channels_last)
         r_lo, r_hi = self.trunk(x)
         return self.heads_f32(r_lo.float().contiguous(), r_hi.float().contiguous(), channels_last)
 

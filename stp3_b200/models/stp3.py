@@ -133,6 +133,10 @@ class STP3(nn.Module):
         the reference's keys (stp3.py:132-184)."""
         S = self.receptive_field
         image = image[:, :S].contiguous()
+        if self.encoder.native:
+            dev = image.device
+            h = {k: v.to(dev) for k, v in self.prepare_inputs(intrinsics, extrinsics, future_egomotion).items()}
+            return self.forward_images_device(image, **h)
         b, s, n = image.shape[:3]
         r_lo, r_hi = self.encoder.trunk(image.view(b * s * n, *image.shape[3:]))
         r_lo = r_lo.float().contiguous().view(b, s, n, *r_lo.shape[1:])
@@ -147,6 +151,17 @@ class STP3(nn.Module):
         dev = r_lo.device
         h = {k: v.to(dev) for k, v in self.prepare_inputs(intrinsics, extrinsics, future_egomotion).items()}
         return self.forward_heads_device(r_lo[:, :S].contiguous(), r_hi[:, :S].contiguous(), **h)
+
+    def forward_images_device(self, image, cam_M, cam_t, ego_R, ego_t, const):
+        """Device-only from images (B,S,N,3,H,W) fp32 through the native trunk: trunk -> heads -> forward_device
+        (capturable in a CUDA graph, GraphedPerception(entry="images"))."""
+        b, s, n = image.shape[:3]
+        self._mark("start_trunk")
+        feat, depth = self.encoder.features_native(image.reshape(b * s * n, *image.shape[3:]), channels_last=True)
+        feat = feat.view(b, s, n, *feat.shape[1:])
+        depth = depth.view(b, s, n, *depth.shape[1:]) if depth is not None else None
+        self._mark("encoder")
+        return self.forward_device(feat, depth, cam_M, cam_t, ego_R, ego_t, const, feat_channels_last=True)
 
     def forward_heads_device(self, r_lo, r_hi, cam_M, cam_t, ego_R, ego_t, const):
         """Device-only: encoder heads -> forward_device (capturable in a CUDA graph)."""
@@ -297,7 +312,9 @@ class GraphedPerception:
     def __init__(self, model: STP3, batch: int, n_cameras: int, device=None, entry: str = "lift"):
         """entry "lift": the step enters at the encoder outputs (feat, depth_logits), STP3.forward_features;
         entry "heads": at the trunk endpoints (r_lo, r_hi), STP3.forward_trunk_features (encoder heads included);
-        entry "sharded": like "lift" but frame-sharded over the ranks of the default process group (latency mode)."""
+        entry "sharded": like "lift" but frame-sharded over the ranks of the default process group (latency mode);
+        entry "images": from the camera images (B,S,N,3,H,W) through the native trunk, STP3.forward -- the first two
+        arguments of __call__ / stage_inputs are then (image, None)."""
         if model.decoder.training:
             raise RuntimeError("GraphedPerception: the decoder is in train mode (batch statistics, running-statistics "
                                "updates, autograd); a CUDA graph replays the inference forward only -- call .eval()")
@@ -323,6 +340,13 @@ class GraphedPerception:
             first = {"r_lo": torch.zeros((batch, S, N, c_lo, Hf, Wf), **f32),
                      "r_hi": torch.zeros((batch, S, N, c_hi, Hf // 2, Wf // 2), **f32)}
             self._fwd = model.forward_heads_device
+        elif entry == "images":
+            if not model.encoder.native:
+                raise ValueError('entry="images" needs the native trunk (Encoder backbone="native")')
+            H, W = model.cfg.IMAGE.FINAL_DIM
+            self.big = ("image",)
+            first = {"image": torch.zeros((batch, S, N, 3, H, W), **f32)}
+            self._fwd = model.forward_images_device
         else:
             raise ValueError(entry)
         self.static = {
@@ -371,8 +395,9 @@ class GraphedPerception:
             self.static[k].copy_(self.pinned[k], non_blocking=True)
         self.h2d_done.record(stream if stream is not None else torch.cuda.current_stream(self.static["cam_M"].device))
         S = self.model.receptive_field
-        self.static[self.big[0]].copy_(feat[:, :S], non_blocking=True)          # (feat, depth_logits) or (r_lo, r_hi)
-        self.static[self.big[1]].copy_(depth_logits[:, :S], non_blocking=True)
+        self.static[self.big[0]].copy_(feat[:, :S], non_blocking=True)          # (feat, depth_logits), (r_lo, r_hi), (image,)
+        if len(self.big) > 1:
+            self.static[self.big[1]].copy_(depth_logits[:, :S], non_blocking=True)
 
     def __call__(self, feat, depth_logits, intrinsics, extrinsics, future_egomotion):
         """Inputs are consumed asynchronously (pinned host tensors must stay untouched until the step has run); the
