@@ -318,19 +318,23 @@ int stp3_upsample2x_add(const void* x_hi, const void* x_lo, int n_img, int h, in
                         int C, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------
- * Train mode of the BEV decoder (stp3/models/decoder.py in train(): BatchNorm with batch statistics, autograd).
+ * Train mode of the BEV decoder and the DeepLab head (stp3/models/decoder.py, stp3/layers/convolutions.py:227-280 in
+ * train(): BatchNorm with batch statistics, dropout, autograd).
  * Tensors are fp32 channels-last (n_pix, cstride) with the channels at [0, C) of each row unless noted; every
  * reduction is deterministic (per-block partials in `scratch`, summed in a fixed order, no float atomics), so two calls
  * on the same inputs return bitwise-identical results.  The input gradient of a convolution is stp3_conv_fwd itself
  * (transposed weights, mirrored taps; stride 2 as four phase convolutions joined by stp3_phase_interleave).
  *
- * Weight gradient of a (kh x kw, stride, zero padding pad) convolution, reference layout (cout, cin, kh, kw):
- *   dw[co][ci][ky][kx] = sum over the n_img*Ho*Wo output pixels p of g[p][co] * x[p*stride + (ky-pad, kx-pad)][ci]
- *   x (n_img, H, W, x_cstride), g (n_img, Ho, Wo, g_cstride); scratch: stp3_conv_wgrad_scratch_bytes() bytes. */
-size_t stp3_conv_wgrad_scratch_bytes(int n_img, int Ho, int Wo, int cout, int cin, int kh, int kw);
+ * Weight gradient of a (kh x kw, stride, zero padding pad, dilation d >= 1) convolution, reference layout
+ * (cout, cin, kh, kw):
+ *   dw[co][ci][ky][kx] = sum over the n_img*Ho*Wo output pixels p of g[p][co] * x[p*stride + (ky*d-pad, kx*d-pad)][ci]
+ *   x (n_img, H, W, x_cstride), g (n_img, Ho, Wo, g_cstride); scratch: stp3_conv_wgrad_scratch_bytes() bytes.
+ *   A tap whose shifted window lies in the zero padding for every output pixel gets exact zeros (its pixels are not
+ *   read).  The input gradient of a dilated convolution is stp3_conv_fwd with the mirrored taps e = pad - k*d. */
+size_t stp3_conv_wgrad_scratch_bytes(int n_img, int Ho, int Wo, int cout, int cin, int kh, int kw, int dilation);
 int stp3_conv_wgrad(const float* x, int n_img, int H, int W, int x_cstride, int cin, const float* g, int Ho, int Wo,
-                    int g_cstride, int cout, int kh, int kw, int stride, int pad, void* scratch, size_t scratch_bytes,
-                    float* dw, void* stream);
+                    int g_cstride, int cout, int kh, int kw, int stride, int pad, int dilation, void* scratch,
+                    size_t scratch_bytes, float* dw, void* stream);
 /* BatchNorm batch statistics over n_pix rows (two passes: mean, then the centred sum of squares; fp64 partials):
  * mean[C], var[C] (biased; may be NULL), invstd = 1/sqrt(var + eps); when running_mean/var are given they are updated
  * like nn.BatchNorm2d: r = (1 - momentum) r + momentum b, with the unbiased variance var * n/(n-1).
@@ -340,15 +344,27 @@ int stp3_bn_stats(const float* x, long long n_pix, int C, int x_cstride, float e
                   float* running_var, float* mean, float* var, float* invstd, void* scratch, size_t scratch_bytes,
                   void* stream);
 /* y = relu?((x - mean) * invstd * gamma + beta (+ res)) -> fp32 y (may be NULL) and/or bf16 hi/lo planes (n_pix,
- * hl_cstride) for the next stp3_conv_fwd (channels [C, hl_cstride) written as zeros).  C % 8 == 0, 16-byte rows. */
+ * hl_cstride) for the next stp3_conv_fwd (channels [C, hl_cstride) written as zeros).  C % 8 == 0, 16-byte rows.
+ * Dropout (0 <= dropout_p < 1; 0 = none, bit for bit): y is then multiplied by m / (1 - p), where the keep bit m of
+ * element (pixel, c) depends only on (seed, offset + pixel * C + c): word e % 4 of Philox-4x32-10 with key seed and
+ * counter (e / 4, 0) (64-bit values as (low, high) words), read as (word >> 8) / 2^24, keeps when it is >= p.  So a
+ * tensor split across launches (offset = the elements before each part) gets the same mask as one launch.  Both y and
+ * the bf16 planes carry the dropped values; a kept, positive element is exactly one with y > 0. */
 int stp3_bn_apply(const float* x, long long n_pix, int C, int x_cstride, const float* mean, const float* invstd,
-                  const float* gamma, const float* beta, const float* res, int res_cstride, int relu, float* y,
-                  int y_cstride, void* y_hi, void* y_lo, int hl_cstride, void* stream);
+                  const float* gamma, const float* beta, const float* res, int res_cstride, int relu, float dropout_p,
+                  unsigned long long seed, unsigned long long offset, float* y, int y_cstride, void* y_hi, void* y_lo,
+                  int hl_cstride, void* stream);
 /* sum_g[c] = sum_p g'[p][c] (= dbeta, or a conv bias gradient when x is NULL) and sum_gxhat[c] = sum_p g' xhat (= dgamma),
  * g' = g where y > 0 (the ReLU mask of the BN's activated output y; y NULL = no mask), xhat = (x - mean) * invstd. */
 int stp3_bn_bwd_reduce(const float* g, int g_cstride, const float* y, int y_cstride, const float* x, int x_cstride,
                        const float* mean, const float* invstd, long long n_pix, int C, float* sum_g, float* sum_gxhat,
                        void* scratch, size_t scratch_bytes, void* stream);
+/* sums[img][c] = sum over the hw rows of image img of x[img * hw + p][c], x (n_img * hw, x_cstride) fp32: per-image
+ * channel sums in a fixed order (fp64 partials in scratch), bitwise repeatable -- the global-pool branch of the DeepLab
+ * head and its backward.  sums (n_img, C); scratch: stp3_image_channel_sums_scratch_bytes() bytes. */
+size_t stp3_image_channel_sums_scratch_bytes(int n_img, long long hw, int C);
+int stp3_image_channel_sums(const float* x, int n_img, long long hw, int C, int x_cstride, float* sums, void* scratch,
+                            size_t scratch_bytes, void* stream);
 /* dx = gamma * invstd * (g' - sum_g/n - xhat * sum_gxhat/n); g_masked (optional) receives g' (the gradient of a residual
  * that was added before the ReLU). */
 int stp3_bn_bwd_apply(const float* g, int g_cstride, const float* y, int y_cstride, const float* x, int x_cstride,

@@ -19,6 +19,7 @@ _I = ctypes.c_int
 _F = ctypes.c_float
 _SZ = ctypes.c_size_t
 _LL = ctypes.c_longlong
+_ULL = ctypes.c_ulonglong
 
 
 class LiftSplatDesc(ctypes.Structure):
@@ -95,12 +96,14 @@ SIGNATURES = {
     "stp3_bev_discount": (_I, [_V, _I, _I, _I, _I, _I, _F, _V, _V, _V]),
     "stp3_conv_fwd": (_I, [ctypes.POINTER(ConvDesc), _V, _V, _V, _V, _V, _V, _V, _V, _V, _V, ctypes.POINTER(ConvHead), _V]),
     "stp3_lift_splat_fwd": (_I, [_LSD, _V, _V, _V, _V, _V, _SZ, _V, _I, _I, ctypes.POINTER(_V), _V]),
-    # train mode of the decoder
-    "stp3_conv_wgrad_scratch_bytes": (_SZ, [_I, _I, _I, _I, _I, _I, _I]),
-    "stp3_conv_wgrad": (_I, [_V, _I, _I, _I, _I, _I, _V, _I, _I, _I, _I, _I, _I, _I, _I, _V, _SZ, _V, _V]),
+    # train mode of the decoder and the DeepLab head
+    "stp3_conv_wgrad_scratch_bytes": (_SZ, [_I, _I, _I, _I, _I, _I, _I, _I]),
+    "stp3_conv_wgrad": (_I, [_V, _I, _I, _I, _I, _I, _V, _I, _I, _I, _I, _I, _I, _I, _I, _I, _V, _SZ, _V, _V]),
     "stp3_bn_scratch_bytes": (_SZ, [_LL, _I]),
     "stp3_bn_stats": (_I, [_V, _LL, _I, _I, _F, _F, _V, _V, _V, _V, _V, _V, _SZ, _V]),
-    "stp3_bn_apply": (_I, [_V, _LL, _I, _I, _V, _V, _V, _V, _V, _I, _I, _V, _I, _V, _V, _I, _V]),
+    "stp3_bn_apply": (_I, [_V, _LL, _I, _I, _V, _V, _V, _V, _V, _I, _I, _F, _ULL, _ULL, _V, _I, _V, _V, _I, _V]),
+    "stp3_image_channel_sums_scratch_bytes": (_SZ, [_I, _LL, _I]),
+    "stp3_image_channel_sums": (_I, [_V, _I, _LL, _I, _I, _V, _V, _SZ, _V]),
     "stp3_bn_bwd_reduce": (_I, [_V, _I, _V, _I, _V, _I, _V, _V, _LL, _I, _V, _V, _V, _SZ, _V]),
     "stp3_bn_bwd_apply": (_I, [_V, _I, _V, _I, _V, _I, _V, _V, _V, _V, _V, _LL, _I, _V, _I, _V, _I, _V]),
     "stp3_upsample2x_f32": (_I, [_V, _I, _I, _I, _I, _V, _V]),

@@ -18,10 +18,10 @@ int set_error(int code, const char* fmt, ...) {
 
 }  // namespace stp3
 
-extern "C" int stp3_abi_version(void) { return 6; }
+extern "C" int stp3_abi_version(void) { return 7; }
 
 extern "C" const char* stp3_build_info(void) {
-  return "stp3_b200 abi 6; sm_90a; nvcc " __DATE__ " " __TIME__;
+  return "stp3_b200 abi 7; sm_90a; nvcc " __DATE__ " " __TIME__;
 }
 
 extern "C" const char* stp3_last_error(void) { return stp3::error_buffer(); }

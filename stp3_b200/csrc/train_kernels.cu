@@ -1,6 +1,7 @@
-// Train-mode pieces of the dense path (the BEV decoder, stp3/models/decoder.py): convolution weight gradient,
-// BatchNorm with batch statistics (stats / apply / backward), fp32 bilinear x2 and its backward, the interleave of the
-// four stride-2 input-gradient phases, and the sigmoid backward.  Tensors are fp32 channels-last (n_pix, cstride) unless
+// Train-mode pieces of the dense path (the BEV decoder, stp3/models/decoder.py, and the DeepLab head,
+// convolutions.py:272-280): convolution weight gradient (dilated too), BatchNorm with batch statistics (stats / apply with
+// fused dropout / backward), per-image channel sums, fp32 bilinear x2 and its backward, the interleave of the four
+// stride-2 input-gradient phases, and the sigmoid backward.  Tensors are fp32 channels-last (n_pix, cstride) unless
 // noted.  Every reduction is deterministic: per-block partials go to caller scratch and are summed in a fixed order
 // (no float atomics), and the block decomposition depends only on the problem shape, so two calls on the same inputs
 // return bitwise-identical results.
@@ -13,7 +14,7 @@
 namespace stp3 {
 
 // ------------------------------------------------------------------------------------------------ weight gradient
-// dW[co][ci][ky][kx] = sum over output pixels p of g[p][co] * x[p * stride + (ky - pad, kx - pad)][ci]   (zero outside)
+// dW[co][ci][ky][kx] = sum over output pixels p of g[p][co] * x[p * stride + (ky*d - pad, kx*d - pad)][ci]  (zero outside)
 // as a GEMM on the tensor cores: M = co, N = ci, K = output pixels.  Both operands are channels-last, i.e. MN-major for
 // this GEMM: a K row (one pixel) holds 64 consecutive co (A) or ci (B).  One CTA = one warpgroup = one tap x 64 co x
 // 64 ci x one contiguous range of output pixels (the K split).  Each 64-pixel stage is staged as bf16 hi / lo planes
@@ -24,8 +25,14 @@ constexpr int kWgTile = 64, kWgK = 64;
 constexpr int kWgTileBytes = kWgK * kWgTile * 2;          // one bf16 plane of one operand: 64 pixels x 128 B
 
 struct WgradShape {
-  int n_img, H, W, x_cstride, cin, Ho, Wo, g_cstride, cout, stride, kh, kw, pad;
+  int n_img, H, W, x_cstride, cin, Ho, Wo, g_cstride, cout, stride, kh, kw, pad, dil;
 };
+
+// does an output axis of n_out positions, read at o * stride + d, touch the input extent [0, n_in) at all?
+__device__ __forceinline__ bool tap_in_image(int d, int n_out, int stride, int n_in) {
+  const int o = d >= 0 ? 0 : (-d + stride - 1) / stride;       // first o with o * stride + d >= 0
+  return o < n_out && o * stride + d < n_in;
+}
 
 __host__ __device__ inline long long wgrad_pixels(const WgradShape& s) { return (long long)s.n_img * s.Ho * s.Wo; }
 
@@ -69,7 +76,10 @@ wgrad_partial_kernel(const float* __restrict__ x, const float* __restrict__ g, W
   const int cit = t % ci_tiles; t /= ci_tiles;
   const int cot = t % co_tiles; t /= co_tiles;
   const int tap = t;                                   // ky * kw + kx
-  const int dy = tap / s.kw - s.pad, dx = tap % s.kw - s.pad;
+  const int dy = tap / s.kw * s.dil - s.pad, dx = tap % s.kw * s.dil - s.pad;
+  // a tap whose window lies in the zero padding for every output pixel (large dilations on small maps) contributes
+  // exact zeros: the CTA stores them without streaming the pixels
+  const bool live = tap_in_image(dy, s.Ho, s.stride, s.H) && tap_in_image(dx, s.Wo, s.stride, s.W);
   const long long P = wgrad_pixels(s);
   const long long p_begin = (long long)blockIdx.x * px_per_split;
   const long long p_end = p_begin + px_per_split < P ? p_begin + px_per_split : P;
@@ -79,7 +89,7 @@ wgrad_partial_kernel(const float* __restrict__ x, const float* __restrict__ g, W
   float acc[32];
 #pragma unroll
   for (int i = 0; i < 32; ++i) acc[i] = 0.f;
-  for (long long p0 = p_begin; p0 < p_end; p0 += kWgK) {
+  for (long long p0 = p_begin; live && p0 < p_end; p0 += kWgK) {
     // stage: 64 pixel rows x 8 chunks of 8 channels, per operand; chunk c of row r lives at chunk c ^ (r % 8)
 #pragma unroll
     for (int k = 0; k < (kWgK * 8) / 128; ++k) {
@@ -152,8 +162,9 @@ __global__ void wgrad_reduce_kernel(const float* __restrict__ part, int n_split,
 }
 
 // ------------------------------------------------------------------------------------------------ channel reductions
-// Per-channel sums over n_pix rows, deterministic: grid (channel tiles of 32, kRedParts row ranges), block (32, 8);
-// fp64 accumulation; partials [part][C] to scratch, then one thread per channel adds the parts in order.
+// Per-channel sums over n_pix rows, deterministic: grid (channel tiles of 32, kRedParts row ranges, images), block
+// (32, 8); fp64 accumulation; partials [image][part][C] to scratch, then one thread per channel adds the parts in order.
+// grid.z > 1 (mode 0 only) sums each of gridDim.z consecutive images of n_pix rows on its own.
 constexpr int kRedParts = 128;
 
 inline int red_parts(long long n_pix) { return (int)(n_pix < kRedParts ? n_pix : kRedParts); }
@@ -167,6 +178,8 @@ chan_partial_kernel(int mode, const float* __restrict__ a, int a_cs, const float
   __shared__ double red[2][8][33];
   const int c = blockIdx.x * 32 + threadIdx.x;
   const int n_part = gridDim.y;
+  a += (long long)blockIdx.z * n_pix * a_cs;
+  part += (size_t)blockIdx.z * n_part * 2 * C;
   const long long per = (n_pix + n_part - 1) / n_part;
   const long long p0 = blockIdx.y * per, p1 = p0 + per < n_pix ? p0 + per : n_pix;
   double s0 = 0.0, s1 = 0.0;
@@ -231,10 +244,13 @@ __global__ void var_finalize_kernel(const double* __restrict__ part, int n_part,
   }
 }
 
+// grid.y = images: image i reads its own partials and writes sum_g[i * C + c]
 __global__ void sums_finalize_kernel(const double* __restrict__ part, int n_part, int C, float* __restrict__ sum_g,
                                      float* __restrict__ sum_gx) {
   const int c = blockIdx.x * blockDim.x + threadIdx.x;
   if (c >= C) return;
+  part += (size_t)blockIdx.y * n_part * 2 * C;
+  sum_g += (size_t)blockIdx.y * C;
   double t0, t1;
   sum_parts(part, n_part, C, c, t0, t1);
   sum_g[c] = (float)t0;
@@ -242,13 +258,46 @@ __global__ void sums_finalize_kernel(const double* __restrict__ part, int n_part
 }
 
 // ------------------------------------------------------------------------------------------------ elementwise
-// y = relu?((x - mean) * invstd * gamma + beta (+ res)); one thread = one pixel x 8 channels (two 128-bit loads);
-// groups of 8 channels in [C, y_cs) of the bf16 planes are written as zeros (padding of the next conv's K blocks)
+// Philox-4x32-10 (Salmon et al., SC'11): four 32-bit words of counter-based random output for (key, counter)
+__device__ __forceinline__ uint4 philox4x32_10(uint32_t k0, uint32_t k1, uint4 c) {
+#pragma unroll
+  for (int r = 0; r < 10; ++r) {
+    const uint32_t hi0 = __umulhi(0xD2511F53u, c.x), lo0 = 0xD2511F53u * c.x;
+    const uint32_t hi1 = __umulhi(0xCD9E8D57u, c.z), lo1 = 0xCD9E8D57u * c.z;
+    c = make_uint4(hi1 ^ c.y ^ k0, lo1, hi0 ^ c.w ^ k1, lo0);
+    k0 += 0x9E3779B9u;
+    k1 += 0xBB67AE85u;
+  }
+  return c;
+}
+
+// dropout keep bits of the 8 flat elements e0 .. e0 + 7: element e keeps when word e % 4 of
+// philox(key = seed, counter = e / 4), read as a 24-bit uniform u in [0, 1), has u >= p
+__device__ __forceinline__ uint32_t dropout_keep8(unsigned long long seed, unsigned long long e0, float p) {
+  uint32_t bits = 0;
+  uint4 r = make_uint4(0u, 0u, 0u, 0u);
+#pragma unroll
+  for (int k = 0; k < 8; ++k) {
+    const unsigned long long e = e0 + k;
+    if (k == 0 || (e & 3) == 0) {
+      const unsigned long long q = e >> 2;
+      r = philox4x32_10((uint32_t)seed, (uint32_t)(seed >> 32), make_uint4((uint32_t)q, (uint32_t)(q >> 32), 0u, 0u));
+    }
+    const uint32_t w = (e & 3) == 0 ? r.x : (e & 3) == 1 ? r.y : (e & 3) == 2 ? r.z : r.w;
+    if ((float)(w >> 8) * (1.f / 16777216.f) >= p) bits |= 1u << k;
+  }
+  return bits;
+}
+
+// y = relu?((x - mean) * invstd * gamma + beta (+ res)) [* keep / (1 - p)]; one thread = one pixel x 8 channels (two
+// 128-bit loads); groups of 8 channels in [C, y_cs) of the bf16 planes are written as zeros (padding of the next conv's
+// K blocks).  Dropout (p > 0): the keep bit of element (pixel, c) depends only on (seed, offset + pixel * C + c).
 __global__ void __launch_bounds__(256)
 bn_apply_kernel(const float* __restrict__ x, int x_cs, const float* __restrict__ mean, const float* __restrict__ invstd,
                 const float* __restrict__ gamma, const float* __restrict__ beta, const float* __restrict__ res, int res_cs,
-                int relu, long long n_pix, int C, float* __restrict__ y, int y_cs, __nv_bfloat16* __restrict__ yh,
-                __nv_bfloat16* __restrict__ yl, int hl_cs) {
+                int relu, float drop_p, unsigned long long seed, unsigned long long offset, long long n_pix, int C,
+                float* __restrict__ y, int y_cs, __nv_bfloat16* __restrict__ yh, __nv_bfloat16* __restrict__ yl,
+                int hl_cs) {
   const int groups = (hl_cs > C ? hl_cs : C) / 8;
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n_pix * groups) return;
@@ -271,6 +320,12 @@ bn_apply_kernel(const float* __restrict__ x, int x_cs, const float* __restrict__
       const int c = c0 + k;
       float t = (v[k] - mean[c]) * invstd[c] * gamma[c] + beta[c] + r[k];
       v[k] = relu ? fmaxf(t, 0.f) : t;
+    }
+    if (drop_p > 0.f) {
+      const uint32_t keep = dropout_keep8(seed, offset + (unsigned long long)p * C + c0, drop_p);
+      const float scale = 1.f / (1.f - drop_p);
+#pragma unroll
+      for (int k = 0; k < 8; ++k) v[k] = (keep >> k) & 1u ? v[k] * scale : 0.f;
     }
     if (y) {
       *reinterpret_cast<float4*>(y + p * y_cs + c0) = make_float4(v[0], v[1], v[2], v[3]);
@@ -433,24 +488,26 @@ using namespace stp3;
 
 static bool al16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
-extern "C" size_t stp3_conv_wgrad_scratch_bytes(int n_img, int Ho, int Wo, int cout, int cin, int kh, int kw) {
-  if (n_img <= 0 || Ho <= 0 || Wo <= 0 || cout <= 0 || cin <= 0 || kh <= 0 || kw <= 0) return 0;
+extern "C" size_t stp3_conv_wgrad_scratch_bytes(int n_img, int Ho, int Wo, int cout, int cin, int kh, int kw,
+                                                int dilation) {
+  if (n_img <= 0 || Ho <= 0 || Wo <= 0 || cout <= 0 || cin <= 0 || kh <= 0 || kw <= 0 || dilation < 1) return 0;
   WgradShape s{};
   s.n_img = n_img; s.Ho = Ho; s.Wo = Wo; s.cout = cout; s.cin = cin; s.kh = kh; s.kw = kw;
   return (size_t)wgrad_splits(s) * kh * kw * (size_t)cout * cin * sizeof(float);
 }
 
 extern "C" int stp3_conv_wgrad(const float* x, int n_img, int H, int W, int x_cstride, int cin, const float* g, int Ho,
-                               int Wo, int g_cstride, int cout, int kh, int kw, int stride, int pad, void* scratch,
-                               size_t scratch_bytes, float* dw, void* stream) {
+                               int Wo, int g_cstride, int cout, int kh, int kw, int stride, int pad, int dilation,
+                               void* scratch, size_t scratch_bytes, float* dw, void* stream) {
   STP3_CHECK_ARG(x && g && dw && scratch, "stp3_conv_wgrad: null pointer argument");
   STP3_CHECK_ARG(n_img > 0 && H > 0 && W > 0 && Ho > 0 && Wo > 0 && cin > 0 && cout > 0 && kh > 0 && kw > 0 && pad >= 0,
                  "stp3_conv_wgrad: non-positive dimension");
   STP3_CHECK_ARG(stride == 1 || stride == 2, "stp3_conv_wgrad: stride must be 1 or 2");
+  STP3_CHECK_ARG(dilation >= 1, "stp3_conv_wgrad: dilation must be >= 1");
   STP3_CHECK_ARG(cin <= x_cstride && cout <= g_cstride, "stp3_conv_wgrad: channel count exceeds the row stride");
-  const size_t need = stp3_conv_wgrad_scratch_bytes(n_img, Ho, Wo, cout, cin, kh, kw);
+  const size_t need = stp3_conv_wgrad_scratch_bytes(n_img, Ho, Wo, cout, cin, kh, kw, dilation);
   STP3_CHECK_ARG(scratch_bytes >= need, "stp3_conv_wgrad: scratch smaller than stp3_conv_wgrad_scratch_bytes()");
-  WgradShape s{n_img, H, W, x_cstride, cin, Ho, Wo, g_cstride, cout, stride, kh, kw, pad};
+  WgradShape s{n_img, H, W, x_cstride, cin, Ho, Wo, g_cstride, cout, stride, kh, kw, pad, dilation};
   const int n_split = wgrad_splits(s);
   const long long P = wgrad_pixels(s);
   long long per = (P + n_split - 1) / n_split;
@@ -499,9 +556,11 @@ extern "C" int stp3_bn_stats(const float* x, long long n_pix, int C, int x_cstri
 
 extern "C" int stp3_bn_apply(const float* x, long long n_pix, int C, int x_cstride, const float* mean,
                              const float* invstd, const float* gamma, const float* beta, const float* res,
-                             int res_cstride, int relu, float* y, int y_cstride, void* y_hi, void* y_lo, int hl_cstride,
+                             int res_cstride, int relu, float dropout_p, unsigned long long seed,
+                             unsigned long long offset, float* y, int y_cstride, void* y_hi, void* y_lo, int hl_cstride,
                              void* stream) {
   STP3_CHECK_ARG(x && mean && invstd && gamma && beta && (y || y_hi) && n_pix > 0 && C > 0, "stp3_bn_apply: bad argument");
+  STP3_CHECK_ARG(dropout_p >= 0.f && dropout_p < 1.f, "stp3_bn_apply: dropout p must be in [0, 1)");
   STP3_CHECK_ARG((y_hi == nullptr) == (y_lo == nullptr), "stp3_bn_apply: give both bf16 planes or neither");
   STP3_CHECK_ARG(C % 8 == 0 && x_cstride % 4 == 0 && C <= x_cstride && al16(x), "stp3_bn_apply: C % 8, 16-byte rows");
   STP3_CHECK_ARG(!res || (res_cstride % 4 == 0 && C <= res_cstride && al16(res)), "stp3_bn_apply: bad residual");
@@ -511,7 +570,8 @@ extern "C" int stp3_bn_apply(const float* x, long long n_pix, int C, int x_cstri
   const int groups = ((y_hi && hl_cstride > C) ? hl_cstride : C) / 8;
   const long long total = n_pix * groups;
   bn_apply_kernel<<<blocks_for(total), 256, 0, (cudaStream_t)stream>>>(
-      x, x_cstride, mean, invstd, gamma, beta, res, res_cstride, relu, n_pix, C, y, y_cstride, (__nv_bfloat16*)y_hi,
+      x, x_cstride, mean, invstd, gamma, beta, res, res_cstride, relu, dropout_p, seed, offset, n_pix, C, y, y_cstride,
+      (__nv_bfloat16*)y_hi,
       (__nv_bfloat16*)y_lo, y_hi ? hl_cstride : 0);
   STP3_CUDA_OK(cudaGetLastError());
   return STP3_OK;
@@ -531,6 +591,29 @@ extern "C" int stp3_bn_bwd_reduce(const float* g, int g_cstride, const float* y,
                                                                           mean, invstd, n_pix, C, part);
   STP3_CUDA_OK(cudaGetLastError());
   sums_finalize_kernel<<<ceil_div(C, 128), 128, 0, st>>>(part, parts, C, sum_g, x ? sum_gxhat : nullptr);
+  STP3_CUDA_OK(cudaGetLastError());
+  return STP3_OK;
+}
+
+extern "C" size_t stp3_image_channel_sums_scratch_bytes(int n_img, long long hw, int C) {
+  if (n_img <= 0) return 0;
+  return (size_t)n_img * stp3_bn_scratch_bytes(hw, C);
+}
+
+extern "C" int stp3_image_channel_sums(const float* x, int n_img, long long hw, int C, int x_cstride, float* sums,
+                                       void* scratch, size_t scratch_bytes, void* stream) {
+  STP3_CHECK_ARG(x && sums && scratch && n_img > 0 && hw > 0 && C > 0 && C <= x_cstride,
+                 "stp3_image_channel_sums: bad argument");
+  STP3_CHECK_ARG(n_img <= 65535, "stp3_image_channel_sums: more than 65535 images");
+  STP3_CHECK_ARG(scratch_bytes >= stp3_image_channel_sums_scratch_bytes(n_img, hw, C),
+                 "stp3_image_channel_sums: scratch smaller than stp3_image_channel_sums_scratch_bytes()");
+  cudaStream_t st = (cudaStream_t)stream;
+  const int parts = red_parts(hw);
+  double* part = (double*)scratch;
+  chan_partial_kernel<<<dim3(ceil_div(C, 32), parts, n_img), dim3(32, 8), 0, st>>>(0, x, x_cstride, nullptr, 0, nullptr, 0,
+                                                                                 nullptr, nullptr, hw, C, part);
+  STP3_CUDA_OK(cudaGetLastError());
+  sums_finalize_kernel<<<dim3(ceil_div(C, 128), n_img), 128, 0, st>>>(part, parts, C, sums, nullptr);
   STP3_CUDA_OK(cudaGetLastError());
   return STP3_OK;
 }

@@ -1,7 +1,7 @@
-"""Host side of the train-mode dense path (the BEV decoder in train(), include/stp3_b200.h "Train mode"):
-convolution without folded BatchNorm, BatchNorm with batch statistics (stats / apply / backward), the input gradient of
-a convolution on stp3_conv_fwd (transposed weights, mirrored taps; stride 2 as four phase convolutions), the weight
-gradient, and the bilinear x2 pair.
+"""Host side of the train-mode dense path (the BEV decoder and the DeepLab head in train(), include/stp3_b200.h "Train
+mode"): convolution without folded BatchNorm, BatchNorm with batch statistics (stats / apply with dropout / backward),
+the input gradient of a convolution on stp3_conv_fwd (transposed weights, mirrored taps, dilated too; stride 2 as four
+phase convolutions), the weight gradient, per-image channel sums, and the bilinear x2 pair.
 
 Tensors are fp32 channels-last (N, H, W, C) contiguous; the inputs of the tensor-core convolutions are the usual
 bf16 hi/lo planes (dense.HL with T = 1).  Nothing here falls back to ATen convolutions or F.batch_norm.
@@ -26,6 +26,16 @@ def _stream(dev):
 def _f32_cl(t: torch.Tensor) -> torch.Tensor:
     assert t.dtype == torch.float32 and t.is_contiguous() and t.is_cuda and t.dim() == 4, (t.dtype, t.shape)
     return t
+
+
+def _row_stride(t: torch.Tensor) -> int:
+    """Row stride of an fp32 (N, H, W, C) tensor whose pixel rows hold C contiguous channels at one stride: a contiguous
+    tensor, or a channel slice t[..., a:b] of a wider channels-last one (the DeepLab head's concat tensor)."""
+    assert t.dtype == torch.float32 and t.is_cuda and t.dim() == 4, (t.dtype, t.shape)
+    N, H, W, C = t.shape
+    cs = t.stride(2)
+    assert t.stride(3) == 1 and t.stride(1) == W * cs and t.stride(0) == H * W * cs and C <= cs, t.stride()
+    return cs
 
 
 def to_hl(x: torch.Tensor, cp: Optional[int] = None) -> dense.HL:
@@ -58,13 +68,17 @@ def _pack_taps(mats: List[torch.Tensor], taps: List[Tuple[int, int]], cin: int, 
                             dense._PACK_COUNTER)
 
 
-def dgrad_taps(kh: int, kw: int, stride: int, pad: int):
+def dgrad_taps(kh: int, kw: int, stride: int, pad: int, dilation: int = 1):
     """Input gradient of y[o] = sum_t W_t x[o*stride + d_t] as stride-1 convolutions of the output gradient G:
     a list of ((py, px), [(ky, kx, ey, ex)]) -- phase (py, px) of the input (every pixel for stride 1) receives
-    sum over the listed taps of W[:, :, ky, kx]^T G[i + ey, j + ex].  Stride 1: e = -d.  Stride 2: input pixel
-    2i + py is read by tap d when py - d is even, from output i + (py - d) / 2."""
+    sum over the listed taps of W[:, :, ky, kx]^T G[i + ey, j + ex].  Stride 1: e = -d (d = k * dilation - pad).
+    Stride 2 (undilated): input pixel 2i + py is read by tap d when py - d is even, from output i + (py - d) / 2."""
+    if dilation < 1:
+        raise ValueError(f"dilation must be >= 1, got {dilation}")
     if stride == 1:
-        return [((0, 0), [(ky, kx, pad - ky, pad - kx) for ky in range(kh) for kx in range(kw)])]
+        return [((0, 0), [(ky, kx, pad - ky * dilation, pad - kx * dilation) for ky in range(kh) for kx in range(kw)])]
+    if dilation != 1:
+        raise NotImplementedError("input gradient of a dilated stride-2 convolution")
     phases = []
     for py in range(2):
         for px in range(2):
@@ -74,13 +88,13 @@ def dgrad_taps(kh: int, kw: int, stride: int, pad: int):
     return phases
 
 
-def pack_dgrad(weight: torch.Tensor, stride: int, pad: int):
+def pack_dgrad(weight: torch.Tensor, stride: int, pad: int, dilation: int = 1):
     """weight (cout, cin, kh, kw) -> [((py, px), PackedConv or None)]: the transposed (cin x cout) tap matrices of every
     phase, for stp3_conv_fwd on the output gradient."""
     w = weight.detach().float()
     cout, cin, kh, kw = w.shape
     out = []
-    for ph, taps in dgrad_taps(kh, kw, stride, pad):
+    for ph, taps in dgrad_taps(kh, kw, stride, pad, dilation):
         if not taps:
             out.append((ph, None))
             continue
@@ -90,38 +104,42 @@ def pack_dgrad(weight: torch.Tensor, stride: int, pad: int):
 
 
 def conv_raw(x: dense.HL, weight: torch.Tensor, stride: int, bias: Optional[torch.Tensor] = None,
-             sigmoid: bool = False, nchw: bool = False) -> torch.Tensor:
-    """Convolution without folded BatchNorm ('same' zero padding, like every decoder convolution) on stp3_conv_fwd:
-    (N, Ho, Wo, cout) fp32 channels-last, or (N, cout, Ho, Wo) with nchw (the reference's logits layout, optional
-    sigmoid)."""
+             sigmoid: bool = False, nchw: bool = False, dilation: int = 1,
+             img_bias: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """Convolution without folded BatchNorm ('same' zero padding, like every decoder and DeepLab convolution) on
+    stp3_conv_fwd: (N, Ho, Wo, cout) fp32 channels-last, or (N, cout, Ho, Wo) with nchw (the reference's logits layout,
+    optional sigmoid).  img_bias (N, out_tile(cout)) replaces the bias per image."""
     cout = weight.shape[0]
     b = bias.detach().float() if bias is not None else torch.zeros(cout, device=weight.device)
-    pc = dense.pack_conv(weight.detach().float(), b, stride=stride)
+    pc = dense.pack_conv(weight.detach().float(), b, stride=stride, dilation=dilation)
     N, _, H, W, _ = x.hi.shape
     Ho, Wo = (H + stride - 1) // stride, (W + stride - 1) // stride
     if nchw:
         out = torch.empty((N, cout, Ho, Wo), dtype=torch.float32, device=x.hi.device)
     else:
         out = torch.empty((N, Ho, Wo, cout), dtype=torch.float32, device=x.hi.device)
-    dense.conv(x, pc, out_f32=out, n_valid=cout, out_f32_nhwc=not nchw, sigmoid=sigmoid, store=False, tune=(0, 0))
+    dense.conv(x, pc, out_f32=out, n_valid=cout, out_f32_nhwc=not nchw, sigmoid=sigmoid, store=False, tune=(0, 0),
+               img_bias=img_bias)
     return out
 
 
 def conv_dgrad(g: torch.Tensor, weight: torch.Tensor, stride: int, H: int, W: int,
-               packed=None) -> torch.Tensor:
-    """dL/dx (N, H, W, cin) of a 'same'-padded convolution from g = dL/dy (N, Ho, Wo, cout)."""
+               packed=None, dilation: int = 1, img_bias: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """dL/dx (N, H, W, cin) of a 'same'-padded convolution from g = dL/dy (N, Ho, Wo, cout).  Stride 1 only: img_bias
+    (N, out_tile(cin)) is added to every pixel of image n (a spatially constant gradient term, for free)."""
     _f32_cl(g)
     cout, cin, kh, kw = weight.shape
-    pad = (kh - 1) // 2
+    pad = (kh - 1) * dilation // 2
     N = g.shape[0]
-    packed = packed if packed is not None else pack_dgrad(weight, stride, pad)
+    packed = packed if packed is not None else pack_dgrad(weight, stride, pad, dilation)
     g_hl = to_hl(g)
     dev = g.device
     if stride == 1:
         out = torch.empty((N, H, W, cin), dtype=torch.float32, device=dev)
         dense.conv(g_hl, packed[0][1], out_f32=out, n_valid=cin, out_f32_nhwc=True, out_hw=(H, W), store=False,
-                   tune=(0, 0))
+                   tune=(0, 0), img_bias=img_bias)
         return out
+    assert img_bias is None
     phases = []
     for (py, px), pc in packed:
         if pc is None:
@@ -138,18 +156,19 @@ def conv_dgrad(g: torch.Tensor, weight: torch.Tensor, stride: int, H: int, W: in
     return out
 
 
-def conv_wgrad(x: torch.Tensor, g: torch.Tensor, kh: int, kw: int, stride: int) -> torch.Tensor:
+def conv_wgrad(x: torch.Tensor, g: torch.Tensor, kh: int, kw: int, stride: int, dilation: int = 1) -> torch.Tensor:
     """dL/dW (cout, cin, kh, kw) of a 'same'-padded convolution: x (N, H, W, cin) its input, g (N, Ho, Wo, cout)."""
     _f32_cl(x), _f32_cl(g)
     N, H, W, cin = x.shape
     _, Ho, Wo, cout = g.shape
     L = _lib.lib()
-    nbytes = L.stp3_conv_wgrad_scratch_bytes(N, Ho, Wo, cout, cin, kh, kw)
+    nbytes = L.stp3_conv_wgrad_scratch_bytes(N, Ho, Wo, cout, cin, kh, kw, dilation)
     scratch = torch.empty(nbytes, dtype=torch.uint8, device=x.device)
     dw = torch.empty((cout, cin, kh, kw), dtype=torch.float32, device=x.device)
     with torch.cuda.device(x.device):
         code = L.stp3_conv_wgrad(x.data_ptr(), N, H, W, cin, cin, g.data_ptr(), Ho, Wo, cout, cout, kh, kw, stride,
-                                 (kh - 1) // 2, scratch.data_ptr(), nbytes, dw.data_ptr(), _stream(x.device))
+                                 (kh - 1) * dilation // 2, dilation, scratch.data_ptr(), nbytes, dw.data_ptr(),
+                                 _stream(x.device))
     _lib.check(code, "stp3_conv_wgrad")
     return dw
 
@@ -211,12 +230,18 @@ def bn_stats_module(x: torch.Tensor, bn: nn.BatchNorm2d) -> BNStats:
 
 
 def bn_apply(x: torch.Tensor, st: BNStats, gamma: torch.Tensor, beta: torch.Tensor, relu: bool,
-             res: Optional[torch.Tensor] = None, hl: bool = True) -> Tuple[torch.Tensor, Optional[dense.HL]]:
-    """y = relu?(xhat * gamma + beta (+ res)) -> (fp32 (N, H, W, C), HL planes for the next convolution or None)."""
+             res: Optional[torch.Tensor] = None, hl: bool = True, dropout: Tuple[float, int, int] = (0.0, 0, 0),
+             y_out: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, Optional[dense.HL]]:
+    """y = relu?(xhat * gamma + beta (+ res)) [* keep / (1 - p)] -> (fp32 (N, H, W, C), HL planes for the next
+    convolution or None).  dropout = (p, seed, offset): the keep bits of stp3_bn_apply.  y_out: where y goes (default a
+    new tensor; a channel slice of a wider channels-last tensor is fine)."""
     _f32_cl(x)
     N, H, W, C = x.shape
     dev = x.device
-    y = torch.empty_like(x)
+    y = torch.empty_like(x) if y_out is None else y_out
+    assert y.shape == x.shape
+    y_cs = _row_stride(y)
+    p, seed, offset = dropout
     out = dense.HL.empty(N, 1, H, W, C, dev) if hl else None
     g, b = gamma.detach().float().contiguous(), beta.detach().float().contiguous()
     if res is not None:
@@ -224,7 +249,8 @@ def bn_apply(x: torch.Tensor, st: BNStats, gamma: torch.Tensor, beta: torch.Tens
         assert res.shape == x.shape
     with torch.cuda.device(dev):
         code = _lib.lib().stp3_bn_apply(x.data_ptr(), N * H * W, C, C, st.mean.data_ptr(), st.invstd.data_ptr(),
-                                        g.data_ptr(), b.data_ptr(), _p(res), C, int(relu), y.data_ptr(), C,
+                                        g.data_ptr(), b.data_ptr(), _p(res), C, int(relu), float(p), int(seed),
+                                        int(offset), y.data_ptr(), y_cs,
                                         _p(out.hi if out else None), _p(out.lo if out else None),
                                         out.hi.shape[-1] if out else 0, _stream(dev))
     _lib.check(code, "stp3_bn_apply")
@@ -247,30 +273,47 @@ def channel_sums(g: torch.Tensor) -> torch.Tensor:
 
 def bn_backward(g: torch.Tensor, x: torch.Tensor, st: BNStats, gamma: torch.Tensor, y_mask: Optional[torch.Tensor],
                 want_masked: bool = False):
-    """Backward of y = relu?(BN_batch(x) (+ res)): g = dL/dy, y_mask = the forward output y when a ReLU follows.
+    """Backward of y = relu?(BN_batch(x) (+ res)): g = dL/dy, y_mask = the forward output y when a ReLU follows (after
+    dropout, y > 0 marks the kept positive elements; the 1 / (1 - p) factor is the caller's).  g, x and y_mask may be
+    channel slices of wider channels-last tensors.
     -> (dL/dx, dgamma, dbeta, g masked by the ReLU (the gradient of the residual) or None)."""
-    for t in (g, x) + ((y_mask,) if y_mask is not None else ()):
-        _f32_cl(t)
-    C = x.shape[-1]
-    n = x.numel() // C
+    g_cs, x_cs = _row_stride(g), _row_stride(x)
+    y_cs = _row_stride(y_mask) if y_mask is not None else 0
+    N, H, W, C = x.shape
+    n = N * H * W
     dev = x.device
     sum_g = torch.empty(C, dtype=torch.float32, device=dev)
     sum_gx = torch.empty(C, dtype=torch.float32, device=dev)
     scratch, nbytes = _bn_scratch(n, C, dev)
-    gm = torch.empty_like(g) if want_masked else None
-    dx = torch.empty_like(x)
+    gm = torch.empty((N, H, W, C), dtype=torch.float32, device=dev) if want_masked else None
+    dx = torch.empty((N, H, W, C), dtype=torch.float32, device=dev)
     gam = gamma.detach().float().contiguous()
     L = _lib.lib()
     with torch.cuda.device(dev):
-        code = L.stp3_bn_bwd_reduce(g.data_ptr(), C, _p(y_mask), C, x.data_ptr(), C, st.mean.data_ptr(),
+        code = L.stp3_bn_bwd_reduce(g.data_ptr(), g_cs, _p(y_mask), y_cs, x.data_ptr(), x_cs, st.mean.data_ptr(),
                                     st.invstd.data_ptr(), n, C, sum_g.data_ptr(), sum_gx.data_ptr(), scratch.data_ptr(),
                                     nbytes, _stream(dev))
         _lib.check(code, "stp3_bn_bwd_reduce")
-        code = L.stp3_bn_bwd_apply(g.data_ptr(), C, _p(y_mask), C, x.data_ptr(), C, st.mean.data_ptr(),
+        code = L.stp3_bn_bwd_apply(g.data_ptr(), g_cs, _p(y_mask), y_cs, x.data_ptr(), x_cs, st.mean.data_ptr(),
                                    st.invstd.data_ptr(), gam.data_ptr(), sum_g.data_ptr(), sum_gx.data_ptr(), n, C,
                                    dx.data_ptr(), C, _p(gm), C, _stream(dev))
     _lib.check(code, "stp3_bn_bwd_apply")
     return dx, sum_gx, sum_g, gm
+
+
+def image_channel_sums(x: torch.Tensor) -> torch.Tensor:
+    """(N, C) fp32 sums over the H*W pixels of every image of x (N, H, W, C), in a fixed order (stp3_image_channel_sums)."""
+    _f32_cl(x)
+    N, H, W, C = x.shape
+    L = _lib.lib()
+    nbytes = L.stp3_image_channel_sums_scratch_bytes(N, H * W, C)
+    scratch = torch.empty(nbytes, dtype=torch.uint8, device=x.device)
+    out = torch.empty((N, C), dtype=torch.float32, device=x.device)
+    with torch.cuda.device(x.device):
+        code = L.stp3_image_channel_sums(x.data_ptr(), N, H * W, C, C, out.data_ptr(), scratch.data_ptr(), nbytes,
+                                         _stream(x.device))
+    _lib.check(code, "stp3_image_channel_sums")
+    return out
 
 
 # ------------------------------------------------------------------------------------------------ elementwise

@@ -4,15 +4,17 @@
   UpsamplingAdd  : bilinear x2 -> 1x1 conv -> BN, + skip.   Executed as 1x1 conv + folded BN at LOW resolution and a
                    fused upsample+add kernel (the interpolation weights sum to one, so the affine map commutes).
   ASPP / DeepLabHead : the five ASPP branches write straight into one channels-last concat tensor; the global-pool
-                   branch is spatially constant and becomes a per-image bias of the 1x1 projection.
+                   branch is spatially constant and becomes a per-image bias of the 1x1 projection.  DeepLabHead also
+                   runs in train() (batch statistics, dropout, autograd; dense_train.py).
 """
 import os
 from typing import Optional
 
 import torch
 import torch.nn as nn
+from torch.autograd.function import once_differentiable
 
-from .. import dense
+from .. import dense, dense_train
 from ._packing import PackedModule
 
 
@@ -149,9 +151,154 @@ class DeepLabHead(nn.Sequential, PackedModule):
         return dense.conv(y, P["cls"], out=out)
 
     def forward(self, x):
-        """x (N,Cin,H,W) fp32 -> (N,num_classes,H,W) fp32."""
+        """x (N,Cin,H,W) fp32 -> (N,num_classes,H,W) fp32.  In train mode every BatchNorm uses batch statistics (and
+        updates its running ones), the projection's Dropout draws its mask from torch's default generator, and the output
+        carries a grad_fn whose backward fills every parameter's .grad (and x's, when x requires grad)."""
+        if self.training:
+            return self._forward_train(x)
         y = self.forward_hl(dense.from_f32(x.unsqueeze(1)))
         return dense.to_f32(y, 0, self.num_classes).squeeze(1)
+
+    # ------------------------------------------------------------------------------------------------ train mode
+    def _forward_train(self, x: torch.Tensor) -> torch.Tensor:
+        for name, m in self.named_modules():
+            if isinstance(m, nn.modules.batchnorm._BatchNorm):
+                dense_train.check_bn(m, f"DeepLabHead.{name}")
+        if not x.is_cuda or not self[1].weight.is_cuda:
+            raise RuntimeError("stp3_b200 dense ops run on CUDA tensors only (there is no CPU path)")
+        if x.dim() != 4 or x.shape[1] != self.in_channels:
+            raise ValueError(f"DeepLabHead: expected (N, {self.in_channels}, H, W), got {tuple(x.shape)}")
+        if x.shape[0] < 2:
+            # the pooling branch's BatchNorm sees one value per image and channel (nn.BatchNorm2d raises the same)
+            raise ValueError("DeepLabHead (train mode): Expected more than 1 value per channel when training, got input "
+                             f"size {(x.shape[0], self.hidden, 1, 1)} in the ASPP pooling branch")
+        return _DeepLabTrainFn.apply(self, x.float(), *self.parameters())
+
+    def _train_forward(self, x: torch.Tensor):
+        """x (N, Cin, H, W) fp32 -> (logits (N, num_classes, H, W), tape for _train_backward)."""
+        aspp: ASPP = self[0]
+        h, nb = self.hidden, 1 + len(aspp.rates)
+        N, cin, H, W = x.shape
+        dev = x.device
+        x_cl = x.detach().permute(0, 2, 3, 1).contiguous()
+        x_hl = dense_train.to_hl(x_cl)
+        # the nb spatial branches write their activated outputs side by side: the projection's input
+        cat = torch.empty((N, H, W, nb * h), dtype=torch.float32, device=dev)
+        branches = []
+        for i in range(nb):
+            conv, bn = aspp.convs[i][0], aspp.convs[i][1]
+            raw = dense_train.conv_raw(x_hl, conv.weight, 1, dilation=conv.dilation[0])
+            st = dense_train.bn_stats_module(raw, bn)
+            dense_train.bn_apply(raw, st, bn.weight, bn.bias, relu=True, hl=False, y_out=cat[..., i * h:(i + 1) * h])
+            branches.append((conv, bn, raw, st))
+        # global-pool branch: per-image means -> 1x1 -> BatchNorm over the N images -> ReLU; spatially constant, so it
+        # enters the projection as a per-image bias and the broadcast map is never built
+        pconv, pbn = aspp.convs[nb][1], aspp.convs[nb][2]
+        mean = dense_train.image_channel_sums(x_cl) * (1.0 / (H * W))
+        v_raw = torch.empty((N, 1, 1, h), dtype=torch.float32, device=dev)
+        dense.small_linear(mean, pconv.weight.detach().float().reshape(h, cin).contiguous(), v_raw.view(N, h), False)
+        pst = dense_train.bn_stats_module(v_raw, pbn)
+        v, _ = dense_train.bn_apply(v_raw, pst, pbn.weight, pbn.bias, relu=True, hl=False)
+        proj, proj_bn, drop = aspp.project[0], aspp.project[1], aspp.project[3]
+        w_proj = proj.weight.detach().float().reshape(h, (nb + 1) * h)
+        pbias = torch.zeros((N, dense.out_tile(h)), dtype=torch.float32, device=dev)
+        dense.small_linear(v.view(N, h), w_proj[:, nb * h:].contiguous(), pbias, False)
+        praw = dense_train.conv_raw(dense_train.to_hl(cat), w_proj[:, :nb * h].reshape(h, nb * h, 1, 1), 1,
+                                    img_bias=pbias)
+        proj_st = dense_train.bn_stats_module(praw, proj_bn)
+        p = float(drop.p) if drop.training else 0.0
+        seed = int(torch.randint(0, 2 ** 63 - 1, (1,)).item()) if p > 0 else 0     # torch.manual_seed reproduces it
+        z, z_hl = dense_train.bn_apply(praw, proj_st, proj_bn.weight, proj_bn.bias, relu=True, dropout=(p, seed, 0))
+        raw3 = dense_train.conv_raw(z_hl, self[1].weight, 1)
+        st3 = dense_train.bn_stats_module(raw3, self[2])
+        y3, y3_hl = dense_train.bn_apply(raw3, st3, self[2].weight, self[2].bias, relu=True)
+        out = dense_train.conv_raw(y3_hl, self[4].weight, 1, bias=self[4].bias, nchw=True)
+        tape = {"x": x_cl, "cat": cat, "branches": branches, "mean": mean, "v_raw": v_raw, "pst": pst, "v": v,
+                "praw": praw, "proj_st": proj_st, "p": p, "z": z, "raw3": raw3, "st3": st3, "y3": y3}
+        return out, tape
+
+    def _train_backward(self, tape, g_out: torch.Tensor, need_x: bool):
+        """Reverse walk of _train_forward -> (dL/dx (N, Cin, H, W) or None, {parameter: gradient})."""
+        aspp: ASPP = self[0]
+        h, nb = self.hidden, 1 + len(aspp.rates)
+        x_cl = tape["x"]
+        N, H, W, cin = x_cl.shape
+        dev = x_cl.device
+        grads = {}
+        conv3, bn3, cls = self[1], self[2], self[4]
+        g = g_out.float().permute(0, 2, 3, 1).contiguous()
+        grads[cls.bias] = dense_train.channel_sums(g)
+        grads[cls.weight] = dense_train.conv_wgrad(tape["y3"], g, 1, 1, 1)
+        g = dense_train.conv_dgrad(g, cls.weight, 1, H, W)
+        g, grads[bn3.weight], grads[bn3.bias], _ = dense_train.bn_backward(g, tape["raw3"], tape["st3"], bn3.weight,
+                                                                          tape["y3"])
+        grads[conv3.weight] = dense_train.conv_wgrad(tape["z"], g, 3, 3, 1)
+        # dropout: z > 0 marks the kept positive elements (the projection BN's mask below); the 1 / (1 - p) factor of
+        # the kept ones rides on the transposed 3x3 weights
+        p = tape["p"]
+        w3 = conv3.weight.detach().float() * (1.0 / (1.0 - p)) if p > 0 else conv3.weight
+        g = dense_train.conv_dgrad(g, w3, 1, H, W)
+        proj, proj_bn = aspp.project[0], aspp.project[1]
+        g, grads[proj_bn.weight], grads[proj_bn.bias], _ = dense_train.bn_backward(g, tape["praw"], tape["proj_st"],
+                                                                                  proj_bn.weight, tape["z"])
+        # projection: the spatial branches' columns from the concat tensor, the pooled ones from the per-image sums of g
+        w_proj = proj.weight.detach().float().reshape(h, (nb + 1) * h)
+        gsum = dense_train.image_channel_sums(g)
+        dw_pool = dense_train.conv_wgrad(tape["v"], gsum.view(N, 1, 1, h), 1, 1, 1)
+        grads[proj.weight] = torch.cat([dense_train.conv_wgrad(tape["cat"], g, 1, 1, 1), dw_pool], dim=1)
+        g_v = torch.empty((N, 1, 1, h), dtype=torch.float32, device=dev)
+        dense.small_linear(gsum, w_proj[:, nb * h:].t().contiguous(), g_v.view(N, h), False)
+        pconv, pbn = aspp.convs[nb][1], aspp.convs[nb][2]
+        g_v, grads[pbn.weight], grads[pbn.bias], _ = dense_train.bn_backward(g_v, tape["v_raw"], tape["pst"],
+                                                                            pbn.weight, tape["v"])
+        grads[pconv.weight] = dense_train.conv_wgrad(tape["mean"].view(N, 1, 1, cin), g_v, 1, 1, 1)
+        gx = None
+        if need_x:
+            # the pooled branch's input gradient, W1^T g_v / (H W) per image, is added by the first branch's dgrad
+            # epilogue as its per-image bias
+            w1t = pconv.weight.detach().float().reshape(h, cin).t() * (1.0 / (H * W))
+            gx_pool = torch.zeros((N, dense.out_tile(cin)), dtype=torch.float32, device=dev)
+            dense.small_linear(g_v.view(N, h), w1t.contiguous(), gx_pool, False)
+        for i, (conv, bn, raw, st) in enumerate(tape["branches"]):
+            sl = slice(i * h, (i + 1) * h)
+            gb = dense_train.conv_dgrad(g, w_proj[:, sl].reshape(h, h, 1, 1), 1, H, W)
+            gb, grads[bn.weight], grads[bn.bias], _ = dense_train.bn_backward(gb, raw, st, bn.weight,
+                                                                             tape["cat"][..., sl])
+            k, d = conv.kernel_size[0], conv.dilation[0]
+            grads[conv.weight] = dense_train.conv_wgrad(x_cl, gb, k, k, 1, dilation=d)
+            if need_x:
+                gxi = dense_train.conv_dgrad(gb, conv.weight, 1, H, W, dilation=d,
+                                             img_bias=gx_pool if i == 0 else None)
+                gx = gxi if gx is None else gx.add_(gxi)
+        return (gx.permute(0, 3, 1, 2).contiguous() if need_x else None), grads
+
+
+class _DeepLabTrainFn(torch.autograd.Function):
+    """The train-mode DeepLab head as one autograd node, like the decoder's (_DecoderTrainFn): forward keeps the
+    activations and statistics, backward walks the layers in reverse on the train-mode kernels.  The backward is not
+    itself differentiable, runs once per forward (retain_graph is refused), and refuses weights modified in place
+    between forward and backward."""
+
+    @staticmethod
+    def forward(ctx, head, x, *params):
+        out, tape = head._train_forward(x)
+        ctx.head, ctx.tape, ctx.params = head, tape, params
+        ctx.versions = [p._version for p in params]
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g_out):
+        if ctx.tape is None:
+            raise RuntimeError("DeepLabHead (train mode): backward ran a second time through the same forward; the "
+                               "activations are released after the first backward (retain_graph is not supported) -- "
+                               "run the forward again")
+        if any(p._version != v for p, v in zip(ctx.params, ctx.versions)):
+            raise RuntimeError("DeepLabHead (train mode): a head parameter was modified in place between forward and "
+                               "backward (e.g. optimizer.step() before loss.backward())")
+        tape, ctx.tape = ctx.tape, None
+        gx, grads = ctx.head._train_backward(tape, g_out, ctx.needs_input_grad[1])
+        return (None, gx) + tuple(grads.get(p) for p in ctx.params)
 
 
 class UpsamplingConcat(PackedModule):

@@ -193,6 +193,9 @@ class STP3(nn.Module):
         C = self.encoder_out_channels
         off, res, dim = self._bev_host()
         output = {'depth_prediction': depth_logits, 'cam_front': None}
+        if self._head_training() and not self.decoder.training:
+            raise RuntimeError("STP3: temporal_model.final_conv is in train mode but the decoder is in eval mode, so no "
+                               "gradient could reach the head -- call model.decoder.train() as well")
 
         self._mark("start")
         planes = torch.empty((2, B, S, X, Y, C), dtype=torch.bfloat16, device=dev)
@@ -214,9 +217,13 @@ class STP3(nn.Module):
         else:
             states = self.temporal_model.forward_hl(x, const=const if use_ego else None, sums=sums)
         self._mark("temporal_model")
-        output.update(self.decoder.forward_hl(states))
+        # a train-mode head hands over fp32 (B, S, C, X, Y) with a grad_fn, for the train-mode decoder
+        output.update(self.decoder(states) if torch.is_tensor(states) else self.decoder.forward_hl(states))
         self._mark("decoder")
         return output
+
+    def _head_training(self) -> bool:
+        return isinstance(self.temporal_model, TemporalModel) and self.temporal_model.final_conv.training
 
     def forward_features_frame_sharded(self, feat, depth_logits, intrinsics, extrinsics, future_egomotion, gather="nccl"):
         """Latency mode for a global batch smaller than the number of GPUs (SURVEY.md §8e): the B*S camera frames are
@@ -276,6 +283,9 @@ class STP3(nn.Module):
         use_ego = self.cfg.MODEL.TEMPORAL_MODEL.INPUT_EGOPOSE
         if isinstance(self.temporal_model, TemporalModelIdentity):
             raise NotImplementedError("frame-sharded mode is wired for the temporal_block model")
+        if self._head_training():
+            raise RuntimeError("frame-sharded forward: temporal_model.final_conv is in train mode; the sharded path runs "
+                               "the inference forward only -- call .eval() on it")
         states = self.temporal_model.forward_hl(x, const=h["const"] if use_ego else None, sums=None)
         output.update(self.decoder.forward_hl(states))
         return output
@@ -318,6 +328,9 @@ class GraphedPerception:
         if model.decoder.training:
             raise RuntimeError("GraphedPerception: the decoder is in train mode (batch statistics, running-statistics "
                                "updates, autograd); a CUDA graph replays the inference forward only -- call .eval()")
+        if model._head_training():
+            raise RuntimeError("GraphedPerception: temporal_model.final_conv is in train mode (batch statistics, "
+                               "dropout, autograd); a CUDA graph replays the inference forward only -- call .eval()")
         self.model = model
         self.entry = entry
         dev = torch.device(device) if device is not None else next(model.parameters()).device

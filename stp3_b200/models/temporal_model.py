@@ -26,7 +26,9 @@ class TemporalModel(nn.Module):
         self.final_conv = DeepLabHead(block_out, block_out, hidden_channel=128)
         self.model = nn.Sequential(*blocks)
 
-    def forward_hl(self, x: dense.HL, const=None, sums=None) -> dense.HL:
+    def forward_hl(self, x: dense.HL, const=None, sums=None):
+        """x: HL (B, S, H, W, .) -> HL with the head's channels; with final_conv in train mode (and the blocks in eval
+        mode) an fp32 (B, S, C, H, W) tensor with a grad_fn instead (the head's batch statistics, dropout, autograd)."""
         n_img = x.hi.shape[0] * x.hi.shape[1]
         for i, block in enumerate(self.model):
             # a 64-channel block hands the spatial sums of its output (the next block's pyramid pooling / the head's
@@ -36,12 +38,16 @@ class TemporalModel(nn.Module):
                 nxt = torch.empty((n_img, 64), dtype=torch.float32, device=x.hi.device)
             x = block.forward_hl(x, const if i == 0 else None, sums, out_sums=nxt)
             sums = nxt
+        if self.final_conv.training:
+            B, S = x.hi.shape[:2]
+            y = self.final_conv(dense.to_f32(x, 0, self.final_conv.in_channels).flatten(0, 1))
+            return y.view(B, S, *y.shape[1:])
         return self.final_conv.forward_hl(x, sums=sums)
 
     def forward(self, x):
         """x (B, S, C, H, W) fp32 -> (B, S, Cout, H, W) fp32."""
         y = self.forward_hl(dense.from_f32(x))
-        return dense.to_f32(y, 0, self.final_conv.num_classes)
+        return y if torch.is_tensor(y) else dense.to_f32(y, 0, self.final_conv.num_classes)
 
 
 class TemporalModelIdentity(nn.Module):
