@@ -318,8 +318,9 @@ int stp3_upsample2x_add(const void* x_hi, const void* x_lo, int n_img, int h, in
                         int C, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------
- * Train mode of the BEV decoder and the DeepLab head (stp3/models/decoder.py, stp3/layers/convolutions.py:227-280 in
- * train(): BatchNorm with batch statistics, dropout, autograd).
+ * Train mode of the BEV decoder, the DeepLab head and the TemporalBlocks (stp3/models/decoder.py,
+ * stp3/layers/convolutions.py:227-280, stp3/layers/temporal.py:252-489 in train(): BatchNorm with batch statistics,
+ * dropout, autograd).
  * Tensors are fp32 channels-last (n_pix, cstride) with the channels at [0, C) of each row unless noted; every
  * reduction is deterministic (per-block partials in `scratch`, summed in a fixed order, no float atomics), so two calls
  * on the same inputs return bitwise-identical results.  The input gradient of a convolution is stp3_conv_fwd itself
@@ -335,6 +336,18 @@ size_t stp3_conv_wgrad_scratch_bytes(int n_img, int Ho, int Wo, int cout, int ci
 int stp3_conv_wgrad(const float* x, int n_img, int H, int W, int x_cstride, int cin, const float* g, int Ho, int Wo,
                     int g_cstride, int cout, int kh, int kw, int stride, int pad, int dilation, void* scratch,
                     size_t scratch_bytes, float* dw, void* stream);
+/* Weight gradient of a causal (kt, kh, kw) 3-D convolution (stride 1, 'same' spatial padding (kh-1)/2, kh == kw odd,
+ * time padded on the left by kt - 1: the TemporalBlock's CausalConv3d, temporal.py:252-269), reference layout
+ * (cout, cin, kt, kh, kw):
+ *   dw[co][ci][it][ky][kx] = sum over b, t and pixels of g[b][t][p][co] * x[b][t + it - (kt-1)][p + (ky, kx) - pad][ci]
+ *   x (B, T, H, W, x_cstride), g (B, T, H, W, g_cstride); frames and pixels outside the tensor are zeros.  A time tap
+ *   that reads padding for every output frame (kt - 1 - it >= T) stores exact zeros without reading pixels.
+ *   scratch: stp3_conv3d_wgrad_scratch_bytes() bytes.  The same GEMM, split and ordered reduction as stp3_conv_wgrad
+ *   (deterministic).  The input gradient is stp3_conv_fwd with the mirrored taps (kt-1-it, pad-ky, pad-kx): their time
+ *   offsets are >= 0, and frames at or past T read as zero. */
+size_t stp3_conv3d_wgrad_scratch_bytes(int B, int T, int H, int W, int cout, int cin, int kt, int kh, int kw);
+int stp3_conv3d_wgrad(const float* x, int B, int T, int H, int W, int x_cstride, int cin, const float* g, int g_cstride,
+                      int cout, int kt, int kh, int kw, void* scratch, size_t scratch_bytes, float* dw, void* stream);
 /* BatchNorm batch statistics over n_pix rows (two passes: mean, then the centred sum of squares; fp64 partials):
  * mean[C], var[C] (biased; may be NULL), invstd = 1/sqrt(var + eps); when running_mean/var are given they are updated
  * like nn.BatchNorm2d: r = (1 - momentum) r + momentum b, with the unbiased variance var * n/(n-1).
@@ -344,7 +357,9 @@ int stp3_bn_stats(const float* x, long long n_pix, int C, int x_cstride, float e
                   float* running_var, float* mean, float* var, float* invstd, void* scratch, size_t scratch_bytes,
                   void* stream);
 /* y = relu?((x - mean) * invstd * gamma + beta (+ res)) -> fp32 y (may be NULL) and/or bf16 hi/lo planes (n_pix,
- * hl_cstride) for the next stp3_conv_fwd (channels [C, hl_cstride) written as zeros).  C % 8 == 0, 16-byte rows.
+ * hl_cstride) for the next stp3_conv_fwd (channels [C, hl_cstride) written as zeros).  Any C and fp32 row strides (8
+ * channels per thread when C % 8 == 0 and every fp32 row is 16-byte aligned, else one element per thread: the same
+ * values); the bf16 planes need hl_cstride % 8 == 0 and 16-byte alignment.
  * Dropout (0 <= dropout_p < 1; 0 = none, bit for bit): y is then multiplied by m / (1 - p), where the keep bit m of
  * element (pixel, c) depends only on (seed, offset + pixel * C + c): word e % 4 of Philox-4x32-10 with key seed and
  * counter (e / 4, 0) (64-bit values as (low, high) words), read as (word >> 8) / 2^24, keeps when it is >= p.  So a
@@ -366,7 +381,7 @@ size_t stp3_image_channel_sums_scratch_bytes(int n_img, long long hw, int C);
 int stp3_image_channel_sums(const float* x, int n_img, long long hw, int C, int x_cstride, float* sums, void* scratch,
                             size_t scratch_bytes, void* stream);
 /* dx = gamma * invstd * (g' - sum_g/n - xhat * sum_gxhat/n); g_masked (optional) receives g' (the gradient of a residual
- * that was added before the ReLU). */
+ * that was added before the ReLU).  Any C and row strides (vector path under the conditions of stp3_bn_apply). */
 int stp3_bn_bwd_apply(const float* g, int g_cstride, const float* y, int y_cstride, const float* x, int x_cstride,
                       const float* mean, const float* invstd, const float* gamma, const float* sum_g,
                       const float* sum_gxhat, long long n_pix, int C, float* dx, int dx_cstride, float* g_masked,
@@ -381,6 +396,14 @@ int stp3_phase_interleave(const float* p00, const float* p01, const float* p10, 
                           int C, float* out, void* stream);
 /* dz = g * s * (1 - s), s = sigmoid(z) the forward output (instance_center head, decoder.py:70) */
 int stp3_sigmoid_bwd(const float* g, const float* s, long long n, float* dz, void* stream);
+/* The pyramid-pooling branch of a TemporalBlock in time (AvgPool3d((2, H, W)), time padding 1,
+ * count_include_pad=False; temporal.py:375-423) on per-frame means m (B, T, C) fp32:
+ *   adjoint == 0: the T + 1 pooled frames out (B, T + 1, C): out[b][0] = m[b][0], out[b][t] = (m[b][t-1] + m[b][t]) / 2
+ *   for 1 <= t < T, out[b][T] = m[b][T-1].  The reference drops frame T only after the branch's BatchNorm, so its
+ *   batch statistics cover B * (T + 1) values.
+ *   adjoint != 0 (its transpose): m is a gradient (B, T + 1, C), out (B, T, C): out[b][t] = c_t m[b][t] + m[b][t+1] / 2
+ *   for t + 1 < T, c_t m[b][t] + m[b][T] for t = T - 1; c_0 = 1, c_t = 1/2 for t >= 1.  out must not alias m. */
+int stp3_temporal_pair_mean(const float* m, int B, int T, int C, int adjoint, float* out, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------
  * EfficientNet trunk (efficientnet-pytorch 0.7.0, truncated like stp3/models/encoder.py:39-55).  The 1x1 expand and

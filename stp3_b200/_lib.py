@@ -110,6 +110,10 @@ SIGNATURES = {
     "stp3_upsample2x_bwd": (_I, [_V, _I, _I, _I, _I, _V, _V]),
     "stp3_phase_interleave": (_I, [_V, _V, _V, _V, _I, _I, _I, _I, _V, _V]),
     "stp3_sigmoid_bwd": (_I, [_V, _V, _LL, _V, _V]),
+    # train mode of the TemporalBlocks
+    "stp3_conv3d_wgrad_scratch_bytes": (_SZ, [_I, _I, _I, _I, _I, _I, _I, _I, _I]),
+    "stp3_conv3d_wgrad": (_I, [_V, _I, _I, _I, _I, _I, _I, _V, _I, _I, _I, _I, _I, _V, _SZ, _V, _V]),
+    "stp3_temporal_pair_mean": (_I, [_V, _I, _I, _I, _I, _V, _V]),
     # EfficientNet trunk
     "stp3_effnet_stem": (_I, [_V, _I, _I, _I, _I, _I, _I, _I, _V, _V, _I, _I, _V, _V, _V]),
     "stp3_dw_sums_scratch_bytes": (_SZ, [ctypes.POINTER(DwDesc)]),

@@ -5,6 +5,8 @@
 // noted.  Every reduction is deterministic: per-block partials go to caller scratch and are summed in a fixed order
 // (no float atomics), and the block decomposition depends only on the problem shape, so two calls on the same inputs
 // return bitwise-identical results.
+#include <climits>
+
 #include <cuda_bf16.h>
 
 #include "common.cuh"
@@ -24,8 +26,11 @@ namespace stp3 {
 constexpr int kWgTile = 64, kWgK = 64;
 constexpr int kWgTileBytes = kWgK * kWgTile * 2;          // one bf16 plane of one operand: 64 pixels x 128 B
 
+// n_img = B * T images, frame-major within a sample; kt > 1: causal time taps, output frame t of a sample reads frame
+// t + it - (kt - 1) of the same sample (frames outside [0, T) are zeros).  T = kt = 1 is the 2-D convolution.
 struct WgradShape {
   int n_img, H, W, x_cstride, cin, Ho, Wo, g_cstride, cout, stride, kh, kw, pad, dil;
+  int T = 1, kt = 1;
 };
 
 // does an output axis of n_out positions, read at o * stride + d, touch the input extent [0, n_in) at all?
@@ -38,7 +43,7 @@ __host__ __device__ inline long long wgrad_pixels(const WgradShape& s) { return 
 
 // the K split: a function of the shape only (determinism), ~4 CTAs per SM of an H100, >= 256 pixels per CTA
 inline int wgrad_splits(const WgradShape& s) {
-  const long long tiles = (long long)s.kh * s.kw * ceil_div(s.cout, kWgTile) * ceil_div(s.cin, kWgTile);
+  const long long tiles = (long long)s.kt * s.kh * s.kw * ceil_div(s.cout, kWgTile) * ceil_div(s.cin, kWgTile);
   const long long px = wgrad_pixels(s);
   long long n = (132 * 4 + tiles - 1) / tiles;
   const long long max_by_px = (px + 255) / 256;
@@ -75,11 +80,12 @@ wgrad_partial_kernel(const float* __restrict__ x, const float* __restrict__ g, W
   int t = blockIdx.y;
   const int cit = t % ci_tiles; t /= ci_tiles;
   const int cot = t % co_tiles; t /= co_tiles;
-  const int tap = t;                                   // ky * kw + kx
-  const int dy = tap / s.kw * s.dil - s.pad, dx = tap % s.kw * s.dil - s.pad;
-  // a tap whose window lies in the zero padding for every output pixel (large dilations on small maps) contributes
-  // exact zeros: the CTA stores them without streaming the pixels
-  const bool live = tap_in_image(dy, s.Ho, s.stride, s.H) && tap_in_image(dx, s.Wo, s.stride, s.W);
+  const int tap = t;                                   // (it * kh + ky) * kw + kx
+  const int dy = tap / s.kw % s.kh * s.dil - s.pad, dx = tap % s.kw * s.dil - s.pad;
+  const int dt = tap / (s.kw * s.kh) - (s.kt - 1);     // <= 0: causal
+  // a tap whose window lies in the zero padding for every output pixel (large dilations on small maps, a time offset
+  // of T frames or more) contributes exact zeros: the CTA stores them without streaming the pixels
+  const bool live = tap_in_image(dy, s.Ho, s.stride, s.H) && tap_in_image(dx, s.Wo, s.stride, s.W) && -dt < s.T;
   const long long P = wgrad_pixels(s);
   const long long p_begin = (long long)blockIdx.x * px_per_split;
   const long long p_end = p_begin + px_per_split < P ? p_begin + px_per_split : P;
@@ -104,8 +110,9 @@ wgrad_partial_kernel(const float* __restrict__ x, const float* __restrict__ g, W
         const int oy = (int)(q % s.Ho);
         const long long img = q / s.Ho;
         grow = g + p * s.g_cstride + co0;
-        const int iy = oy * s.stride + dy, ix = ox * s.stride + dx;
-        if (iy >= 0 && iy < s.H && ix >= 0 && ix < s.W) xrow = x + ((img * s.H + iy) * s.W + ix) * s.x_cstride + ci0;
+        const int iy = oy * s.stride + dy, ix = ox * s.stride + dx, it = (int)(img % s.T) + dt;
+        if (iy >= 0 && iy < s.H && ix >= 0 && ix < s.W && it >= 0)
+          xrow = x + (((img + dt) * s.H + iy) * s.W + ix) * s.x_cstride + ci0;
       }
       uint4 gh, gl, xh, xl;
       load8_split(grow, c * 8, s.cout - co0, vec_g, gh, gl);
@@ -135,7 +142,7 @@ wgrad_partial_kernel(const float* __restrict__ x, const float* __restrict__ g, W
     __syncthreads();                                   // every warp's MMAs have read the stage before it is rewritten
   }
   // part[split][tap][co][ci]; accumulator fragment: row = co, column = ci (wgmma.cuh)
-  float* dst = part + ((size_t)blockIdx.x * s.kh * s.kw + tap) * (size_t)s.cout * s.cin;
+  float* dst = part + ((size_t)blockIdx.x * s.kt * s.kh * s.kw + tap) * (size_t)s.cout * s.cin;
   const int w = tid >> 5, l = tid & 31;
 #pragma unroll
   for (int i = 0; i < 32; ++i) {
@@ -384,6 +391,80 @@ bn_bwd_apply_kernel(const float* __restrict__ g, int g_cs, const float* __restri
   }
 }
 
+// keep bit of one flat element e (the bit dropout_keep8 gives it)
+__device__ __forceinline__ bool dropout_keep1(unsigned long long seed, unsigned long long e, float p) {
+  const unsigned long long q = e >> 2;
+  const uint4 r = philox4x32_10((uint32_t)seed, (uint32_t)(seed >> 32), make_uint4((uint32_t)q, (uint32_t)(q >> 32), 0u, 0u));
+  const uint32_t w = (e & 3) == 0 ? r.x : (e & 3) == 1 ? r.y : (e & 3) == 2 ? r.z : r.w;
+  return (float)(w >> 8) * (1.f / 16777216.f) >= p;
+}
+
+// bn_apply_kernel for any C and row stride (channel windows at odd offsets, C % 8 != 0): one thread = one element of
+// the n_cols = max(C, hl_cs) columns; the same arithmetic per element as the vector kernel
+__global__ void __launch_bounds__(256)
+bn_apply_scalar_kernel(const float* __restrict__ x, int x_cs, const float* __restrict__ mean,
+                       const float* __restrict__ invstd, const float* __restrict__ gamma, const float* __restrict__ beta,
+                       const float* __restrict__ res, int res_cs, int relu, float drop_p, unsigned long long seed,
+                       unsigned long long offset, long long n_pix, int C, int n_cols, float* __restrict__ y, int y_cs,
+                       __nv_bfloat16* __restrict__ yh, __nv_bfloat16* __restrict__ yl, int hl_cs) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n_pix * n_cols) return;
+  const int c = (int)(i % n_cols);
+  const long long p = i / n_cols;
+  float v = 0.f;
+  if (c < C) {
+    const float r = res ? res[p * res_cs + c] : 0.f;
+    const float t = (x[p * x_cs + c] - mean[c]) * invstd[c] * gamma[c] + beta[c] + r;
+    v = relu ? fmaxf(t, 0.f) : t;
+    if (drop_p > 0.f) v = dropout_keep1(seed, offset + (unsigned long long)p * C + c, drop_p) ? v * (1.f / (1.f - drop_p)) : 0.f;
+    if (y) y[p * y_cs + c] = v;
+  }
+  if (yh && c < hl_cs) ptx::split_hilo(v, yh[p * hl_cs + c], yl[p * hl_cs + c]);
+}
+
+// bn_bwd_apply_kernel for any C and row stride: one thread = one element
+__global__ void __launch_bounds__(256)
+bn_bwd_apply_scalar_kernel(const float* __restrict__ g, int g_cs, const float* __restrict__ y, int y_cs,
+                           const float* __restrict__ x, int x_cs, const float* __restrict__ mean,
+                           const float* __restrict__ invstd, const float* __restrict__ gamma,
+                           const float* __restrict__ sum_g, const float* __restrict__ sum_gx, long long n_pix, int C,
+                           float* __restrict__ dx, int dx_cs, float* __restrict__ gm, int gm_cs) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n_pix * C) return;
+  const int c = (int)(i % C);
+  const long long p = i / C;
+  const float inv_n = 1.f / (float)n_pix;
+  float gv = g[p * g_cs + c];
+  if (y && !(y[p * y_cs + c] > 0.f)) gv = 0.f;
+  const float xh = (x[p * x_cs + c] - mean[c]) * invstd[c];
+  dx[p * dx_cs + c] = gamma[c] * invstd[c] * (gv - sum_g[c] * inv_n - xh * sum_gx[c] * inv_n);
+  if (gm) gm[p * gm_cs + c] = gv;
+}
+
+// The pooled branch of a TemporalBlock in time (AvgPool3d((2, H, W)), time padding 1, count_include_pad=False) on
+// per-image means m (B, T, C): the T + 1 pooled frames p (B, T + 1, C), p[0] = m[0], p[t] = (m[t-1] + m[t]) / 2 for
+// 1 <= t < T, p[T] = m[T-1] (the reference drops that frame only after its BatchNorm).  adjoint: g (B, T + 1, C) ->
+// (B, T, C), out[t] = c_t g[t] + (t + 1 < T ? g[t+1] / 2 : g[T]), c_0 = 1, c_t = 1/2.  One thread per output element.
+__global__ void __launch_bounds__(256)
+temporal_pair_mean_kernel(const float* __restrict__ m, int T, int C, long long total, int adjoint,
+                          float* __restrict__ out) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= total) return;
+  const int c = (int)(i % C);
+  if (!adjoint) {                                      // i over (B, T + 1, C)
+    const int t = (int)(i / C % (T + 1));
+    const long long b = i / C / (T + 1);
+    const float* mb = m + b * T * C + c;
+    out[i] = t == 0 ? mb[0] : t == T ? mb[(long long)(T - 1) * C] : 0.5f * (mb[(long long)(t - 1) * C] + mb[(long long)t * C]);
+  } else {                                             // i over (B, T, C)
+    const int t = (int)(i / C % T);
+    const long long b = i / C / T;
+    const float* gb = m + b * (T + 1) * C + c;
+    const float a = t == 0 ? gb[0] : 0.5f * gb[(long long)t * C];
+    out[i] = a + (t + 1 < T ? 0.5f * gb[(long long)(t + 1) * C] : gb[(long long)T * C]);
+  }
+}
+
 // bilinear x2, align_corners=False (nn.Upsample of UpsamplingAdd): source coordinate (o + 0.5) / 2 - 0.5 clamped at 0
 __device__ __forceinline__ void up_coord(int o, int n, int& i0, int& i1, float& w0, float& w1) {
   const float f = fmaxf((o + 0.5f) * 0.5f - 0.5f, 0.f);
@@ -496,6 +577,28 @@ extern "C" size_t stp3_conv_wgrad_scratch_bytes(int n_img, int Ho, int Wo, int c
   return (size_t)wgrad_splits(s) * kh * kw * (size_t)cout * cin * sizeof(float);
 }
 
+// the partial GEMMs and the ordered reduction of one (validated) weight gradient
+static int launch_wgrad(const WgradShape& s, const float* x, const float* g, float* scratch, float* dw, cudaStream_t st,
+                        const char* what) {
+  const int n_split = wgrad_splits(s);
+  const long long P = wgrad_pixels(s);
+  long long per = (P + n_split - 1) / n_split;
+  per = (per + kWgK - 1) / kWgK * kWgK;
+  const int ntaps = s.kt * s.kh * s.kw;
+  const long long tiles = (long long)ntaps * ceil_div(s.cout, kWgTile) * ceil_div(s.cin, kWgTile);
+  if (tiles >= 65536) return stp3::set_error(STP3_EINVAL, "%s: too many output tiles", what);
+  // float4 loads need 16-byte aligned rows
+  const int vec_x = s.x_cstride % 4 == 0 && (reinterpret_cast<uintptr_t>(x) & 15) == 0;
+  const int vec_g = s.g_cstride % 4 == 0 && (reinterpret_cast<uintptr_t>(g) & 15) == 0;
+  const size_t smem = 4 * kWgTileBytes + 1024;
+  wgrad_partial_kernel<<<dim3(n_split, (unsigned)tiles), 128, smem, st>>>(x, g, s, per, vec_x, vec_g, scratch);
+  STP3_CUDA_OK(cudaGetLastError());
+  const long long n = (long long)ntaps * s.cout * s.cin;
+  wgrad_reduce_kernel<<<blocks_for(n), 256, 0, st>>>(scratch, n_split, ntaps, s.cout, s.cin, dw);
+  STP3_CUDA_OK(cudaGetLastError());
+  return STP3_OK;
+}
+
 extern "C" int stp3_conv_wgrad(const float* x, int n_img, int H, int W, int x_cstride, int cin, const float* g, int Ho,
                                int Wo, int g_cstride, int cout, int kh, int kw, int stride, int pad, int dilation,
                                void* scratch, size_t scratch_bytes, float* dw, void* stream) {
@@ -508,23 +611,31 @@ extern "C" int stp3_conv_wgrad(const float* x, int n_img, int H, int W, int x_cs
   const size_t need = stp3_conv_wgrad_scratch_bytes(n_img, Ho, Wo, cout, cin, kh, kw, dilation);
   STP3_CHECK_ARG(scratch_bytes >= need, "stp3_conv_wgrad: scratch smaller than stp3_conv_wgrad_scratch_bytes()");
   WgradShape s{n_img, H, W, x_cstride, cin, Ho, Wo, g_cstride, cout, stride, kh, kw, pad, dilation};
-  const int n_split = wgrad_splits(s);
-  const long long P = wgrad_pixels(s);
-  long long per = (P + n_split - 1) / n_split;
-  per = (per + kWgK - 1) / kWgK * kWgK;
-  const long long tiles = (long long)kh * kw * ceil_div(cout, kWgTile) * ceil_div(cin, kWgTile);
-  STP3_CHECK_ARG(tiles < 65536, "stp3_conv_wgrad: too many output tiles");
-  // float4 loads need 16-byte aligned rows
-  const int vec_x = x_cstride % 4 == 0 && (reinterpret_cast<uintptr_t>(x) & 15) == 0;
-  const int vec_g = g_cstride % 4 == 0 && (reinterpret_cast<uintptr_t>(g) & 15) == 0;
-  cudaStream_t st = (cudaStream_t)stream;
-  const size_t smem = 4 * kWgTileBytes + 1024;
-  wgrad_partial_kernel<<<dim3(n_split, (unsigned)tiles), 128, smem, st>>>(x, g, s, per, vec_x, vec_g, (float*)scratch);
-  STP3_CUDA_OK(cudaGetLastError());
-  const long long n = (long long)kh * kw * cout * cin;
-  wgrad_reduce_kernel<<<blocks_for(n), 256, 0, st>>>((const float*)scratch, n_split, kh * kw, cout, cin, dw);
-  STP3_CUDA_OK(cudaGetLastError());
-  return STP3_OK;
+  return launch_wgrad(s, x, g, (float*)scratch, dw, (cudaStream_t)stream, "stp3_conv_wgrad");
+}
+
+extern "C" size_t stp3_conv3d_wgrad_scratch_bytes(int B, int T, int H, int W, int cout, int cin, int kt, int kh, int kw) {
+  if (B <= 0 || T <= 0 || H <= 0 || W <= 0 || cout <= 0 || cin <= 0 || kt <= 0 || kh <= 0 || kw <= 0) return 0;
+  if ((long long)B * T > INT_MAX) return 0;
+  WgradShape s{};
+  s.n_img = B * T; s.Ho = H; s.Wo = W; s.cout = cout; s.cin = cin; s.kh = kh; s.kw = kw; s.T = T; s.kt = kt;
+  return (size_t)wgrad_splits(s) * kt * kh * kw * (size_t)cout * cin * sizeof(float);
+}
+
+extern "C" int stp3_conv3d_wgrad(const float* x, int B, int T, int H, int W, int x_cstride, int cin, const float* g,
+                                 int g_cstride, int cout, int kt, int kh, int kw, void* scratch, size_t scratch_bytes,
+                                 float* dw, void* stream) {
+  STP3_CHECK_ARG(x && g && dw && scratch, "stp3_conv3d_wgrad: null pointer argument");
+  STP3_CHECK_ARG(B > 0 && T > 0 && H > 0 && W > 0 && cin > 0 && cout > 0 && kt > 0 && kh > 0 && kw > 0,
+                 "stp3_conv3d_wgrad: non-positive dimension");
+  STP3_CHECK_ARG((long long)B * T <= INT_MAX, "stp3_conv3d_wgrad: too many frames");
+  STP3_CHECK_ARG(kh == kw && kh % 2 == 1, "stp3_conv3d_wgrad: the spatial kernel must be square and odd");
+  STP3_CHECK_ARG(cin <= x_cstride && cout <= g_cstride, "stp3_conv3d_wgrad: channel count exceeds the row stride");
+  const size_t need = stp3_conv3d_wgrad_scratch_bytes(B, T, H, W, cout, cin, kt, kh, kw);
+  STP3_CHECK_ARG(scratch_bytes >= need, "stp3_conv3d_wgrad: scratch smaller than stp3_conv3d_wgrad_scratch_bytes()");
+  WgradShape s{B * T, H, W, x_cstride, cin, H, W, g_cstride, cout, 1, kh, kw, (kh - 1) / 2, 1};
+  s.T = T; s.kt = kt;
+  return launch_wgrad(s, x, g, (float*)scratch, dw, (cudaStream_t)stream, "stp3_conv3d_wgrad");
 }
 
 extern "C" size_t stp3_bn_scratch_bytes(long long n_pix, int C) {
@@ -562,11 +673,22 @@ extern "C" int stp3_bn_apply(const float* x, long long n_pix, int C, int x_cstri
   STP3_CHECK_ARG(x && mean && invstd && gamma && beta && (y || y_hi) && n_pix > 0 && C > 0, "stp3_bn_apply: bad argument");
   STP3_CHECK_ARG(dropout_p >= 0.f && dropout_p < 1.f, "stp3_bn_apply: dropout p must be in [0, 1)");
   STP3_CHECK_ARG((y_hi == nullptr) == (y_lo == nullptr), "stp3_bn_apply: give both bf16 planes or neither");
-  STP3_CHECK_ARG(C % 8 == 0 && x_cstride % 4 == 0 && C <= x_cstride && al16(x), "stp3_bn_apply: C % 8, 16-byte rows");
-  STP3_CHECK_ARG(!res || (res_cstride % 4 == 0 && C <= res_cstride && al16(res)), "stp3_bn_apply: bad residual");
-  STP3_CHECK_ARG(!y || (y_cstride % 4 == 0 && C <= y_cstride && al16(y)), "stp3_bn_apply: bad fp32 output");
+  STP3_CHECK_ARG(C <= x_cstride, "stp3_bn_apply: C exceeds the row stride");
+  STP3_CHECK_ARG(!res || C <= res_cstride, "stp3_bn_apply: bad residual");
+  STP3_CHECK_ARG(!y || C <= y_cstride, "stp3_bn_apply: bad fp32 output");
   STP3_CHECK_ARG(!y_hi || (hl_cstride % 8 == 0 && C <= hl_cstride && al16(y_hi) && al16(y_lo)),
                  "stp3_bn_apply: bad bf16 planes");
+  // 8 channels per thread with 128-bit accesses when every row allows it, else one element per thread
+  const bool vec = C % 8 == 0 && x_cstride % 4 == 0 && al16(x) && (!res || (res_cstride % 4 == 0 && al16(res))) &&
+                   (!y || (y_cstride % 4 == 0 && al16(y)));
+  if (!vec) {
+    const int n_cols = (y_hi && hl_cstride > C) ? hl_cstride : C;
+    bn_apply_scalar_kernel<<<blocks_for(n_pix * n_cols), 256, 0, (cudaStream_t)stream>>>(
+        x, x_cstride, mean, invstd, gamma, beta, res, res_cstride, relu, dropout_p, seed, offset, n_pix, C, n_cols, y,
+        y_cstride, (__nv_bfloat16*)y_hi, (__nv_bfloat16*)y_lo, y_hi ? hl_cstride : 0);
+    STP3_CUDA_OK(cudaGetLastError());
+    return STP3_OK;
+  }
   const int groups = ((y_hi && hl_cstride > C) ? hl_cstride : C) / 8;
   const long long total = n_pix * groups;
   bn_apply_kernel<<<blocks_for(total), 256, 0, (cudaStream_t)stream>>>(
@@ -624,10 +746,19 @@ extern "C" int stp3_bn_bwd_apply(const float* g, int g_cstride, const float* y, 
                                  int dx_cstride, float* g_masked, int gm_cstride, void* stream) {
   STP3_CHECK_ARG(g && x && mean && invstd && gamma && sum_g && sum_gxhat && dx && n_pix > 0 && C > 0,
                  "stp3_bn_bwd_apply: bad argument");
-  STP3_CHECK_ARG(C % 8 == 0 && g_cstride % 4 == 0 && x_cstride % 4 == 0 && dx_cstride % 4 == 0 && C <= g_cstride &&
-                 C <= x_cstride && C <= dx_cstride && al16(g) && al16(x) && al16(dx), "stp3_bn_bwd_apply: C % 8, 16-byte rows");
-  STP3_CHECK_ARG(!y || (y_cstride % 4 == 0 && C <= y_cstride && al16(y)), "stp3_bn_bwd_apply: bad mask tensor");
-  STP3_CHECK_ARG(!g_masked || (gm_cstride % 4 == 0 && C <= gm_cstride && al16(g_masked)), "stp3_bn_bwd_apply: bad g_masked");
+  STP3_CHECK_ARG(C <= g_cstride && C <= x_cstride && C <= dx_cstride, "stp3_bn_bwd_apply: C exceeds a row stride");
+  STP3_CHECK_ARG(!y || C <= y_cstride, "stp3_bn_bwd_apply: bad mask tensor");
+  STP3_CHECK_ARG(!g_masked || C <= gm_cstride, "stp3_bn_bwd_apply: bad g_masked");
+  const bool vec = C % 8 == 0 && g_cstride % 4 == 0 && x_cstride % 4 == 0 && dx_cstride % 4 == 0 && al16(g) && al16(x) &&
+                   al16(dx) && (!y || (y_cstride % 4 == 0 && al16(y))) &&
+                   (!g_masked || (gm_cstride % 4 == 0 && al16(g_masked)));
+  if (!vec) {
+    bn_bwd_apply_scalar_kernel<<<blocks_for(n_pix * C), 256, 0, (cudaStream_t)stream>>>(
+        g, g_cstride, y, y_cstride, x, x_cstride, mean, invstd, gamma, sum_g, sum_gxhat, n_pix, C, dx, dx_cstride,
+        g_masked, gm_cstride);
+    STP3_CUDA_OK(cudaGetLastError());
+    return STP3_OK;
+  }
   const long long total = n_pix * (C / 8);
   bn_bwd_apply_kernel<<<blocks_for(total), 256, 0, (cudaStream_t)stream>>>(
       g, g_cstride, y, y_cstride, x, x_cstride, mean, invstd, gamma, sum_g, sum_gxhat, n_pix, C, dx, dx_cstride,
@@ -665,6 +796,15 @@ extern "C" int stp3_phase_interleave(const float* p00, const float* p01, const f
 extern "C" int stp3_sigmoid_bwd(const float* g, const float* s, long long n, float* dz, void* stream) {
   STP3_CHECK_ARG(g && s && dz && n > 0, "stp3_sigmoid_bwd: bad argument");
   sigmoid_bwd_kernel<<<blocks_for(n), 256, 0, (cudaStream_t)stream>>>(g, s, n, dz);
+  STP3_CUDA_OK(cudaGetLastError());
+  return STP3_OK;
+}
+
+extern "C" int stp3_temporal_pair_mean(const float* m, int B, int T, int C, int adjoint, float* out, void* stream) {
+  STP3_CHECK_ARG(m && out && B > 0 && T > 0 && C > 0, "stp3_temporal_pair_mean: bad argument");
+  STP3_CHECK_ARG(m != out, "stp3_temporal_pair_mean: out must not alias m");
+  const long long total = (long long)B * (adjoint ? T : T + 1) * C;
+  temporal_pair_mean_kernel<<<blocks_for(total), 256, 0, (cudaStream_t)stream>>>(m, T, C, total, adjoint != 0, out);
   STP3_CUDA_OK(cudaGetLastError());
   return STP3_OK;
 }

@@ -1,7 +1,9 @@
-"""Host side of the train-mode dense path (the BEV decoder and the DeepLab head in train(), include/stp3_b200.h "Train
-mode"): convolution without folded BatchNorm, BatchNorm with batch statistics (stats / apply with dropout / backward),
-the input gradient of a convolution on stp3_conv_fwd (transposed weights, mirrored taps, dilated too; stride 2 as four
-phase convolutions), the weight gradient, per-image channel sums, and the bilinear x2 pair.
+"""Host side of the train-mode dense path (the BEV decoder, the DeepLab head and the TemporalBlocks in train(),
+include/stp3_b200.h "Train mode"): convolution without folded BatchNorm (2-D, and causal 3-D on (B, T, ...) planes),
+BatchNorm with batch statistics (stats / apply with dropout / backward), the input gradient of a convolution on
+stp3_conv_fwd (transposed weights, mirrored taps, dilated too; stride 2 as four phase convolutions; anti-causal time
+taps for the 3-D ones), the weight gradient (2-D and causal 3-D), per-image channel sums, the temporal pair mean of
+the pyramid-pooling branch, and the bilinear x2 pair.
 
 Tensors are fp32 channels-last (N, H, W, C) contiguous; the inputs of the tensor-core convolutions are the usual
 bf16 hi/lo planes (dense.HL with T = 1).  Nothing here falls back to ATen convolutions or F.batch_norm.
@@ -51,8 +53,9 @@ def to_hl(x: torch.Tensor, cp: Optional[int] = None) -> dense.HL:
 
 
 # ------------------------------------------------------------------------------------------------ convolutions
-def _pack_taps(mats: List[torch.Tensor], taps: List[Tuple[int, int]], cin: int, cout: int) -> dense.PackedConv:
-    """Weight matrices (cout, cin) of arbitrary (dy, dx) taps -> the tap-major / K-major layout of stp3_conv_fwd."""
+def _pack_taps(mats: List[torch.Tensor], taps: List[Tuple[int, ...]], cin: int, cout: int) -> dense.PackedConv:
+    """Weight matrices (cout, cin) of arbitrary (dy, dx) or (dt, dy, dx) taps -> the tap-major / K-major layout of
+    stp3_conv_fwd."""
     cin_p, bn = dense.pad_to(cin), dense.out_tile(cout)
     dev = mats[0].device
     m = torch.zeros((len(mats), bn, cin_p), dtype=torch.float32, device=dev)
@@ -64,8 +67,8 @@ def _pack_taps(mats: List[torch.Tensor], taps: List[Tuple[int, int]], cin: int, 
     packed = packed.permute(1, 3, 0, 2, 4).contiguous()
     bias = torch.zeros(bn, dtype=torch.float32, device=dev)
     dense._PACK_COUNTER += 1
-    return dense.PackedConv(packed, bias, [(0, dy, dx) for dy, dx in taps], cin_p, bn, cout, 1, 0, cin_p,
-                            dense._PACK_COUNTER)
+    return dense.PackedConv(packed, bias, [tuple(t) if len(t) == 3 else (0, *t) for t in taps], cin_p, bn, cout, 1, 0,
+                            cin_p, dense._PACK_COUNTER)
 
 
 def dgrad_taps(kh: int, kw: int, stride: int, pad: int, dilation: int = 1):
@@ -88,6 +91,26 @@ def dgrad_taps(kh: int, kw: int, stride: int, pad: int, dilation: int = 1):
     return phases
 
 
+def dgrad_taps_3d(kt: int, kh: int, kw: int):
+    """Input gradient of the causal y[t, p] = sum W_k x[t + it - (kt-1), p + (ky, kx) - pad] (stride 1, 'same' spatial
+    padding, pad = (kh-1)//2 = (kw-1)//2) as one convolution of the output gradient G: [(it, ky, kx, et, ey, ex)], x
+    receives sum over the list of W[:, :, it, ky, kx]^T G[t + et, p + (ey, ex)].  et = (kt-1) - it >= 0 (anti-causal:
+    frames at or past T are zero padding), ey = pad - ky, ex = pad - kx."""
+    if kh != kw or kh % 2 != 1:
+        raise ValueError(f"the spatial kernel must be square and odd, got {kh}x{kw}")
+    pad = (kh - 1) // 2
+    return [(it, ky, kx, kt - 1 - it, pad - ky, pad - kx) for it in range(kt) for ky in range(kh) for kx in range(kw)]
+
+
+def pack_dgrad3d(weight: torch.Tensor) -> dense.PackedConv:
+    """weight (cout, cin, kt, kh, kw) of a causal 3-D convolution -> the transposed (cin x cout) tap matrices with the
+    anti-causal taps of dgrad_taps_3d, for stp3_conv_fwd on the output gradient."""
+    w = weight.detach().float()
+    cout, cin, kt, kh, kw = w.shape
+    taps = dgrad_taps_3d(kt, kh, kw)
+    return _pack_taps([w[:, :, it, ky, kx].t() for it, ky, kx, _, _, _ in taps], [t[3:] for t in taps], cout, cin)
+
+
 def pack_dgrad(weight: torch.Tensor, stride: int, pad: int, dilation: int = 1):
     """weight (cout, cin, kh, kw) -> [((py, px), PackedConv or None)]: the transposed (cin x cout) tap matrices of every
     phase, for stp3_conv_fwd on the output gradient."""
@@ -108,11 +131,14 @@ def conv_raw(x: dense.HL, weight: torch.Tensor, stride: int, bias: Optional[torc
              img_bias: Optional[torch.Tensor] = None) -> torch.Tensor:
     """Convolution without folded BatchNorm ('same' zero padding, like every decoder and DeepLab convolution) on
     stp3_conv_fwd: (N, Ho, Wo, cout) fp32 channels-last, or (N, cout, Ho, Wo) with nchw (the reference's logits layout,
-    optional sigmoid).  img_bias (N, out_tile(cout)) replaces the bias per image."""
+    optional sigmoid), N = B*T images of x (B, T, H, W, .).  A 5-D weight (cout, cin, kt, kh, kw) is the causal 3-D
+    convolution of the TemporalBlocks (time padded on the left, stride 1).  img_bias (N, out_tile(cout)) replaces the
+    bias per image."""
     cout = weight.shape[0]
     b = bias.detach().float() if bias is not None else torch.zeros(cout, device=weight.device)
     pc = dense.pack_conv(weight.detach().float(), b, stride=stride, dilation=dilation)
-    N, _, H, W, _ = x.hi.shape
+    B, T, H, W, _ = x.hi.shape
+    N = B * T
     Ho, Wo = (H + stride - 1) // stride, (W + stride - 1) // stride
     if nchw:
         out = torch.empty((N, cout, Ho, Wo), dtype=torch.float32, device=x.hi.device)
@@ -124,10 +150,23 @@ def conv_raw(x: dense.HL, weight: torch.Tensor, stride: int, bias: Optional[torc
 
 
 def conv_dgrad(g: torch.Tensor, weight: torch.Tensor, stride: int, H: int, W: int,
-               packed=None, dilation: int = 1, img_bias: Optional[torch.Tensor] = None) -> torch.Tensor:
+               packed=None, dilation: int = 1, img_bias: Optional[torch.Tensor] = None, T: int = 1) -> torch.Tensor:
     """dL/dx (N, H, W, cin) of a 'same'-padded convolution from g = dL/dy (N, Ho, Wo, cout).  Stride 1 only: img_bias
-    (N, out_tile(cin)) is added to every pixel of image n (a spatially constant gradient term, for free)."""
+    (N, out_tile(cin)) is added to every pixel of image n (a spatially constant gradient term, for free).  A 5-D weight
+    (cout, cin, kt, kh, kw) is the causal 3-D convolution of conv_raw on N = B*T frames (T given): its input gradient is
+    one stp3_conv_fwd with the anti-causal taps of dgrad_taps_3d."""
     _f32_cl(g)
+    if weight.dim() == 5:
+        N, _, _, cout = g.shape
+        cin = weight.shape[1]
+        assert N % T == 0 and stride == 1 and dilation == 1
+        pc = packed if packed is not None else pack_dgrad3d(weight)
+        g_hl = to_hl(g)
+        g_hl = dense.HL(g_hl.hi.view(N // T, T, *g_hl.hi.shape[2:]), g_hl.lo.view(N // T, T, *g_hl.lo.shape[2:]), cout)
+        out = torch.empty((N, H, W, cin), dtype=torch.float32, device=g.device)
+        dense.conv(g_hl, pc, out_f32=out, n_valid=cin, out_f32_nhwc=True, out_hw=(H, W), store=False, tune=(0, 0),
+                   img_bias=img_bias)
+        return out
     cout, cin, kh, kw = weight.shape
     pad = (kh - 1) * dilation // 2
     N = g.shape[0]
@@ -156,12 +195,28 @@ def conv_dgrad(g: torch.Tensor, weight: torch.Tensor, stride: int, H: int, W: in
     return out
 
 
-def conv_wgrad(x: torch.Tensor, g: torch.Tensor, kh: int, kw: int, stride: int, dilation: int = 1) -> torch.Tensor:
-    """dL/dW (cout, cin, kh, kw) of a 'same'-padded convolution: x (N, H, W, cin) its input, g (N, Ho, Wo, cout)."""
+def conv_wgrad(x: torch.Tensor, g: torch.Tensor, kh: int, kw: int, stride: int, dilation: int = 1,
+               kt: Optional[int] = None) -> torch.Tensor:
+    """dL/dW (cout, cin, kh, kw) of a 'same'-padded convolution: x (N, H, W, cin) its input, g (N, Ho, Wo, cout).
+    x and g 5-D (B, T, H, W, .) with kt: the causal 3-D convolution of conv_raw, dL/dW (cout, cin, kt, kh, kw)
+    (stp3_conv3d_wgrad)."""
+    L = _lib.lib()
+    if x.dim() == 5:
+        assert kt is not None and stride == 1 and dilation == 1 and x.shape[:4] == g.shape[:4]
+        assert x.is_contiguous() and g.is_contiguous() and x.dtype == g.dtype == torch.float32
+        B, T, H, W, cin = x.shape
+        cout = g.shape[-1]
+        nbytes = L.stp3_conv3d_wgrad_scratch_bytes(B, T, H, W, cout, cin, kt, kh, kw)
+        scratch = torch.empty(nbytes, dtype=torch.uint8, device=x.device)
+        dw = torch.empty((cout, cin, kt, kh, kw), dtype=torch.float32, device=x.device)
+        with torch.cuda.device(x.device):
+            code = L.stp3_conv3d_wgrad(x.data_ptr(), B, T, H, W, cin, cin, g.data_ptr(), cout, cout, kt, kh, kw,
+                                       scratch.data_ptr(), nbytes, dw.data_ptr(), _stream(x.device))
+        _lib.check(code, "stp3_conv3d_wgrad")
+        return dw
     _f32_cl(x), _f32_cl(g)
     N, H, W, cin = x.shape
     _, Ho, Wo, cout = g.shape
-    L = _lib.lib()
     nbytes = L.stp3_conv_wgrad_scratch_bytes(N, Ho, Wo, cout, cin, kh, kw, dilation)
     scratch = torch.empty(nbytes, dtype=torch.uint8, device=x.device)
     dw = torch.empty((cout, cin, kh, kw), dtype=torch.float32, device=x.device)
@@ -175,12 +230,13 @@ def conv_wgrad(x: torch.Tensor, g: torch.Tensor, kh: int, kw: int, stride: int, 
 
 # ------------------------------------------------------------------------------------------------ BatchNorm
 def check_bn(bn: nn.Module, owner: str):
-    """The train-mode kernels implement nn.BatchNorm2d with running statistics and a fixed momentum."""
+    """The train-mode kernels implement nn.BatchNorm2d / nn.BatchNorm3d (the TemporalBlocks') with running statistics
+    and a fixed momentum."""
     if isinstance(bn, nn.SyncBatchNorm):
         raise NotImplementedError(f"{owner}: SyncBatchNorm (sync_batchnorm=True / DDP) is not supported in train mode; "
-                                  "use plain BatchNorm2d")
-    if not isinstance(bn, nn.BatchNorm2d):
-        raise NotImplementedError(f"{owner}: expected nn.BatchNorm2d, got {type(bn).__name__}")
+                                  "use plain BatchNorm2d / BatchNorm3d")
+    if not isinstance(bn, (nn.BatchNorm2d, nn.BatchNorm3d)):
+        raise NotImplementedError(f"{owner}: expected nn.BatchNorm2d or nn.BatchNorm3d, got {type(bn).__name__}")
     if not bn.track_running_stats or bn.running_mean is None:
         raise NotImplementedError(f"{owner}: BatchNorm2d(track_running_stats=False) is not supported in train mode")
     if bn.momentum is None:
@@ -272,10 +328,10 @@ def channel_sums(g: torch.Tensor) -> torch.Tensor:
 
 
 def bn_backward(g: torch.Tensor, x: torch.Tensor, st: BNStats, gamma: torch.Tensor, y_mask: Optional[torch.Tensor],
-                want_masked: bool = False):
+                want_masked: bool = False, dx_out: Optional[torch.Tensor] = None):
     """Backward of y = relu?(BN_batch(x) (+ res)): g = dL/dy, y_mask = the forward output y when a ReLU follows (after
     dropout, y > 0 marks the kept positive elements; the 1 / (1 - p) factor is the caller's).  g, x and y_mask may be
-    channel slices of wider channels-last tensors.
+    channel slices of wider channels-last tensors; so may dx_out, where dL/dx goes (default a new tensor).
     -> (dL/dx, dgamma, dbeta, g masked by the ReLU (the gradient of the residual) or None)."""
     g_cs, x_cs = _row_stride(g), _row_stride(x)
     y_cs = _row_stride(y_mask) if y_mask is not None else 0
@@ -286,7 +342,9 @@ def bn_backward(g: torch.Tensor, x: torch.Tensor, st: BNStats, gamma: torch.Tens
     sum_gx = torch.empty(C, dtype=torch.float32, device=dev)
     scratch, nbytes = _bn_scratch(n, C, dev)
     gm = torch.empty((N, H, W, C), dtype=torch.float32, device=dev) if want_masked else None
-    dx = torch.empty((N, H, W, C), dtype=torch.float32, device=dev)
+    dx = torch.empty((N, H, W, C), dtype=torch.float32, device=dev) if dx_out is None else dx_out
+    assert dx.shape == x.shape
+    dx_cs = _row_stride(dx)
     gam = gamma.detach().float().contiguous()
     L = _lib.lib()
     with torch.cuda.device(dev):
@@ -296,7 +354,7 @@ def bn_backward(g: torch.Tensor, x: torch.Tensor, st: BNStats, gamma: torch.Tens
         _lib.check(code, "stp3_bn_bwd_reduce")
         code = L.stp3_bn_bwd_apply(g.data_ptr(), g_cs, _p(y_mask), y_cs, x.data_ptr(), x_cs, st.mean.data_ptr(),
                                    st.invstd.data_ptr(), gam.data_ptr(), sum_g.data_ptr(), sum_gx.data_ptr(), n, C,
-                                   dx.data_ptr(), C, _p(gm), C, _stream(dev))
+                                   dx.data_ptr(), dx_cs, _p(gm), C, _stream(dev))
     _lib.check(code, "stp3_bn_bwd_apply")
     return dx, sum_gx, sum_g, gm
 
@@ -313,6 +371,21 @@ def image_channel_sums(x: torch.Tensor) -> torch.Tensor:
         code = L.stp3_image_channel_sums(x.data_ptr(), N, H * W, C, C, out.data_ptr(), scratch.data_ptr(), nbytes,
                                          _stream(x.device))
     _lib.check(code, "stp3_image_channel_sums")
+    return out
+
+
+def temporal_pair_mean(m: torch.Tensor, T: int, adjoint: bool = False) -> torch.Tensor:
+    """The time part of a TemporalBlock's pyramid pooling (stp3_temporal_pair_mean): per-frame means m (B*T, C) -> the
+    B*(T+1) pooled frames (frame t: m[0] at t = 0, (m[t-1] + m[t]) / 2 for t < T, m[T-1] at t = T); adjoint: a gradient
+    (B*(T+1), C) -> (B*T, C)."""
+    assert m.dtype == torch.float32 and m.is_contiguous() and m.is_cuda and m.dim() == 2
+    B = m.shape[0] // (T + 1 if adjoint else T)
+    assert m.shape[0] == B * (T + 1 if adjoint else T)
+    out = torch.empty((B * (T if adjoint else T + 1), m.shape[1]), dtype=torch.float32, device=m.device)
+    with torch.cuda.device(m.device):
+        code = _lib.lib().stp3_temporal_pair_mean(m.data_ptr(), B, T, m.shape[1], int(adjoint), out.data_ptr(),
+                                                  _stream(m.device))
+    _lib.check(code, "stp3_temporal_pair_mean")
     return out
 
 

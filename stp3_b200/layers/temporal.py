@@ -9,6 +9,10 @@ TemporalBlock data flow on the device (channels-last hi/lo planes, o = half roun
     out = relu(BN(1x1x1(agg))) + (projection(x) | x)
 Spatially constant input channels (the broadcast ego-motion of stp3.py:145-152) are never materialised: they enter
 every 1x1x1 convolution that reads x as a per-image bias.
+
+Train mode (batch statistics, autograd) runs only inside TemporalModel, which wraps the whole block stack in one
+autograd node (temporal_model._TemporalBlocksTrainFn) built on _train_forward / _train_backward below; a block called
+on its own keeps refusing train().
 """
 import os
 from collections import OrderedDict
@@ -17,7 +21,7 @@ from typing import Optional
 import torch
 import torch.nn as nn
 
-from .. import dense
+from .. import dense, dense_train
 from ._packing import PackedModule
 
 
@@ -315,6 +319,184 @@ class TemporalBlock(PackedModule):
         y = dense.block_tail(mid, x, P["tail"], hid, pbias, rbias, col_sums=out_sums)
         y.c = self.out_channels
         return y
+
+    def _require_eval(self):
+        if self.training:
+            raise NotImplementedError(
+                "TemporalBlock: train mode runs through TemporalModel, which trains its blocks and its head together "
+                "(TemporalModel.train()); a block on its own implements the inference forward only -- call .eval()")
+
+    # ------------------------------------------------------------------------------------------------ train mode
+    def _x_convs(self):
+        """The 1x1x1 convolutions that read x, in the row order of the backward's pre-BN gradient tensor: the three
+        entry convolutions of the paths, then the projection."""
+        p0, p1, p2 = self.convolution_paths
+        convs = [p0[0].conv, p1[0].conv, p2.conv]
+        return convs + ([self.projection[0]] if self.projection is not None else [])
+
+    def _train_forward(self, x: torch.Tensor, const: Optional[torch.Tensor], B: int, T: int):
+        """x (B*T, H, W, cs) fp32 channels-last: the spatial input channels; const (B*T, n_const) fp32 or None: the
+        spatially constant ones.  Every BatchNorm3d uses batch statistics over B*T*H*W (the pooled branch's over the B*T
+        values) and updates its running statistics.  -> (y (B*T, H, W, cout) fp32, tape for _train_backward)."""
+        N, H, W, cs = x.shape
+        nc = 0 if const is None else const.shape[1]
+        assert nc == self.n_const and cs + nc == self.in_channels
+        if self.projection is None and nc:
+            raise NotImplementedError("TemporalBlock: an identity skip cannot carry spatially constant extra channels")
+        h, cout = self.half_channels, self.out_channels
+        dev = x.device
+        TT = dense_train
+        x_hl = TT.to_hl(x)
+
+        def x_conv(conv):                  # 1x1x1 convolution of x; the constant channels enter as a per-image bias
+            w = conv.weight.detach().float().reshape(conv.out_channels, -1)
+            ib = None
+            if nc:
+                ib = torch.zeros((N, dense.out_tile(w.shape[0])), dtype=torch.float32, device=dev)
+                dense.small_linear(const, w[:, cs:].contiguous(), ib, False)
+            return TT.conv_raw(x_hl, w[:, :cs].reshape(w.shape[0], cs, 1, 1).contiguous(), 1, img_bias=ib)
+
+        # the three paths write their activated outputs side by side: the aggregation's spatial input
+        cat = torch.empty((N, H, W, 3 * h), dtype=torch.float32, device=dev)
+        entry, mids = [], []
+        for i, path in enumerate(self.convolution_paths):
+            e = path[0] if i < 2 else path
+            raw = x_conv(e.conv)
+            st = TT.bn_stats_module(raw, e.norm)
+            if i < 2:
+                y, y_hl = TT.bn_apply(raw, st, e.norm.weight, e.norm.bias, relu=True)
+                cc = path[1]
+                y_hl = dense.HL(y_hl.hi.view(B, T, *y_hl.hi.shape[2:]), y_hl.lo.view(B, T, *y_hl.lo.shape[2:]), h)
+                raw2 = TT.conv_raw(y_hl, cc.conv.weight, 1)
+                st2 = TT.bn_stats_module(raw2, cc.norm)
+                TT.bn_apply(raw2, st2, cc.norm.weight, cc.norm.bias, relu=True, hl=False, y_out=cat[..., i * h:(i + 1) * h])
+                mids.append((cc, raw2, st2))
+            else:
+                y = cat[..., 2 * h:]
+                TT.bn_apply(raw, st, e.norm.weight, e.norm.bias, relu=True, hl=False, y_out=y)
+            entry.append((e, raw, st, y))
+        agg = self.aggregation[0]
+        wg = agg.conv.weight.detach().float().reshape(cout, -1)
+        tape = {"x": x, "const": const, "B": B, "T": T, "cat": cat, "entry": entry, "mids": mids}
+        pbias = None
+        if self.use_pyramid_pooling:
+            # per-frame means -> temporal pair mean (AvgPool3d with count_include_pad=False: T + 1 frames) -> 1x1x1 ->
+            # BatchNorm over the B*(T+1) values -> ReLU -> last frame dropped (that order is the reference's,
+            # temporal.py:414): spatially constant, so it enters the aggregation as a per-image bias and the broadcast
+            # map is never built
+            ph, pw = self.pyramid_pooling.pool_sizes[0][1:]
+            assert (ph, pw) == (H, W), "pyramid pooling must span the whole map (as configured by TemporalModel)"
+            pcbr = self.pyramid_pooling.features[0].conv_bn_relu
+            red = pcbr.conv.out_channels
+            mean = torch.empty((N, self.in_channels), dtype=torch.float32, device=dev)
+            mean[:, :cs] = TT.image_channel_sums(x) * (1.0 / (H * W))
+            if nc:
+                mean[:, cs:] = const
+            m = TT.temporal_pair_mean(mean, T)
+            Np = m.shape[0]
+            v_raw = torch.empty((Np, 1, 1, red), dtype=torch.float32, device=dev)
+            dense.small_linear(m, pcbr.conv.weight.detach().float().reshape(red, -1).contiguous(), v_raw.view(Np, red),
+                               False)
+            pst = TT.bn_stats_module(v_raw, pcbr.norm)
+            v_full, _ = TT.bn_apply(v_raw, pst, pcbr.norm.weight, pcbr.norm.bias, relu=True, hl=False)
+            v = v_full.view(B, T + 1, red)[:, :T].reshape(N, 1, 1, red).contiguous()
+            pbias = torch.zeros((N, dense.out_tile(cout)), dtype=torch.float32, device=dev)
+            dense.small_linear(v.view(N, red), wg[:, 3 * h:].contiguous(), pbias, False)
+            tape.update(m=m, v_raw=v_raw, pst=pst, v_full=v_full, v=v)
+        araw = TT.conv_raw(TT.to_hl(cat), wg[:, :3 * h].reshape(cout, 3 * h, 1, 1).contiguous(), 1, img_bias=pbias)
+        ast = TT.bn_stats_module(araw, agg.norm)
+        ya, _ = TT.bn_apply(araw, ast, agg.norm.weight, agg.norm.bias, relu=True, hl=False)
+        tape.update(araw=araw, ast=ast, ya=ya)
+        if self.projection is not None:
+            jbn = self.projection[1]
+            jraw = x_conv(self.projection[0])
+            jst = TT.bn_stats_module(jraw, jbn)
+            out, _ = TT.bn_apply(jraw, jst, jbn.weight, jbn.bias, relu=False, hl=False)
+            out.add_(ya)
+            tape.update(jraw=jraw, jst=jst)
+        else:
+            out = ya + x
+        return out, tape
+
+    def _train_backward(self, tape, g: torch.Tensor, need_x: bool):
+        """Reverse walk of _train_forward: g = dL/dy (B*T, H, W, cout) contiguous fp32 -> (dL/dx (B*T, H, W, cs) or
+        None, {parameter: gradient}).  No gradient reaches the constant channels (host-derived input data)."""
+        TT = dense_train
+        x, const, B, T, cat = tape["x"], tape["const"], tape["B"], tape["T"], tape["cat"]
+        N, H, W, cs = x.shape
+        nc = 0 if const is None else const.shape[1]
+        h, cout = self.half_channels, self.out_channels
+        dev = x.device
+        grads = {}
+        convs = self._x_convs()
+        K = 3 * h + (cout if self.projection is not None else 0)
+        # pre-BN gradients of every 1x1x1 convolution that reads x, side by side: one wgrad and one transposed
+        # convolution serve all of them
+        graw = torch.empty((N, H, W, K), dtype=torch.float32, device=dev)
+        if self.projection is not None:
+            jbn = self.projection[1]
+            _, grads[jbn.weight], grads[jbn.bias], _ = TT.bn_backward(g, tape["jraw"], tape["jst"], jbn.weight, None,
+                                                                      dx_out=graw[..., 3 * h:])
+        agg = self.aggregation[0]
+        wg = agg.conv.weight.detach().float().reshape(cout, -1)
+        ga, grads[agg.norm.weight], grads[agg.norm.bias], _ = TT.bn_backward(g, tape["araw"], tape["ast"],
+                                                                            agg.norm.weight, tape["ya"])
+        dw_agg = TT.conv_wgrad(cat, ga, 1, 1, 1).reshape(cout, 3 * h)
+        g_cat = TT.conv_dgrad(ga, wg[:, :3 * h].reshape(cout, 3 * h, 1, 1), 1, H, W)
+        gx_pool = None
+        if self.use_pyramid_pooling:
+            pcbr = self.pyramid_pooling.features[0].conv_bn_relu
+            red = pcbr.conv.out_channels
+            gsum = TT.image_channel_sums(ga)
+            v = tape["v"]
+            dw_agg = torch.cat([dw_agg, TT.conv_wgrad(v, gsum.view(N, 1, 1, cout), 1, 1, 1).reshape(cout, red)], 1)
+            g_vk = torch.empty((N, red), dtype=torch.float32, device=dev)
+            dense.small_linear(gsum, wg[:, 3 * h:].t().contiguous(), g_vk, False)
+            m = tape["m"]
+            Np = m.shape[0]
+            g_v = torch.zeros((B, T + 1, red), dtype=torch.float32, device=dev)    # the dropped frame gets none
+            g_v[:, :T] = g_vk.view(B, T, red)
+            g_v, grads[pcbr.norm.weight], grads[pcbr.norm.bias], _ = TT.bn_backward(
+                g_v.view(Np, 1, 1, red), tape["v_raw"], tape["pst"], pcbr.norm.weight, tape["v_full"])
+            grads[pcbr.conv.weight] = TT.conv_wgrad(m.view(Np, 1, 1, -1), g_v, 1, 1, 1).view_as(pcbr.conv.weight)
+            if need_x:
+                # d mean = pair-mean adjoint of W1^T g_v; its spatial channels spread evenly over the H*W pixels and
+                # enter the input gradient as the per-image bias of the transposed convolution below
+                wp = pcbr.conv.weight.detach().float().reshape(red, -1)
+                g_m = torch.empty((Np, self.in_channels), dtype=torch.float32, device=dev)
+                dense.small_linear(g_v.view(Np, red), wp.t().contiguous(), g_m, False)
+                g_mean = TT.temporal_pair_mean(g_m, T, adjoint=True)
+                gx_pool = torch.zeros((N, dense.out_tile(cs)), dtype=torch.float32, device=dev)
+                gx_pool[:, :cs] = g_mean[:, :cs] * (1.0 / (H * W))
+        grads[agg.conv.weight] = dw_agg.view_as(agg.conv.weight)
+        for i, (e, raw, st, y) in enumerate(tape["entry"]):
+            sl = slice(i * h, (i + 1) * h)
+            gi = g_cat[..., sl]
+            if i < 2:
+                cc, raw2, st2 = tape["mids"][i]
+                g2, grads[cc.norm.weight], grads[cc.norm.bias], _ = TT.bn_backward(gi, raw2, st2, cc.norm.weight,
+                                                                                  cat[..., sl])
+                kt = cc.conv.kernel_size[0]
+                grads[cc.conv.weight] = TT.conv_wgrad(y.view(B, T, H, W, h), g2.view(B, T, H, W, h), 3, 3, 1, kt=kt)
+                gi = TT.conv_dgrad(g2, cc.conv.weight, 1, H, W, T=T)
+            _, grads[e.norm.weight], grads[e.norm.bias], _ = TT.bn_backward(gi, raw, st, e.norm.weight, y,
+                                                                            dx_out=graw[..., sl])
+        dw_x = TT.conv_wgrad(x, graw, 1, 1, 1).reshape(K, cs)
+        if nc:
+            # the constant channels' columns: sum over images of (per-image sums of the pre-BN gradient) x const
+            gs = TT.image_channel_sums(graw)
+            dw_x = torch.cat([dw_x, TT.conv_wgrad(const.view(N, 1, 1, nc), gs.view(N, 1, 1, K), 1, 1, 1).reshape(K, nc)], 1)
+        row = 0
+        for conv in convs:
+            grads[conv.weight] = dw_x[row:row + conv.out_channels].reshape(conv.weight.shape).contiguous()
+            row += conv.out_channels
+        gx = None
+        if need_x:
+            w_x = torch.cat([conv.weight.detach().float().reshape(conv.out_channels, -1)[:, :cs] for conv in convs], 0)
+            gx = TT.conv_dgrad(graw, w_x.reshape(K, cs, 1, 1).contiguous(), 1, H, W, img_bias=gx_pool)
+            if self.projection is None:
+                gx.add_(g)
+        return gx, grads
 
     def forward(self, *inputs):
         """x (B, C, T, H, W) fp32 -> (B, Cout, T, H, W) fp32, like the reference module."""

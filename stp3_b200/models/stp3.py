@@ -196,6 +196,24 @@ class STP3(nn.Module):
         if self._head_training() and not self.decoder.training:
             raise RuntimeError("STP3: temporal_model.final_conv is in train mode but the decoder is in eval mode, so no "
                                "gradient could reach the head -- call model.decoder.train() as well")
+        use_ego = self.cfg.MODEL.TEMPORAL_MODEL.INPUT_EGOPOSE
+        if isinstance(self.temporal_model, TemporalModel) and self.temporal_model.blocks_training():
+            # train-mode TemporalBlocks take fp32 BEV features; through the lift-splat's autograd when feat / depth
+            # require grad
+            needs_grad = torch.is_grad_enabled() and (feat.requires_grad or
+                                                      (depth_logits is not None and depth_logits.requires_grad))
+            if needs_grad and feat_channels_last:
+                raise NotImplementedError("STP3: gradients to channels-last feat are not supported; pass (B,S,N,C,Hf,Wf)")
+            kw = dict(use_depth_distribution=self.cfg.MODEL.ENCODER.USE_DEPTH_DISTRIBUTION, workspace=self._ws)
+            if needs_grad:
+                bev = ops.lift_splat_autograd(feat, depth_logits, cam_M, cam_t, ego_R, ego_t, *self._axes(), off, res,
+                                              dim, float(self.discount), **kw)
+            else:
+                bev = ops.lift_splat(feat, depth_logits, cam_M, cam_t, ego_R, ego_t, *self._axes(), off, res, dim,
+                                     float(self.discount), feat_channels_last=feat_channels_last, **kw)
+            states = self.temporal_model(bev, const=const if use_ego else None)
+            output.update(self.decoder(states))
+            return output
 
         self._mark("start")
         planes = torch.empty((2, B, S, X, Y, C), dtype=torch.bfloat16, device=dev)
@@ -208,7 +226,6 @@ class STP3(nn.Module):
         x = dense.HL(planes[0], planes[1], C)
         self._mark("lift_splat")
 
-        use_ego = self.cfg.MODEL.TEMPORAL_MODEL.INPUT_EGOPOSE
         if isinstance(self.temporal_model, TemporalModelIdentity):
             bev = dense.to_f32(x, 0, C)
             if use_ego:
@@ -224,6 +241,9 @@ class STP3(nn.Module):
 
     def _head_training(self) -> bool:
         return isinstance(self.temporal_model, TemporalModel) and self.temporal_model.final_conv.training
+
+    def _blocks_training(self) -> bool:
+        return isinstance(self.temporal_model, TemporalModel) and any(b.training for b in self.temporal_model.model)
 
     def forward_features_frame_sharded(self, feat, depth_logits, intrinsics, extrinsics, future_egomotion, gather="nccl"):
         """Latency mode for a global batch smaller than the number of GPUs (SURVEY.md §8e): the B*S camera frames are
@@ -283,6 +303,9 @@ class STP3(nn.Module):
         use_ego = self.cfg.MODEL.TEMPORAL_MODEL.INPUT_EGOPOSE
         if isinstance(self.temporal_model, TemporalModelIdentity):
             raise NotImplementedError("frame-sharded mode is wired for the temporal_block model")
+        if self._blocks_training():
+            raise RuntimeError("frame-sharded forward: the TemporalBlocks are in train mode; the sharded path runs the "
+                               "inference forward only -- call .eval() on temporal_model.model")
         if self._head_training():
             raise RuntimeError("frame-sharded forward: temporal_model.final_conv is in train mode; the sharded path runs "
                                "the inference forward only -- call .eval() on it")
@@ -328,6 +351,9 @@ class GraphedPerception:
         if model.decoder.training:
             raise RuntimeError("GraphedPerception: the decoder is in train mode (batch statistics, running-statistics "
                                "updates, autograd); a CUDA graph replays the inference forward only -- call .eval()")
+        if model._blocks_training():
+            raise RuntimeError("GraphedPerception: the TemporalBlocks are in train mode (batch statistics, autograd); a "
+                               "CUDA graph replays the inference forward only -- call .eval() on temporal_model.model")
         if model._head_training():
             raise RuntimeError("GraphedPerception: temporal_model.final_conv is in train mode (batch statistics, "
                                "dropout, autograd); a CUDA graph replays the inference forward only -- call .eval()")
