@@ -114,6 +114,32 @@ int stp3_lift_splat_fwd(const stp3_lift_splat_desc* desc, const float* feat, con
                         int32_t* ranks_out, float* pool_sum, void* workspace, size_t workspace_bytes,
                         float* out, int out_layout, int n_peers, void* const* peer_out, void* stream);
 
+/* The kernels stp3_lift_splat_fwd would launch for these arguments; stp3_lift_splat_fwd launches exactly this plan.
+ * Host only: launches nothing and never dereferences feat or depth_logits (their addresses decide the alignment rule
+ * and are encoded into the TMA descriptors).  Refuses what stp3_lift_splat_fwd refuses for the descriptor, out_layout
+ * and n_peers, with the same messages.
+ *   tma_rules       the TMA-staged scatter kernel is admissible: TW 4, Wf % 4 == 0, C % 64 == 0, D <= 256, Hf <= 32,
+ *                   16-byte aligned feat / depth_logits, its tile fits in shared memory, STP3_LIFT_NO_TMA unset or 0
+ *   scatter         1: the TMA-staged kernel runs (tma_rules and the driver encoded both tensor maps); 0: the generic one
+ *   scatter_tw      image columns per generic scatter CTA (4, 2 or 1; 4 whenever tma_rules holds)
+ *   finalize        0: lane-per-pillar kernel; 1: channels-last kernel (out_layout != 0, C in {32, 64, 128}, <= 4 frames)
+ *   finalize_vec    lane-per-pillar kernel with 8-channel vector accesses (C % 8 == 0); 0 for the channels-last kernel
+ *   finalize_smax   frames the finalize kernel is instantiated for (4 or 8)
+ *   finalize_lpp    channels-last kernel: lanes per pillar, C / 16 (2, 4 or 8); 0 for the lane-per-pillar kernel
+ *   channel_groups  finalize CTAs per pillar block; > 1 (C > 64, lane-per-pillar) adds the occupancy-clearing kernel */
+typedef struct stp3_lift_splat_kernel_plan {
+  int tma_rules;
+  int scatter;
+  int scatter_tw;
+  int finalize;
+  int finalize_vec;
+  int finalize_smax;
+  int finalize_lpp;
+  int channel_groups;
+} stp3_lift_splat_kernel_plan;
+int stp3_lift_splat_plan(const stp3_lift_splat_desc* desc, const float* feat, const float* depth_logits, int out_layout,
+                         int n_peers, stp3_lift_splat_kernel_plan* plan);
+
 /* Backward of stp3_lift_splat_fwd (training through the drop-in, SURVEY.md row f2): given grad_out = dLoss/d out
  * (B,S,C,nx,ny) fp32 it returns grad_feat (B,S,N,C,Hf,Wf) and grad_depth_logits (B,S,N,D,Hf,Wf; may be NULL, and is not
  * written when use_depth_distribution == 0).  Replaces the autograd chain of the reference:

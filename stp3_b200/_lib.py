@@ -33,6 +33,12 @@ class LiftSplatDesc(ctypes.Structure):
 _LSD = ctypes.POINTER(LiftSplatDesc)
 
 
+class LiftSplatPlan(ctypes.Structure):
+    """Mirror of stp3_lift_splat_kernel_plan (include/stp3_b200.h)."""
+    _fields_ = [("tma_rules", _I), ("scatter", _I), ("scatter_tw", _I), ("finalize", _I), ("finalize_vec", _I),
+                ("finalize_smax", _I), ("finalize_lpp", _I), ("channel_groups", _I)]
+
+
 class ConvDesc(ctypes.Structure):
     """Mirror of stp3_conv_desc (include/stp3_b200.h)."""
     _fields_ = [("B", _I), ("T", _I), ("H", _I), ("W", _I), ("T_total", _I), ("t0", _I), ("in_cstride", _I), ("cin_off", _I), ("cin", _I),
@@ -96,6 +102,7 @@ SIGNATURES = {
     "stp3_bev_discount": (_I, [_V, _I, _I, _I, _I, _I, _F, _V, _V, _V]),
     "stp3_conv_fwd": (_I, [ctypes.POINTER(ConvDesc), _V, _V, _V, _V, _V, _V, _V, _V, _V, _V, ctypes.POINTER(ConvHead), _V]),
     "stp3_lift_splat_fwd": (_I, [_LSD, _V, _V, _V, _V, _V, _SZ, _V, _I, _I, ctypes.POINTER(_V), _V]),
+    "stp3_lift_splat_plan": (_I, [_LSD, _V, _V, _I, _I, ctypes.POINTER(LiftSplatPlan)]),
     # train mode of the decoder and the DeepLab head
     "stp3_conv_wgrad_scratch_bytes": (_SZ, [_I, _I, _I, _I, _I, _I, _I, _I]),
     "stp3_conv_wgrad": (_I, [_V, _I, _I, _I, _I, _I, _V, _I, _I, _I, _I, _I, _I, _I, _I, _I, _V, _SZ, _V, _V]),

@@ -1067,6 +1067,119 @@ int stp3::check_lift_splat_desc(const char* fn, const stp3_lift_splat_desc* d, c
   return STP3_OK;
 }
 
+// The scatter and finalize launches of one forward call: the public plan plus what the launch needs beyond it.
+namespace {
+struct LiftLaunch {
+  stp3_lift_splat_kernel_plan plan;
+  LiftSplatTmaMaps maps;   // valid when plan.scatter == 1
+  size_t smem;             // generic scatter kernel
+  size_t smem_tma;         // TMA scatter kernel
+};
+
+// The one place that decides which kernels run (stp3_lift_splat_plan, stp3_lift_splat_fwd).  Checks the descriptor and
+// the output choice; host only -- the tensor-map encode reads nothing behind the pointers.
+int plan_lift_splat(const char* fn, const stp3_lift_splat_desc* desc, const float* feat, const float* depth_logits,
+                    int out_layout, int n_peers, BevQuant& q, LiftLaunch& L) {
+  if (const int rc = check_lift_splat_desc(fn, desc, feat, depth_logits, kMaxFrames, q)) return rc;
+  const int B = desc->B, S = desc->S, N = desc->N, D = desc->D, Hf = desc->Hf, Wf = desc->Wf, C = desc->C;
+  const int feat_layout = desc->feat_layout;
+  const bool raw = desc->f_count > 0;
+  const int Sw = raw ? 1 : S;                                   // frames per sample of the scatter grid / finalize
+  STP3_CHECK_ARG(n_peers >= 0 && n_peers <= kMaxPeers, "n_peers must be in [0, %d], with peer_out when it is not 0",
+                 kMaxPeers);
+  STP3_CHECK_ARG(raw || n_peers == 0, "peer outputs need frame mode (f_count > 0)");
+  STP3_CHECK_ARG(out_layout >= 0 && out_layout <= 2, "out_layout must be 0 (C,X,Y), 1 (X,Y,C) or 2 (bf16 hi/lo X,Y,C)");
+  STP3_CHECK_ARG(!raw || out_layout == 1, "frame mode writes fp32 channels-last frames (out_layout 1)");
+  STP3_CHECK_ARG(n_peers == 0 || C == 32 || C == 64 || C == 128,
+                 "peer outputs need C in {32, 64, 128} (channels-last finalize kernel)");
+  STP3_CHECK_ARG(out_layout != 2 || C % 8 == 0, "out_layout 2 needs C %% 8 == 0");
+  stp3_lift_splat_kernel_plan& P = L.plan;
+  memset(&P, 0, sizeof(P));
+
+  // generic scatter: tile width as wide as shared memory allows (<= 4 columns), at least 1
+  const int HP = (Hf + 3) & ~3;
+  auto smem_for = [&](int tw) {
+    return (size_t)D * tw * HP * 8 + (size_t)D * tw * 4 +
+           (size_t)(kCChunk * ((((Hf + kHChunk - 1) / kHChunk) * kHChunk * tw) | 1) + 12 * kMaxFrames + Hf + D +
+                    kScatterThreads) * sizeof(float);
+  };
+  int TW = 4;
+  while (TW > 1 && smem_for(TW) > 110 * 1024) TW >>= 1;
+  L.smem = smem_for(TW);
+  STP3_CHECK_ARG(L.smem <= 227 * 1024, "D*Hf = %d too large for one image column in shared memory", D * Hf);
+  P.scatter_tw = TW;
+
+  // TMA-staged scatter: 16-byte aligned rows for the tensor maps, whole 64-channel chunks for the fixed transaction
+  // counts, two mma k-steps (Hf <= 32), and a tile that leaves room for two CTAs per SM
+  const int npix = Hf * kTmaTW, feat_floats = npix * kCChunk;
+  L.smem_tma = 128 + ((size_t)((D * npix + 31) & ~31) + ((feat_floats + 31) & ~31) + 2 * (size_t)D * kTmaTW * HP +
+                      (kSegPasses + 1) * (size_t)D * kTmaTW + 4 + 12 * kMaxFrames + Hf + D + kScatterThreads + 2) * 4 + 16;
+  static const int no_tma = [] { const char* e = getenv("STP3_LIFT_NO_TMA"); return e ? atoi(e) : 0; }();
+  P.tma_rules = !no_tma && TW == kTmaTW && Wf % 4 == 0 && C % kCChunk == 0 && D <= 256 && Hf <= 32 &&
+                (reinterpret_cast<uintptr_t>(feat) & 15) == 0 &&
+                (!depth_logits || (reinterpret_cast<uintptr_t>(depth_logits) & 15) == 0) && L.smem_tma <= 113 * 1024;
+  if (P.tma_rules) {
+    const TmapEncodeFn enc = tmap_encode_fn();
+    if (enc) {   // otherwise (or when an encode fails) the generic kernel runs
+      const long long n_img = (long long)B * S * N;
+      const cuuint32_t es[3] = {1, 1, 1};
+      CUresult r1 = CUDA_SUCCESS, r2;
+      if (desc->use_depth_distribution) {
+        const cuuint64_t dims[3] = {(cuuint64_t)Wf, (cuuint64_t)Hf, (cuuint64_t)(D * n_img)};
+        const cuuint64_t strides[2] = {(cuuint64_t)Wf * 4, (cuuint64_t)Hf * Wf * 4};
+        const cuuint32_t box[3] = {4, (cuuint32_t)Hf, (cuuint32_t)D};
+        r1 = enc(&L.maps.depth, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(depth_logits), dims, strides, box,
+                 es, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                 CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+      } else {
+        memset(&L.maps.depth, 0, sizeof(L.maps.depth));
+      }
+      if (feat_layout == 0) {
+        const cuuint64_t dims[3] = {(cuuint64_t)Wf, (cuuint64_t)Hf, (cuuint64_t)(C * n_img)};
+        const cuuint64_t strides[2] = {(cuuint64_t)Wf * 4, (cuuint64_t)Hf * Wf * 4};
+        const cuuint32_t box[3] = {4, (cuuint32_t)Hf, (cuuint32_t)kCChunk};
+        r2 = enc(&L.maps.feat, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(feat), dims, strides, box, es,
+                 CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                 CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+      } else {
+        const cuuint64_t dims[3] = {(cuuint64_t)C, (cuuint64_t)Wf, (cuuint64_t)(Hf * n_img)};
+        const cuuint64_t strides[2] = {(cuuint64_t)C * 4, (cuuint64_t)Wf * C * 4};
+        const cuuint32_t box[3] = {(cuuint32_t)kCChunk, 4, (cuuint32_t)Hf};
+        r2 = enc(&L.maps.feat, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(feat), dims, strides, box, es,
+                 CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                 CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+      }
+      P.scatter = r1 == CUDA_SUCCESS && r2 == CUDA_SUCCESS;
+    }
+  }
+
+  // finalize: channels-last outputs with 32 / 64 / 128 channels and few frames take the sector-exact kernel
+  // (one thread = 16 channels); everything else the lane-per-pillar kernel (8 warps x 8 channels per CTA)
+  P.finalize = out_layout != 0 && (C == 32 || C == 64 || C == 128) && Sw <= 4;
+  if (P.finalize) {
+    P.finalize_smax = 4;
+    P.finalize_lpp = C / 16;
+    P.channel_groups = 1;
+  } else {
+    P.finalize_vec = C % 8 == 0;
+    P.finalize_smax = Sw <= 4 ? 4 : 8;
+    P.channel_groups = ceil_div(C, 64);
+  }
+  return STP3_OK;
+}
+}  // namespace
+
+extern "C" int stp3_lift_splat_plan(const stp3_lift_splat_desc* desc, const float* feat, const float* depth_logits,
+                                    int out_layout, int n_peers, stp3_lift_splat_kernel_plan* plan) {
+  STP3_CHECK_ARG(plan != nullptr, "stp3_lift_splat_plan: null plan");
+  BevQuant q;
+  LiftLaunch L;
+  if (const int rc = plan_lift_splat("stp3_lift_splat_plan", desc, feat, depth_logits, out_layout, n_peers, q, L))
+    return rc;
+  *plan = L.plan;
+  return STP3_OK;
+}
+
 // f_count == 0: all B*S frames, discount recurrence over each sample's S frames.  f_count > 0: frame-sharded call --
 // only the flat frames f_begin + [0, f_count) are splatted and written RAW (no recurrence), one (nx, ny, C) grid per
 // frame, to `out` or to every peer's gathered buffer; the caller all-gathers them and applies stp3_bev_discount.
@@ -1075,23 +1188,18 @@ extern "C" int stp3_lift_splat_fwd(const stp3_lift_splat_desc* desc, const float
                                    float* out, int out_layout, int n_peers, void* const* peer_out, void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   BevQuant q;
-  if (const int rc = check_lift_splat_desc("stp3_lift_splat_fwd", desc, feat, depth_logits, kMaxFrames, q)) return rc;
+  LiftLaunch L;
+  if (const int rc = plan_lift_splat("stp3_lift_splat_fwd", desc, feat, depth_logits, out_layout, n_peers, q, L))
+    return rc;
+  const stp3_lift_splat_kernel_plan& P = L.plan;
   const int nx = desc->nx, ny = desc->ny, nz = desc->nz;
   const int B = desc->B, S = desc->S, N = desc->N, D = desc->D, Hf = desc->Hf, Wf = desc->Wf, C = desc->C;
-  const int feat_layout = desc->feat_layout, use_depth_distribution = desc->use_depth_distribution;
   const bool raw = desc->f_count > 0;
   const float discount = raw ? 0.f : desc->discount;
   const int Bw = raw ? desc->f_count : B, Sw = raw ? 1 : S;     // shape of the scatter grid / finalize launch
-  STP3_CHECK_ARG(n_peers >= 0 && n_peers <= kMaxPeers && (n_peers == 0 || peer_out),
-                 "n_peers must be in [0, %d], with peer_out when it is not 0", kMaxPeers);
+  STP3_CHECK_ARG(n_peers == 0 || peer_out, "n_peers must be in [0, %d], with peer_out when it is not 0", kMaxPeers);
   STP3_CHECK_ARG((out || n_peers > 0) && workspace, "stp3_lift_splat_fwd: null pointer argument");
-  STP3_CHECK_ARG(raw || n_peers == 0, "peer outputs need frame mode (f_count > 0)");
   STP3_CHECK_ARG(!raw || (!ranks_out && !pool_sum), "frame mode writes no ranks_out or pool_sum");
-  STP3_CHECK_ARG(out_layout >= 0 && out_layout <= 2, "out_layout must be 0 (C,X,Y), 1 (X,Y,C) or 2 (bf16 hi/lo X,Y,C)");
-  STP3_CHECK_ARG(!raw || out_layout == 1, "frame mode writes fp32 channels-last frames (out_layout 1)");
-  STP3_CHECK_ARG(n_peers == 0 || C == 32 || C == 64 || C == 128,
-                 "peer outputs need C in {32, 64, 128} (channels-last finalize kernel)");
-  STP3_CHECK_ARG(out_layout != 2 || C % 8 == 0, "out_layout 2 needs C %% 8 == 0");
   PeerOut po;
   po.n = n_peers; po.first_slot = desc->f_begin;
   for (int i = 0; i < kMaxPeers; ++i) po.ptr[i] = i < n_peers ? static_cast<float*>(peer_out[i]) : nullptr;
@@ -1108,118 +1216,51 @@ extern "C" int stp3_lift_splat_fwd(const stp3_lift_splat_desc* desc, const float
   for (int i = 0; i < 3; ++i) { p.off[i] = q.off[i]; p.res[i] = q.res[i]; p.inv[i] = q.inv[i]; p.inv_ok[i] = q.inv_ok[i]; }
   p.nx = nx; p.ny = ny; p.nz = nz;
   p.B = B; p.S = S; p.N = N; p.D = D; p.Hf = Hf; p.Wf = Wf; p.C = C;
-  p.feat_nhwc = feat_layout; p.use_depth = use_depth_distribution;
+  p.feat_nhwc = desc->feat_layout; p.use_depth = desc->use_depth_distribution;
   p.ranks_out = ranks_out;
   p.grid = static_cast<float*>(workspace);
   p.occ = static_cast<unsigned char*>(workspace) + grid_bytes(Bw, Sw, C, nx, ny);
-
-  // tile width: as wide as shared memory allows (<= 4 columns), at least 1
-  int TW = 4;
-  auto smem_for = [&](int tw) {
-    const int HP = (Hf + 3) & ~3;
-    return (size_t)D * tw * HP * 8 + (size_t)D * tw * 4 +
-           (size_t)(kCChunk * ((((Hf + kHChunk - 1) / kHChunk) * kHChunk * tw) | 1) + 12 * kMaxFrames + Hf + D +
-                    kScatterThreads) * sizeof(float);
-  };
-  while (TW > 1 && smem_for(TW) > 110 * 1024) TW >>= 1;
-  const size_t smem = smem_for(TW);
-  STP3_CHECK_ARG(smem <= 227 * 1024, "D*Hf = %d too large for one image column in shared memory", D * Hf);
-  p.TW = TW;
-  p.tiles_w = ceil_div(Wf, TW);
+  p.TW = P.scatter_tw;
+  p.tiles_w = ceil_div(Wf, P.scatter_tw);
   const long long nblk = (long long)Bw * Sw * N * p.tiles_w;
   STP3_CHECK_ARG(nblk < (1ll << 31), "grid too large");
-  auto launch = [&](auto kernel) -> int {
-    STP3_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    kernel<<<(unsigned)nblk, kScatterThreads, smem, stream>>>(p);
-    STP3_CUDA_OK(cudaGetLastError());
-    return STP3_OK;
-  };
-  // fast path: TMA-staged tiles (needs 16-byte aligned rows for the tensor maps)
-  static const int no_tma = [] { const char* e = getenv("STP3_LIFT_NO_TMA"); return e ? atoi(e) : 0; }();
-  const bool tma_ok = !no_tma && TW == 4 && Wf % 4 == 0 && (feat_layout == 0 || C % 4 == 0) && D <= 256 && Hf <= 32 /* two mma k-steps */ &&
-                      (reinterpret_cast<uintptr_t>(feat) & 15) == 0 &&
-                      (!depth_logits || (reinterpret_cast<uintptr_t>(depth_logits) & 15) == 0);
-  int rc = STP3_OK;
-  bool used_tma = false;
-  if (tma_ok) {
-    const TmapEncodeFn enc = tmap_encode_fn();
-    if (enc) {
-      LiftSplatTmaMaps maps;
-      const long long n_img = (long long)B * S * N;
-      CUresult r1 = CUDA_SUCCESS, r2;
-      if (use_depth_distribution) {
-        const cuuint64_t dims[3] = {(cuuint64_t)Wf, (cuuint64_t)Hf, (cuuint64_t)(D * n_img)};
-        const cuuint64_t strides[2] = {(cuuint64_t)Wf * 4, (cuuint64_t)Hf * Wf * 4};
-        const cuuint32_t box[3] = {4, (cuuint32_t)Hf, (cuuint32_t)D};
-        const cuuint32_t es[3] = {1, 1, 1};
-        r1 = enc(&maps.depth, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(depth_logits), dims, strides, box, es,
-                 CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                 CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-      } else {
-        memset(&maps.depth, 0, sizeof(maps.depth));
-      }
-      if (feat_layout == 0) {
-        const cuuint64_t dims[3] = {(cuuint64_t)Wf, (cuuint64_t)Hf, (cuuint64_t)(C * n_img)};
-        const cuuint64_t strides[2] = {(cuuint64_t)Wf * 4, (cuuint64_t)Hf * Wf * 4};
-        const cuuint32_t box[3] = {4, (cuuint32_t)Hf, (cuuint32_t)(C < kCChunk ? C : kCChunk)};
-        const cuuint32_t es[3] = {1, 1, 1};
-        r2 = enc(&maps.feat, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(feat), dims, strides, box, es,
-                 CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                 CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-      } else {
-        const cuuint64_t dims[3] = {(cuuint64_t)C, (cuuint64_t)Wf, (cuuint64_t)(Hf * n_img)};
-        const cuuint64_t strides[2] = {(cuuint64_t)C * 4, (cuuint64_t)Wf * C * 4};
-        const cuuint32_t box[3] = {(cuuint32_t)(C < kCChunk ? C : kCChunk), 4, (cuuint32_t)Hf};
-        const cuuint32_t es[3] = {1, 1, 1};
-        r2 = enc(&maps.feat, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(feat), dims, strides, box, es,
-                 CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                 CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-      }
-      // channel chunks must be whole for the fixed-size transaction counts: C % 64 == 0 (NCHW groups of 8 / NHWC box)
-      if (r1 == CUDA_SUCCESS && r2 == CUDA_SUCCESS && C % kCChunk == 0) {
-        const int HP = (Hf + 3) & ~3, npix = Hf * 4;
-        const int feat_floats = npix * kCChunk;
-        const size_t smem_tma = 128 + ((size_t)((D * npix + 31) & ~31) + ((feat_floats + 31) & ~31) + 2 * (size_t)D * 4 * HP +
-                                       (kSegPasses + 1) * (size_t)D * 4 + 4 + 12 * kMaxFrames + Hf + D + kScatterThreads + 2) * 4 + 16;
-        if (smem_tma <= 113 * 1024) {
-          STP3_CUDA_OK(cudaFuncSetAttribute(lift_splat_scatter_tma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                            (int)smem_tma));
-          lift_splat_scatter_tma_kernel<<<(unsigned)nblk, kScatterThreads, smem_tma, stream>>>(maps, p);
-          STP3_CUDA_OK(cudaGetLastError());
-          used_tma = true;
-        }
-      }
-    }
+
+  if (P.scatter) {
+    STP3_CUDA_OK(cudaFuncSetAttribute(lift_splat_scatter_tma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                      (int)L.smem_tma));
+    lift_splat_scatter_tma_kernel<<<(unsigned)nblk, kScatterThreads, L.smem_tma, stream>>>(L.maps, p);
+  } else {
+    auto launch = [&](auto kernel) -> int {
+      STP3_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L.smem));
+      kernel<<<(unsigned)nblk, kScatterThreads, L.smem, stream>>>(p);
+      return STP3_OK;
+    };
+    const int rc = P.scatter_tw == 4 ? launch(lift_splat_scatter_kernel<4>)
+                 : P.scatter_tw == 2 ? launch(lift_splat_scatter_kernel<2>) : launch(lift_splat_scatter_kernel<1>);
+    if (rc != STP3_OK) return rc;
   }
-  if (!used_tma)
-    rc = TW == 4 ? launch(lift_splat_scatter_kernel<4>)
-       : TW == 2 ? launch(lift_splat_scatter_kernel<2>) : launch(lift_splat_scatter_kernel<1>);
-  if (rc != STP3_OK) return rc;
+  STP3_CUDA_OK(cudaGetLastError());
 
   const int nvox = nx * ny * nz;
-  const int groups = ceil_div(C, 64);                 // 8 warps x 8 channels per CTA
-  dim3 fgrid(ceil_div(nvox, 32), Bw, groups), fblock(32, C >= 64 ? 8 : ceil_div(C, 8));
   float* pool_part = pool_sum ? reinterpret_cast<float*>(p.occ + occ_bytes(Bw, Sw, nx, ny)) : nullptr;
-  // channels-last outputs with 32 / 64 / 128 channels and few frames: sector-exact kernel (one thread = 16 channels)
-  const bool cl = out_layout != 0 && (C == 32 || C == 64 || C == 128) && Sw <= 4;
   int pool_blocks = ceil_div(nvox, 32);
-  if (cl) {
-    const int ppb = 256 / (C / 16);
-    pool_blocks = ceil_div(nvox, ppb);
+  if (P.finalize) {
+    pool_blocks = ceil_div(nvox, 256 / P.finalize_lpp);
     dim3 cgrid(pool_blocks, Bw);
 #define STP3_FIN_CL(LPP_, PEERS_) \
     bev_finalize_cl_kernel<LPP_, 4, PEERS_><<<cgrid, 256, 0, stream>>>(p.grid, p.occ, out, pool_part, Sw, nvox, discount, out_layout, po)
     if (po.n > 0) {
-      if (C == 32) STP3_FIN_CL(2, true); else if (C == 64) STP3_FIN_CL(4, true); else STP3_FIN_CL(8, true);
+      if (P.finalize_lpp == 2) STP3_FIN_CL(2, true); else if (P.finalize_lpp == 4) STP3_FIN_CL(4, true); else STP3_FIN_CL(8, true);
     } else {
-      if (C == 32) STP3_FIN_CL(2, false); else if (C == 64) STP3_FIN_CL(4, false); else STP3_FIN_CL(8, false);
+      if (P.finalize_lpp == 2) STP3_FIN_CL(2, false); else if (P.finalize_lpp == 4) STP3_FIN_CL(4, false); else STP3_FIN_CL(8, false);
     }
 #undef STP3_FIN_CL
   } else {
+    dim3 fgrid(pool_blocks, Bw, P.channel_groups), fblock(32, C >= 64 ? 8 : ceil_div(C, 8));
 #define STP3_FINALIZE(VEC, SMAX) \
   bev_finalize_kernel<VEC, SMAX><<<fgrid, fblock, 0, stream>>>(p.grid, p.occ, out, pool_part, Sw, C, nvox, discount, out_layout)
-  if (C % 8 == 0) { if (Sw <= 4) STP3_FINALIZE(true, 4); else STP3_FINALIZE(true, 8); }
-  else            { if (Sw <= 4) STP3_FINALIZE(false, 4); else STP3_FINALIZE(false, 8); }
+    if (P.finalize_vec) { if (P.finalize_smax == 4) STP3_FINALIZE(true, 4); else STP3_FINALIZE(true, 8); }
+    else                { if (P.finalize_smax == 4) STP3_FINALIZE(false, 4); else STP3_FINALIZE(false, 8); }
 #undef STP3_FINALIZE
   }
   STP3_CUDA_OK(cudaGetLastError());
@@ -1228,14 +1269,13 @@ extern "C" int stp3_lift_splat_fwd(const stp3_lift_splat_desc* desc, const float
     pool_reduce_kernel<<<dim3(Bw * Sw, kPoolSlices), dim3(32, 8), 0, stream>>>(pool_part, pool_blocks, Sw, C, pool_sum);
     STP3_CUDA_OK(cudaGetLastError());
   }
-  if (groups > 1 && !cl) {
+  if (P.channel_groups > 1) {
     const size_t nocc = ((size_t)Bw * Sw * nvox + 255) & ~(size_t)255;
     clear_bytes_kernel<<<(unsigned)((nocc / 16 + 255) / 256), 256, 0, stream>>>(p.occ, nocc);
     STP3_CUDA_OK(cudaGetLastError());
   }
   return STP3_OK;
 }
-
 
 namespace stp3 {
 // out[b,t] = out[b,t-1]*discount + raw[b,t] over channels-last fp32 raw splats, written as bf16 hi/lo planes

@@ -263,6 +263,13 @@ extern "C" int stp3_lift_splat_bwd(const stp3_lift_splat_desc* desc, const float
   const size_t need = stp3_lift_splat_bwd_scratch_bytes(desc);
   if (scratch_bytes < need) return set_error(STP3_ENOSPC, "scratch too small: %zu < %zu", scratch_bytes, need);
   const int nvox = desc->nx * desc->ny * desc->nz;
+  // every refusal comes before the first launch
+  const int npix = Hf * kBwdTW;
+  const size_t smem = ((size_t)3 * D * npix + (size_t)kBwdC * (npix | 1) + 12 * kBwdMaxFrames + Hf + D) * sizeof(float) + 16;
+  STP3_CHECK_ARG(smem <= 227 * 1024, "D*Hf = %d too large for the backward tile in shared memory", D * Hf);
+  const int tiles_w = ceil_div(Wf, kBwdTW);
+  const long long nblk = (long long)B * S * N * tiles_w;
+  STP3_CHECK_ARG(nblk < (1ll << 31), "grid too large");
 
   dim3 g1(ceil_div(nvox, 32), ceil_div(C, 32), B);
   bev_grad_to_grid_kernel<<<g1, dim3(32, 8), 0, stream>>>(grad_out, static_cast<float*>(scratch), S, C, nvox,
@@ -273,15 +280,10 @@ extern "C" int stp3_lift_splat_bwd(const stp3_lift_splat_desc* desc, const float
   p.ego_t = desc->ego_t; p.xs = desc->xs; p.ys = desc->ys; p.ds = desc->ds;
   p.B = B; p.S = S; p.N = N; p.D = D; p.Hf = Hf; p.Wf = Wf; p.C = C;
   p.use_depth = desc->use_depth_distribution;
-  p.tiles_w = ceil_div(Wf, kBwdTW);
+  p.tiles_w = tiles_w;
   p.ggrid = static_cast<const float*>(scratch);
   p.gfeat = grad_feat; p.gdepth = grad_depth_logits;
-  const int npix = Hf * kBwdTW;
-  const size_t smem = ((size_t)3 * D * npix + (size_t)kBwdC * (npix | 1) + 12 * kBwdMaxFrames + Hf + D) * sizeof(float) + 16;
-  STP3_CHECK_ARG(smem <= 227 * 1024, "D*Hf = %d too large for the backward tile in shared memory", D * Hf);
   STP3_CUDA_OK(cudaFuncSetAttribute(lift_splat_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  const long long nblk = (long long)B * S * N * p.tiles_w;
-  STP3_CHECK_ARG(nblk < (1ll << 31), "grid too large");
   lift_splat_bwd_kernel<<<(unsigned)nblk, 32 * kBwdTW, smem, stream>>>(p);
   STP3_CUDA_OK(cudaGetLastError());
   return STP3_OK;

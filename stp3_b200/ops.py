@@ -133,6 +133,25 @@ def lift_splat(feat, depth_logits, cam_M, cam_t, ego_R, ego_t, xs, ys, ds, bev_o
     return res if len(res) > 1 else out
 
 
+def lift_splat_plan(feat, depth_logits, cam_M, cam_t, ego_R, ego_t, xs, ys, ds, bev_off, bev_res, bev_dim,
+                    discount: float, *, feat_channels_last: bool = False, out_channels_last: bool = False,
+                    use_depth_distribution: bool = True, return_ranks: bool = False, pool_sum: bool = False,
+                    workspace: Optional[Workspace] = None, out: Optional[torch.Tensor] = None,
+                    out_hilo: Optional[torch.Tensor] = None, f_begin: int = 0, f_count: int = 0, n_peers: int = 0) -> dict:
+    """The kernels lift_splat() (or, with f_count > 0, lift_splat_frames()) launches for these arguments:
+    stp3_lift_splat_plan (include/stp3_b200.h) as a dict of its fields.  Launches nothing.  return_ranks, pool_sum,
+    workspace and out do not change the plan; they are accepted so that lift_splat()'s arguments can be passed as they
+    are."""
+    desc, feat, depth_logits = _lift_desc(feat, depth_logits, cam_M, cam_t, ego_R, ego_t, xs, ys, ds, bev_off, bev_res,
+                                          bev_dim, discount, feat_channels_last, use_depth_distribution, f_begin, f_count)
+    layout = 2 if out_hilo is not None else 1 if (out_channels_last or f_count > 0) else 0
+    plan = _lib.LiftSplatPlan()
+    code = _lib.lib().stp3_lift_splat_plan(desc, feat.data_ptr(), _ptr(depth_logits), layout, int(n_peers),
+                                           ctypes.byref(plan))
+    _lib.check(code, "stp3_lift_splat_plan")
+    return {name: getattr(plan, name) for name, _ in _lib.LiftSplatPlan._fields_}
+
+
 def lift_splat_backward(grad_out, feat, depth_logits, cam_M, cam_t, ego_R, ego_t, xs, ys, ds, bev_off, bev_res, bev_dim,
                         discount: float, *, use_depth_distribution: bool = True):
     """Gradients of lift_splat()'s (B,S,C,X,Y) output w.r.t. feat (B,S,N,C,Hf,Wf) and depth_logits (B,S,N,D,Hf,Wf):
