@@ -16,14 +16,15 @@
 //              serves the three dy taps of a 3x3) and B_hi, B_lo (BN x 64; small weight tensors stay resident in
 //              smem) through separate rings; each warpgroup issues 4 (K = 16) x 3 wgmma per tap for its 64 rows
 //   CTA      : persistent, one per SM, walks tiles blockIdx.x + i*gridDim.x
-//   warps    : 0..7 = two MMA warpgroups (rows 0..63 / 64..127 of the tile) that also run the epilogue (registers ->
-//              shared accumulator tile -> global), 8 = TMA producer, which keeps loading the next tile's operands
-//              while the epilogue drains
+//   warps    : 0..7 = two MMA warpgroups (rows 0..63 / 64..127 of the tile): wgmma only, then their fragments into
+//              the shared accumulator tile; 8..15 = two epilogue warpgroups (shared accumulator tile -> global) that
+//              drain tile u while the MMA warpgroups multiply tile u+1; 16 = TMA producer (17..19 leave at once)
 //
 // Reference layers: stp3/layers/temporal.py:252-489, stp3/layers/convolutions.py:183-280, stp3/models/decoder.py.
 #include <cuda_bf16.h>
 
 #include <cstdlib>
+#include <type_traits>
 
 #include "common.cuh"
 #include "pipeline.cuh"
@@ -32,8 +33,22 @@
 
 namespace stp3 {
 
+constexpr int kMmaWarps = 8;                     // two warpgroups, 64 accumulator rows each
 constexpr int kEpiWarps = 8;                     // two warps per 32-row quarter of the tile, each owning half of the columns
-constexpr int kConvThreads = kEpiWarps * 32 + 32;
+constexpr int kProducerWarp = kMmaWarps + kEpiWarps;
+constexpr int kConvThreads = (kProducerWarp + 4) * 32;   // the producer has a warpgroup of its own for setmaxnreg
+// per-thread registers of each role (setmaxnreg): the MMA warpgroups hold the accumulator (64 registers for BN = 128
+// and for the stacked BN = 64), the epilogue its chunk, residual, column-sum and head arrays.  ptxas -v reports no
+// spills in any instantiation with this split.  setmaxnreg.inc only takes registers that another warpgroup of the CTA
+// gave back with setmaxnreg.dec: the five roles together must fit the CTA's launch allocation (96 per thread for 640
+// threads), or an inc waits forever.
+constexpr int kProducerRegs = 24, kMmaRegs = 96, kEpiRegs = 128;
+constexpr int kLaunchRegs = 65536 / kConvThreads / 8 * 8;
+static_assert(kProducerRegs + 2 * kMmaRegs + 2 * kEpiRegs <= 5 * kLaunchRegs, "setmaxnreg split exceeds the CTA's registers");
+// the single shared accumulator tile is handed over with two named barriers of the MMA and epilogue threads (ids
+// 1..4 are the epilogue's column-half pairs): "full" (MMA arrive, epilogue sync) and "free" (the reverse)
+constexpr int kBarAccFull = 5, kBarAccFree = 6;
+constexpr int kHandoverThreads = (kMmaWarps + kEpiWarps) * 32;
 constexpr int kSubH = 8, kTileW = 16;           // one tile = 8 x 16 pixels = 128 accumulator rows
 constexpr int kBK = 64;                         // channels per K step (one 128-byte swizzle row of bf16)
 constexpr int kMaxTaps = 49;
@@ -108,12 +123,11 @@ struct ConvParams {
 
 // STACK (BN = 64 only): the hi and lo weight planes of a K step form ONE B operand of 2*BN rows, so a product is two
 // MMAs instead of three -- A_hi x [W_hi; W_lo] (N = 2*BN) and A_lo x W_hi (N = BN) -- and the activation tile is read
-// from shared memory twice instead of three times.  The accumulator has 2*BN columns; the epilogue adds columns c and
-// n_mma + c.
-template <int BN, bool STACK = false>
+// from shared memory twice instead of three times.  The register accumulator has 2*BN columns; the MMA warpgroups add
+// columns c and b_rows + c on their way to the shared accumulator tile, which has BN columns either way.
+template <int BN>
 struct ConvSmem {
-  static constexpr int kAccCols = STACK ? 2 * BN : BN;                 // accumulator columns
-  static constexpr int kAccStride = kAccCols + 4;                      // floats per row of the shared accumulator tile
+  static constexpr int kAccStride = BN + 4;                            // floats per row of the shared accumulator tile
   // the tail behind the operand rings (or the resident weights), byte offsets from its start
   static constexpr int bias = 0;                                       // fp32 [BN]
   static constexpr int head = bias + BN * 4;                           // fp32 [kMaxHeadOut][BN] fused head weights
@@ -151,8 +165,9 @@ __device__ __forceinline__ void ld_acc16(const float* src, uint32_t (&r)[16]) { 
 //     the same smem tile at row offsets 0, 16, 32 (2 KB steps keep the 1024-byte swizzle alignment).
 //   * wgmma groups are committed per tap; a ring slot is released once the group after the one that read it has been
 //     issued and the reading group has retired (wgmma.wait_group 1), so the tensor pipe always has the next tap queued.
-//   * At the end of a tile the accumulators go to a shared [128 rows][columns] fp32 tile; the epilogue gives every
-//     thread one pixel (row) and half of the columns.
+//   * At the end of a tile the MMA warpgroups wait until the epilogue has released the shared [128 rows][columns] fp32
+//     accumulator tile, write their accumulators into it and go on with the next tile; the epilogue warpgroups give
+//     every thread one pixel (row) and half of the columns.
 // FULLK: every K = 16 step of every K block carries data (ks_first == 0, ks_end == 4).  Then a tap is a branch-free run
 // of wgmma with N fixed at compile time (BN, 2 * BN for the stacked operand), which ptxas pipelines; any branch around
 // the MMAs (skipped K steps, an N chosen at run time) makes it serialise them.
@@ -160,9 +175,9 @@ template <int BN, bool STACK, bool FULLK>
 __global__ void __launch_bounds__(kConvThreads, 1)
 conv_igemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ CUtensorMap tm_a_lo,
                   const __grid_constant__ CUtensorMap tm_w, const ConvParams p) {
-  using S = ConvSmem<BN, STACK>;
+  using S = ConvSmem<BN>;
   static_assert(!STACK || BN == 64, "stacked weight operand: BN = 64 only");
-  constexpr int kAccRegs = S::kAccCols / 2;        // accumulator registers per thread (64 rows x kAccCols per warpgroup)
+  constexpr int kAccRegs = (STACK ? 2 * BN : BN) / 2;   // accumulator registers per thread (64 rows x columns per warpgroup)
   const int kBRows = p.b_rows;
   const int cta = (int)blockIdx.x, n_cta = (int)gridDim.x;
   extern __shared__ unsigned char smem_raw[];
@@ -196,7 +211,7 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
   // has left; this grid's own set-up ran while its predecessor drained.  Only module constants (bias, weights, head
   // weights) are read before griddep_wait().
   ptx::griddep_launch_dependents();
-  if (warp == kEpiWarps && lane == 0) {
+  if (warp == kProducerWarp && lane == 0) {
     ptx::prefetch_tmap(&tm_a_hi); ptx::prefetch_tmap(&tm_a_lo); ptx::prefetch_tmap(&tm_w);
     ra.init(2); rb.init(2);
     ptx::mbar_init(bres_bar, 1);
@@ -209,7 +224,9 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
   const int n_groups = p.n_groups;
   const int tile_h = kSubH;
 
-  if (warp == kEpiWarps) {
+  if (warp >= kProducerWarp) {
+    ptx::setmaxnreg_dec<kProducerRegs>();
+    if (warp != kProducerWarp) return;
     // ===================== TMA producer (whole warp walks the loops; one elected lane issues) =====================
     // load_b: the weight tile of K step `it` into `dst` (called by the elected lane; transaction bytes on `bar`)
     auto load_b = [&](unsigned char* dst, int it, uint64_t* bar, int img_w) {
@@ -250,8 +267,9 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
         }
       }
     }
-  } else {
-    // ===================== two MMA warpgroups, then the epilogue =====================
+  } else if (warp < kMmaWarps) {
+    // ===================== two MMA warpgroups =====================
+    ptx::setmaxnreg_inc<kMmaRegs>();
     const int wg = warp >> 2;                    // warpgroup: accumulator rows [64 wg, 64 wg + 64)
     const bool wg_leader = (threadIdx.x & 127) == 0;
     float accr[kAccRegs];
@@ -328,21 +346,42 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
       }
       wg::wait<0>();
       pend.release();
-      // registers -> s_acc (columns the MMAs computed)
-      const int ncols = STACK ? 2 * kBRows : kBRows;
+      ptx::bar_sync(kBarAccFree, kHandoverThreads);      // the epilogue has read the previous tile's accumulators
+      // registers -> s_acc (columns the MMAs computed).  Register i holds column 8 (i / 4) + 2 (lane % 4) + i % 2, so
+      // the stacked operand's A_hi x W_lo partner of column c (column b_rows + c) is register i + kLo, kLo = b_rows / 2
       const int row0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+      auto to_smem = [&](auto lo) {
+        constexpr int kLo = decltype(lo)::value;             // 0: not stacked
 #pragma unroll
-      for (int i = 0; i < kAccRegs; i += 2) {
-        const int col = 8 * (i >> 2) + 2 * (lane & 3);
-        if (col < ncols) {
-          const int row = row0 + 8 * ((i >> 1) & 1);
-          *reinterpret_cast<float2*>(s_acc + (size_t)row * S::kAccStride + col) = make_float2(accr[i], accr[i + 1]);
+        for (int i = 0; i < (kLo ? kLo : kAccRegs); i += 2) {
+          const int col = 8 * (i >> 2) + 2 * (lane & 3);
+          if (kLo || col < kBRows) {
+            const int row = row0 + 8 * ((i >> 1) & 1);
+            float2 v = make_float2(accr[i], accr[i + 1]);
+            if constexpr (kLo > 0) { v.x += accr[i + kLo]; v.y += accr[i + 1 + kLo]; }
+            *reinterpret_cast<float2*>(s_acc + (size_t)row * S::kAccStride + col) = v;
+          }
+        }
+      };
+      if constexpr (!STACK) {
+        to_smem(std::integral_constant<int, 0>{});
+      } else if constexpr (FULLK) {
+        to_smem(std::integral_constant<int, BN / 2>{});
+      } else {
+        switch (kBRows) {                                     // n_mma: 16, 32, 48 or 64
+          case 16: to_smem(std::integral_constant<int, 8>{}); break;
+          case 32: to_smem(std::integral_constant<int, 16>{}); break;
+          case 48: to_smem(std::integral_constant<int, 24>{}); break;
+          default: to_smem(std::integral_constant<int, 32>{}); break;
         }
       }
-      ptx::bar_sync(5, kEpiWarps * 32);
+      ptx::bar_arrive(kBarAccFull, kHandoverThreads);
     };
-    // ----- epilogue: shared accumulator tile -> registers -> global
-    const int e = warp;
+    for (int tile = cta; tile < p.n_tiles; tile += n_cta) mma_tile(tile);
+  } else {
+    // ===================== two epilogue warpgroups: shared accumulator tile -> registers -> global =====================
+    ptx::setmaxnreg_inc<kEpiRegs>();
+    const int e = warp - kMmaWarps;
     const int q = warp & 3;                      // 32-row quarter of the tile this warp drains
     const int half = e >> 2;                     // which half of the BN columns this warp handles
     constexpr int kColsPerWarp = BN / 2;
@@ -384,6 +423,7 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
     };
     ptx::griddep_wait();                          // residual / per-image bias reads and every global write come after
     for (int tile = cta; tile < p.n_tiles; tile += n_cta) {
+      ptx::bar_arrive(kBarAccFree, kHandoverThreads);   // done with the previous tile's accumulators (if any)
       const int img = tile / tiles_per_img, rem = tile % tiles_per_img;
       const int oy_t = (rem / p.tiles_x) * kSubH, ox = (rem % p.tiles_x) * kTileW + (r & 15);
       if (kSums && p.sum_part && img != sum_img) {      // tiles come in image order: hand the finished image over
@@ -391,7 +431,7 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
         sum_img = img;
       }
       // latency hiding: the residual of the first chunk and this warp's slice of the per-image bias are requested
-      // before waiting for the accumulator; every later residual chunk is requested one chunk ahead
+      // before waiting for the accumulator; every later residual chunk as soon as the previous one has been added
       uint32_t nh[8], nl[8];
       auto request_residual = [&](int j) {
         const int oy = oy_t + (r >> 4);
@@ -424,7 +464,7 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
         __syncwarp();
         bsrc = wb - col0;
       }
-      mma_tile(tile);
+      ptx::bar_sync(kBarAccFull, kHandoverThreads);     // the MMA warpgroups have written this tile's accumulators
       {
         const int oy = oy_t + (r >> 4);
         const bool valid = oy < p.Ho && ox < p.Wo;
@@ -437,47 +477,33 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
         for (int j = 0; j < kColsPerWarp / 16; ++j) {
           const int cb = col0 + j * 16;              // first output channel of this chunk
           uint32_t acc[16];
-          uint32_t acc2[16];                         // stacked operand: the hi x lo products live b_rows columns further
           const bool computed = cb < p.n_mma;        // columns beyond n_mma: zero weights, never multiplied
           if (computed) {
             ld_acc16(acc_row + j * 16, acc);
-            if constexpr (STACK) ld_acc16(acc_row + kBRows + j * 16, acc2);
           } else {
 #pragma unroll
-            for (int i = 0; i < 16; ++i) { acc[i] = 0u; acc2[i] = 0u; }
-          }
-          uint32_t rhw[8], rlw[8];                   // residual of this chunk (requested one chunk ago)
-          if (p.res_mode) {
-#pragma unroll
-            for (int i = 0; i < 8; ++i) { rhw[i] = nh[i]; rlw[i] = nl[i]; }
-            const bool last_j = j + 1 == kColsPerWarp / 16;
-            if (!last_j) request_residual(j + 1);
+            for (int i = 0; i < 16; ++i) acc[i] = 0u;
           }
           if (valid) {
             float v[16];
 #pragma unroll
             for (int g = 0; g < 4; ++g) {          // bias: per-image slice (conv bias already folded in) or the conv's own
               const float4 b4 = *reinterpret_cast<const float4*>(bsrc + cb + 4 * g);
-              if constexpr (STACK) {
-                v[4 * g + 0] = (__uint_as_float(acc[4 * g + 0]) + __uint_as_float(acc2[4 * g + 0])) + b4.x;
-                v[4 * g + 1] = (__uint_as_float(acc[4 * g + 1]) + __uint_as_float(acc2[4 * g + 1])) + b4.y;
-                v[4 * g + 2] = (__uint_as_float(acc[4 * g + 2]) + __uint_as_float(acc2[4 * g + 2])) + b4.z;
-                v[4 * g + 3] = (__uint_as_float(acc[4 * g + 3]) + __uint_as_float(acc2[4 * g + 3])) + b4.w;
-              } else {
-                v[4 * g + 0] = __uint_as_float(acc[4 * g + 0]) + b4.x;
-                v[4 * g + 1] = __uint_as_float(acc[4 * g + 1]) + b4.y;
-                v[4 * g + 2] = __uint_as_float(acc[4 * g + 2]) + b4.z;
-                v[4 * g + 3] = __uint_as_float(acc[4 * g + 3]) + b4.w;
-              }
+              v[4 * g + 0] = __uint_as_float(acc[4 * g + 0]) + b4.x;
+              v[4 * g + 1] = __uint_as_float(acc[4 * g + 1]) + b4.y;
+              v[4 * g + 2] = __uint_as_float(acc[4 * g + 2]) + b4.z;
+              v[4 * g + 3] = __uint_as_float(acc[4 * g + 3]) + b4.w;
             }
             if (p.res_mode) {
 #pragma unroll
               for (int e2 = 0; e2 < 8; ++e2) {
-                const float2 r = ptx::join_hilo(rhw[e2], rlw[e2]);
+                const float2 r = ptx::join_hilo(nh[e2], nl[e2]);
                 float& a0 = v[e2 * 2], &a1 = v[e2 * 2 + 1];
                 if (p.res_mode == 1) { a0 += r.x; a1 += r.y; if (d_relu) { a0 = fmaxf(a0, 0.f); a1 = fmaxf(a1, 0.f); } }
                 else { if (d_relu) { a0 = fmaxf(a0, 0.f); a1 = fmaxf(a1, 0.f); } a0 += r.x; a1 += r.y; }
               }
+              // the next chunk's residual is in flight while this chunk is stored (one buffer of residual registers)
+              if (j + 1 < kColsPerWarp / 16) request_residual(j + 1);
             } else if (d_relu) {
 #pragma unroll
               for (int i = 0; i < 16; ++i) v[i] = fmaxf(v[i], 0.f);
@@ -572,7 +598,6 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
           ptx::bar_sync(1 + q, 64);
         }
       }
-      ptx::bar_sync(5, kEpiWarps * 32);        // every warp has read the accumulator tile before the next tile overwrites it
     }
     if (kSums && p.sum_part && sum_img >= 0) flush_sums(sum_img);
   }
@@ -616,7 +641,7 @@ int launch_col_sum_reduce(const float* part, int n_part, int n_img, float* out, 
 template <int BN, bool STACK, bool FULLK>
 static int launch_conv(ConvParams& p, const CUtensorMap& tm_hi, const CUtensorMap& tm_lo, const CUtensorMap& tm_w,
                        int n_mma, int k_iters, bool stream_weights, unsigned grid, cudaStream_t stream) {
-  using SM = ConvSmem<BN, STACK>;
+  using SM = ConvSmem<BN>;
   const size_t smem_cap = 227 * 1024;
   const size_t a_stage = 2 * (size_t)p.a_plane_bytes;
   p.b_rows = FULLK ? BN : n_mma;

@@ -145,6 +145,8 @@ __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.
 
 // named barrier over `count` threads (a multiple of 32) of the CTA
 __device__ __forceinline__ void bar_sync(int id, int count) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory"); }
+// arrive without waiting: a producer's half of a named-barrier hand-over whose consumers bar_sync on the same id
+__device__ __forceinline__ void bar_arrive(int id, int count) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(count) : "memory"); }
 
 }  // namespace ptx
 }  // namespace stp3
