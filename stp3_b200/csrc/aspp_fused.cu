@@ -157,6 +157,7 @@ aspp_fused_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
       ptx::bar_sync(1 + wg, 128);                // the previous tile's output has read the per-image bias
       // written by the preceding (PDL-overlapped) pool_bias kernel: coherent loads
       wb[wtid] = *(reinterpret_cast<const volatile float*>(p.img_bias) + (size_t)img * kAsppHidden + wtid);
+      ptx::bar_sync(1 + wg, 128);                // the output reads entries other warps of the warpgroup wrote
       float acc2[kAsppHidden / 2];
       for (int s = 0; s < p.n_br; ++s) {
         // ---- main(s): acc1 = sum over the branch's taps
@@ -256,7 +257,6 @@ extern "C" int stp3_aspp_fused_fwd(const stp3_aspp_desc* d, const void* x_hi, co
   STP3_CHECK_ARG(d->out_cstride % 16 == 0 && d->out_coff % 16 == 0 && d->out_coff + n_store <= d->out_cstride &&
                  (reinterpret_cast<uintptr_t>(y_hi) & 31) == 0 && (reinterpret_cast<uintptr_t>(y_lo) & 31) == 0,
                  "output planes: n_store channels at a 16-channel aligned offset, 32-byte aligned");
-  if (!tmap_encode_fn()) return set_error(STP3_ECUDA, "cuTensorMapEncodeTiled is not available from the driver");
   AsppParams p;
   p.n_img = d->B * d->T; p.T = d->T; p.T_total = d->T; p.H = d->H; p.W = d->W;
   p.tiles_x = ceil_div(d->W, 16); p.tiles_y = ceil_div(d->H, 8);
@@ -280,6 +280,8 @@ extern "C" int stp3_aspp_fused_fwd(const stp3_aspp_desc* d, const void* x_hi, co
   p.out_hi = static_cast<__nv_bfloat16*>(y_hi); p.out_lo = static_cast<__nv_bfloat16*>(y_lo);
   p.out_cstride = d->out_cstride; p.out_coff = d->out_coff;
   p.relu_out = d->no_relu ? 0 : 1; p.n_store = n_store;
+  // every descriptor check comes before the driver lookup: a bad descriptor is reported as such without a GPU
+  if (!tmap_encode_fn()) return set_error(STP3_ECUDA, "cuTensorMapEncodeTiled is not available from the driver");
 
   CUtensorMap tm_hi, tm_lo, tm_w;
   {

@@ -405,7 +405,6 @@ extern "C" int stp3_block_fused_fwd(const stp3_block_desc* d, const void* mid_hi
   STP3_CHECK_ARG((d->has_res_proj != 0) == (res_bias != nullptr), "res_bias is given exactly when the block has a projection");
   auto al32 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 31) == 0; };
   STP3_CHECK_ARG(al32(y_hi) && al32(y_lo) && al32(x_hi) && al32(x_lo), "planes must be 32-byte aligned");
-  if (!tmap_encode_fn()) return set_error(STP3_ECUDA, "cuTensorMapEncodeTiled is not available from the driver");
 
   BlkParams p;
   p.n_img = d->B * d->T; p.T = d->T; p.H = d->H; p.W = d->W;
@@ -472,6 +471,8 @@ extern "C" int stp3_block_fused_fwd(const stp3_block_desc* d, const void* mid_hi
                    "chain %d of %d: (N, pieces of P) = (%d, %d) is not a compiled chain layout", c, p.n_chain, ch.n_mma, npc);
   }
   for (; pp < 16; ++pp) STP3_CHECK_ARG(d->piece_col[pp] < 0, "piece %d of P: the chains' pieces are consecutive, zeros follow", pp);
+  // every descriptor check comes before the driver lookup: a bad descriptor is reported as such without a GPU
+  if (!tmap_encode_fn()) return set_error(STP3_ECUDA, "cuTensorMapEncodeTiled is not available from the driver");
   p.hid_bias = hid_bias; p.img_bias = img_bias; p.res_bias = res_bias;
   p.res_hi = static_cast<const __nv_bfloat16*>(x_hi); p.res_lo = static_cast<const __nv_bfloat16*>(x_lo);
   p.res_cstride = d->x_cstride;

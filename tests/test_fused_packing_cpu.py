@@ -2,7 +2,8 @@
 descriptors, piece map and bias tables that `DeepLabHead._pack` / `TemporalBlock._pack` hand to stp3_aspp_fused_fwd /
 stp3_block_fused_fwd are run through a plain fp64 emulation of what the kernels do with them (the indexing documented in
 include/stp3_b200.h and stp3_b200/csrc/{aspp,block}_fused.cu: block order, weight rows of an N-wide chain, K-step ranges,
-hidden-accumulator columns, pieces of P) and compared with the fp64 oracle of the same module.  A packing / table mistake shows up here as
+hidden-accumulator columns, pieces of P; tests/fused_reference.py, the same reference the GPU contract test uses) and
+compared with the fp64 oracle of the same module.  A packing / table mistake shows up here as
 an O(1) error; the bf16 hi+lo split of the weights leaves ~1e-5.
 """
 import os
@@ -15,6 +16,7 @@ import torch.nn.functional as F
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
 from oracle import torch_dense as TD  # noqa: E402
+from tests import fused_reference as FR  # noqa: E402
 from stp3_b200.layers.convolutions import DeepLabHead  # noqa: E402
 from stp3_b200.layers.temporal import TemporalBlock  # noqa: E402
 
@@ -24,44 +26,10 @@ def f64(m):
     return copy.deepcopy(m).double()
 
 
-def shifted(x, dt, dy, dx):
-    """x (B,T,H,W,C) -> y[b,t,h,w] = x[b,t+dt,h+dy,w+dx] with zeros outside (what a TMA box delivers)."""
-    B, T, H, W, C = x.shape
-    p = F.pad(x, (0, 0, abs(dx), abs(dx), abs(dy), abs(dy), abs(dt), abs(dt)))
-    return p[:, abs(dt) + dt:abs(dt) + dt + T, abs(dy) + dy:abs(dy) + dy + H, abs(dx) + dx:abs(dx) + dx + W]
-
-
-def blocks_f64(w):
-    """(n_blocks, 2, 128, 64) bf16 [hi | lo] -> (n_blocks, 128, 64) fp64"""
-    return w[:, 0].double() + w[:, 1].double()
-
-
-# ----------------------------------------------------------------------------------------------- aspp_fused
 def emulate_aspp(x, pa, img_bias, relu=True):
-    """aspp_fused.cu: per branch s, acc1 = sum over its taps t and K blocks kb of x[.., kb] . W[t * kblocks + kb]^T (taps
-    numbered through all branches); P = relu(acc1 + br_bias[s]); acc2 += P[:, kb2] . W[proj_blk0 + 2 s + kb2]^T;
-    y = [relu](acc2 + img_bias[image])."""
-    W = blocks_f64(pa.w)
-    B, T, H, Wd, cin_p = x.shape
-    assert cin_p == pa.cin_p
-    kbs = cin_p // 64
-    n_taps = sum(len(t) for t in pa.taps)
-    proj_blk0 = n_taps * kbs
-    assert W.shape[0] == proj_blk0 + 2 * len(pa.taps)
-    acc2 = torch.zeros((B, T, H, Wd, 128), dtype=torch.float64)
-    t = 0
-    for s, taps in enumerate(pa.taps):
-        acc1 = torch.zeros((B, T, H, Wd, 128), dtype=torch.float64)
-        for (dy, dx) in taps:
-            xs = shifted(x, 0, dy, dx)
-            for kb in range(kbs):
-                acc1 += xs[..., kb * 64:(kb + 1) * 64] @ W[t * kbs + kb].T
-            t += 1
-        P = torch.relu(acc1 + pa.br_bias[s].double())
-        for kb2 in range(2):
-            acc2 += P[..., kb2 * 64:(kb2 + 1) * 64] @ W[proj_blk0 + 2 * s + kb2].T
-    y = acc2 + img_bias.double().view(B, T, 1, 1, 128)
-    return torch.relu(y) if relu else y
+    """the fp64 reference of the kernel (tests/fused_reference.py) on fp64 activations: (B, T, H, W, 128)"""
+    B, T, H, W, _ = x.shape
+    return FR.aspp(x, torch.zeros_like(x), pa, img_bias, relu=relu).view(B, T, H, W, 128)
 
 
 @pytest.mark.parametrize("cin,classes,H,W", [(64, 64, 40, 44)])
@@ -90,50 +58,22 @@ def test_deeplab_head_fused_packing_vs_oracle(cin, classes, H, W):
 
 
 # ----------------------------------------------------------------------------------------------- block_fused
-def unpair(blk, n):
-    """inverse of dense._pair_rows: rows [0, n/2) and [64, 64 + n/2) of a 128-row block -> the chain's n weight rows"""
-    return torch.cat([blk[:n // 2], blk[64:64 + n - n // 2]])
-
-
 def emulate_block_tail(mid, x, pb, hid_bias, img_bias, res_bias):
-    """block_fused.cu: chain c accumulates sum over its taps of src[.., cin_off : cin_off + 64] (shifted) . W_tap^T into
-    columns [tmem_col, tmem_col + n_mma) of the hidden accumulator (only K steps [k_lo, k_hi) are issued); piece pp of P =
-    relu(acc[piece_col[pp] : +8] + hid_bias[8 pp : +8]) (zeros for -1); out = relu(P . W_agg^T + img_bias) + (x . W_res^T +
-    res_bias | x)."""
-    W = blocks_f64(pb.w)
-    B, T, H, Wd, _ = x.shape
-    acc = torch.zeros((B, T, H, Wd, 160), dtype=torch.float64)
+    """the fp64 reference of the kernel on fp64 activations: (B, T, H, W, 64).  Also checks the packing invariant the
+    kernel's K-step ranges rely on: every weight outside a chain's issued K steps [k_lo, k_hi) is zero."""
+    W = pb.w[:, 0].double() + pb.w[:, 1].double()
     blk = 0
-    for src, cin_off, taps, n_mma, tmem_col, k_lo, k_hi in pb.chains:
-        assert n_mma % 16 == 0 and tmem_col + n_mma <= 160 and k_lo % 16 == 0 and k_hi % 16 == 0
-        inp = (x if src else mid)[..., cin_off:cin_off + 64]
-        assert inp.shape[-1] == 64
-        for (dt, dy, dx) in taps:
-            w = unpair(W[blk], n_mma)
-            assert float(w[:, :k_lo].abs().max() if k_lo else 0) == 0 and float(w[:, k_hi:].abs().max() if k_hi < 64 else 0) == 0, \
-                "weights outside the issued K steps"
-            acc[..., tmem_col:tmem_col + n_mma] += shifted(inp, dt, dy, dx)[..., k_lo:k_hi] @ w[:, k_lo:k_hi].T
+    for _, _, taps, n_mma, _, k_lo, k_hi in pb.chains + ([pb.res] if pb.res is not None else []):
+        if blk == sum(len(c[2]) for c in pb.chains):
+            blk += 2                                   # the aggregation blocks precede the projection
+        for _ in taps:
+            w = FR.unpair(W[blk], n_mma)
+            assert float(w[:, :k_lo].abs().max() if k_lo else 0) == 0 and \
+                float(w[:, k_hi:].abs().max() if k_hi < 64 else 0) == 0, "weights outside the issued K steps"
             blk += 1
-    P = torch.zeros((B, T, H, Wd, 128), dtype=torch.float64)
-    hb = hid_bias.double().view(B, T, 1, 1, 128)
-    for pp, col in enumerate(pb.piece_col):
-        if col >= 0:
-            P[..., 8 * pp:8 * pp + 8] = torch.relu(acc[..., col:col + 8] + hb[..., 8 * pp:8 * pp + 8])
-    out = torch.zeros((B, T, H, Wd, 64), dtype=torch.float64)
-    for kb2 in range(2):
-        out += P[..., kb2 * 64:(kb2 + 1) * 64] @ unpair(W[blk], 64).T
-        blk += 1
-    out = torch.relu(out + img_bias.double().view(B, T, 1, 1, 64))
-    if pb.res is not None:
-        _, cin_off, _, n_mma, _, k_lo, k_hi = pb.res
-        w = unpair(W[blk], n_mma)
-        blk += 1
-        assert float(w[:, k_hi:].abs().max() if k_hi < 64 else 0) == 0
-        out += x[..., cin_off + k_lo:cin_off + k_hi] @ w[:, k_lo:k_hi].T + res_bias.double().view(B, T, 1, 1, 64)
-    else:
-        out += x[..., :64]
-    assert blk == W.shape[0]
-    return out
+    B, T, H, Wd, _ = x.shape
+    out, _ = FR.block_tail(mid, torch.zeros_like(mid), x, torch.zeros_like(x), pb, hid_bias, img_bias, res_bias)
+    return out.view(B, T, H, Wd, 64)
 
 
 @pytest.mark.parametrize("cin,nc", [(70, 6), (64, 0)])
