@@ -199,7 +199,7 @@ typedef struct stp3_conv_desc {
   int tune_n_sub;        /* accepted and ignored: the CTA tile is always 8x16 pixels */
   int tune_group;        /* 0 = automatic; 1 = never share an activation load between the dy taps of a 3x3; 3 = share;
                             +4 = stream the weights through the smem ring even if they would fit (more activation stages);
-                            +8 = (bn 64) one stacked [W_hi; W_lo] operand: 2 MMAs per product instead of 3 */
+                            +8 = (64-column blocks) one stacked [W_hi; W_lo] operand: 2 MMAs per product instead of 3 */
   int n_cols;            /* output columns that carry weights (0 = bn): rows [n_cols, bn) of every weight block and the
                             bias are zero padding, so the kernel neither loads nor multiplies them (bn <= 128) */
   /* optional (bn = 64): col_sums[img][c] = sum over the output pixels of the activated output (fp32, (B*T, 64)) -- the
@@ -226,6 +226,11 @@ typedef struct stp3_conv_desc {
   long long w_img_stride; /* 0: one weight tensor for every image; > 0: image i's weights start at w + i * w_img_stride
                             (bf16 elements, a multiple of 64) -- the squeeze-excite gated projections (stp3_se_gate).  Such
                             weights are streamed through the shared-memory ring, never resident */
+  int tune_bn;           /* column-block width: 0 = automatic (bn up to 128 in one block, 256 as two of 128), 64 or 128
+                            (<= bn).  A convolution of several blocks is ONE launch whose work items are (pixel tile,
+                            column block) pairs: more and smaller items for the layers with few tiles, and at 64 the
+                            stacked operand (tune_group +8) and deeper shared-memory rings.  Its weights are streamed.
+                            Not with a fused head, a second destination or col_sums: they need every column in one CTA */
 } stp3_conv_desc;
 
 /* Optional fused 1x1 "head" evaluated on the activated output tile while it is still in registers:
@@ -245,6 +250,15 @@ typedef struct stp3_conv_head {
 
 /* bytes of device scratch stp3_conv_desc.col_sums needs for n_img images */
 size_t stp3_conv_col_sums_scratch_bytes(int n_img, int bn);
+/* How stp3_conv_fwd would run desc on a device of n_sm SMs, from the descriptor alone (host arithmetic, no device):
+ * work items = tiles of 8x16 pixels x column blocks, walked by `ctas` persistent CTAs; the shared-memory ring depths
+ * (b_stages = 0 and resident = 1: the weights stay in shared memory).  Same argument errors as stp3_conv_fwd. */
+typedef struct stp3_conv_tiling_info {
+  int bn_blk, stacked;
+  int tiles, items, ctas;
+  int a_stages, b_stages, resident;
+} stp3_conv_tiling_info;
+int stp3_conv_tiling(const stp3_conv_desc* desc, int n_sm, stp3_conv_tiling_info* out);
 int stp3_conv_fwd(const stp3_conv_desc* desc, const void* x_hi, const void* x_lo, const void* w, const float* bias,
                   const float* img_bias, const void* res_hi, const void* res_lo, void* y_hi, void* y_lo,
                   float* y_f32, const stp3_conv_head* head /* may be NULL */, void* stream);

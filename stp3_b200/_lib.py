@@ -47,7 +47,13 @@ class ConvDesc(ctypes.Structure):
                 ("res_cstride", _I), ("res_coff", _I), ("n_valid", _I), ("sigmoid", _I), ("tune_n_sub", _I), ("tune_group", _I),
                 ("n_cols", _I), ("col_sums", _V), ("col_sums_scratch", _V), ("col_sums_scratch_bytes", _SZ),
                 ("y2_hi", _V), ("y2_lo", _V), ("out2_cstride", _I), ("out2_coff", _I), ("n_store2", _I), ("relu2", _I),
-                ("k_lo", _I), ("k_hi", _I), ("f32_layout", _I), ("swish", _I), ("w_img_stride", _LL)]
+                ("k_lo", _I), ("k_hi", _I), ("f32_layout", _I), ("swish", _I), ("w_img_stride", _LL), ("tune_bn", _I)]
+
+
+class ConvTilingInfo(ctypes.Structure):
+    """Mirror of stp3_conv_tiling_info (include/stp3_b200.h)."""
+    _fields_ = [("bn_blk", _I), ("stacked", _I), ("tiles", _I), ("items", _I), ("ctas", _I), ("a_stages", _I),
+                ("b_stages", _I), ("resident", _I)]
 
 
 class DwDesc(ctypes.Structure):
@@ -84,6 +90,7 @@ class ConvHead(ctypes.Structure):
 SIGNATURES = {
     "stp3_abi_version": (_I, []),
     "stp3_conv_col_sums_scratch_bytes": (_SZ, [_I, _I]),
+    "stp3_conv_tiling": (_I, [ctypes.POINTER(ConvDesc), _I, ctypes.POINTER(ConvTilingInfo)]),
     "stp3_build_info": (ctypes.c_char_p, []),
     "stp3_last_error": (ctypes.c_char_p, []),
     "stp3_lift_splat_workspace_bytes": (_SZ, [_LSD]),

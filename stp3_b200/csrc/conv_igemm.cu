@@ -11,11 +11,13 @@
 // the weights/bias on the host; bias, per-image bias (pyramid-pool / ASPP-pool / ego-motion branches), ReLU,
 // residual add and the concat offset are fused in the epilogue.
 //
-//   tile     : 128 output pixels (8 x 16 of one image) x BN output channels (64 / 128; 256 runs as two launches)
+//   item     : 128 output pixels (8 x 16 of one image) x one block of BN output channels (64 / 128).  A convolution
+//              wider than its column block (256 columns, or 128 / 256 in 64-column blocks) is still ONE launch: the
+//              blocks of a pixel tile are consecutive work items, so the tile's activation windows stay hot in L2
 //   K loop   : taps x (Cin / 64); TMA brings A_hi, A_lo (128 or 160 pixel rows x 64 bf16, 128B-swizzled; one load
 //              serves the three dy taps of a 3x3) and B_hi, B_lo (BN x 64; small weight tensors stay resident in
 //              smem) through separate rings; each warpgroup issues 4 (K = 16) x 3 wgmma per tap for its 64 rows
-//   CTA      : persistent, one per SM, walks tiles blockIdx.x + i*gridDim.x
+//   CTA      : persistent, one per SM, walks items blockIdx.x + i*gridDim.x
 //   warps    : 0..7 = two MMA warpgroups (rows 0..63 / 64..127 of the tile): wgmma only, then their fragments into
 //              the shared accumulator tile; 8..15 = two epilogue warpgroups (shared accumulator tile -> global) that
 //              drain tile u while the MMA warpgroups multiply tile u+1; 16 = TMA producer (17..19 leave at once)
@@ -54,6 +56,7 @@ constexpr int kBK = 64;                         // channels per K step (one 128-
 constexpr int kMaxTaps = 49;
 constexpr int kMaxAStages = 4, kMaxBStages = 8;
 constexpr int kMaxHeadOut = 8;
+constexpr size_t kSmemCap = 227 * 1024;           // dynamic shared memory one CTA may ask for
 
 struct ConvParams {
   int n_img, T, t0, Ho, Wo;
@@ -62,6 +65,9 @@ struct ConvParams {
   int skip_t;               // skip tap groups whose window lies entirely in the zero padding for the whole tile (frame
                             // outside [0, T_total): causal convs at t = 0; rows / columns outside the image: dilated convs)
   int tiles_x, tiles_y, n_tiles;
+  int n_nblk;               // column blocks of BN output channels per pixel tile; work item i = (tile i / n_nblk, block
+                            // i % n_nblk).  Block nb owns columns [nb * BN, nb * BN + BN) of the weights, the bias, the
+                            // residual and every output
   int stride;
   int kblocks;              // Cin / 64 of this convolution
   int cin_off;              // first input channel inside the (wider) input tensor, multiple of 64
@@ -81,9 +87,8 @@ struct ConvParams {
   int b_tile_bytes;         // shared-memory bytes of one K step's weights (hi and lo parts)
   int b_load_bytes;         // bytes TMA brings per K step: 2 * n_mma rows
   int w_rows;               // rows per (tap, kb, plane) block of the packed weight tensor (the convolution's padded Cout)
-  int w_row_off;            // first row of this launch inside that block (a 256-channel conv runs as two launches)
   signed char tap[kMaxTaps][4];   // (dt, dy, dx): input coordinate = output coordinate * stride + d
-  const float* bias;        // [BN]
+  const float* bias;        // [n_nblk * BN]
   const float* img_bias;    // [n_img][img_bias_stride] or null (replaces bias)
   int img_bias_stride;
   int relu;
@@ -96,7 +101,7 @@ struct ConvParams {
   int out_cstride, out_coff, n_store;
   int vec256;               // bit 0: output rows / windows are 32-byte aligned (256-bit stores), bit 1: residual likewise
   float* out_f32;           // optional (n_img, n_valid, Ho, Wo) fp32, the reference's NCHW layout
-  int n_valid, f32_coff;    // channel offset of this launch inside out_f32
+  int n_valid;
   int f32_nhwc;             // out_f32 is channels-last (n_img, Ho, Wo, n_valid): 16 channels of a pixel = two 32-byte stores
   int sigmoid;              // apply to out_f32 (instance_center head)
   int na_stages, nb_stages; // smem ring depths chosen by the host
@@ -129,7 +134,8 @@ template <int BN>
 struct ConvSmem {
   static constexpr int kAccStride = BN + 4;                            // floats per row of the shared accumulator tile
   // the tail behind the operand rings (or the resident weights), byte offsets from its start
-  static constexpr int bias = 0;                                       // fp32 [BN]
+  static constexpr int bias = 0;                                       // fp32 [n_nblk * BN]: the blocks beyond the first
+                                                                       // lie over the head weights (n_nblk > 1: no head)
   static constexpr int head = bias + BN * 4;                           // fp32 [kMaxHeadOut][BN] fused head weights
   static constexpr int hx = head + kMaxHeadOut * BN * 4;               // fp32 [kMaxHeadOut][128] head partials handed between column halves
   static constexpr int wb = hx + kMaxHeadOut * 128 * 4;                // fp32 [kEpiWarps][64] per-image bias slice of each epilogue warp
@@ -159,7 +165,8 @@ __device__ __forceinline__ void ld_acc16(const float* src, uint32_t (&r)[16]) { 
 }
 
 // Persistent, warp-specialised implicit-GEMM convolution.
-//   * A CTA walks output tiles blockIdx.x + i*gridDim.x; a tile is 8x16 pixels = 128 accumulator rows, 64 per warpgroup.
+//   * A CTA walks work items blockIdx.x + i*gridDim.x: (pixel tile, column block) pairs, the blocks of a tile next to
+//     each other.  A tile is 8x16 pixels = 128 accumulator rows, 64 per warpgroup.
 //   * Activations and weights travel through separate shared-memory rings filled by one producer warp.  For 3x3 /
 //     stride 1 / dilation 1 kernels one activation load of 10 image rows serves the three dy taps: their A operands are
 //     the same smem tile at row offsets 0, 16, 32 (2 KB steps keep the 1024-byte swizzle alignment).
@@ -217,30 +224,33 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
     ptx::mbar_init(bres_bar, 1);
     ptx::fence_mbar_init();
   }
-  for (int i = threadIdx.x; i < BN; i += blockDim.x) s_bias[i] = p.bias[i];
+  static_assert(kMaxHeadOut * BN >= 256 - BN, "the bias of every column block fits in the bias and head-weight areas");
+  for (int i = threadIdx.x; i < p.n_nblk * BN; i += blockDim.x) s_bias[i] = p.bias[i];
   for (int i = threadIdx.x; i < p.head_ko * BN; i += blockDim.x) s_head[i] = p.head_w[i];
   __syncthreads();
   const int tiles_per_img = p.tiles_x * p.tiles_y;
   const int n_groups = p.n_groups;
   const int tile_h = kSubH;
+  const int n_items = p.n_tiles * p.n_nblk;
 
   if (warp >= kProducerWarp) {
     ptx::setmaxnreg_dec<kProducerRegs>();
     if (warp != kProducerWarp) return;
     // ===================== TMA producer (whole warp walks the loops; one elected lane issues) =====================
     // load_b: the weight tile of K step `it` into `dst` (called by the elected lane; transaction bytes on `bar`)
-    auto load_b = [&](unsigned char* dst, int it, uint64_t* bar, int img_w) {
-      const int row_hi = (int)((it * 2) * p.w_rows + p.w_row_off + img_w * p.w_img_rows), row_lo = row_hi + p.w_rows;
+    auto load_b = [&](unsigned char* dst, int it, uint64_t* bar, int img_w, int nb) {
+      const int row_hi = (int)((it * 2) * p.w_rows + nb * BN + img_w * p.w_img_rows), row_lo = row_hi + p.w_rows;
       ptx::tma_load_2d(dst, &tm_w, bar, 0, row_hi);                       // [W_hi; W_lo], also the stacked operand
       ptx::tma_load_2d(dst + kBRows * kBK * 2, &tm_w, bar, 0, row_lo);
     };
     if (resident && ptx::elect_one_sync()) {
       ptx::mbar_arrive_expect_tx(bres_bar, (uint32_t)(k_iters * p.b_load_bytes));
-      for (int it = 0; it < k_iters; ++it) load_b(b_ring + (size_t)it * p.b_tile_bytes, it, bres_bar, 0);
+      for (int it = 0; it < k_iters; ++it) load_b(b_ring + (size_t)it * p.b_tile_bytes, it, bres_bar, 0, 0);
     }
     __syncwarp();
     ptx::griddep_wait();                        // activations come from the preceding kernel
-    for (int tile = cta; tile < p.n_tiles; tile += n_cta) {
+    for (int item = cta; item < n_items; item += n_cta) {
+      const int tile = item / p.n_nblk, nb = item % p.n_nblk;
       const int img = tile / tiles_per_img, rem = tile % tiles_per_img;
       const int oy0 = (rem / p.tiles_x) * tile_h, ox0 = (rem % p.tiles_x) * kTileW;
       const int bidx = img / p.T, tidx = p.t0 + img % p.T;
@@ -261,7 +271,7 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
             for (int j = 0; j < gsz; ++j) {
               const int it = (tap0 + j) * p.kblocks + kb;          // [tap][kb][plane][rows] blocks of 64-wide rows
               rb.produce((uint32_t)p.b_load_bytes,
-                         [&](int s, uint64_t* bar) { load_b(b_ring + (size_t)s * p.b_tile_bytes, it, bar, img); });
+                         [&](int s, uint64_t* bar) { load_b(b_ring + (size_t)s * p.b_tile_bytes, it, bar, img, nb); });
             }
           }
         }
@@ -377,7 +387,7 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
       }
       ptx::bar_arrive(kBarAccFull, kHandoverThreads);
     };
-    for (int tile = cta; tile < p.n_tiles; tile += n_cta) mma_tile(tile);
+    for (int item = cta; item < n_items; item += n_cta) mma_tile(item / p.n_nblk);   // whichever column block: the producer chose the weights
   } else {
     // ===================== two epilogue warpgroups: shared accumulator tile -> registers -> global =====================
     ptx::setmaxnreg_inc<kEpiRegs>();
@@ -422,8 +432,10 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
       }
     };
     ptx::griddep_wait();                          // residual / per-image bias reads and every global write come after
-    for (int tile = cta; tile < p.n_tiles; tile += n_cta) {
-      ptx::bar_arrive(kBarAccFree, kHandoverThreads);   // done with the previous tile's accumulators (if any)
+    for (int item = cta; item < n_items; item += n_cta) {
+      ptx::bar_arrive(kBarAccFree, kHandoverThreads);   // done with the previous item's accumulators (if any)
+      const int tile = item / p.n_nblk;
+      const int cblk = (item % p.n_nblk) * BN;          // first column of this item's block in the whole convolution
       const int img = tile / tiles_per_img, rem = tile % tiles_per_img;
       const int oy_t = (rem / p.tiles_x) * kSubH, ox = (rem % p.tiles_x) * kTileW + (r & 15);
       if (kSums && p.sum_part && img != sum_img) {      // tiles come in image order: hand the finished image over
@@ -436,7 +448,7 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
       auto request_residual = [&](int j) {
         const int oy = oy_t + (r >> 4);
         if (oy < p.Ho && ox < p.Wo) {
-          const size_t off = (((size_t)img * p.Ho + oy) * p.Wo + ox) * p.res_cstride + p.res_coff + col0 + j * 16;
+          const size_t off = (((size_t)img * p.Ho + oy) * p.Wo + ox) * p.res_cstride + p.res_coff + cblk + col0 + j * 16;
           // coherent loads: the residual (like the per-image bias below) is written by a PRECEDING kernel that this grid
           // may overlap under programmatic dependent launch, so the read-only (.nc) path is not allowed for it
           if (p.vec256 & 2) {
@@ -454,9 +466,9 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
         }
       };
       if (p.res_mode) request_residual(0);
-      const float* bsrc = s_bias;                 // bias of column c at bsrc[c]
+      const float* bsrc = s_bias + cblk;          // bias of the block's column c at bsrc[c]
       if (p.img_bias) {
-        const float* ib = p.img_bias + (size_t)img * p.img_bias_stride + col0;
+        const float* ib = p.img_bias + (size_t)img * p.img_bias_stride + cblk + col0;
         float* wb = s_wb + e * 64;
         __syncwarp();                             // every lane is done with the previous tile's slice
 #pragma unroll
@@ -475,7 +487,8 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
         const float* acc_row = s_acc + (size_t)r * S::kAccStride + col0;
 #pragma unroll 1
         for (int j = 0; j < kColsPerWarp / 16; ++j) {
-          const int cb = col0 + j * 16;              // first output channel of this chunk
+          const int cb = col0 + j * 16;              // first column of this chunk in the block,
+          const int cg = cblk + cb;                  // in the convolution
           uint32_t acc[16];
           const bool computed = cb < p.n_mma;        // columns beyond n_mma: zero weights, never multiplied
           if (computed) {
@@ -512,26 +525,26 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
 #pragma unroll
               for (int i = 0; i < 16; ++i) v[i] = v[i] / (1.f + __expf(-v[i]));
             }
-            if (d_hi && cb < d_nstore) {
-              __nv_bfloat16* ohp = d_hi + pix * d_cstride + d_coff + cb;
-              __nv_bfloat16* olp = d_lo + pix * d_cstride + d_coff + cb;
+            if (d_hi && cg < d_nstore) {
+              __nv_bfloat16* ohp = d_hi + pix * d_cstride + d_coff + cg;
+              __nv_bfloat16* olp = d_lo + pix * d_cstride + d_coff + cg;
               uint32_t hw[8], lw[8];
 #pragma unroll
               for (int e2 = 0; e2 < 8; ++e2) ptx::split_hilo(v[e2 * 2], v[e2 * 2 + 1], hw[e2], lw[e2]);
-              if (d_vec && cb + 16 <= d_nstore) {               // one full 32-byte sector per plane and lane
+              if (d_vec && cg + 16 <= d_nstore) {               // one full 32-byte sector per plane and lane
                 ptx::st_global_v8(ohp, hw);
                 ptx::st_global_v8(olp, lw);
               } else {
                 reinterpret_cast<uint4*>(ohp)[0] = make_uint4(hw[0], hw[1], hw[2], hw[3]);
                 reinterpret_cast<uint4*>(olp)[0] = make_uint4(lw[0], lw[1], lw[2], lw[3]);
-                if (cb + 8 < d_nstore) {
+                if (cg + 8 < d_nstore) {
                   reinterpret_cast<uint4*>(ohp)[1] = make_uint4(hw[4], hw[5], hw[6], hw[7]);
                   reinterpret_cast<uint4*>(olp)[1] = make_uint4(lw[4], lw[5], lw[6], lw[7]);
                 }
               }
             }
             if (p.out_f32 && p.f32_nhwc) {
-              const int c0 = p.f32_coff + cb;
+              const int c0 = cg;
               float* dst = p.out_f32 + pix * p.n_valid + c0;
               if (c0 + 16 <= p.n_valid && (p.n_valid & 7) == 0) {          // rows are 32-byte aligned (host checks the base)
                 ptx::st_global_v8f(dst, v);
@@ -544,7 +557,7 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
             } else if (p.out_f32) {
 #pragma unroll
               for (int i = 0; i < 16; ++i) {
-                const int c = p.f32_coff + cb + i;
+                const int c = cg + i;
                 if (c < p.n_valid) {
                   float x = v[i];
                   if (p.sigmoid) x = 1.f / (1.f + __expf(-x));
@@ -637,18 +650,116 @@ int launch_col_sum_reduce(const float* part, int n_part, int n_img, float* out, 
   return STP3_OK;
 }
 
-// Ring depths for this instantiation's shared-memory tail, then the launch.  p.a_plane_bytes is set.
 template <int BN, bool STACK, bool FULLK>
-static int launch_conv(ConvParams& p, const CUtensorMap& tm_hi, const CUtensorMap& tm_lo, const CUtensorMap& tm_w,
-                       int n_mma, int k_iters, bool stream_weights, unsigned grid, cudaStream_t stream) {
-  using SM = ConvSmem<BN>;
-  const size_t smem_cap = 227 * 1024;
+static int launch_conv(const ConvParams& p, const CUtensorMap& tm_hi, const CUtensorMap& tm_lo, const CUtensorMap& tm_w,
+                       size_t smem_bytes, unsigned grid, cudaStream_t stream) {
+  constexpr auto kern = conv_igemm_kernel<BN, STACK, FULLK>;
+  STP3_CUDA_OK(set_max_dynamic_smem<kern>((int)kSmemCap));
+  STP3_CUDA_OK(launch_pdl(kPdlConv, kern, dim3(grid), dim3(kConvThreads), smem_bytes, stream, tm_hi, tm_lo, tm_w, p));
+  return STP3_OK;
+}
+
+// What the host decides from the descriptor alone: the instantiation, the work items and the ring depths.
+// stp3_conv_fwd launches it, stp3_conv_tiling reports it.
+struct ConvPlan {
+  int bn_blk;               // column-block width = the kernel's BN
+  bool stack, full_k;
+  int box_h;                // image rows of one activation stage
+  int k_iters;
+  unsigned grid;
+  size_t smem_bytes;
+};
+
+// Checks every rule of the descriptor that needs no tensor pointer and fills the geometry, tiling and ring fields of p.
+static int plan_conv(const stp3_conv_desc* d, bool has_head, int n_sm, ConvParams& p, ConvPlan& t) {
+  STP3_CHECK_ARG(d->B > 0 && d->T > 0 && d->H > 0 && d->W > 0 && d->Ho > 0 && d->Wo > 0, "non-positive dimension");
+  const int T_total = d->T_total > 0 ? d->T_total : d->T;
+  STP3_CHECK_ARG(d->t0 >= 0 && d->t0 + d->T <= T_total, "frame window [t0, t0+T) outside the input tensor");
+  const int n_store = d->n_store > 0 ? d->n_store : d->bn;
+  STP3_CHECK_ARG(n_store % 8 == 0 && n_store <= d->bn, "n_store must be a multiple of 8 and <= bn");
+  STP3_CHECK_ARG(d->in_cstride % 64 == 0 && d->cin % 64 == 0 && d->cin_off % 64 == 0 && d->cin > 0 &&
+                 d->cin_off + d->cin <= d->in_cstride, "input channels must be padded to multiples of 64");
+  STP3_CHECK_ARG(d->bn == 64 || d->bn == 128 || d->bn == 256, "bn (padded output channels) must be 64, 128 or 256");
+  STP3_CHECK_ARG(d->stride == 1 || d->stride == 2, "stride must be 1 or 2");
+  STP3_CHECK_ARG(d->ntaps >= 1 && d->ntaps <= kMaxTaps, "ntaps out of range");
+  STP3_CHECK_ARG(!d->swish || (!d->relu && d->res_mode != 2 && !d->y2_hi), "swish: not with relu, res_mode 2 or a second destination");
+  if (d->w_img_stride)
+    STP3_CHECK_ARG(d->w_img_stride > 0 && d->w_img_stride % 64 == 0 &&
+                   d->w_img_stride >= (long long)d->ntaps * (d->cin / 64) * 2 * d->bn * 64,
+                   "w_img_stride: a multiple of 64 elements, at least one image's weight blocks");
+  STP3_CHECK_ARG(d->f32_layout == 0 || d->f32_layout == 1, "f32_layout must be 0 (n_img, n_valid, Ho, Wo) or 1 (n_img, Ho, Wo, n_valid)");
+
+  // column blocks: tune_bn, or as wide as the kernel goes (128)
+  STP3_CHECK_ARG(d->tune_bn == 0 || ((d->tune_bn == 64 || d->tune_bn == 128) && d->tune_bn <= d->bn),
+                 "tune_bn (column-block width) must be 0, 64 or 128 and <= bn");
+  t.bn_blk = d->tune_bn ? d->tune_bn : (d->bn == 256 ? 128 : d->bn);
+  p.n_nblk = d->bn / t.bn_blk;
+  STP3_CHECK_ARG(p.n_nblk == 1 || (!has_head && !d->y2_hi && !d->col_sums),
+                 "a fused head, a second destination and col_sums need the convolution's columns in one block (tune_bn)");
+
+  // tuning knobs (0 = automatic): desc->tune_group, or the STP3_CONV_GROUP environment variable.  tune_n_sub is
+  // accepted for ABI compatibility; the tile is always 8 x 16 pixels.
+  static const int env_group = [] { const char* e = getenv("STP3_CONV_GROUP"); return e ? atoi(e) : 0; }();
+  const int want_group_raw = d->tune_group ? d->tune_group : env_group;
+  const int want_group = want_group_raw & 3;
+  // +4: keep the weights in the ring even if they would fit; per-image weights always stream, and so do the weights
+  // of several column blocks (a CTA meets all of them)
+  const bool stream_weights = (want_group_raw & 4) != 0 || d->w_img_stride != 0 || p.n_nblk > 1;
+  // +8: stacked [W_hi; W_lo] operand (64-column blocks only).  Untuned (tune_group == 0) multi-tap layers in 64-column
+  // blocks use it: it reads the activation tile twice instead of three times
+  t.stack = t.bn_blk == 64 && ((want_group_raw & 8) != 0 || (want_group_raw == 0 && d->ntaps > 1));
+  // taps that can share one activation load: runs (<= 4) of consecutive taps with the same (dt, dx) and dy advancing
+  // by the stride
+  p.n_groups = 0; p.gmax = 1;
+  for (int i = 0; i < d->ntaps;) {
+    int g = 1;
+    if (want_group != 1)
+      while (g < 4 && i + g < d->ntaps && d->taps[i + g][0] == d->taps[i][0] && d->taps[i + g][2] == d->taps[i][2] &&
+             d->taps[i + g][1] == d->taps[i][1] + g * d->stride)
+        ++g;
+    p.gstart[p.n_groups] = (unsigned char)i; p.gsize[p.n_groups] = (unsigned char)g; ++p.n_groups;
+    if (g > p.gmax) p.gmax = g;
+    i += g;
+  }
+  t.box_h = kSubH + (p.gmax - 1);                                        // image rows one CTA loads per stage
+
+  const int kblocks = d->cin / kBK;
+  // the MMAs cover only the columns that carry weights (n_cols, rounded up to a multiple of 16); with several column
+  // blocks every block runs at full width (the padding rows are zeros)
+  const int n_mma = p.n_nblk == 1 && d->n_cols > 0 && d->n_cols < d->bn ? ((d->n_cols + 15) / 16) * 16 : t.bn_blk;
+  p.n_img = d->B * d->T; p.T = d->T; p.t0 = d->t0; p.Ho = d->Ho; p.Wo = d->Wo;
+  p.T_total = T_total;
+  p.H = d->H; p.W = d->W;
+  p.skip_t = 0;                                     // safe only if some tap always stays inside: the centre tap
+  for (int i = 0; i < d->ntaps; ++i) if (d->taps[i][0] == 0 && d->taps[i][1] == 0 && d->taps[i][2] == 0) p.skip_t = 1;
+  p.tiles_x = ceil_div(d->Wo, kTileW); p.tiles_y = ceil_div(d->Ho, kSubH);
+  p.stride = d->stride; p.kblocks = kblocks; p.cin_off = d->cin_off; p.ntaps = d->ntaps;
+  {
+    const int k_lo = d->k_hi > 0 ? d->k_lo : 0, k_hi = d->k_hi > 0 ? d->k_hi : d->cin;
+    STP3_CHECK_ARG(k_lo % 16 == 0 && k_hi % 16 == 0 && k_lo >= 0 && k_lo < k_hi && k_hi <= d->cin &&
+                   k_lo < kBK && k_hi > d->cin - kBK, "k_lo / k_hi: multiples of 16 inside the first / last 64-channel block");
+    p.ks_first = k_lo / 16;
+    p.ks_end = (k_hi - (kblocks - 1) * kBK) / 16;
+    STP3_CHECK_ARG(kblocks > 1 || p.ks_first < p.ks_end, "empty K range");
+  }
+  p.a_plane_bytes = t.box_h * kTileW * kBK * 2; p.w_rows = d->bn; p.n_mma = n_mma;
+  for (int i = 0; i < d->ntaps; ++i) { p.tap[i][0] = d->taps[i][0]; p.tap[i][1] = d->taps[i][1]; p.tap[i][2] = d->taps[i][2]; p.tap[i][3] = 0; }
+  t.k_iters = d->ntaps * kblocks;
+  t.full_k = p.ks_first == 0 && p.ks_end == kBK / 16;
+  const long long ntile = (long long)p.n_img * p.tiles_x * p.tiles_y;
+  STP3_CHECK_ARG(ntile > 0 && ntile * p.n_nblk < (1ll << 31), "grid too large");
+  p.n_tiles = (int)ntile;
+  const long long items = ntile * p.n_nblk;
+  t.grid = (unsigned)(items < n_sm ? items : n_sm);                      // persistent: one CTA per SM
+
+  // ring depths beside this block width's shared-memory tail
+  const size_t tail = t.bn_blk == 64 ? ConvSmem<64>::tail_bytes() : ConvSmem<128>::tail_bytes();
   const size_t a_stage = 2 * (size_t)p.a_plane_bytes;
-  p.b_rows = FULLK ? BN : n_mma;
+  p.b_rows = t.full_k ? t.bn_blk : n_mma;
   p.b_tile_bytes = 2 * p.b_rows * kBK * 2;
   p.b_load_bytes = 2 * n_mma * kBK * 2;
-  const size_t avail = smem_cap - 1024 - SM::tail_bytes();
-  const size_t wbytes = (size_t)k_iters * (size_t)p.b_tile_bytes;
+  const size_t avail = kSmemCap - 1024 - tail;
+  const size_t wbytes = (size_t)t.k_iters * (size_t)p.b_tile_bytes;
   // small weight tensors stay resident in smem next to >= 2 activation stages
   const bool res = !stream_weights && wbytes + 2 * a_stage <= avail;
   int na, nb;
@@ -666,10 +777,7 @@ static int launch_conv(ConvParams& p, const CUtensorMap& tm_hi, const CUtensorMa
   if (na > kMaxAStages) na = kMaxAStages;
   if (nb > kMaxBStages) nb = kMaxBStages;
   p.na_stages = na; p.nb_stages = nb; p.b_resident = res ? 1 : 0;
-  const size_t smem_bytes = 1024 + na * a_stage + (res ? wbytes : (size_t)nb * (size_t)p.b_tile_bytes) + SM::tail_bytes();
-  constexpr auto kern = conv_igemm_kernel<BN, STACK, FULLK>;
-  STP3_CUDA_OK(set_max_dynamic_smem<kern>((int)smem_cap));
-  STP3_CUDA_OK(launch_pdl(kPdlConv, kern, dim3(grid), dim3(kConvThreads), smem_bytes, stream, tm_hi, tm_lo, tm_w, p));
+  t.smem_bytes = 1024 + na * a_stage + (res ? wbytes : (size_t)nb * (size_t)p.b_tile_bytes) + tail;
   return STP3_OK;
 }
 
@@ -679,6 +787,16 @@ using namespace stp3;
 
 extern "C" size_t stp3_conv_col_sums_scratch_bytes(int n_img, int bn) {
   return (size_t)num_sms() * 4 * (size_t)(n_img > 0 ? n_img : 0) * (size_t)(bn > 0 ? bn : 0) * sizeof(float);
+}
+
+extern "C" int stp3_conv_tiling(const stp3_conv_desc* d, int n_sm, stp3_conv_tiling_info* out) {
+  STP3_CHECK_ARG(d && out && n_sm > 0, "stp3_conv_tiling: null pointer argument or no SM");
+  ConvParams p;
+  ConvPlan t;
+  if (const int rc = plan_conv(d, false, n_sm, p, t)) return rc;
+  out->bn_blk = t.bn_blk; out->stacked = t.stack; out->tiles = p.n_tiles; out->items = p.n_tiles * p.n_nblk;
+  out->ctas = (int)t.grid; out->a_stages = p.na_stages; out->b_stages = p.nb_stages; out->resident = p.b_resident;
+  return STP3_OK;
 }
 
 extern "C" int stp3_conv_fwd(const stp3_conv_desc* d, const void* x_hi, const void* x_lo, const void* w,
@@ -692,98 +810,39 @@ extern "C" int stp3_conv_fwd(const stp3_conv_desc* d, const void* x_hi, const vo
     STP3_CHECK_ARG(d->bn <= 128, "a fused head needs bn <= 128");
     for (int k = 0; k < head->n_out; ++k) STP3_CHECK_ARG(head->out[k] != nullptr, "fused head: null output plane");
   }
-  STP3_CHECK_ARG(d->B > 0 && d->T > 0 && d->H > 0 && d->W > 0 && d->Ho > 0 && d->Wo > 0, "non-positive dimension");
-  const int T_total = d->T_total > 0 ? d->T_total : d->T;
-  STP3_CHECK_ARG(d->t0 >= 0 && d->t0 + d->T <= T_total, "frame window [t0, t0+T) outside the input tensor");
+  ConvParams p;
+  ConvPlan t;
+  if (const int rc = plan_conv(d, head != nullptr, num_sms(), p, t)) return rc;
   const int n_store = d->n_store > 0 ? d->n_store : d->bn;
-  STP3_CHECK_ARG(n_store % 8 == 0 && n_store <= d->bn, "n_store must be a multiple of 8 and <= bn");
-  STP3_CHECK_ARG(d->in_cstride % 64 == 0 && d->cin % 64 == 0 && d->cin_off % 64 == 0 && d->cin > 0 &&
-                 d->cin_off + d->cin <= d->in_cstride, "input channels must be padded to multiples of 64");
-  STP3_CHECK_ARG(d->bn == 64 || d->bn == 128 || d->bn == 256, "bn (padded output channels) must be 64, 128 or 256");
-  STP3_CHECK_ARG(d->stride == 1 || d->stride == 2, "stride must be 1 or 2");
-  STP3_CHECK_ARG(d->ntaps >= 1 && d->ntaps <= kMaxTaps, "ntaps out of range");
   if (y_hi) STP3_CHECK_ARG(d->out_cstride % 8 == 0 && d->out_coff % 8 == 0 && d->out_coff + n_store <= d->out_cstride,
                            "output channel window does not fit the output tensor");
   if (d->res_mode) STP3_CHECK_ARG(res_hi && res_lo && d->res_cstride % 8 == 0 && d->res_coff % 8 == 0 &&
                                   d->res_coff + d->bn <= d->res_cstride, "bad residual tensor");
   if (y_f32) STP3_CHECK_ARG(d->n_valid > 0 && d->n_valid <= d->bn, "n_valid out of range");
-  STP3_CHECK_ARG(!d->swish || (!d->relu && d->res_mode != 2 && !d->y2_hi), "swish: not with relu, res_mode 2 or a second destination");
-  if (d->w_img_stride)
-    STP3_CHECK_ARG(d->w_img_stride > 0 && d->w_img_stride % 64 == 0 &&
-                   d->w_img_stride >= (long long)d->ntaps * (d->cin / 64) * 2 * d->bn * 64,
-                   "w_img_stride: a multiple of 64 elements, at least one image's weight blocks");
   if (!tmap_encode_fn()) return set_error(STP3_ECUDA, "cuTensorMapEncodeTiled is not available from the driver");
-
-  // tuning knobs (0 = automatic): desc->tune_group, or the STP3_CONV_GROUP environment variable.  tune_n_sub is
-  // accepted for ABI compatibility; the tile is always 8 x 16 pixels.
-  static const int env_group = [] { const char* e = getenv("STP3_CONV_GROUP"); return e ? atoi(e) : 0; }();
-  const int want_group_raw = d->tune_group ? d->tune_group : env_group;
-  const int want_group = want_group_raw & 3;
-  // +4: keep the weights in the ring even if they would fit; per-image weights always stream
-  const bool stream_weights = (want_group_raw & 4) != 0 || d->w_img_stride != 0;
-  // +8: stacked [W_hi; W_lo] operand (bn = 64 only).  Untuned (tune_group == 0) multi-tap 64-column layers use it: it
-  // reads the activation tile twice instead of three times
-  const bool stack = d->bn == 64 && ((want_group_raw & 8) != 0 || (want_group_raw == 0 && d->ntaps > 1));
-  // taps that can share one activation load: runs (<= 4) of consecutive taps with the same (dt, dx) and dy advancing
-  // by the stride
-  ConvParams p;
-  p.n_groups = 0; p.gmax = 1;
-  for (int i = 0; i < d->ntaps;) {
-    int g = 1;
-    if (want_group != 1)
-      while (g < 4 && i + g < d->ntaps && d->taps[i + g][0] == d->taps[i][0] && d->taps[i + g][2] == d->taps[i][2] &&
-             d->taps[i + g][1] == d->taps[i][1] + g * d->stride)
-        ++g;
-    p.gstart[p.n_groups] = (unsigned char)i; p.gsize[p.n_groups] = (unsigned char)g; ++p.n_groups;
-    if (g > p.gmax) p.gmax = g;
-    i += g;
-  }
-  const int group = p.gmax;
-  const int tile_h = kSubH;
-  const int box_h = kSubH + (group - 1);                                 // image rows one CTA loads per stage
 
   CUtensorMap tm_hi, tm_lo, tm_w;
   {
-    const int box_w = (kTileW - 1) * d->stride + 1, box_rows = (box_h - 1) * d->stride + 1;
-    const CUresult r1 = encode_act_5d(&tm_hi, x_hi, d->in_cstride, d->W, d->H, T_total, d->B, box_w, box_rows, d->stride);
-    const CUresult r2 = encode_act_5d(&tm_lo, x_lo, d->in_cstride, d->W, d->H, T_total, d->B, box_w, box_rows, d->stride);
+    const int box_w = (kTileW - 1) * d->stride + 1, box_rows = (t.box_h - 1) * d->stride + 1;
+    const CUresult r1 = encode_act_5d(&tm_hi, x_hi, d->in_cstride, d->W, d->H, p.T_total, d->B, box_w, box_rows, d->stride);
+    const CUresult r2 = encode_act_5d(&tm_lo, x_lo, d->in_cstride, d->W, d->H, p.T_total, d->B, box_w, box_rows, d->stride);
     if (r1 != CUDA_SUCCESS || r2 != CUDA_SUCCESS)
       return set_error(STP3_ECUDA, "cuTensorMapEncodeTiled(activation) failed: %d %d", (int)r1, (int)r2);
   }
-  const int kblocks = d->cin / kBK;
-  const int bn_launch = d->bn == 256 ? 128 : d->bn;     // 256 output channels run as two 128-column launches
-  // the MMAs cover only the columns that carry weights (n_cols, rounded up to a multiple of 16)
-  const int n_mma = d->bn <= 128 && d->n_cols > 0 && d->n_cols < d->bn ? ((d->n_cols + 15) / 16) * 16 : bn_launch;
   {
-    const long long rows = d->w_img_stride ? (long long)(d->B * d->T - 1) * (d->w_img_stride / 64) + (long long)d->ntaps * kblocks * 2 * d->bn
-                                           : (long long)d->ntaps * kblocks * 2 * d->bn;
-    const CUresult r = encode_rows_2d(&tm_w, w, rows, n_mma);
+    const long long rows = d->w_img_stride ? (long long)(d->B * d->T - 1) * (d->w_img_stride / 64) + (long long)t.k_iters * 2 * d->bn
+                                           : (long long)t.k_iters * 2 * d->bn;
+    const CUresult r = encode_rows_2d(&tm_w, w, rows, p.n_mma);
     if (r != CUDA_SUCCESS) return set_error(STP3_ECUDA, "cuTensorMapEncodeTiled(weights) failed: %d", (int)r);
   }
 
-  p.n_img = d->B * d->T; p.T = d->T; p.t0 = d->t0; p.Ho = d->Ho; p.Wo = d->Wo;
-  p.T_total = T_total;
-  p.H = d->H; p.W = d->W;
-  p.skip_t = 0;                                     // safe only if some tap always stays inside: the centre tap
-  for (int i = 0; i < d->ntaps; ++i) if (d->taps[i][0] == 0 && d->taps[i][1] == 0 && d->taps[i][2] == 0) p.skip_t = 1;
-  p.tiles_x = ceil_div(d->Wo, kTileW); p.tiles_y = ceil_div(d->Ho, tile_h);
-  p.stride = d->stride; p.kblocks = kblocks; p.cin_off = d->cin_off; p.ntaps = d->ntaps;
-  {
-    const int k_lo = d->k_hi > 0 ? d->k_lo : 0, k_hi = d->k_hi > 0 ? d->k_hi : d->cin;
-    STP3_CHECK_ARG(k_lo % 16 == 0 && k_hi % 16 == 0 && k_lo >= 0 && k_lo < k_hi && k_hi <= d->cin &&
-                   k_lo < kBK && k_hi > d->cin - kBK, "k_lo / k_hi: multiples of 16 inside the first / last 64-channel block");
-    p.ks_first = k_lo / 16;
-    p.ks_end = (k_hi - (kblocks - 1) * kBK) / 16;
-    STP3_CHECK_ARG(kblocks > 1 || p.ks_first < p.ks_end, "empty K range");
-  }
-  p.a_plane_bytes = box_h * kTileW * kBK * 2; p.w_rows = d->bn; p.n_mma = n_mma;
-  for (int i = 0; i < d->ntaps; ++i) { p.tap[i][0] = d->taps[i][0]; p.tap[i][1] = d->taps[i][1]; p.tap[i][2] = d->taps[i][2]; p.tap[i][3] = 0; }
+  p.bias = bias; p.img_bias = img_bias; p.img_bias_stride = d->bn;
   p.relu = d->relu; p.res_mode = d->res_mode;
   p.swish = d->swish; p.w_img_rows = d->w_img_stride / 64;
   p.res_hi = static_cast<const __nv_bfloat16*>(res_hi); p.res_lo = static_cast<const __nv_bfloat16*>(res_lo);
-  p.res_cstride = d->res_cstride;
+  p.res_cstride = d->res_cstride; p.res_coff = d->res_coff;
   p.out_hi = static_cast<__nv_bfloat16*>(y_hi); p.out_lo = static_cast<__nv_bfloat16*>(y_lo);
-  p.out_cstride = d->out_cstride;
+  p.out_cstride = d->out_cstride; p.out_coff = d->out_coff; p.n_store = n_store;
   p.out2_hi = static_cast<__nv_bfloat16*>(d->y2_hi); p.out2_lo = static_cast<__nv_bfloat16*>(d->y2_lo);
   p.out2_cstride = d->out2_cstride; p.out2_coff = d->out2_coff; p.relu2 = d->relu2;
   p.n_store2 = d->n_store2 > 0 ? d->n_store2 : 64;
@@ -796,24 +855,15 @@ extern "C" int stp3_conv_fwd(const stp3_conv_desc* d, const void* x_hi, const vo
   }
   p.out_f32 = y_f32; p.n_valid = d->n_valid; p.sigmoid = d->sigmoid;
   p.f32_nhwc = d->f32_layout;
-  STP3_CHECK_ARG(d->f32_layout == 0 || d->f32_layout == 1, "f32_layout must be 0 (n_img, n_valid, Ho, Wo) or 1 (n_img, Ho, Wo, n_valid)");
   if (y_f32 && d->f32_layout == 1)
     STP3_CHECK_ARG((reinterpret_cast<uintptr_t>(y_f32) & 31) == 0 && !d->sigmoid,
                    "channels-last y_f32 must be 32-byte aligned (and carries no sigmoid)");
-  p.img_bias_stride = d->bn;
   p.head_ko = 0; p.head_w = nullptr; p.head_b = nullptr; p.head_sigmoid_mask = 0;
   for (int k = 0; k < kMaxHeadOut; ++k) { p.head_out[k] = nullptr; p.head_img_stride[k] = 0; }
   if (head) {
     p.head_ko = head->n_out; p.head_w = head->w; p.head_b = head->b; p.head_sigmoid_mask = head->sigmoid_mask;
     for (int k = 0; k < head->n_out; ++k) { p.head_out[k] = head->out[k]; p.head_img_stride[k] = head->img_stride[k]; }
   }
-  const int k_iters = d->ntaps * kblocks;
-  const bool full_k = p.ks_first == 0 && p.ks_end == kBK / 16;
-  const long long nblk = (long long)p.n_img * p.tiles_x * p.tiles_y;
-  STP3_CHECK_ARG(nblk > 0 && nblk < (1ll << 31), "grid too large");
-  p.n_tiles = (int)nblk;
-  const int n_sm = num_sms();
-  const unsigned grid = (unsigned)(nblk < n_sm ? nblk : n_sm);           // persistent: one CTA per SM
   p.sum_part = nullptr;
   if (d->col_sums) {
     STP3_CHECK_ARG(d->bn == 64, "col_sums: 64-column convolutions only");
@@ -821,38 +871,28 @@ extern "C" int stp3_conv_fwd(const stp3_conv_desc* d, const void* x_hi, const vo
                    "col_sums: scratch buffer missing or smaller than stp3_conv_col_sums_scratch_bytes()");
     p.sum_part = static_cast<float*>(d->col_sums_scratch);
     // CTAs that never see an image leave its partial rows untouched: start from zeros
-    STP3_CUDA_OK(cudaMemsetAsync(p.sum_part, 0, (size_t)grid * 4 * p.n_img * 64 * sizeof(float), stream));
+    STP3_CUDA_OK(cudaMemsetAsync(p.sum_part, 0, (size_t)t.grid * 4 * p.n_img * 64 * sizeof(float), stream));
   }
-
-  for (int part = 0; part * bn_launch < d->bn; ++part) {
-    const int coff = part * bn_launch;
-    p.w_row_off = coff;
-    p.bias = bias + coff;
-    p.img_bias = img_bias ? img_bias + coff : nullptr;
-    p.res_coff = d->res_coff + coff;
-    p.out_coff = d->out_coff + coff;
-    p.n_store = n_store - coff < bn_launch ? (n_store - coff > 0 ? n_store - coff : 0) : bn_launch;
-    p.f32_coff = coff;
-    auto al32 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 31) == 0; };
-    p.vec256 = (y_hi && d->out_cstride % 16 == 0 && p.out_coff % 16 == 0 && al32(y_hi) && al32(y_lo) ? 1 : 0) |
-               (d->res_mode && d->res_cstride % 16 == 0 && p.res_coff % 16 == 0 && al32(res_hi) && al32(res_lo) ? 2 : 0) |
-               (d->y2_hi && d->out2_cstride % 16 == 0 && d->out2_coff % 16 == 0 && al32(d->y2_hi) && al32(d->y2_lo) ? 4 : 0);
-    int rc;
-    if (bn_launch == 64 && stack)
-      rc = full_k ? launch_conv<64, true, true>(p, tm_hi, tm_lo, tm_w, n_mma, k_iters, stream_weights, grid, stream)
-                  : launch_conv<64, true, false>(p, tm_hi, tm_lo, tm_w, n_mma, k_iters, stream_weights, grid, stream);
-    else if (bn_launch == 64)
-      rc = full_k ? launch_conv<64, false, true>(p, tm_hi, tm_lo, tm_w, n_mma, k_iters, stream_weights, grid, stream)
-                  : launch_conv<64, false, false>(p, tm_hi, tm_lo, tm_w, n_mma, k_iters, stream_weights, grid, stream);
-    else
-      rc = full_k ? launch_conv<128, false, true>(p, tm_hi, tm_lo, tm_w, n_mma, k_iters, stream_weights, grid, stream)
-                  : launch_conv<128, false, false>(p, tm_hi, tm_lo, tm_w, n_mma, k_iters, stream_weights, grid, stream);
-    if (rc) return rc;
-    STP3_CUDA_OK(cudaGetLastError());
-  }
+  // every column block starts a multiple of 64 channels further: one alignment answer for all of them
+  auto al32 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 31) == 0; };
+  p.vec256 = (y_hi && d->out_cstride % 16 == 0 && d->out_coff % 16 == 0 && al32(y_hi) && al32(y_lo) ? 1 : 0) |
+             (d->res_mode && d->res_cstride % 16 == 0 && d->res_coff % 16 == 0 && al32(res_hi) && al32(res_lo) ? 2 : 0) |
+             (d->y2_hi && d->out2_cstride % 16 == 0 && d->out2_coff % 16 == 0 && al32(d->y2_hi) && al32(d->y2_lo) ? 4 : 0);
+  int rc;
+  if (t.bn_blk == 64 && t.stack)
+    rc = t.full_k ? launch_conv<64, true, true>(p, tm_hi, tm_lo, tm_w, t.smem_bytes, t.grid, stream)
+                  : launch_conv<64, true, false>(p, tm_hi, tm_lo, tm_w, t.smem_bytes, t.grid, stream);
+  else if (t.bn_blk == 64)
+    rc = t.full_k ? launch_conv<64, false, true>(p, tm_hi, tm_lo, tm_w, t.smem_bytes, t.grid, stream)
+                  : launch_conv<64, false, false>(p, tm_hi, tm_lo, tm_w, t.smem_bytes, t.grid, stream);
+  else
+    rc = t.full_k ? launch_conv<128, false, true>(p, tm_hi, tm_lo, tm_w, t.smem_bytes, t.grid, stream)
+                  : launch_conv<128, false, false>(p, tm_hi, tm_lo, tm_w, t.smem_bytes, t.grid, stream);
+  if (rc) return rc;
+  STP3_CUDA_OK(cudaGetLastError());
   if (p.sum_part) {
     STP3_CUDA_OK(launch_pdl(kPdlAux, col_sum_reduce_kernel, dim3(p.n_img), dim3(64, 16), 0, stream,
-                            (const float*)p.sum_part, (int)grid * 4, p.n_img, 64, static_cast<float*>(d->col_sums)));
+                            (const float*)p.sum_part, (int)t.grid * 4, p.n_img, 64, static_cast<float*>(d->col_sums)));
   }
   return STP3_OK;
 }

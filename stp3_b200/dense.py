@@ -139,10 +139,11 @@ def pack_conv(weight: torch.Tensor, bias: torch.Tensor, *, stride: int = 1, dila
 
 # ------------------------------------------------------------------------------------------------ autotuner
 # The conv kernel has tiling knobs (sharing one activation load between the dy taps of a 3x3, streaming the weights
-# through the ring instead of keeping them resident, the stacked hi/lo weight operand).  Which combination wins depends
-# on the layer (K depth, N width, image size, whether the weights are smem-resident), so the first eager call of every
-# (layer, shape) times the candidates back to back and the winner is cached; CUDA-graph capture then records the tuned
-# launches.  STP3_CONV_AUTOTUNE=0 disables it (kernel heuristics).
+# through the ring instead of keeping them resident, the stacked hi/lo weight operand, 64-column blocks for layers of
+# 128 / 256 columns).  Which combination wins depends on the layer (K depth, N width, image size, whether the weights
+# are smem-resident), so the first eager call of every (layer, shape) times the candidates back to back and the winner
+# is cached; CUDA-graph capture then records the tuned launches.  STP3_CONV_AUTOTUNE=0 disables it (kernel heuristics,
+# and untuned_blocks() for the column blocks).
 import os as _os
 
 _TUNED = {}
@@ -150,9 +151,13 @@ _AUTOTUNE = _os.environ.get("STP3_CONV_AUTOTUNE", "1") != "0"
 TUNE_LOG = []      # (description, {config: ms}) for reports
 
 
+BLOCKS64 = 16      # bit of a tiling's group: 64-column blocks (stp3_conv_desc.tune_bn = 64)
+
+
 def tune_candidates(pc: PackedConv, per_image: bool = False) -> List[Tuple[int, int]]:
     """The (n_sub, group) tilings the autotuner times for this packed convolution.  Per-image weights are never
-    resident: only the streamed (+4) tilings are offered for them."""
+    resident: only the streamed (+4) tilings are offered for them.  Convolutions of 128 / 256 columns are also offered
+    in 64-column blocks (+16), plain and with the stacked operand (+8); their weights stream either way."""
     taps = pc.taps
     groupable = any(taps[i + 1][0] == taps[i][0] and taps[i + 1][2] == taps[i][2] and
                     taps[i + 1][1] == taps[i][1] + pc.stride for i in range(len(taps) - 1))
@@ -163,7 +168,15 @@ def tune_candidates(pc: PackedConv, per_image: bool = False) -> List[Tuple[int, 
         cands += [(ns, g + 4) for ns, g in cands]
     if pc.bn == 64:     # stacked [W_hi; W_lo] operand: two MMAs per product instead of three
         cands += [(ns, g + 8) for ns, g in cands]
+    else:
+        cands += [(1, g + (4 if per_image else 0) + BLOCKS64 + s) for s in (8, 0) for g in sorted({g & 3 for _, g in cands})]
     return cands
+
+
+def untuned_blocks(pc: PackedConv, tiles: int, n_sm: int) -> int:
+    """The group bits of the column blocks when nothing was timed: 64-column stacked blocks where 128-column items
+    would not fill two waves of the SMs, else the kernel's own choice."""
+    return BLOCKS64 + 8 if pc.bn >= 128 and tiles * (pc.bn // 128) < 2 * n_sm else 0
 
 
 def _tune(key, desc, launch, cands):
@@ -196,7 +209,8 @@ def conv(x: HL, pc: PackedConv, *, cin_off: int = 0, out: Optional[HL] = None, o
     relu2 -- two 64-column convolutions of the same input in one launch.
     col_sums (B*T, 64) fp32 (bn = 64 layers): receives the per-image sums over pixels of the activated output.
     tune = (n_sub, group) forces a tiling (n_sub is ignored: the tile is 8x16 pixels; group +4 = streamed weights,
-    +8 = stacked hi/lo weight operand) instead of the autotuned one.
+    +8 = stacked hi/lo weight operand, +16 = 64-column blocks) instead of the autotuned one.  A fused head and a
+    second destination need all columns in one block: +16 is dropped for them.
     swish: x * sigmoid(x) instead of ReLU.  w_img_stride > 0: pc.w holds image 0's weights and image i's start
     w_img_stride bf16 elements further (squeeze-excite gated projections, se_gate())."""
     B, T_total, H, W, cs = x.hi.shape
@@ -253,8 +267,11 @@ def conv(x: HL, pc: PackedConv, *, cin_off: int = 0, out: Optional[HL] = None, o
     dev = x.hi.device
     ptr = lambda t: t.data_ptr() if t is not None else None
 
+    one_block = hd is not None or out2 is not None
+
     def launch(n_sub=0, group=0):
-        d.tune_n_sub, d.tune_group = n_sub, group
+        d.tune_n_sub, d.tune_group = n_sub, group & ~BLOCKS64
+        d.tune_bn = 64 if group & BLOCKS64 and not one_block else 0
         with torch.cuda.device(dev):
             code = _lib.lib().stp3_conv_fwd(
                 ctypes.byref(d), x.hi.data_ptr(), x.lo.data_ptr(), pc.w.data_ptr(), pc.bias.data_ptr(), ptr(img_bias),
@@ -272,7 +289,12 @@ def conv(x: HL, pc: PackedConv, *, cin_off: int = 0, out: Optional[HL] = None, o
         ins = {x.hi.data_ptr(), x.lo.data_ptr()} | ({residual.hi.data_ptr(), residual.lo.data_ptr()} if residual is not None else set())
         outs = {t.data_ptr() for t in ((out.hi, out.lo) if out is not None else ()) + ((out2.hi, out2.lo) if out2 is not None else ())}
         assert not (ins & outs), "stp3_b200.dense.conv: output aliases an input (in-place convolution is not supported)"
-        cfg = _tune(key, desc, launch, tune_candidates(pc, per_image=w_img_stride > 0))
+        cfg = _tune(key, desc, launch, [c for c in tune_candidates(pc, per_image=w_img_stride > 0)
+                                        if not (one_block and c[1] & BLOCKS64)])
+    elif cfg is None and not _AUTOTUNE and not one_block and pc.bn >= 128:
+        tiles = B * T * -(-Ho // 8) * -(-Wo // 16)
+        cfg = _TUNED[key] = (0, untuned_blocks(pc, tiles, torch.cuda.get_device_properties(dev).multi_processor_count))
+        TUNE_LOG.append((f"{len(pc.taps)}tap cin{pc.cin_p} bn{pc.bn} s{pc.stride} {B * T}x{Ho}x{Wo}", {cfg: float("nan")}))
     launch(*(cfg or (0, 0)))
     return out
 

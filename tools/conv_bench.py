@@ -5,12 +5,16 @@ with L2 flushed before every repetition.  Per layer: taps x Cin -> Cout, output 
 tensor-bound fraction (3 bf16 products per MAC at the data-sheet rate, scaled to the SM clock sampled during the
 timed loop).
 
-    python tools/conv_bench.py [--heads] [--reps 100] [--save DIR | --compare DIR] [--lib PATH]
+    python tools/conv_bench.py [--heads] [--reps 100] [--blocks 128|64s|64p] [--save DIR | --compare DIR] [--lib PATH]
+    python tools/conv_bench.py --count-only [--sms 132]     # host counts of the decoder's 25x25 / 50x50 layers, no GPU
 
 --save DIR writes the tilings and a SHA-256 digest of every output of every call (hi / lo planes, second destination,
 fp32 outputs, fused-head planes, column sums, each snapshotted right after its call); --compare DIR runs under the
 tilings another build saved there and reports which outputs are not bitwise identical.  --lib loads another build of
-libstp3_b200.so, so that two builds can be timed alternately on the same card.  One JSON line.
+libstp3_b200.so, so that two builds can be timed alternately on the same card.  --blocks replaces the tuner's
+column-block choice for every convolution of 128 / 256 columns that may run in blocks (128-column blocks, 64-column
+stacked, 64-column plain), so each width is timed alone.  --count-only prints, for the decoder trunk's low-resolution
+layers under each block width, what stp3_conv_tiling answers: work items, waves over the SMs, ring depths.  One JSON line.
 """
 import argparse
 import hashlib
@@ -26,6 +30,38 @@ sys.path.insert(0, os.path.join(ROOT, "tools"))
 from head_bench import FLOP_PER_CLK_SM, ClockSampler, gpu_info  # noqa: E402
 
 BATCH = 4
+BLOCKS = {"128": 0, "64s": 16 + 8, "64p": 16}        # group bits of dense.conv's tune
+# (taps, cin, cout, stride, input map, output map) of the decoder trunk's calls on the 25 x 25 and 50 x 50 maps of one
+# perceive step (ResNet-18 layer2 / layer3 and the 1x1 of the two upsampling stages), B * T = 12 images
+LOW_RES_LAYERS = [(9, 128, 256, 2, 50, 25), (1, 128, 256, 2, 50, 25)] + [(9, 256, 256, 1, 25, 25)] * 3 + \
+                 [(1, 256, 128, 1, 25, 25), (9, 64, 128, 2, 100, 50), (1, 64, 128, 2, 100, 50)] + \
+                 [(9, 128, 128, 1, 50, 50)] * 3 + [(1, 128, 64, 1, 50, 50)]
+
+
+def count_layers(n_sm, n_img=3 * BATCH):
+    """stp3_conv_tiling of every LOW_RES_LAYERS entry under each column-block width (host arithmetic only)."""
+    import ctypes
+    import torch
+    from stp3_b200 import _lib, dense
+    rows = []
+    for taps, cin, cout, stride, hw_in, hw_out in LOW_RES_LAYERS:
+        k = 3 if taps == 9 else 1
+        pc = dense.pack_conv(torch.zeros(cout, cin, k, k), torch.zeros(cout), stride=stride)
+        d = _lib.ConvDesc(B=n_img, T=1, H=hw_in, W=hw_in, in_cstride=cin, cin=cin, Ho=hw_out, Wo=hw_out, stride=stride,
+                          ntaps=taps, bn=pc.bn)
+        for i, t in enumerate(pc.taps):
+            d.taps[i][0], d.taps[i][1], d.taps[i][2] = t
+        row = {"layer": f"{taps}x{cin}->{cout}" + (f" s{stride}" if stride > 1 else ""), "map": f"{n_img}x{hw_out}x{hw_out}"}
+        for name, bits in BLOCKS.items():
+            if pc.bn < 128 and name != "128":
+                continue
+            d.tune_group, d.tune_bn = bits & 15, 64 if bits & dense.BLOCKS64 else 0
+            info = _lib.ConvTilingInfo()
+            _lib.check(_lib.lib().stp3_conv_tiling(ctypes.byref(d), n_sm, ctypes.byref(info)), "stp3_conv_tiling")
+            row[name] = {"items": info.items, "waves": round(info.items / n_sm, 2), "a_stages": info.a_stages,
+                         "b_stages": info.b_stages, "resident": bool(info.resident)}
+        rows.append(row)
+    return rows
 
 
 def outputs_of(a, k, ret):
@@ -82,7 +118,7 @@ def record_step(model, dev, heads, tilings):
     seen = []
 
     def fwd_rec(d, *rest):
-        seen.append(d._obj.tune_group)
+        seen.append(d._obj.tune_group | (dense.BLOCKS64 if d._obj.tune_bn == 64 else 0))
         return fwd(d, *rest)
 
     calls = []
@@ -156,7 +192,13 @@ def main():
     ap.add_argument("--save", metavar="DIR", help="write the tilings and output digests of every call")
     ap.add_argument("--compare", metavar="DIR", help="run under the tilings saved in DIR and compare output digests")
     ap.add_argument("--lib", metavar="PATH", help="libstp3_b200.so to load instead of the package's own")
+    ap.add_argument("--blocks", choices=list(BLOCKS), help="column blocks of every 128 / 256-column convolution")
+    ap.add_argument("--count-only", action="store_true", help="host counts of the low-resolution decoder layers")
+    ap.add_argument("--sms", type=int, default=132, help="SM count for --count-only")
     args = ap.parse_args()
+    if args.count_only:
+        print(json.dumps({"sms": args.sms, "layers": count_layers(args.sms)}))
+        return
     import torch
     from stp3_b200 import _lib
     if args.lib:
@@ -171,6 +213,11 @@ def main():
         assert ref["heads"] == args.heads, "--compare needs the --heads setting of the saved run"
     model = bench.build_model(dev)
     calls = record_step(model, dev, args.heads, [c["tiling"] for c in ref["calls"]] if ref else None)
+    if args.blocks:      # the tuned tap sharing of every call, the column blocks as asked
+        def in_blocks(a, k):
+            return a[1].bn >= 128 and k.get("head") is None and k.get("out2") is None
+        calls = record_step(model, dev, args.heads, [(t & 3) | BLOCKS[args.blocks] if in_blocks(a, k) else t
+                                                     for a, k, t, _ in calls])
     us, mhz = time_calls(calls, args.reps, dev)
     n_sm = torch.cuda.get_device_properties(0).multi_processor_count
     rows, saved = [], []
