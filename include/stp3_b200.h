@@ -153,6 +153,14 @@ size_t stp3_lift_splat_bwd_scratch_bytes(const stp3_lift_splat_desc* desc);
 int stp3_lift_splat_bwd(const stp3_lift_splat_desc* desc, const float* grad_out, const float* feat,
                         const float* depth_logits, void* scratch, size_t scratch_bytes, float* grad_feat,
                         float* grad_depth_logits, void* stream);
+/* stp3_lift_splat_bwd for channels-last context features, the layout the encoder heads hand to stp3_lift_splat_fwd
+ * (desc->feat_layout 1, required): feat and grad_feat are (B,S,N,Hf,Wf,C), 8-byte aligned, C even; depth_logits and
+ * grad_depth_logits stay (B,S,N,D,Hf,Wf).  Same descriptor rules, scratch query and kernels; only the addresses of feat
+ * and grad_feat differ (a lane's channel pair is one float2 of a pixel's row), and every sum keeps its order: the
+ * results equal stp3_lift_splat_bwd's on the transposed tensors bit for bit. */
+int stp3_lift_splat_bwd_cl(const stp3_lift_splat_desc* desc, const float* grad_out, const float* feat,
+                           const float* depth_logits, void* scratch, size_t scratch_bytes, float* grad_feat,
+                           float* grad_depth_logits, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------
  * Dense layers: implicit-GEMM convolution on the Hopper tensor cores (wgmma, register accumulators, TMA-fed operands).
@@ -430,6 +438,17 @@ int stp3_bn_bwd_apply(const float* g, int g_cstride, const float* y, int y_cstri
  * its adjoint (a gather over the outputs each input feeds; no atomics) */
 int stp3_upsample2x_f32(const float* x, int n_img, int h, int w, int C, float* y, void* stream);
 int stp3_upsample2x_bwd(const float* gy, int n_img, int h, int w, int C, float* gx, void* stream);
+/* The same pair on a channel window of a wider channels-last tensor (the concat tensor of UpsamplingConcat in train
+ * mode, convolutions.py:183-201: the upsampled coarse map sits behind the fine map, and its gradient is read from there):
+ *   forward: x dense (n_img, h, w, C) -> channels [y_coff, y_coff + C) of y (n_img, 2h, 2w, y_cstride); the other
+ *            channels of y are not touched
+ *   adjoint: channels [gy_coff, gy_coff + C) of gy (n_img, 2h, 2w, gy_cstride) -> gx dense (n_img, h, w, C)
+ * 16-byte accesses when C, the row stride and the offset are multiples of 4 and both pointers are 16-byte aligned, one
+ * float per thread otherwise: the same values.  With the stride C and offset 0 these are the two functions above. */
+int stp3_upsample2x_window_f32(const float* x, int n_img, int h, int w, int C, float* y, int y_cstride, int y_coff,
+                               void* stream);
+int stp3_upsample2x_window_bwd(const float* gy, int gy_cstride, int gy_coff, int n_img, int h, int w, int C, float* gx,
+                               void* stream);
 /* out (n_img, H, W, C)[y][x] = p_{y%2 x%2}[y/2][x/2], phase p_ab of size (n_img, (H-a+1)/2, (W-b+1)/2, C) or NULL = 0:
  * the four phases of a stride-2 convolution's input gradient */
 int stp3_phase_interleave(const float* p00, const float* p01, const float* p10, const float* p11, int n_img, int H, int W,

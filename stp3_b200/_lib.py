@@ -106,6 +106,7 @@ SIGNATURES = {
     "stp3_aspp_fused_fwd": (_I, [ctypes.POINTER(AsppDesc), _V, _V, _V, _V, _V, _V, _V, _V]),
     "stp3_lift_splat_bwd_scratch_bytes": (_SZ, [_LSD]),
     "stp3_lift_splat_bwd": (_I, [_LSD, _V, _V, _V, _V, _SZ, _V, _V, _V]),
+    "stp3_lift_splat_bwd_cl": (_I, [_LSD, _V, _V, _V, _V, _SZ, _V, _V, _V]),
     "stp3_bev_discount": (_I, [_V, _I, _I, _I, _I, _I, _F, _V, _V, _V]),
     "stp3_conv_fwd": (_I, [ctypes.POINTER(ConvDesc), _V, _V, _V, _V, _V, _V, _V, _V, _V, _V, ctypes.POINTER(ConvHead), _V]),
     "stp3_lift_splat_fwd": (_I, [_LSD, _V, _V, _V, _V, _V, _SZ, _V, _I, _I, ctypes.POINTER(_V), _V]),
@@ -122,6 +123,8 @@ SIGNATURES = {
     "stp3_bn_bwd_apply": (_I, [_V, _I, _V, _I, _V, _I, _V, _V, _V, _V, _V, _LL, _I, _V, _I, _V, _I, _V]),
     "stp3_upsample2x_f32": (_I, [_V, _I, _I, _I, _I, _V, _V]),
     "stp3_upsample2x_bwd": (_I, [_V, _I, _I, _I, _I, _V, _V]),
+    "stp3_upsample2x_window_f32": (_I, [_V, _I, _I, _I, _I, _V, _I, _I, _V]),
+    "stp3_upsample2x_window_bwd": (_I, [_V, _I, _I, _I, _I, _I, _I, _V, _V]),
     "stp3_phase_interleave": (_I, [_V, _V, _V, _V, _I, _I, _I, _I, _V, _V]),
     "stp3_sigmoid_bwd": (_I, [_V, _V, _LL, _V, _V]),
     # train mode of the TemporalBlocks

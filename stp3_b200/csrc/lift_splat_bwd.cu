@@ -10,6 +10,9 @@
 //   K1  bev_grad_to_grid_kernel : g_grid[b,t',pillar,c] = sum_{t >= t'} discount^(t-t') * g_out[b,t,c,pillar]
 //         (channels-last, so that a point's gradient row is one contiguous 4*C-byte gather)
 //   K2  lift_splat_bwd_kernel   : one CTA per (b, t, camera, 4 image columns), one warp per column, lanes = channel pairs
+//         (one body for both feature layouts: NCHW, and channels-last -- what the encoder heads produce -- where a
+//          lane's channel pair is one float2 of a pixel's contiguous row; only the addresses of feat / g_feat differ,
+//          every sum keeps its order, so the two instantiations agree bit for bit)
 //         g_feat[c,h,w]  = sum_d prob[d,h,w] * g_grid[rank(d,h,w), c]
 //         g_prob[d,h,w]  = sum_c feat[c,h,w] * g_grid[rank(d,h,w), c]      (halving butterfly over the lanes)
 //         g_logit[d,h,w] = prob[d,h,w] * (g_prob[d,h,w] - sum_d' prob[d',h,w] * g_prob[d',h,w])
@@ -28,7 +31,7 @@ constexpr int kBwdC = 64;            // channels per pass (2 per lane)
 constexpr int kBwdMaxFrames = 8;
 
 struct LiftBwdParams {
-  const float* feat;      // (B,S,N,C,Hf,Wf)
+  const float* feat;      // (B,S,N,C,Hf,Wf), channels-last instantiation: (B,S,N,Hf,Wf,C)
   const float* depth;     // (B,S,N,D,Hf,Wf) or null
   const float* cam_M; const float* cam_t; const float* ego_R; const float* ego_t;
   const float* xs; const float* ys; const float* ds;
@@ -37,7 +40,7 @@ struct LiftBwdParams {
   int use_depth;
   int tiles_w;
   const float* ggrid;     // (B,S,nvox,C)
-  float* gfeat;           // (B,S,N,C,Hf,Wf)
+  float* gfeat;           // same layout as feat
   float* gdepth;          // (B,S,N,D,Hf,Wf) or null
 };
 
@@ -66,6 +69,7 @@ bev_grad_to_grid_kernel(const float* __restrict__ gout, float* __restrict__ ggri
   }
 }
 
+template <bool kChannelsLast>
 __global__ void __launch_bounds__(32 * kBwdTW, 2)
 lift_splat_bwd_kernel(const LiftBwdParams p) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -143,12 +147,24 @@ lift_splat_bwd_kernel(const LiftBwdParams p) {
   const int wl = warp, w = w0 + wl;
   for (int c0 = 0; c0 < C; c0 += kBwdC) {
     __syncthreads();
-    for (int i = tid; i < kBwdC * npix; i += nthr) {                // context features of channels [c0, c0+64) of the tile
-      const int cl = i / npix, px = i % npix;
-      const int ww = w0 + px % TW, hh = px / TW;
-      float v = 0.f;
-      if (ww < Wf && c0 + cl < C) v = __ldg(p.feat + (((size_t)img * C + c0 + cl) * Hf + hh) * Wf + ww);
-      s_feat[(((cl & 1) << 5) | (cl >> 1)) * fstride + px] = v;     // channels (2l, 2l+1) in rows l and l + 32
+    if constexpr (kChannelsLast) {                                  // a warp reads one pixel's 64 channels: 256 contiguous bytes
+      for (int i = tid; i < (kBwdC / 2) * npix; i += nthr) {
+        const int l = i & 31, px = i >> 5;
+        const int ww = w0 + px % TW, hh = px / TW;
+        float2 v = make_float2(0.f, 0.f);
+        if (ww < Wf && c0 + 2 * l < C)                              // C is even: the pair is inside together
+          v = __ldg(reinterpret_cast<const float2*>(p.feat + (((size_t)img * Hf + hh) * Wf + ww) * C + c0 + 2 * l));
+        s_feat[l * fstride + px] = v.x;
+        s_feat[(l + 32) * fstride + px] = v.y;
+      }
+    } else {
+      for (int i = tid; i < kBwdC * npix; i += nthr) {              // context features of channels [c0, c0+64) of the tile
+        const int cl = i / npix, px = i % npix;
+        const int ww = w0 + px % TW, hh = px / TW;
+        float v = 0.f;
+        if (ww < Wf && c0 + cl < C) v = __ldg(p.feat + (((size_t)img * C + c0 + cl) * Hf + hh) * Wf + ww);
+        s_feat[(((cl & 1) << 5) | (cl >> 1)) * fstride + px] = v;   // channels (2l, 2l+1) in rows l and l + 32
+      }
     }
     __syncthreads();
     if (w >= Wf) continue;
@@ -217,8 +233,12 @@ lift_splat_bwd_kernel(const LiftBwdParams p) {
       for (int j = 0; j < kBwdH; ++j) {
         const int h = h0 + j;
         if (h < Hf && c < C) {
-          p.gfeat[(((size_t)img * C + c) * Hf + h) * Wf + w] = a0[j];
-          if (c + 1 < C) p.gfeat[(((size_t)img * C + c + 1) * Hf + h) * Wf + w] = a1[j];
+          if constexpr (kChannelsLast) {
+            *reinterpret_cast<float2*>(p.gfeat + (((size_t)img * Hf + h) * Wf + w) * C + c) = make_float2(a0[j], a1[j]);
+          } else {
+            p.gfeat[(((size_t)img * C + c) * Hf + h) * Wf + w] = a0[j];
+            if (c + 1 < C) p.gfeat[(((size_t)img * C + c + 1) * Hf + h) * Wf + w] = a1[j];
+          }
         }
       }
     }
@@ -250,15 +270,12 @@ extern "C" size_t stp3_lift_splat_bwd_scratch_bytes(const stp3_lift_splat_desc* 
   return (size_t)d->B * d->S * d->nx * d->ny * d->C * sizeof(float);
 }
 
-extern "C" int stp3_lift_splat_bwd(const stp3_lift_splat_desc* desc, const float* grad_out, const float* feat,
-                                   const float* depth_logits, void* scratch, size_t scratch_bytes, float* grad_feat,
-                                   float* grad_depth_logits, void* stream_) {
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  LiftBwdParams p;
-  if (const int rc = check_lift_splat_desc("stp3_lift_splat_bwd", desc, feat, depth_logits, kBwdMaxFrames, p.q)) return rc;
-  STP3_CHECK_ARG(grad_out && scratch && grad_feat, "stp3_lift_splat_bwd: null pointer argument");
-  STP3_CHECK_ARG(desc->feat_layout == 0, "stp3_lift_splat_bwd: feat must be NCHW (feat_layout 0)");
-  STP3_CHECK_ARG(desc->f_count == 0, "stp3_lift_splat_bwd: every frame is processed (f_count 0)");
+// Both entry points: the checks they share, K1, then K2 instantiated for the layout.  `fn` names the caller in messages.
+template <bool kChannelsLast>
+static int lift_splat_bwd_launch(const char* fn, const stp3_lift_splat_desc* desc, const float* grad_out, const float* feat,
+                                 const float* depth_logits, void* scratch, size_t scratch_bytes, float* grad_feat,
+                                 float* grad_depth_logits, cudaStream_t stream, LiftBwdParams& p) {
+  STP3_CHECK_ARG(desc->f_count == 0, "%s: every frame is processed (f_count 0)", fn);
   const int B = desc->B, S = desc->S, N = desc->N, D = desc->D, Hf = desc->Hf, Wf = desc->Wf, C = desc->C;
   const size_t need = stp3_lift_splat_bwd_scratch_bytes(desc);
   if (scratch_bytes < need) return set_error(STP3_ENOSPC, "scratch too small: %zu < %zu", scratch_bytes, need);
@@ -283,8 +300,34 @@ extern "C" int stp3_lift_splat_bwd(const stp3_lift_splat_desc* desc, const float
   p.tiles_w = tiles_w;
   p.ggrid = static_cast<const float*>(scratch);
   p.gfeat = grad_feat; p.gdepth = grad_depth_logits;
-  STP3_CUDA_OK(cudaFuncSetAttribute(lift_splat_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  lift_splat_bwd_kernel<<<(unsigned)nblk, 32 * kBwdTW, smem, stream>>>(p);
+  STP3_CUDA_OK(cudaFuncSetAttribute(lift_splat_bwd_kernel<kChannelsLast>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                    (int)smem));
+  lift_splat_bwd_kernel<kChannelsLast><<<(unsigned)nblk, 32 * kBwdTW, smem, stream>>>(p);
   STP3_CUDA_OK(cudaGetLastError());
   return STP3_OK;
+}
+
+extern "C" int stp3_lift_splat_bwd(const stp3_lift_splat_desc* desc, const float* grad_out, const float* feat,
+                                   const float* depth_logits, void* scratch, size_t scratch_bytes, float* grad_feat,
+                                   float* grad_depth_logits, void* stream_) {
+  LiftBwdParams p;
+  if (const int rc = check_lift_splat_desc("stp3_lift_splat_bwd", desc, feat, depth_logits, kBwdMaxFrames, p.q)) return rc;
+  STP3_CHECK_ARG(grad_out && scratch && grad_feat, "stp3_lift_splat_bwd: null pointer argument");
+  STP3_CHECK_ARG(desc->feat_layout == 0, "stp3_lift_splat_bwd: feat must be NCHW (feat_layout 0)");
+  return lift_splat_bwd_launch<false>("stp3_lift_splat_bwd", desc, grad_out, feat, depth_logits, scratch, scratch_bytes,
+                                      grad_feat, grad_depth_logits, reinterpret_cast<cudaStream_t>(stream_), p);
+}
+
+extern "C" int stp3_lift_splat_bwd_cl(const stp3_lift_splat_desc* desc, const float* grad_out, const float* feat,
+                                      const float* depth_logits, void* scratch, size_t scratch_bytes, float* grad_feat,
+                                      float* grad_depth_logits, void* stream_) {
+  LiftBwdParams p;
+  if (const int rc = check_lift_splat_desc("stp3_lift_splat_bwd_cl", desc, feat, depth_logits, kBwdMaxFrames, p.q)) return rc;
+  STP3_CHECK_ARG(grad_out && scratch && grad_feat, "stp3_lift_splat_bwd_cl: null pointer argument");
+  STP3_CHECK_ARG(desc->feat_layout == 1, "stp3_lift_splat_bwd_cl: feat must be channels-last (feat_layout 1)");
+  STP3_CHECK_ARG(desc->C % 2 == 0 && reinterpret_cast<uintptr_t>(feat) % 8 == 0 &&
+                     reinterpret_cast<uintptr_t>(grad_feat) % 8 == 0,
+                 "stp3_lift_splat_bwd_cl: C must be even and feat / grad_feat 8-byte aligned (float2 accesses)");
+  return lift_splat_bwd_launch<true>("stp3_lift_splat_bwd_cl", desc, grad_out, feat, depth_logits, scratch,
+                                     scratch_bytes, grad_feat, grad_depth_logits, reinterpret_cast<cudaStream_t>(stream_), p);
 }

@@ -474,14 +474,35 @@ __device__ __forceinline__ void up_coord(int o, int n, int& i0, int& i1, float& 
   w0 = 1.f - w1;
 }
 
-// y (n_img, 2h, 2w, C) = bilinear_x2(x (n_img, h, w, C)); one thread per output element
+// V consecutive fp32 channels (V = 4: one 16-byte access; V = 1: any alignment)
+template <int V>
+__device__ __forceinline__ void ld_vec(const float* p, float (&v)[V]) {
+  if constexpr (V == 4) {
+    const float4 t = *reinterpret_cast<const float4*>(p);
+    v[0] = t.x; v[1] = t.y; v[2] = t.z; v[3] = t.w;
+  } else {
+    v[0] = *p;
+  }
+}
+template <int V>
+__device__ __forceinline__ void st_vec(float* p, const float (&v)[V]) {
+  if constexpr (V == 4) *reinterpret_cast<float4*>(p) = make_float4(v[0], v[1], v[2], v[3]);
+  else *p = v[0];
+}
+
+// y[.., y_coff + c] = bilinear_x2(x (n_img, h, w, C))[.., c]: y has rows of y_cstride floats (a channel window of a wider
+// channels-last tensor, or y_cstride = C, y_coff = 0 for a dense one); one thread per V channels of an output pixel
+template <int V>
 __global__ void __launch_bounds__(256)
-upsample2x_f32_kernel(const float* __restrict__ x, int h, int w, int C, long long total, float* __restrict__ y) {
+upsample2x_f32_kernel(const float* __restrict__ x, int h, int w, int C, long long total, float* __restrict__ y,
+                      int y_cstride, int y_coff) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= total) return;
-  const int c = (int)(i % C);
-  long long r = i / C;
-  const int ox = (int)(r % (2 * w)); r /= 2 * w;
+  const int c = (int)(i % (C / V)) * V;
+  long long r = i / (C / V);
+  const int ox = (int)(r % (2 * w));
+  const long long orow = r;                         // output pixel index (img, oy, ox)
+  r /= 2 * w;
   const int oy = (int)(r % (2 * h));
   const long long img = r / (2 * h);
   int y0, y1, x0, x1;
@@ -489,9 +510,14 @@ upsample2x_f32_kernel(const float* __restrict__ x, int h, int w, int C, long lon
   up_coord(oy, h, y0, y1, wy0, wy1);
   up_coord(ox, w, x0, x1, wx0, wx1);
   const float* b = x + img * h * w * C + c;
-  const float v = wy0 * (wx0 * b[((long long)y0 * w + x0) * C] + wx1 * b[((long long)y0 * w + x1) * C]) +
-                  wy1 * (wx0 * b[((long long)y1 * w + x0) * C] + wx1 * b[((long long)y1 * w + x1) * C]);
-  y[i] = v;
+  float v00[V], v01[V], v10[V], v11[V], v[V];
+  ld_vec<V>(b + ((long long)y0 * w + x0) * C, v00);
+  ld_vec<V>(b + ((long long)y0 * w + x1) * C, v01);
+  ld_vec<V>(b + ((long long)y1 * w + x0) * C, v10);
+  ld_vec<V>(b + ((long long)y1 * w + x1) * C, v11);
+#pragma unroll
+  for (int k = 0; k < V; ++k) v[k] = wy0 * (wx0 * v00[k] + wx1 * v01[k]) + wy1 * (wx0 * v10[k] + wx1 * v11[k]);
+  st_vec<V>(y + orow * y_cstride + y_coff + c, v);
 }
 
 // weight of low-resolution index i in output o along one axis (both corners may coincide at the border)
@@ -502,32 +528,44 @@ __device__ __forceinline__ float up_weight(int o, int n, int i) {
   return (i0 == i ? w0 : 0.f) + (i1 == i ? w1 : 0.f);
 }
 
-// gx (n_img, h, w, C) = adjoint of bilinear_x2 applied to gy (n_img, 2h, 2w, C): a gather over the outputs 2i-1 .. 2i+2
-// of every axis (fixed order, no atomics)
+// gx (n_img, h, w, C) = adjoint of bilinear_x2 applied to channels [gy_coff, gy_coff + C) of gy (n_img, 2h, 2w,
+// gy_cstride): a gather over the outputs 2i-1 .. 2i+2 of every axis (fixed order, no atomics)
+template <int V>
 __global__ void __launch_bounds__(256)
-upsample2x_bwd_kernel(const float* __restrict__ gy, int h, int w, int C, long long total, float* __restrict__ gx) {
+upsample2x_bwd_kernel(const float* __restrict__ gy, int gy_cstride, int gy_coff, int h, int w, int C, long long total,
+                      float* __restrict__ gx) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= total) return;
-  const int c = (int)(i % C);
-  long long r = i / C;
+  const int c = (int)(i % (C / V)) * V;
+  long long r = i / (C / V);
   const int ix = (int)(r % w); r /= w;
   const int iy = (int)(r % h);
   const long long img = r / h;
-  const float* b = gy + img * 4 * h * w * C + c;
-  float acc = 0.f;
+  const float* b = gy + img * 4 * h * w * gy_cstride + gy_coff + c;
+  float acc[V];
+#pragma unroll
+  for (int k = 0; k < V; ++k) acc[k] = 0.f;
   for (int oy = 2 * iy - 1; oy <= 2 * iy + 2; ++oy) {
     if (oy < 0 || oy >= 2 * h) continue;
     const float wy = up_weight(oy, h, iy);
     if (wy == 0.f) continue;
-    float row = 0.f;
+    float row[V];
+#pragma unroll
+    for (int k = 0; k < V; ++k) row[k] = 0.f;
     for (int ox = 2 * ix - 1; ox <= 2 * ix + 2; ++ox) {
       if (ox < 0 || ox >= 2 * w) continue;
       const float wx = up_weight(ox, w, ix);
-      if (wx != 0.f) row = fmaf(wx, b[((long long)oy * 2 * w + ox) * C], row);
+      if (wx != 0.f) {
+        float g[V];
+        ld_vec<V>(b + ((long long)oy * 2 * w + ox) * gy_cstride, g);
+#pragma unroll
+        for (int k = 0; k < V; ++k) row[k] = fmaf(wx, g[k], row[k]);
+      }
     }
-    acc = fmaf(wy, row, acc);
+#pragma unroll
+    for (int k = 0; k < V; ++k) acc[k] = fmaf(wy, row[k], acc[k]);
   }
-  gx[i] = acc;
+  st_vec<V>(gx + i * V, acc);                       // gx is dense: thread i owns its elements [i * V, i * V + V)
 }
 
 // out (n_img, H, W, C)[y][x] = phase[y % 2][x % 2] (n_img, (H - y%2 + 1) / 2, (W - x%2 + 1) / 2, C)[y / 2][x / 2]
@@ -767,20 +805,52 @@ extern "C" int stp3_bn_bwd_apply(const float* g, int g_cstride, const float* y, 
   return STP3_OK;
 }
 
-extern "C" int stp3_upsample2x_f32(const float* x, int n_img, int h, int w, int C, float* y, void* stream) {
-  STP3_CHECK_ARG(x && y && n_img > 0 && h > 0 && w > 0 && C > 0, "stp3_upsample2x_f32: bad argument");
-  const long long total = (long long)n_img * 4 * h * w * C;
-  upsample2x_f32_kernel<<<blocks_for(total), 256, 0, (cudaStream_t)stream>>>(x, h, w, C, total, y);
+// 16-byte accesses when every row of the dense tensor and of the window starts 16-byte aligned; else one float per thread
+static bool upsample_vec(const void* dense, const void* win, int C, int cstride, int coff) {
+  return C % 4 == 0 && cstride % 4 == 0 && coff % 4 == 0 && reinterpret_cast<uintptr_t>(dense) % 16 == 0 &&
+         reinterpret_cast<uintptr_t>(win) % 16 == 0;
+}
+
+extern "C" int stp3_upsample2x_window_f32(const float* x, int n_img, int h, int w, int C, float* y, int y_cstride,
+                                          int y_coff, void* stream) {
+  STP3_CHECK_ARG(x && y && n_img > 0 && h > 0 && w > 0 && C > 0, "stp3_upsample2x_window_f32: bad argument");
+  STP3_CHECK_ARG(y_coff >= 0 && y_coff + C <= y_cstride,
+                 "stp3_upsample2x_window_f32: channels [%d, %d) outside rows of %d", y_coff, y_coff + C, y_cstride);
+  const long long pix = (long long)n_img * 4 * h * w;
+  if (upsample_vec(x, y, C, y_cstride, y_coff))
+    upsample2x_f32_kernel<4><<<blocks_for(pix * (C / 4)), 256, 0, (cudaStream_t)stream>>>(x, h, w, C, pix * (C / 4), y,
+                                                                                         y_cstride, y_coff);
+  else
+    upsample2x_f32_kernel<1><<<blocks_for(pix * C), 256, 0, (cudaStream_t)stream>>>(x, h, w, C, pix * C, y, y_cstride,
+                                                                                   y_coff);
   STP3_CUDA_OK(cudaGetLastError());
   return STP3_OK;
 }
 
-extern "C" int stp3_upsample2x_bwd(const float* gy, int n_img, int h, int w, int C, float* gx, void* stream) {
-  STP3_CHECK_ARG(gy && gx && n_img > 0 && h > 0 && w > 0 && C > 0, "stp3_upsample2x_bwd: bad argument");
-  const long long total = (long long)n_img * h * w * C;
-  upsample2x_bwd_kernel<<<blocks_for(total), 256, 0, (cudaStream_t)stream>>>(gy, h, w, C, total, gx);
+extern "C" int stp3_upsample2x_window_bwd(const float* gy, int gy_cstride, int gy_coff, int n_img, int h, int w, int C,
+                                          float* gx, void* stream) {
+  STP3_CHECK_ARG(gy && gx && n_img > 0 && h > 0 && w > 0 && C > 0, "stp3_upsample2x_window_bwd: bad argument");
+  STP3_CHECK_ARG(gy_coff >= 0 && gy_coff + C <= gy_cstride,
+                 "stp3_upsample2x_window_bwd: channels [%d, %d) outside rows of %d", gy_coff, gy_coff + C, gy_cstride);
+  const long long pix = (long long)n_img * h * w;
+  if (upsample_vec(gx, gy, C, gy_cstride, gy_coff))
+    upsample2x_bwd_kernel<4><<<blocks_for(pix * (C / 4)), 256, 0, (cudaStream_t)stream>>>(gy, gy_cstride, gy_coff, h, w,
+                                                                                         C, pix * (C / 4), gx);
+  else
+    upsample2x_bwd_kernel<1><<<blocks_for(pix * C), 256, 0, (cudaStream_t)stream>>>(gy, gy_cstride, gy_coff, h, w, C,
+                                                                                   pix * C, gx);
   STP3_CUDA_OK(cudaGetLastError());
   return STP3_OK;
+}
+
+extern "C" int stp3_upsample2x_f32(const float* x, int n_img, int h, int w, int C, float* y, void* stream) {
+  STP3_CHECK_ARG(x && y && n_img > 0 && h > 0 && w > 0 && C > 0, "stp3_upsample2x_f32: bad argument");
+  return stp3_upsample2x_window_f32(x, n_img, h, w, C, y, C, 0, stream);
+}
+
+extern "C" int stp3_upsample2x_bwd(const float* gy, int n_img, int h, int w, int C, float* gx, void* stream) {
+  STP3_CHECK_ARG(gy && gx && n_img > 0 && h > 0 && w > 0 && C > 0, "stp3_upsample2x_bwd: bad argument");
+  return stp3_upsample2x_window_bwd(gy, C, 0, n_img, h, w, C, gx, stream);
 }
 
 extern "C" int stp3_phase_interleave(const float* p00, const float* p01, const float* p10, const float* p11, int n_img,

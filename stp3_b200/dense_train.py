@@ -3,7 +3,7 @@ include/stp3_b200.h "Train mode"): convolution without folded BatchNorm (2-D, an
 BatchNorm with batch statistics (stats / apply with dropout / backward), the input gradient of a convolution on
 stp3_conv_fwd (transposed weights, mirrored taps, dilated too; stride 2 as four phase convolutions; anti-causal time
 taps for the 3-D ones), the weight gradient (2-D and causal 3-D), per-image channel sums, the temporal pair mean of
-the pyramid-pooling branch, and the bilinear x2 pair.
+the pyramid-pooling branch, and the bilinear x2 pair (dense, and on a channel window of a wider tensor).
 
 Tensors are fp32 channels-last (N, H, W, C) contiguous; the inputs of the tensor-core convolutions are the usual
 bf16 hi/lo planes (dense.HL with T = 1).  Nothing here falls back to ATen convolutions or F.batch_norm.
@@ -410,6 +410,32 @@ def upsample2x_backward(gy: torch.Tensor) -> torch.Tensor:
     with torch.cuda.device(gy.device):
         code = _lib.lib().stp3_upsample2x_bwd(gy.data_ptr(), N, H2 // 2, W2 // 2, C, gx.data_ptr(), _stream(gy.device))
     _lib.check(code, "stp3_upsample2x_bwd")
+    return gx
+
+
+def upsample2x_into(x: torch.Tensor, y: torch.Tensor, coff: int) -> torch.Tensor:
+    """upsample2x of x (N, h, w, C) written into channels [coff, coff + C) of the wider channels-last y (N, 2h, 2w, Cy)
+    (UpsamplingConcat's concat tensor: no torch.cat); the other channels of y are not touched."""
+    _f32_cl(x), _f32_cl(y)
+    N, h, w, C = x.shape
+    assert tuple(y.shape[:3]) == (N, 2 * h, 2 * w) and 0 <= coff and coff + C <= y.shape[3], (x.shape, y.shape, coff)
+    with torch.cuda.device(x.device):
+        code = _lib.lib().stp3_upsample2x_window_f32(x.data_ptr(), N, h, w, C, y.data_ptr(), y.shape[3], coff,
+                                                     _stream(x.device))
+    _lib.check(code, "stp3_upsample2x_window_f32")
+    return y
+
+
+def upsample2x_backward_from(gy: torch.Tensor, coff: int, C: int) -> torch.Tensor:
+    """Adjoint of upsample2x applied to channels [coff, coff + C) of gy (N, 2h, 2w, Cy) -> dense (N, h, w, C)."""
+    _f32_cl(gy)
+    N, H2, W2, Cy = gy.shape
+    assert H2 % 2 == 0 and W2 % 2 == 0 and 0 <= coff and coff + C <= Cy
+    gx = torch.empty((N, H2 // 2, W2 // 2, C), dtype=torch.float32, device=gy.device)
+    with torch.cuda.device(gy.device):
+        code = _lib.lib().stp3_upsample2x_window_bwd(gy.data_ptr(), Cy, coff, N, H2 // 2, W2 // 2, C, gx.data_ptr(),
+                                                     _stream(gy.device))
+    _lib.check(code, "stp3_upsample2x_window_bwd")
     return gx
 
 

@@ -6,6 +6,8 @@
   ASPP / DeepLabHead : the five ASPP branches write straight into one channels-last concat tensor; the global-pool
                    branch is spatially constant and becomes a per-image bias of the 1x1 projection.  DeepLabHead also
                    runs in train() (batch statistics, dropout, autograd; dense_train.py).
+  UpsamplingConcat : bilinear x2 of the coarse map into its channel window of the concat tensor, two 3x3 conv/BN/ReLU;
+                   also in train().
 """
 import os
 from typing import Optional
@@ -368,6 +370,99 @@ class UpsamplingConcat(PackedModule):
         dense.conv(y, P["c1"], relu=True, out_f32=out_f32, n_valid=self.out_channels, out_f32_nhwc=out_f32_nhwc, store=False)
         return out_f32
 
-    def forward(self, x_to_upsample, x):
+    def forward(self, x_to_upsample, x, channels_last: bool = False):
+        """x_to_upsample (N,Cc,h,w), x (N,Cf,2h,2w) fp32 -> (N,Cout,2h,2w) like the reference module.  In train mode
+        both BatchNorms use batch statistics (and update their running ones) and the output carries a grad_fn whose
+        backward fills the four parameters' .grad and the gradients of the inputs that require one; channels_last
+        (train mode only) returns (N,2h,2w,Cout) and takes its gradient in that layout -- what the lift-splat reads and
+        its backward writes, so the encoder's train path transposes neither."""
+        if self.training:
+            return self._forward_train(x_to_upsample, x, channels_last)
+        if channels_last:
+            raise ValueError("UpsamplingConcat.forward: channels_last is the train path's; in eval mode use forward_hl("
+                             "out_f32=..., out_f32_nhwc=True)")
         y = self.forward_hl(dense.from_f32(x_to_upsample.unsqueeze(1)), x)
         return dense.to_f32(y, 0, self.out_channels).squeeze(1)
+
+    # ------------------------------------------------------------------------------------------------ train mode
+    def _forward_train(self, x_up: torch.Tensor, x: torch.Tensor, channels_last: bool) -> torch.Tensor:
+        for i in (1, 4):
+            dense_train.check_bn(self.conv[i], f"UpsamplingConcat.conv.{i}")
+        if not x.is_cuda or not x_up.is_cuda or not self.conv[0].weight.is_cuda:
+            raise RuntimeError("stp3_b200 dense ops run on CUDA tensors only (there is no CPU path)")
+        if x.dim() != 4 or x_up.dim() != 4 or x.shape[1] + x_up.shape[1] != self.in_channels or \
+                x.shape[0] != x_up.shape[0] or tuple(x.shape[2:]) != (2 * x_up.shape[2], 2 * x_up.shape[3]):
+            raise ValueError(f"UpsamplingConcat: expected (N, Cc, h, w) and (N, {self.in_channels} - Cc, 2h, 2w), got "
+                             f"{tuple(x_up.shape)} and {tuple(x.shape)}")
+        return _UpsamplingConcatTrainFn.apply(self, x_up.float(), x.float(), channels_last, *self.parameters())
+
+    def _train_forward(self, x_up: torch.Tensor, x: torch.Tensor, channels_last: bool):
+        """-> (output (N, Cout, 2h, 2w), or (N, 2h, 2w, Cout) with channels_last; tape for _train_backward)."""
+        N, cf, H, W = x.shape
+        cc = x_up.shape[1]
+        # the concat tensor [fine | upsampled coarse], channels-last: the fine map is copied into its window, the
+        # upsample kernel writes the coarse map's
+        cat = torch.empty((N, H, W, cf + cc), dtype=torch.float32, device=x.device)
+        cat[..., :cf].copy_(x.detach().permute(0, 2, 3, 1))
+        dense_train.upsample2x_into(x_up.detach().permute(0, 2, 3, 1).contiguous(), cat, cf)
+        conv0, bn0, conv1, bn1 = self.conv[0], self.conv[1], self.conv[3], self.conv[4]
+        raw0 = dense_train.conv_raw(dense_train.to_hl(cat), conv0.weight, 1)
+        st0 = dense_train.bn_stats_module(raw0, bn0)
+        y0, y0_hl = dense_train.bn_apply(raw0, st0, bn0.weight, bn0.bias, relu=True)
+        raw1 = dense_train.conv_raw(y0_hl, conv1.weight, 1)
+        st1 = dense_train.bn_stats_module(raw1, bn1)
+        y1, _ = dense_train.bn_apply(raw1, st1, bn1.weight, bn1.bias, relu=True, hl=False)
+        tape = {"cat": cat, "cf": cf, "raw0": raw0, "st0": st0, "y0": y0, "raw1": raw1, "st1": st1, "y1": y1}
+        return (y1 if channels_last else y1.permute(0, 3, 1, 2).contiguous()), tape
+
+    def _train_backward(self, tape, g_out: torch.Tensor, channels_last: bool, need_up: bool, need_x: bool):
+        """Reverse walk of _train_forward -> (dL/dx_to_upsample or None, dL/dx or None (both NCHW), {parameter: gradient})."""
+        conv0, bn0, conv1, bn1 = self.conv[0], self.conv[1], self.conv[3], self.conv[4]
+        cat, cf = tape["cat"], tape["cf"]
+        N, H, W, ccat = cat.shape
+        grads = {}
+        g = g_out.float().contiguous() if channels_last else g_out.float().permute(0, 2, 3, 1).contiguous()
+        g, grads[bn1.weight], grads[bn1.bias], _ = dense_train.bn_backward(g, tape["raw1"], tape["st1"], bn1.weight,
+                                                                          tape["y1"])
+        grads[conv1.weight] = dense_train.conv_wgrad(tape["y0"], g, 3, 3, 1)
+        g = dense_train.conv_dgrad(g, conv1.weight, 1, H, W)
+        g, grads[bn0.weight], grads[bn0.bias], _ = dense_train.bn_backward(g, tape["raw0"], tape["st0"], bn0.weight,
+                                                                          tape["y0"])
+        grads[conv0.weight] = dense_train.conv_wgrad(cat, g, 3, 3, 1)
+        g_up = g_x = None
+        if need_up or need_x:
+            # the concat gradient splits: the fine map's channels as they are, the coarse map's through the adjoint of
+            # the upsample, read from their window
+            g_cat = dense_train.conv_dgrad(g, conv0.weight, 1, H, W)
+            if need_x:
+                g_x = g_cat[..., :cf].permute(0, 3, 1, 2).contiguous()
+            if need_up:
+                g_up = dense_train.upsample2x_backward_from(g_cat, cf, ccat - cf).permute(0, 3, 1, 2).contiguous()
+        return g_up, g_x, grads
+
+
+class _UpsamplingConcatTrainFn(torch.autograd.Function):
+    """UpsamplingConcat in train mode as one autograd node, with the guards of _DeepLabTrainFn: the backward is not
+    itself differentiable, runs once per forward, and refuses parameters modified in place in between."""
+
+    @staticmethod
+    def forward(ctx, mod, x_up, x, channels_last, *params):
+        out, tape = mod._train_forward(x_up, x, channels_last)
+        ctx.mod, ctx.tape, ctx.params, ctx.channels_last = mod, tape, params, channels_last
+        ctx.versions = [p._version for p in params]
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g_out):
+        if ctx.tape is None:
+            raise RuntimeError("UpsamplingConcat (train mode): backward ran a second time through the same forward; the "
+                               "activations are released after the first backward (retain_graph is not supported) -- "
+                               "run the forward again")
+        if any(p._version != v for p, v in zip(ctx.params, ctx.versions)):
+            raise RuntimeError("UpsamplingConcat (train mode): a parameter was modified in place between forward and "
+                               "backward (e.g. optimizer.step() before loss.backward())")
+        tape, ctx.tape = ctx.tape, None
+        g_up, g_x, grads = ctx.mod._train_backward(tape, g_out, ctx.channels_last, ctx.needs_input_grad[1],
+                                                   ctx.needs_input_grad[2])
+        return (None, g_up, g_x, None) + tuple(grads.get(p) for p in ctx.params)

@@ -6,7 +6,12 @@ The trunk (efficientnet-pytorch 0.7.0, not vendored by the reference; SURVEY.md 
   None          efficientnet_pytorch's pretrained model when the package is importable, else the native trunk;
   a module      injected: maps (M,3,H,W) -> (reduction_3 (M,c3,H/8,W/8), reduction_4 (M,c4,H/16,W/16)).
 The heads -- DeepLabHead + UpsamplingConcat -- run on the wgmma kernels.  With the native trunk the endpoints reach the
-heads as hi/lo planes: block 9 writes reduction_3 straight into the heads' concat tensor."""
+heads as hi/lo planes: block 9 writes reduction_3 straight into the heads' concat tensor.
+
+The heads also run in train mode (batch statistics, dropout, autograd; DeepLabHead.forward and
+UpsamplingConcat.forward on fp32 endpoints).  The native trunk is eval-only: with it the endpoints are computed under
+no_grad and train_heads() gives the frozen-trunk fine-tune; an injected torch trunk follows nn.Module.train() and
+receives the gradients of both endpoints through torch autograd."""
 import math
 
 import torch
@@ -52,6 +57,34 @@ class Encoder(nn.Module):
         self.feature_layer_1 = DeepLabHead(c_hi, c_hi, hidden_channel=64)
         self.feature_layer_2 = UpsamplingConcat(c_hi + c_lo, self.C)
 
+    def _head_modules(self):
+        mods = [self.feature_layer_1, self.feature_layer_2]
+        if self.use_depth_distribution:
+            mods += [self.depth_layer_1, self.depth_layer_2]
+        return mods
+
+    def heads_training(self) -> bool:
+        """True when the head modules are in train mode; they must all be in the same mode."""
+        modes = {m.training for m in self._head_modules()}
+        if len(modes) > 1:
+            raise RuntimeError("Encoder: the head modules (feature_layer_1/2, depth_layer_1/2) are in mixed train / eval "
+                               "modes; call encoder.train_heads(True) or encoder.train_heads(False)")
+        return modes.pop()
+
+    def train_heads(self, mode: bool = True):
+        """Sets the four head modules' mode and leaves the trunk alone (the native trunk is eval-only):
+        model.eval(); model.encoder.train_heads() is the frozen-trunk recipe.  Returns self."""
+        for m in self._head_modules():
+            m.train(mode)
+        return self
+
+    def heads_train(self, r_lo: torch.Tensor, r_hi: torch.Tensor, channels_last: bool = False):
+        """heads_f32 with the heads in train mode: outputs carry a grad_fn; both heads read the same endpoints, autograd
+        adds their two gradients."""
+        feat = self.feature_layer_2(self.feature_layer_1(r_hi), r_lo, channels_last=channels_last)
+        depth = self.depth_layer_2(self.depth_layer_1(r_hi), r_lo) if self.use_depth_distribution else None
+        return feat, depth
+
     def heads_hl(self, r_lo: torch.Tensor, r_hi: torch.Tensor):
         """r_lo (M,c3,H/8,W/8), r_hi (M,c4,H/16,W/16) fp32 -> (feature HL, depth-logit HL or None)."""
         x = dense.from_f32(r_hi.unsqueeze(1))
@@ -65,6 +98,8 @@ class Encoder(nn.Module):
         """Both heads with fp32 outputs written straight from the last convolution's epilogue: context features
         (M,C,Hf,Wf) -- or channels-last (M,Hf,Wf,C), the layout the lift-splat kernel stages with one TMA box per tile
         (SURVEY.md row f1) -- and depth logits (M,D,Hf,Wf) (the reference's layout: they are also a model output)."""
+        if self.heads_training():
+            return self.heads_train(r_lo, r_hi, channels_last)
         M, _, Hf, Wf = r_lo.shape
         dev = r_lo.device
         x = dense.from_f32(r_hi.unsqueeze(1))
@@ -82,6 +117,10 @@ class Encoder(nn.Module):
 
     def features_native(self, x: torch.Tensor, channels_last: bool = False):
         """(M,3,H,W) fp32 images -> heads_f32's outputs through the native trunk, hi/lo from the stem to the heads."""
+        if self.heads_training():
+            with torch.no_grad():                 # the native trunk is frozen: fp32 endpoints, no graph behind them
+                r_lo, r_hi = self.backbone(x)
+            return self.heads_train(r_lo, r_hi, channels_last)
         M, _, H, W = x.shape
         ds = self.downsample
         index = int(math.log2(ds))

@@ -116,15 +116,17 @@ class STP3(nn.Module):
         const = self._shifted_egomotion(ego).reshape(-1, 6).contiguous()
         return {"cam_M": cam_M, "cam_t": cam_t, "ego_R": ego_R, "ego_t": ego_t, "const": const}
 
-    def projection_to_birds_eye_view(self, feat, depth_logits, intrinsics, extrinsics, future_egomotion):
-        """(B,S,N,C,Hf,Wf) features + (B,S,N,D,Hf,Wf) depth logits -> (B,S,C,X,Y) fp32, as stp3.py:226-301 (which takes
-        the materialised outer product and geometry instead; both are fused away here)."""
+    def projection_to_birds_eye_view(self, feat, depth_logits, intrinsics, extrinsics, future_egomotion,
+                                     feat_channels_last=False):
+        """(B,S,N,C,Hf,Wf) features [or (B,S,N,Hf,Wf,C) with feat_channels_last] + (B,S,N,D,Hf,Wf) depth logits ->
+        (B,S,C,X,Y) fp32, as stp3.py:226-301 (which takes the materialised outer product and geometry instead; both are
+        fused away here)."""
         h = self.prepare_inputs(intrinsics, extrinsics, future_egomotion)
         off, res, dim = self._bev_host()
         needs_grad = torch.is_grad_enabled() and (feat.requires_grad or (depth_logits is not None and depth_logits.requires_grad))
         fn = ops.lift_splat_autograd if needs_grad else ops.lift_splat      # training through the lift: SURVEY.md row f2
         return fn(feat, depth_logits, h["cam_M"], h["cam_t"], h["ego_R"], h["ego_t"], *self._axes(), off, res,
-                  dim, float(self.discount),
+                  dim, float(self.discount), feat_channels_last=feat_channels_last,
                   use_depth_distribution=self.cfg.MODEL.ENCODER.USE_DEPTH_DISTRIBUTION, workspace=self._ws)
 
     # ------------------------------------------------------------------------------------------------ forward
@@ -156,6 +158,7 @@ class STP3(nn.Module):
         """Device-only from images (B,S,N,3,H,W) fp32 through the native trunk: trunk -> heads -> forward_device
         (capturable in a CUDA graph, GraphedPerception(entry="images"))."""
         b, s, n = image.shape[:3]
+        self._check_encoder_train()
         self._mark("start_trunk")
         feat, depth = self.encoder.features_native(image.reshape(b * s * n, *image.shape[3:]), channels_last=True)
         feat = feat.view(b, s, n, *feat.shape[1:])
@@ -166,6 +169,7 @@ class STP3(nn.Module):
     def forward_heads_device(self, r_lo, r_hi, cam_M, cam_t, ego_R, ego_t, const):
         """Device-only: encoder heads -> forward_device (capturable in a CUDA graph)."""
         b, s, n = r_lo.shape[:3]
+        self._check_encoder_train()
         self._mark("start_heads")
         feat, depth = self.encoder.heads_f32(r_lo.view(b * s * n, *r_lo.shape[3:]), r_hi.view(b * s * n, *r_hi.shape[3:]),
                                              channels_last=True)
@@ -202,15 +206,10 @@ class STP3(nn.Module):
             # require grad
             needs_grad = torch.is_grad_enabled() and (feat.requires_grad or
                                                       (depth_logits is not None and depth_logits.requires_grad))
-            if needs_grad and feat_channels_last:
-                raise NotImplementedError("STP3: gradients to channels-last feat are not supported; pass (B,S,N,C,Hf,Wf)")
-            kw = dict(use_depth_distribution=self.cfg.MODEL.ENCODER.USE_DEPTH_DISTRIBUTION, workspace=self._ws)
-            if needs_grad:
-                bev = ops.lift_splat_autograd(feat, depth_logits, cam_M, cam_t, ego_R, ego_t, *self._axes(), off, res,
-                                              dim, float(self.discount), **kw)
-            else:
-                bev = ops.lift_splat(feat, depth_logits, cam_M, cam_t, ego_R, ego_t, *self._axes(), off, res, dim,
-                                     float(self.discount), feat_channels_last=feat_channels_last, **kw)
+            fn = ops.lift_splat_autograd if needs_grad else ops.lift_splat
+            bev = fn(feat, depth_logits, cam_M, cam_t, ego_R, ego_t, *self._axes(), off, res, dim, float(self.discount),
+                     feat_channels_last=feat_channels_last, workspace=self._ws,
+                     use_depth_distribution=self.cfg.MODEL.ENCODER.USE_DEPTH_DISTRIBUTION)
             states = self.temporal_model(bev, const=const if use_ego else None)
             output.update(self.decoder(states))
             return output
@@ -242,6 +241,20 @@ class STP3(nn.Module):
     def _head_training(self) -> bool:
         return isinstance(self.temporal_model, TemporalModel) and self.temporal_model.final_conv.training
 
+    def _check_encoder_train(self):
+        """Train-mode encoder heads need a train-mode path behind them: only the train-mode TemporalBlocks take the
+        lift-splat through autograd, and the head and the decoder carry the gradient to them."""
+        if not self.encoder.heads_training():
+            return
+        if not isinstance(self.temporal_model, TemporalModel):
+            raise RuntimeError("STP3: the encoder heads are in train mode, which needs the temporal_block model (the "
+                               "identity temporal model runs the inference forward only) -- call "
+                               "model.encoder.train_heads(False)")
+        if not (self.temporal_model.blocks_training() and self._head_training() and self.decoder.training):
+            raise RuntimeError("STP3: the encoder heads are in train mode but the temporal model or the decoder is in "
+                               "eval mode, so no gradient could reach them -- call model.temporal_model.train() and "
+                               "model.decoder.train() as well")
+
     def _blocks_training(self) -> bool:
         return isinstance(self.temporal_model, TemporalModel) and any(b.training for b in self.temporal_model.model)
 
@@ -255,6 +268,9 @@ class STP3(nn.Module):
         one kernel, bracketed by two device-side barriers."""
         S = self.receptive_field
         dev = feat.device
+        if self.encoder.heads_training():
+            raise RuntimeError("frame-sharded forward: the encoder heads are in train mode; the sharded path runs the "
+                               "inference forward only -- call model.encoder.train_heads(False)")
         h = {k: v.to(dev) for k, v in self.prepare_inputs(intrinsics, extrinsics, future_egomotion).items()}
         feat = feat[:, :S].contiguous()
         depth_logits = depth_logits[:, :S].contiguous() if depth_logits is not None else None
@@ -357,6 +373,10 @@ class GraphedPerception:
         if model._head_training():
             raise RuntimeError("GraphedPerception: temporal_model.final_conv is in train mode (batch statistics, "
                                "dropout, autograd); a CUDA graph replays the inference forward only -- call .eval()")
+        if model.encoder.heads_training():
+            raise RuntimeError("GraphedPerception: the encoder heads are in train mode (batch statistics, dropout, "
+                               "autograd); a CUDA graph replays the inference forward only -- call "
+                               "model.encoder.train_heads(False)")
         self.model = model
         self.entry = entry
         dev = torch.device(device) if device is not None else next(model.parameters()).device

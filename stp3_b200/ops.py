@@ -153,11 +153,12 @@ def lift_splat_plan(feat, depth_logits, cam_M, cam_t, ego_R, ego_t, xs, ys, ds, 
 
 
 def lift_splat_backward(grad_out, feat, depth_logits, cam_M, cam_t, ego_R, ego_t, xs, ys, ds, bev_off, bev_res, bev_dim,
-                        discount: float, *, use_depth_distribution: bool = True):
+                        discount: float, *, use_depth_distribution: bool = True, feat_channels_last: bool = False):
     """Gradients of lift_splat()'s (B,S,C,X,Y) output w.r.t. feat (B,S,N,C,Hf,Wf) and depth_logits (B,S,N,D,Hf,Wf):
-    stp3_lift_splat_bwd (include/stp3_b200.h).  Returns (grad_feat, grad_depth_logits or None)."""
+    stp3_lift_splat_bwd (include/stp3_b200.h).  With feat_channels_last feat and its gradient are (B,S,N,Hf,Wf,C)
+    (stp3_lift_splat_bwd_cl: the same values, no transposes).  Returns (grad_feat, grad_depth_logits or None)."""
     desc, feat, depth_logits = _lift_desc(feat, depth_logits, cam_M, cam_t, ego_R, ego_t, xs, ys, ds, bev_off, bev_res,
-                                          bev_dim, discount, use_depth_distribution=use_depth_distribution)
+                                          bev_dim, discount, feat_channels_last, use_depth_distribution)
     dev = feat.device
     grad_out = _f32c(grad_out)
     assert tuple(grad_out.shape) == (desc.B, desc.S, desc.C, desc.nx, desc.ny)
@@ -166,43 +167,49 @@ def lift_splat_backward(grad_out, feat, depth_logits, cam_M, cam_t, ego_R, ego_t
     scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
     g_feat = torch.empty_like(feat)
     g_depth = torch.empty_like(depth_logits) if (use_depth_distribution and depth_logits is not None) else None
+    name = "stp3_lift_splat_bwd_cl" if feat_channels_last else "stp3_lift_splat_bwd"
     with torch.cuda.device(dev):
-        code = L.stp3_lift_splat_bwd(desc, grad_out.data_ptr(), feat.data_ptr(), _ptr(depth_logits), scratch.data_ptr(),
-                                     nbytes, g_feat.data_ptr(), _ptr(g_depth), torch.cuda.current_stream(dev).cuda_stream)
-    _lib.check(code, "stp3_lift_splat_bwd")
+        code = getattr(L, name)(desc, grad_out.data_ptr(), feat.data_ptr(), _ptr(depth_logits), scratch.data_ptr(),
+                                nbytes, g_feat.data_ptr(), _ptr(g_depth), torch.cuda.current_stream(dev).cuda_stream)
+    _lib.check(code, name)
     return g_feat, g_depth
 
 
 class LiftSplatFunction(torch.autograd.Function):
-    """Differentiable lift-splat: forward = stp3_lift_splat_fwd, backward = stp3_lift_splat_bwd.  Gradients flow to the
+    """Differentiable lift-splat: forward = stp3_lift_splat_fwd, backward = stp3_lift_splat_bwd (stp3_lift_splat_bwd_cl
+    for channels-last feat, whose gradient comes back in that layout).  Gradients flow to the
     context features and the depth logits; calibration, ego-motion and the integer voxel indices carry none (like the
     reference, whose indices pass through .long(), stp3.py:289)."""
 
     @staticmethod
     def forward(ctx, feat, depth_logits, cam_M, cam_t, ego_R, ego_t, xs, ys, ds, bev_off, bev_res, bev_dim, discount,
-                use_depth_distribution, workspace):
+                use_depth_distribution, workspace, feat_channels_last=False):
         out = lift_splat(feat, depth_logits, cam_M, cam_t, ego_R, ego_t, xs, ys, ds, bev_off, bev_res, bev_dim, discount,
-                         use_depth_distribution=use_depth_distribution, workspace=workspace)
+                         use_depth_distribution=use_depth_distribution, workspace=workspace,
+                         feat_channels_last=feat_channels_last)
         ctx.save_for_backward(feat, depth_logits if depth_logits is not None else feat.new_empty(0),
                               cam_M, cam_t, ego_R, ego_t, xs, ys, ds)
-        ctx.host = (bev_off, bev_res, bev_dim, discount, use_depth_distribution, depth_logits is not None)
+        ctx.host = (bev_off, bev_res, bev_dim, discount, use_depth_distribution, depth_logits is not None,
+                    feat_channels_last)
         return out
 
     @staticmethod
     def backward(ctx, grad_out):
         feat, depth_logits, cam_M, cam_t, ego_R, ego_t, xs, ys, ds = ctx.saved_tensors
-        bev_off, bev_res, bev_dim, discount, use_dd, has_depth = ctx.host
+        bev_off, bev_res, bev_dim, discount, use_dd, has_depth, feat_cl = ctx.host
         g_feat, g_depth = lift_splat_backward(grad_out, feat, depth_logits if has_depth else None, cam_M, cam_t, ego_R,
                                               ego_t, xs, ys, ds, bev_off, bev_res, bev_dim, discount,
-                                              use_depth_distribution=use_dd)
-        return (g_feat, g_depth) + (None,) * 13
+                                              use_depth_distribution=use_dd, feat_channels_last=feat_cl)
+        return (g_feat, g_depth) + (None,) * 14
 
 
 def lift_splat_autograd(feat, depth_logits, cam_M, cam_t, ego_R, ego_t, xs, ys, ds, bev_off, bev_res, bev_dim,
-                        discount: float, *, use_depth_distribution: bool = True, workspace: Optional[Workspace] = None):
-    """lift_splat() (reference layout: feat NCHW in, (B,S,C,X,Y) out) with gradients to feat and depth_logits."""
+                        discount: float, *, use_depth_distribution: bool = True, workspace: Optional[Workspace] = None,
+                        feat_channels_last: bool = False):
+    """lift_splat() ((B,S,C,X,Y) out; feat NCHW like the reference, or (B,S,N,Hf,Wf,C) with feat_channels_last) with
+    gradients to feat, in its own layout, and depth_logits."""
     return LiftSplatFunction.apply(feat, depth_logits, cam_M, cam_t, ego_R, ego_t, xs, ys, ds, bev_off, bev_res, bev_dim,
-                                   float(discount), bool(use_depth_distribution), workspace)
+                                   float(discount), bool(use_depth_distribution), workspace, bool(feat_channels_last))
 
 
 def lift_splat_frames(feat, depth_logits, cam_M, cam_t, ego_R, ego_t, xs, ys, ds, bev_off, bev_res, bev_dim,
