@@ -92,9 +92,12 @@ wgrad_partial_kernel(const float* __restrict__ x, const float* __restrict__ g, W
   const int tid = threadIdx.x;
   const int co0 = cot * kWgTile, ci0 = cit * kWgTile;
   const uint32_t s_base = ptx::smem_u32(sm);
-  float acc[32];
+  // each 64-pixel stage is multiplied into `stage` (its first wgmma overwrites it) and then added to `acc` with an
+  // ordinary fp32 add: the tensor cores' accumulation does not round to nearest, and chained over a whole split (up to
+  // thousands of pixels) its error grew with the pixels per split (DESIGN 3.10); chained over one stage it is negligible
+  float acc[32], stage[32];
 #pragma unroll
-  for (int i = 0; i < 32; ++i) acc[i] = 0.f;
+  for (int i = 0; i < 32; ++i) acc[i] = stage[i] = 0.f;
   for (long long p0 = p_begin; live && p0 < p_end; p0 += kWgK) {
     // stage: 64 pixel rows x 8 chunks of 8 channels, per operand; chunk c of row r lives at chunk c ^ (r % 8)
 #pragma unroll
@@ -133,12 +136,14 @@ wgrad_partial_kernel(const float* __restrict__ x, const float* __restrict__ g, W
       const uint64_t a_lo = wg::desc_mn_sw128(s_base + 1 * kWgTileBytes + koff, 1024);
       const uint64_t b_hi = wg::desc_mn_sw128(s_base + 2 * kWgTileBytes + koff, 1024);
       const uint64_t b_lo = wg::desc_mn_sw128(s_base + 3 * kWgTileBytes + koff, 1024);
-      wg::mma_bf16_mn64(acc, a_hi, b_hi, 1);
-      wg::mma_bf16_mn64(acc, a_hi, b_lo, 1);
-      wg::mma_bf16_mn64(acc, a_lo, b_hi, 1);
+      wg::mma_bf16_mn64(stage, a_hi, b_hi, ks > 0);
+      wg::mma_bf16_mn64(stage, a_hi, b_lo, 1);
+      wg::mma_bf16_mn64(stage, a_lo, b_hi, 1);
     }
     wg::commit();
     wg::wait<0>();
+#pragma unroll
+    for (int i = 0; i < 32; ++i) acc[i] += stage[i];
     __syncthreads();                                   // every warp's MMAs have read the stage before it is rewritten
   }
   // part[split][tap][co][ci]; accumulator fragment: row = co, column = ci (wgmma.cuh)

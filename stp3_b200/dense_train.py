@@ -188,9 +188,17 @@ def conv_dgrad(g: torch.Tensor, weight: torch.Tensor, stride: int, H: int, W: in
         t = torch.empty((N, Hp, Wp, cin), dtype=torch.float32, device=dev)
         dense.conv(g_hl, pc, out_f32=t, n_valid=cin, out_f32_nhwc=True, out_hw=(Hp, Wp), store=False, tune=(0, 0))
         phases.append(t)
-    out = torch.empty((N, H, W, cin), dtype=torch.float32, device=dev)
+    return phase_interleave(phases, H, W)
+
+
+def phase_interleave(phases: List[Optional[torch.Tensor]], H: int, W: int) -> torch.Tensor:
+    """The four phases (py, px) = (0,0), (0,1), (1,0), (1,1) of a stride-2 input gradient, phase (py, px) of size
+    (N, (H - py + 1) // 2, (W - px + 1) // 2, C) or None (zeros) -> (N, H, W, C) (stp3_phase_interleave)."""
+    ref = next(t for t in phases if t is not None)
+    N, C, dev = ref.shape[0], ref.shape[-1], ref.device
+    out = torch.empty((N, H, W, C), dtype=torch.float32, device=dev)
     with torch.cuda.device(dev):
-        code = _lib.lib().stp3_phase_interleave(*[_p(t) for t in phases], N, H, W, cin, out.data_ptr(), _stream(dev))
+        code = _lib.lib().stp3_phase_interleave(*[_p(t) for t in phases], N, H, W, C, out.data_ptr(), _stream(dev))
     _lib.check(code, "stp3_phase_interleave")
     return out
 
