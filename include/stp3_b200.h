@@ -335,6 +335,7 @@ int stp3_block_fused_fwd(const stp3_block_desc* desc, const void* mid_hi, const 
 
 /* ---------------------------------------------------------------------------------------------------------
  * Memory-bound helpers of the dense path (all tensors channels-last bf16 hi/lo planes unless noted).
+ * stp3_f32_to_hilo, stp3_hilo_to_f32 and stp3_spatial_sum take n_img <= 65535.
  */
 /* fp32 (n_img,C,H,W) [channels_last=0, the reference's NCHW] or (n_img,H,W,C) [1] -> hi/lo (n_img,H,W,cp), padding 0.
  * Used where a foreign fp32 tensor enters a drop-in module (e.g. TemporalModel.forward, temporal_model.py:50). */
@@ -350,6 +351,7 @@ int stp3_spatial_sum(const void* hi, const void* lo, int n_img, int HW, int cstr
  *       n_const spatially constant ones (their mean is the value); temporal != 0: averaged with the previous frame of
  *       the same sample when it exists -- AvgPool3d((2,H,W), padding (1,0,0), count_include_pad=False), temporal.py:397-415
  *   v = relu(W1 m + b1)  (R);   out[img][co] = (accumulate ? out[img][co] : bias ? bias[co] : 0) + sum_r W2[co][r] v[r]
+ * C + R <= 12288 (m and v live in 48 KiB of shared memory).
  * Replaces PyramidSpatioTemporalPooling (temporal.py:375-423) and ASPPPooling (convolutions.py:227-239). */
 int stp3_pool_bias(const float* sums, int sums_stride, int n_img, int T, int C, float inv_hw, int temporal,
                    const float* const_vals, int n_const, const float* W1, const float* b1, int R, const float* W2, int CO,
@@ -360,7 +362,8 @@ int stp3_small_linear(const float* x, const float* W, int n, int ci, int co, con
                       int accumulate, void* stream);
 /* y[..., y_coff:y_coff+C] = bilinear_x2(x[..., :C]) (+ skip[..., s_coff:s_coff+C] when skip is given); x is
  * (n_img,h,w,.), skip and y are (n_img,2h,2w,.).  UpsamplingAdd tail (convolutions.py:204-215) and the upsample +
- * concat of UpsamplingConcat (convolutions.py:183-201). */
+ * concat of UpsamplingConcat (convolutions.py:183-201).  16-byte vectors: every plane 16-byte aligned, C, the strides
+ * and the offsets multiples of 8. */
 int stp3_upsample2x_add(const void* x_hi, const void* x_lo, int n_img, int h, int w, int x_cstride, const void* s_hi,
                         const void* s_lo, int s_cstride, int s_coff, void* y_hi, void* y_lo, int y_cstride, int y_coff,
                         int C, void* stream);
@@ -471,7 +474,8 @@ int stp3_temporal_pair_mean(const float* m, int B, int T, int C, int adjoint, fl
  * outside the image read as zero, which is the bottom / right pad.  BatchNorm (eps 1e-3) is folded by the caller.
  *
  * Stem: fp32 NCHW images (n_img, 3, H, W) -> 3x3 stride-2 conv (w [cout][3][3][3], bias [cout]) + swish -> hi/lo planes
- * (n_img, Ho, Wo, out_cstride); channels [cout, out_cstride) are written as zeros.  cout <= 64. */
+ * (n_img, Ho, Wo, out_cstride); channels [cout, out_cstride) are written as zeros.  cout <= 64, out_cstride a multiple
+ * of 64, y_hi / y_lo 16-byte aligned, n_img * Ho * Wo * out_cstride / 16 threads in at most 2^31 - 1 blocks of 256. */
 int stp3_effnet_stem(const float* x, int n_img, int H, int W, int Ho, int Wo, int pad_t, int pad_l, const float* w,
                      const float* bias, int cout, int out_cstride, void* y_hi, void* y_lo, void* stream);
 /* Depthwise k x k convolution (k 3 or 5, stride 1 or 2) + folded BN + swish on hi/lo planes, channels [0, C) of

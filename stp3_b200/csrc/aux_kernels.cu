@@ -244,6 +244,7 @@ typedef __nv_bfloat16 bf16;
 extern "C" int stp3_f32_to_hilo(const float* x, int channels_last, int n_img, int C, int H, int W, int cp, void* hi,
                                 void* lo, void* stream) {
   STP3_CHECK_ARG(x && hi && lo && n_img > 0 && C > 0 && H > 0 && W > 0 && cp >= C, "stp3_f32_to_hilo: bad argument");
+  STP3_CHECK_ARG(n_img <= 65535, "stp3_f32_to_hilo: more than 65535 images");
   const int HW = H * W;
   dim3 grid(ceil_div(HW, 32), ceil_div(cp, 32), n_img), block(32, 8);
   f32_to_hilo_kernel<<<grid, block, 0, (cudaStream_t)stream>>>(x, channels_last, C, HW, cp, (bf16*)hi, (bf16*)lo);
@@ -254,6 +255,8 @@ extern "C" int stp3_f32_to_hilo(const float* x, int channels_last, int n_img, in
 extern "C" int stp3_hilo_to_f32(const void* hi, const void* lo, int n_img, int H, int W, int cstride, int c_off, int C,
                                 float* out, void* stream) {
   STP3_CHECK_ARG(hi && lo && out && n_img > 0 && C > 0 && c_off >= 0 && c_off + C <= cstride, "stp3_hilo_to_f32: bad argument");
+  STP3_CHECK_ARG(H > 0 && W > 0, "stp3_hilo_to_f32: non-positive H or W");
+  STP3_CHECK_ARG(n_img <= 65535, "stp3_hilo_to_f32: more than 65535 images");
   const int HW = H * W;
   dim3 grid(ceil_div(HW, 32), ceil_div(C, 32), n_img), block(32, 8);
   hilo_to_f32_kernel<<<grid, block, 0, (cudaStream_t)stream>>>((const bf16*)hi, (const bf16*)lo, cstride, c_off, C, HW, out);
@@ -263,6 +266,7 @@ extern "C" int stp3_hilo_to_f32(const void* hi, const void* lo, int n_img, int H
 
 extern "C" int stp3_spatial_sum(const void* hi, const void* lo, int n_img, int HW, int cstride, float* sums, void* stream) {
   STP3_CHECK_ARG(hi && lo && sums && n_img > 0 && HW > 0 && cstride > 0 && cstride <= 1024, "stp3_spatial_sum: bad argument");
+  STP3_CHECK_ARG(n_img <= 65535, "stp3_spatial_sum: more than 65535 images");
   STP3_CUDA_OK(cudaMemsetAsync(sums, 0, (size_t)n_img * cstride * sizeof(float), (cudaStream_t)stream));
   const int px_per_block = 128;
   dim3 grid(ceil_div(HW, px_per_block), n_img);
@@ -278,6 +282,7 @@ extern "C" int stp3_pool_bias(const float* sums, int sums_stride, int n_img, int
   STP3_CHECK_ARG(sums && W1 && b1 && W2 && out && n_img > 0 && T > 0 && C > 0 && R > 0 && CO > 0 && n_const >= 0 &&
                  n_const < C && C - n_const <= sums_stride && CO <= co_stride && (n_const == 0 || const_vals),
                  "stp3_pool_bias: bad argument");
+  STP3_CHECK_ARG((long long)C + R <= 12288, "stp3_pool_bias: C + R must be <= 12288 (48 KiB of shared memory)");
   STP3_CUDA_OK(launch_pdl(kPdlAux, pool_bias_kernel, dim3(n_img, CO >= 64 ? 4 : 1), dim3(256), (size_t)(C + R) * sizeof(float), (cudaStream_t)stream,
                           sums, sums_stride, T, C, inv_hw, temporal, const_vals, n_const, W1, b1, R, W2, CO, bias, out,
                           co_stride, accumulate));
@@ -301,6 +306,9 @@ extern "C" int stp3_upsample2x_add(const void* x_hi, const void* x_lo, int n_img
   STP3_CHECK_ARG(C % 8 == 0 && C <= x_cstride && s_coff % 8 == 0 && (!s_hi || s_coff + C <= s_cstride) &&
                  y_coff % 8 == 0 && y_coff + C <= y_cstride && x_cstride % 8 == 0 && s_cstride % 8 == 0 &&
                  y_cstride % 8 == 0, "stp3_upsample2x_add: channel windows must be multiples of 8");
+  STP3_CHECK_ARG((reinterpret_cast<uintptr_t>(x_hi) | reinterpret_cast<uintptr_t>(x_lo) | reinterpret_cast<uintptr_t>(s_hi) |
+                  reinterpret_cast<uintptr_t>(s_lo) | reinterpret_cast<uintptr_t>(y_hi) | reinterpret_cast<uintptr_t>(y_lo)) % 16 == 0,
+                 "stp3_upsample2x_add: planes must be 16-byte aligned");
   const size_t total = (size_t)n_img * (2 * h) * (2 * w) * (C / 8);
     STP3_CUDA_OK(launch_pdl(kPdlAux, upsample2x_add_kernel, dim3((unsigned)((total + 255) / 256)), dim3(256), 0, (cudaStream_t)stream,
       (const bf16*)x_hi, (const bf16*)x_lo, h, w, x_cstride, (const bf16*)s_hi, (const bf16*)s_lo, s_cstride, s_coff,

@@ -235,8 +235,10 @@ extern "C" int stp3_effnet_stem(const float* x, int n_img, int H, int W, int Ho,
   STP3_CHECK_ARG(cout > 0 && cout <= kStemMaxCout && out_cstride % 64 == 0 && out_cstride >= cout,
                  "stp3_effnet_stem: cout must be <= 64 and out_cstride a multiple of 64 >= cout");
   STP3_CHECK_ARG(pad_t >= 0 && pad_l >= 0 && pad_t < 3 && pad_l < 3, "stp3_effnet_stem: pad out of range");
+  STP3_CHECK_ARG((reinterpret_cast<uintptr_t>(y_hi) | reinterpret_cast<uintptr_t>(y_lo)) % 16 == 0,
+                 "stp3_effnet_stem: y_hi / y_lo must be 16-byte aligned");
   const long long n = (long long)n_img * Ho * Wo * (out_cstride / 16);
-  STP3_CHECK_ARG(n < (1ll << 40), "stp3_effnet_stem: grid too large");
+  STP3_CHECK_ARG((n + 255) / 256 <= 0x7fffffffll, "stp3_effnet_stem: more than 2^31 - 1 blocks of 256 threads");
   const unsigned grid = (unsigned)((n + 255) / 256);
   STP3_CUDA_OK(launch_pdl(kPdlAux, stem_kernel, dim3(grid), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream_), x,
                           n_img, H, W, Ho, Wo, pad_t, pad_l, w, bias, cout, out_cstride,
