@@ -437,6 +437,31 @@ int stp3_bn_bwd_apply(const float* g, int g_cstride, const float* y, int y_cstri
                       const float* mean, const float* invstd, const float* gamma, const float* sum_g,
                       const float* sum_gxhat, long long n_pix, int C, float* dx, int dx_cstride, float* g_masked,
                       int gm_cstride, void* stream);
+/* SyncBatchNorm (statistics over every rank of a process group; the caller all-gathers the records between the local
+ * and the merge calls).  A moments record is (4, C) fp64, rows n, S = sum x, Q = sum (x - m)^2, m = the fp32-rounded
+ * local mean: stp3_bn_local_moments writes this rank's into out (e.g. its row of the gather buffer), with the two fixed
+ * order passes of stp3_bn_stats; scratch: stp3_bn_scratch_bytes(n_pix, C).
+ * stp3_bn_merge_finalize merges `world` records (world, 4, C) in rank order in fp64: N = sum n, mean = sum S / N,
+ * M2 = sum_r Q_r - 2 (mean - m_r)(S_r - n_r m_r) + n_r (mean - m_r)^2, var = M2 / N (biased), invstd, and the running
+ * statistics with the unbiased M2 / (N - 1), as stp3_bn_stats.  Every rank gets the same bits; world = 1 gives
+ * stp3_bn_stats' bits. */
+int stp3_bn_local_moments(const float* x, long long n_pix, int C, int x_cstride, double* out, void* scratch,
+                          size_t scratch_bytes, void* stream);
+int stp3_bn_merge_finalize(const double* records, int world, int C, float eps, float momentum, float* running_mean,
+                           float* running_var, float* mean, float* var, float* invstd, void* stream);
+/* Backward of a SyncBatchNorm: stp3_bn_bwd_local_sums writes this rank's (2, C) fp64 record (sum g', sum g' xhat) over
+ * its n_pix rows (the arguments of stp3_bn_bwd_reduce); stp3_bn_bwd_merge_sums adds `world` records (world, 2, C) in
+ * rank order into fp32 sum_g / sum_gxhat (world = 1: stp3_bn_bwd_reduce's bits); stp3_bn_bwd_apply_global is
+ * stp3_bn_bwd_apply over this rank's n_pix rows with the group's merged sums and row count n_total:
+ * dx = gamma * invstd * (g' - sum_g/n_total - xhat * sum_gxhat/n_total). */
+int stp3_bn_bwd_local_sums(const float* g, int g_cstride, const float* y, int y_cstride, const float* x, int x_cstride,
+                           const float* mean, const float* invstd, long long n_pix, int C, double* out, void* scratch,
+                           size_t scratch_bytes, void* stream);
+int stp3_bn_bwd_merge_sums(const double* records, int world, int C, float* sum_g, float* sum_gxhat, void* stream);
+int stp3_bn_bwd_apply_global(const float* g, int g_cstride, const float* y, int y_cstride, const float* x,
+                             int x_cstride, const float* mean, const float* invstd, const float* gamma,
+                             const float* sum_g, const float* sum_gxhat, long long n_pix, long long n_total, int C,
+                             float* dx, int dx_cstride, float* g_masked, int gm_cstride, void* stream);
 /* bilinear x2 (align_corners=False, nn.Upsample of UpsamplingAdd) on fp32 (n_img, h, w, C) -> (n_img, 2h, 2w, C), and
  * its adjoint (a gather over the outputs each input feeds; no atomics) */
 int stp3_upsample2x_f32(const float* x, int n_img, int h, int w, int C, float* y, void* stream);

@@ -121,6 +121,11 @@ SIGNATURES = {
     "stp3_image_channel_sums": (_I, [_V, _I, _LL, _I, _I, _V, _V, _SZ, _V]),
     "stp3_bn_bwd_reduce": (_I, [_V, _I, _V, _I, _V, _I, _V, _V, _LL, _I, _V, _V, _V, _SZ, _V]),
     "stp3_bn_bwd_apply": (_I, [_V, _I, _V, _I, _V, _I, _V, _V, _V, _V, _V, _LL, _I, _V, _I, _V, _I, _V]),
+    "stp3_bn_local_moments": (_I, [_V, _LL, _I, _I, _V, _V, _SZ, _V]),
+    "stp3_bn_merge_finalize": (_I, [_V, _I, _I, _F, _F, _V, _V, _V, _V, _V, _V]),
+    "stp3_bn_bwd_local_sums": (_I, [_V, _I, _V, _I, _V, _I, _V, _V, _LL, _I, _V, _V, _SZ, _V]),
+    "stp3_bn_bwd_merge_sums": (_I, [_V, _I, _I, _V, _V, _V]),
+    "stp3_bn_bwd_apply_global": (_I, [_V, _I, _V, _I, _V, _I, _V, _V, _V, _V, _V, _LL, _LL, _I, _V, _I, _V, _I, _V]),
     "stp3_upsample2x_f32": (_I, [_V, _I, _I, _I, _I, _V, _V]),
     "stp3_upsample2x_bwd": (_I, [_V, _I, _I, _I, _I, _V, _V]),
     "stp3_upsample2x_window_f32": (_I, [_V, _I, _I, _I, _I, _V, _I, _I, _V]),

@@ -237,8 +237,15 @@ __global__ void mean_finalize_kernel(const double* __restrict__ part, int n_part
   mean[c] = (float)(t0 / (double)n_pix);
 }
 
-// biased variance, 1/sqrt(var + eps), and the running statistics (unbiased variance, n / (n - 1)) as nn.BatchNorm2d:
-// running = (1 - momentum) * running + momentum * batch
+// running = (1 - momentum) * running + momentum * batch, with the roundings spelled out so that every kernel that
+// updates running statistics gives the same bits (these are the ones var_finalize_kernel has always produced)
+__device__ __forceinline__ void running_update(float* run_mean, float* run_var, int c, float momentum, float mean,
+                                               float unb) {
+  run_mean[c] = __fmaf_rn(run_mean[c], 1.f - momentum, __fmul_rn(mean, momentum));
+  run_var[c] = __fmaf_rn(unb, momentum, __fmul_rn(1.f - momentum, run_var[c]));
+}
+
+// biased variance, 1/sqrt(var + eps), and the running statistics (unbiased variance, n / (n - 1)) as nn.BatchNorm2d
 __global__ void var_finalize_kernel(const double* __restrict__ part, int n_part, int C, long long n_pix, float eps,
                                     float momentum, const float* __restrict__ mean, float* __restrict__ var,
                                     float* __restrict__ invstd, float* __restrict__ run_mean, float* __restrict__ run_var) {
@@ -251,9 +258,82 @@ __global__ void var_finalize_kernel(const double* __restrict__ part, int n_part,
   invstd[c] = (float)(1.0 / sqrt(v + (double)eps));
   if (run_mean) {
     const double unb = n_pix > 1 ? v * (double)n_pix / (double)(n_pix - 1) : v;
-    run_mean[c] = (1.f - momentum) * run_mean[c] + momentum * mean[c];
-    run_var[c] = (1.f - momentum) * run_var[c] + momentum * (float)unb;
+    running_update(run_mean, run_var, c, momentum, mean[c], (float)unb);
   }
+}
+
+// ---- SyncBatchNorm: per-rank fp64 records, merged in rank order (DESIGN.md 3.12)
+// A moments record is (4, C) fp64: rows n, S = sum x, Q = sum (x - m)^2, m = the fp32-rounded local mean.  Between the
+// two passes row 2 holds m as fp32 (the float the centred pass reads); the second finalize then overwrites it with Q.
+__global__ void moments_mean_kernel(const double* __restrict__ part, int n_part, int C, long long n_pix,
+                                    double* __restrict__ rec) {
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= C) return;
+  double t0, t1;
+  sum_parts(part, n_part, C, c, t0, t1);
+  const float m = (float)(t0 / (double)n_pix);                   // mean_finalize_kernel's value
+  rec[c] = (double)n_pix;
+  rec[C + c] = t0;
+  rec[3 * C + c] = (double)m;
+  reinterpret_cast<float*>(rec + 2 * C)[c] = m;
+}
+
+__global__ void moments_q_kernel(const double* __restrict__ part, int n_part, int C, double* __restrict__ rec) {
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= C) return;
+  double t0, t1;
+  sum_parts(part, n_part, C, c, t0, t1);
+  rec[2 * C + c] = t0;
+}
+
+// N = sum n_r, mu = sum S_r / N, M2 = sum_r Q_r - 2 d_r (S_r - n_r m_r) + n_r d_r^2 with d_r = mu - m_r (exact algebra:
+// sum (x - mu)^2 over rank r's rows, from its centred sum about m_r), in fp64 and rank order.  One record keeps d = 0:
+// the variance about the fp32 mean that stp3_bn_stats computes, bit for bit.  The outputs and the running statistics
+// are var_finalize_kernel's.
+__global__ void bn_merge_finalize_kernel(const double* __restrict__ rec, int world, int C, float eps, float momentum,
+                                         float* __restrict__ run_mean, float* __restrict__ run_var,
+                                         float* __restrict__ mean, float* __restrict__ var, float* __restrict__ invstd) {
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= C) return;
+  double n = 0.0, s = 0.0;
+  for (int r = 0; r < world; ++r) { n += rec[(4 * r) * C + c]; s += rec[(4 * r + 1) * C + c]; }
+  const double mu = s / n;
+  double m2 = 0.0;
+  for (int r = 0; r < world; ++r) {
+    const double nr = rec[(4 * r) * C + c], sr = rec[(4 * r + 1) * C + c], qr = rec[(4 * r + 2) * C + c];
+    const double mr = rec[(4 * r + 3) * C + c];
+    const double d = world == 1 ? 0.0 : mu - mr;
+    m2 += qr - 2.0 * d * (sr - nr * mr) + nr * d * d;
+  }
+  const float mf = (float)mu;
+  mean[c] = mf;
+  const double v = m2 / n;
+  if (var) var[c] = (float)v;
+  invstd[c] = (float)(1.0 / sqrt(v + (double)eps));
+  if (run_mean) {
+    const double unb = n > 1.0 ? v * n / (n - 1.0) : v;
+    running_update(run_mean, run_var, c, momentum, mf, (float)unb);
+  }
+}
+
+// backward record (2, C) fp64: sum g', sum g' xhat over this rank's rows
+__global__ void sums_record_kernel(const double* __restrict__ part, int n_part, int C, double* __restrict__ rec) {
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= C) return;
+  double t0, t1;
+  sum_parts(part, n_part, C, c, t0, t1);
+  rec[c] = t0;
+  rec[C + c] = t1;
+}
+
+__global__ void sums_merge_kernel(const double* __restrict__ rec, int world, int C, float* __restrict__ sum_g,
+                                  float* __restrict__ sum_gx) {
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= C) return;
+  double t0 = 0.0, t1 = 0.0;
+  for (int r = 0; r < world; ++r) { t0 += rec[(2 * r) * C + c]; t1 += rec[(2 * r + 1) * C + c]; }
+  sum_g[c] = (float)t0;
+  sum_gx[c] = (float)t1;
 }
 
 // grid.y = images: image i reads its own partials and writes sum_g[i * C + c]
@@ -356,19 +436,21 @@ bn_apply_kernel(const float* __restrict__ x, int x_cs, const float* __restrict__
   }
 }
 
-// dx = gamma * invstd * (g' - sum_g / n - xhat * sum_gx / n), g' = g masked by y > 0 when y is given; g' is also
-// written to gm (the gradient of the residual branch) when gm is given
+// dx = gamma * invstd * (g' - sum_g / n - xhat * sum_gx / n) over n_pix rows, n = n_norm (the rows the statistics and
+// sums cover: n_pix, or the process group's count under SyncBatchNorm), g' = g masked by y > 0 when y is given; g' is
+// also written to gm (the gradient of the residual branch) when gm is given
 __global__ void __launch_bounds__(256)
 bn_bwd_apply_kernel(const float* __restrict__ g, int g_cs, const float* __restrict__ y, int y_cs,
                     const float* __restrict__ x, int x_cs, const float* __restrict__ mean, const float* __restrict__ invstd,
                     const float* __restrict__ gamma, const float* __restrict__ sum_g, const float* __restrict__ sum_gx,
-                    long long n_pix, int C, float* __restrict__ dx, int dx_cs, float* __restrict__ gm, int gm_cs) {
+                    long long n_pix, long long n_norm, int C, float* __restrict__ dx, int dx_cs, float* __restrict__ gm,
+                    int gm_cs) {
   const int groups = C / 8;
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n_pix * groups) return;
   const int c0 = (int)(i % groups) * 8;
   const long long p = i / groups;
-  const float inv_n = 1.f / (float)n_pix;
+  const float inv_n = 1.f / (float)n_norm;
   float gv[8], xv[8], yv[8];
   auto ld8 = [&](const float* src, float* dst) {
     const float4 a = *reinterpret_cast<const float4*>(src), b = *reinterpret_cast<const float4*>(src + 4);
@@ -432,13 +514,13 @@ __global__ void __launch_bounds__(256)
 bn_bwd_apply_scalar_kernel(const float* __restrict__ g, int g_cs, const float* __restrict__ y, int y_cs,
                            const float* __restrict__ x, int x_cs, const float* __restrict__ mean,
                            const float* __restrict__ invstd, const float* __restrict__ gamma,
-                           const float* __restrict__ sum_g, const float* __restrict__ sum_gx, long long n_pix, int C,
-                           float* __restrict__ dx, int dx_cs, float* __restrict__ gm, int gm_cs) {
+                           const float* __restrict__ sum_g, const float* __restrict__ sum_gx, long long n_pix,
+                           long long n_norm, int C, float* __restrict__ dx, int dx_cs, float* __restrict__ gm, int gm_cs) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n_pix * C) return;
   const int c = (int)(i % C);
   const long long p = i / C;
-  const float inv_n = 1.f / (float)n_pix;
+  const float inv_n = 1.f / (float)n_norm;
   float gv = g[p * g_cs + c];
   if (y && !(y[p * y_cs + c] > 0.f)) gv = 0.f;
   const float xh = (x[p * x_cs + c] - mean[c]) * invstd[c];
@@ -783,10 +865,10 @@ extern "C" int stp3_image_channel_sums(const float* x, int n_img, long long hw, 
   return STP3_OK;
 }
 
-extern "C" int stp3_bn_bwd_apply(const float* g, int g_cstride, const float* y, int y_cstride, const float* x,
-                                 int x_cstride, const float* mean, const float* invstd, const float* gamma,
-                                 const float* sum_g, const float* sum_gxhat, long long n_pix, int C, float* dx,
-                                 int dx_cstride, float* g_masked, int gm_cstride, void* stream) {
+static int bn_bwd_apply_impl(const float* g, int g_cstride, const float* y, int y_cstride, const float* x,
+                             int x_cstride, const float* mean, const float* invstd, const float* gamma,
+                             const float* sum_g, const float* sum_gxhat, long long n_pix, long long n_norm, int C,
+                             float* dx, int dx_cstride, float* g_masked, int gm_cstride, void* stream) {
   STP3_CHECK_ARG(g && x && mean && invstd && gamma && sum_g && sum_gxhat && dx && n_pix > 0 && C > 0,
                  "stp3_bn_bwd_apply: bad argument");
   STP3_CHECK_ARG(C <= g_cstride && C <= x_cstride && C <= dx_cstride, "stp3_bn_bwd_apply: C exceeds a row stride");
@@ -797,17 +879,97 @@ extern "C" int stp3_bn_bwd_apply(const float* g, int g_cstride, const float* y, 
                    (!g_masked || (gm_cstride % 4 == 0 && al16(g_masked)));
   if (!vec) {
     bn_bwd_apply_scalar_kernel<<<blocks_for(n_pix * C), 256, 0, (cudaStream_t)stream>>>(
-        g, g_cstride, y, y_cstride, x, x_cstride, mean, invstd, gamma, sum_g, sum_gxhat, n_pix, C, dx, dx_cstride,
-        g_masked, gm_cstride);
+        g, g_cstride, y, y_cstride, x, x_cstride, mean, invstd, gamma, sum_g, sum_gxhat, n_pix, n_norm, C, dx,
+        dx_cstride, g_masked, gm_cstride);
     STP3_CUDA_OK(cudaGetLastError());
     return STP3_OK;
   }
   const long long total = n_pix * (C / 8);
   bn_bwd_apply_kernel<<<blocks_for(total), 256, 0, (cudaStream_t)stream>>>(
-      g, g_cstride, y, y_cstride, x, x_cstride, mean, invstd, gamma, sum_g, sum_gxhat, n_pix, C, dx, dx_cstride,
+      g, g_cstride, y, y_cstride, x, x_cstride, mean, invstd, gamma, sum_g, sum_gxhat, n_pix, n_norm, C, dx, dx_cstride,
       g_masked, gm_cstride);
   STP3_CUDA_OK(cudaGetLastError());
   return STP3_OK;
+}
+
+extern "C" int stp3_bn_bwd_apply(const float* g, int g_cstride, const float* y, int y_cstride, const float* x,
+                                 int x_cstride, const float* mean, const float* invstd, const float* gamma,
+                                 const float* sum_g, const float* sum_gxhat, long long n_pix, int C, float* dx,
+                                 int dx_cstride, float* g_masked, int gm_cstride, void* stream) {
+  return bn_bwd_apply_impl(g, g_cstride, y, y_cstride, x, x_cstride, mean, invstd, gamma, sum_g, sum_gxhat, n_pix, n_pix,
+                           C, dx, dx_cstride, g_masked, gm_cstride, stream);
+}
+
+// ------------------------------------------------------------------------------------------------ SyncBatchNorm
+extern "C" int stp3_bn_local_moments(const float* x, long long n_pix, int C, int x_cstride, double* out, void* scratch,
+                                     size_t scratch_bytes, void* stream) {
+  STP3_CHECK_ARG(x && out && scratch && n_pix > 0 && C > 0 && C <= x_cstride, "stp3_bn_local_moments: bad argument");
+  STP3_CHECK_ARG(scratch_bytes >= stp3_bn_scratch_bytes(n_pix, C),
+                 "stp3_bn_local_moments: scratch smaller than stp3_bn_scratch_bytes()");
+  cudaStream_t st = (cudaStream_t)stream;
+  const int parts = red_parts(n_pix);
+  double* part = (double*)scratch;
+  const dim3 grid(ceil_div(C, 32), parts), block(32, 8);
+  chan_partial_kernel<<<grid, block, 0, st>>>(0, x, x_cstride, nullptr, 0, nullptr, 0, nullptr, nullptr, n_pix, C, part);
+  STP3_CUDA_OK(cudaGetLastError());
+  moments_mean_kernel<<<ceil_div(C, 128), 128, 0, st>>>(part, parts, C, n_pix, out);
+  STP3_CUDA_OK(cudaGetLastError());
+  chan_partial_kernel<<<grid, block, 0, st>>>(1, x, x_cstride, nullptr, 0, nullptr, 0,
+                                              reinterpret_cast<const float*>(out + 2 * C), nullptr, n_pix, C, part);
+  STP3_CUDA_OK(cudaGetLastError());
+  moments_q_kernel<<<ceil_div(C, 128), 128, 0, st>>>(part, parts, C, out);
+  STP3_CUDA_OK(cudaGetLastError());
+  return STP3_OK;
+}
+
+extern "C" int stp3_bn_merge_finalize(const double* records, int world, int C, float eps, float momentum,
+                                      float* running_mean, float* running_var, float* mean, float* var, float* invstd,
+                                      void* stream) {
+  STP3_CHECK_ARG(records && mean && invstd && world > 0 && C > 0, "stp3_bn_merge_finalize: bad argument");
+  STP3_CHECK_ARG((running_mean == nullptr) == (running_var == nullptr),
+                 "stp3_bn_merge_finalize: give both running buffers or neither");
+  bn_merge_finalize_kernel<<<ceil_div(C, 128), 128, 0, (cudaStream_t)stream>>>(records, world, C, eps, momentum,
+                                                                               running_mean, running_var, mean, var,
+                                                                               invstd);
+  STP3_CUDA_OK(cudaGetLastError());
+  return STP3_OK;
+}
+
+extern "C" int stp3_bn_bwd_local_sums(const float* g, int g_cstride, const float* y, int y_cstride, const float* x,
+                                      int x_cstride, const float* mean, const float* invstd, long long n_pix, int C,
+                                      double* out, void* scratch, size_t scratch_bytes, void* stream) {
+  STP3_CHECK_ARG(g && x && mean && invstd && out && scratch && n_pix > 0 && C > 0 && C <= g_cstride && C <= x_cstride,
+                 "stp3_bn_bwd_local_sums: bad argument");
+  STP3_CHECK_ARG(!y || C <= y_cstride, "stp3_bn_bwd_local_sums: bad mask tensor");
+  STP3_CHECK_ARG(scratch_bytes >= stp3_bn_scratch_bytes(n_pix, C),
+                 "stp3_bn_bwd_local_sums: scratch smaller than stp3_bn_scratch_bytes()");
+  cudaStream_t st = (cudaStream_t)stream;
+  const int parts = red_parts(n_pix);
+  double* part = (double*)scratch;
+  chan_partial_kernel<<<dim3(ceil_div(C, 32), parts), dim3(32, 8), 0, st>>>(2, g, g_cstride, y, y_cstride, x, x_cstride,
+                                                                          mean, invstd, n_pix, C, part);
+  STP3_CUDA_OK(cudaGetLastError());
+  sums_record_kernel<<<ceil_div(C, 128), 128, 0, st>>>(part, parts, C, out);
+  STP3_CUDA_OK(cudaGetLastError());
+  return STP3_OK;
+}
+
+extern "C" int stp3_bn_bwd_merge_sums(const double* records, int world, int C, float* sum_g, float* sum_gxhat,
+                                      void* stream) {
+  STP3_CHECK_ARG(records && sum_g && sum_gxhat && world > 0 && C > 0, "stp3_bn_bwd_merge_sums: bad argument");
+  sums_merge_kernel<<<ceil_div(C, 128), 128, 0, (cudaStream_t)stream>>>(records, world, C, sum_g, sum_gxhat);
+  STP3_CUDA_OK(cudaGetLastError());
+  return STP3_OK;
+}
+
+extern "C" int stp3_bn_bwd_apply_global(const float* g, int g_cstride, const float* y, int y_cstride, const float* x,
+                                        int x_cstride, const float* mean, const float* invstd, const float* gamma,
+                                        const float* sum_g, const float* sum_gxhat, long long n_pix, long long n_total,
+                                        int C, float* dx, int dx_cstride, float* g_masked, int gm_cstride,
+                                        void* stream) {
+  STP3_CHECK_ARG(n_total >= n_pix, "stp3_bn_bwd_apply_global: n_total is smaller than n_pix");
+  return bn_bwd_apply_impl(g, g_cstride, y, y_cstride, x, x_cstride, mean, invstd, gamma, sum_g, sum_gxhat, n_pix,
+                           n_total, C, dx, dx_cstride, g_masked, gm_cstride, stream);
 }
 
 // 16-byte accesses when every row of the dense tensor and of the window starts 16-byte aligned; else one float per thread

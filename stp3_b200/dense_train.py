@@ -12,9 +12,10 @@ from dataclasses import dataclass
 from typing import List, Optional, Tuple
 
 import torch
+import torch.distributed as dist
 import torch.nn as nn
 
-from . import _lib, dense
+from . import _lib, dense, parallel
 
 
 def _p(t: Optional[torch.Tensor]):
@@ -239,11 +240,12 @@ def conv_wgrad(x: torch.Tensor, g: torch.Tensor, kh: int, kw: int, stride: int, 
 # ------------------------------------------------------------------------------------------------ BatchNorm
 def check_bn(bn: nn.Module, owner: str):
     """The train-mode kernels implement nn.BatchNorm2d / nn.BatchNorm3d (the TemporalBlocks') with running statistics
-    and a fixed momentum."""
+    and a fixed momentum, and nn.SyncBatchNorm (statistics over its process group) once torch.distributed is up."""
     if isinstance(bn, nn.SyncBatchNorm):
-        raise NotImplementedError(f"{owner}: SyncBatchNorm (sync_batchnorm=True / DDP) is not supported in train mode; "
-                                  "use plain BatchNorm2d / BatchNorm3d")
-    if not isinstance(bn, (nn.BatchNorm2d, nn.BatchNorm3d)):
+        if not (dist.is_available() and dist.is_initialized()):
+            raise NotImplementedError(f"{owner}: SyncBatchNorm (sync_batchnorm=True / DDP) needs torch.distributed: "
+                                      "init the process group before training, or use plain BatchNorm2d / BatchNorm3d")
+    elif not isinstance(bn, (nn.BatchNorm2d, nn.BatchNorm3d)):
         raise NotImplementedError(f"{owner}: expected nn.BatchNorm2d or nn.BatchNorm3d, got {type(bn).__name__}")
     if not bn.track_running_stats or bn.running_mean is None:
         raise NotImplementedError(f"{owner}: BatchNorm2d(track_running_stats=False) is not supported in train mode")
@@ -254,12 +256,45 @@ def check_bn(bn: nn.Module, owner: str):
         raise NotImplementedError(f"{owner}: BatchNorm2d(affine=False) is not supported in train mode")
 
 
+def bn_group(bn: nn.Module):
+    """The process group whose batch a SyncBatchNorm's statistics span (its process_group, None meaning WORLD), or
+    None: plain BatchNorm, or a group of one rank, whose statistics are the local ones bit for bit."""
+    if not isinstance(bn, nn.SyncBatchNorm) or not dist.is_initialized():
+        return None
+    group = bn.process_group if bn.process_group is not None else dist.group.WORLD
+    return group if dist.get_world_size(group) > 1 else None
+
+
+def sync_world(bn: nn.Module, n_local: int, owner: str) -> int:
+    """Ranks over which bn's batch statistics are taken (1: local statistics).  Under SyncBatchNorm every rank must hold
+    at least one image, so the group's batch is at least n_local * world when n_local >= 1: the batch-of-one checks
+    use that count, like torch's SyncBatchNorm."""
+    group = bn_group(bn)
+    if group is None:
+        return 1
+    if n_local < 1:
+        raise ValueError(f"{owner} (train mode, SyncBatchNorm): this rank holds no images; every rank of the process "
+                         "group must train on at least one")
+    return dist.get_world_size(group)
+
+
 @dataclass
 class BNStats:
     mean: torch.Tensor
     var: torch.Tensor          # biased
     invstd: torch.Tensor
-    n: int
+    n: int                     # rows of this rank
+    group: object = None       # SyncBatchNorm: the process group the statistics span
+    counts: Optional[torch.Tensor] = None      # its ranks' row counts, a pinned host copy made after the exchange ...
+    counts_ready: Optional[torch.cuda.Event] = None    # ... and the event that completes it
+
+    @property
+    def n_total(self) -> int:
+        """Rows over the process group: what the backward normalises its merged sums by."""
+        if self.group is None:
+            return self.n
+        self.counts_ready.synchronize()        # recorded in the forward: long done by the backward
+        return int(self.counts.sum().item())
 
 
 def _bn_scratch(n_pix: int, C: int, dev) -> Tuple[torch.Tensor, int]:
@@ -287,10 +322,41 @@ def bn_stats(x: torch.Tensor, eps: float, momentum: float, running_mean: Optiona
 
 
 def bn_stats_module(x: torch.Tensor, bn: nn.BatchNorm2d) -> BNStats:
-    """bn_stats with the module's own eps / momentum; updates its running_mean / running_var / num_batches_tracked."""
-    st = bn_stats(x, bn.eps, bn.momentum, bn.running_mean, bn.running_var)
+    """bn_stats with the module's own eps / momentum; updates its running_mean / running_var / num_batches_tracked.
+    A SyncBatchNorm over more than one rank takes the statistics of the group's batch: each rank's fp64 moments record
+    (stp3_bn_local_moments, into its row of the gather buffer), one all-gather, and the same merge on every rank
+    (stp3_bn_merge_finalize), so every rank gets the same statistics and running-statistic bits."""
+    group = bn_group(bn)
+    st = bn_stats(x, bn.eps, bn.momentum, bn.running_mean, bn.running_var) if group is None else \
+        _bn_stats_sync(x, bn, group)
     bn.num_batches_tracked.add_(1)
     return st
+
+
+def _bn_stats_sync(x: torch.Tensor, bn: nn.SyncBatchNorm, group) -> BNStats:
+    _f32_cl(x)
+    C = x.shape[-1]
+    n = x.numel() // C
+    dev = x.device
+    ws, rank = dist.get_world_size(group), dist.get_rank(group)
+    rec = torch.empty((ws, 4, C), dtype=torch.float64, device=dev)
+    mean, var, invstd = (torch.empty(C, dtype=torch.float32, device=dev) for _ in range(3))
+    scratch, nbytes = _bn_scratch(n, C, dev)
+    L = _lib.lib()
+    with torch.cuda.device(dev):
+        code = L.stp3_bn_local_moments(x.data_ptr(), n, C, C, rec[rank].data_ptr(), scratch.data_ptr(), nbytes,
+                                       _stream(dev))
+        _lib.check(code, "stp3_bn_local_moments")
+        parallel.all_gather_rows(rec, group)
+        code = L.stp3_bn_merge_finalize(rec.data_ptr(), ws, C, float(bn.eps), float(bn.momentum),
+                                        bn.running_mean.data_ptr(), bn.running_var.data_ptr(), mean.data_ptr(),
+                                        var.data_ptr(), invstd.data_ptr(), _stream(dev))
+        _lib.check(code, "stp3_bn_merge_finalize")
+        counts = torch.empty(ws, dtype=torch.float64, pin_memory=True)
+        counts.copy_(rec[:, 0, 0], non_blocking=True)
+        ready = torch.cuda.Event()
+        ready.record()
+    return BNStats(mean, var, invstd, n, group, counts, ready)
 
 
 def bn_apply(x: torch.Tensor, st: BNStats, gamma: torch.Tensor, beta: torch.Tensor, relu: bool,
@@ -355,6 +421,9 @@ def bn_backward(g: torch.Tensor, x: torch.Tensor, st: BNStats, gamma: torch.Tens
     dx_cs = _row_stride(dx)
     gam = gamma.detach().float().contiguous()
     L = _lib.lib()
+    if st.group is not None:
+        _bn_backward_sync(g, g_cs, y_mask, y_cs, x, x_cs, st, gam, sum_g, sum_gx, scratch, nbytes, dx, dx_cs, gm)
+        return dx, sum_gx, sum_g, gm
     with torch.cuda.device(dev):
         code = L.stp3_bn_bwd_reduce(g.data_ptr(), g_cs, _p(y_mask), y_cs, x.data_ptr(), x_cs, st.mean.data_ptr(),
                                     st.invstd.data_ptr(), n, C, sum_g.data_ptr(), sum_gx.data_ptr(), scratch.data_ptr(),
@@ -365,6 +434,30 @@ def bn_backward(g: torch.Tensor, x: torch.Tensor, st: BNStats, gamma: torch.Tens
                                    dx.data_ptr(), dx_cs, _p(gm), C, _stream(dev))
     _lib.check(code, "stp3_bn_bwd_apply")
     return dx, sum_gx, sum_g, gm
+
+
+def _bn_backward_sync(g, g_cs, y_mask, y_cs, x, x_cs, st: BNStats, gam, sum_g, sum_gx, scratch, nbytes, dx, dx_cs, gm):
+    """bn_backward of a SyncBatchNorm: sum_g / sum_gx (dbeta / dgamma) stay this rank's own sums, as torch's
+    SyncBatchNorm returns them (DDP averages them with every other gradient); dx uses the group's sums and row count."""
+    C, n, dev = x.shape[-1], st.n, x.device
+    ws, rank = dist.get_world_size(st.group), dist.get_rank(st.group)
+    rec = torch.empty((ws, 2, C), dtype=torch.float64, device=dev)
+    tot_g, tot_gx = (torch.empty(C, dtype=torch.float32, device=dev) for _ in range(2))
+    L = _lib.lib()
+    with torch.cuda.device(dev):
+        code = L.stp3_bn_bwd_local_sums(g.data_ptr(), g_cs, _p(y_mask), y_cs, x.data_ptr(), x_cs, st.mean.data_ptr(),
+                                        st.invstd.data_ptr(), n, C, rec[rank].data_ptr(), scratch.data_ptr(), nbytes,
+                                        _stream(dev))
+        _lib.check(code, "stp3_bn_bwd_local_sums")
+        code = L.stp3_bn_bwd_merge_sums(rec[rank].data_ptr(), 1, C, sum_g.data_ptr(), sum_gx.data_ptr(), _stream(dev))
+        _lib.check(code, "stp3_bn_bwd_merge_sums")
+        parallel.all_gather_rows(rec, st.group)
+        code = L.stp3_bn_bwd_merge_sums(rec.data_ptr(), ws, C, tot_g.data_ptr(), tot_gx.data_ptr(), _stream(dev))
+        _lib.check(code, "stp3_bn_bwd_merge_sums")
+        code = L.stp3_bn_bwd_apply_global(g.data_ptr(), g_cs, _p(y_mask), y_cs, x.data_ptr(), x_cs, st.mean.data_ptr(),
+                                          st.invstd.data_ptr(), gam.data_ptr(), tot_g.data_ptr(), tot_gx.data_ptr(), n,
+                                          st.n_total, C, dx.data_ptr(), dx_cs, _p(gm), C, _stream(dev))
+    _lib.check(code, "stp3_bn_bwd_apply_global")
 
 
 def image_channel_sums(x: torch.Tensor) -> torch.Tensor:

@@ -170,8 +170,9 @@ class DeepLabHead(nn.Sequential, PackedModule):
             raise RuntimeError("stp3_b200 dense ops run on CUDA tensors only (there is no CPU path)")
         if x.dim() != 4 or x.shape[1] != self.in_channels:
             raise ValueError(f"DeepLabHead: expected (N, {self.in_channels}, H, W), got {tuple(x.shape)}")
-        if x.shape[0] < 2:
-            # the pooling branch's BatchNorm sees one value per image and channel (nn.BatchNorm2d raises the same)
+        if x.shape[0] * dense_train.sync_world(self[0].convs[-1][2], x.shape[0], "DeepLabHead") < 2:
+            # the pooling branch's BatchNorm sees one value per image and channel (nn.BatchNorm2d raises the same);
+            # under SyncBatchNorm it sees the process group's images
             raise ValueError("DeepLabHead (train mode): Expected more than 1 value per channel when training, got input "
                              f"size {(x.shape[0], self.hidden, 1, 1)} in the ASPP pooling branch")
         return _DeepLabTrainFn.apply(self, x.float(), *self.parameters())
@@ -394,6 +395,7 @@ class UpsamplingConcat(PackedModule):
                 x.shape[0] != x_up.shape[0] or tuple(x.shape[2:]) != (2 * x_up.shape[2], 2 * x_up.shape[3]):
             raise ValueError(f"UpsamplingConcat: expected (N, Cc, h, w) and (N, {self.in_channels} - Cc, 2h, 2w), got "
                              f"{tuple(x_up.shape)} and {tuple(x.shape)}")
+        dense_train.sync_world(self.conv[1], x.shape[0], "UpsamplingConcat")
         return _UpsamplingConcatTrainFn.apply(self, x_up.float(), x.float(), channels_last, *self.parameters())
 
     def _train_forward(self, x_up: torch.Tensor, x: torch.Tensor, channels_last: bool):

@@ -180,6 +180,8 @@ class Decoder(PackedModule):
 
     def _forward_train(self, x: torch.Tensor):
         self._check_train()
+        bn = next(m for m in self.modules() if isinstance(m, nn.modules.batchnorm._BatchNorm))
+        dense_train.sync_world(bn, x.shape[0], "Decoder")
         x = x.float()
         params = [p for p in self.parameters()]
         keys = [k for k, _, _ in self._heads()]

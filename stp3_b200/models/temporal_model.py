@@ -84,9 +84,10 @@ class TemporalModel(nn.Module):
         if (0 if const is None else const.shape[-1]) != nc:
             raise ValueError(f"TemporalModel: the first block takes {nc} spatially constant channels (n_const), got "
                              f"const of shape {None if const is None else tuple(const.shape)}")
-        if B * S < 2:
+        if B * S * dense_train.sync_world(self.final_conv[0].convs[-1][2], B * S, "TemporalModel") < 2:
             # a deliberate refusal of the native path, not the reference's error: the head behind the blocks takes its
-            # ASPP pooling statistics over the B*S frames and would see one value per channel
+            # ASPP pooling statistics over the B*S frames (the process group's under SyncBatchNorm) and would see one
+            # value per channel
             raise ValueError("TemporalModel (train mode): B*S = 1 is not supported in train mode (the head's ASPP "
                              "pooling BatchNorm would see one value per channel); train on at least 2 frames")
         const = const.detach().float().reshape(B * S, nc).contiguous() if nc else None

@@ -4,6 +4,7 @@ Every sample is independent through lift-splat -> temporal model -> decoder (the
 stp3.py:265, and eval-mode BatchNorm has no cross-sample coupling), so ranks simply own disjoint slices of the global
 batch.  torch.distributed (NCCL on the GPUs, gloo in the CPU tests) is used for rendezvous, the barrier around timed
 regions, the max-over-ranks reduction of device times and, when a single consumer wants them, gathering the logits.
+Training under SyncBatchNorm adds one small all-gather per BatchNorm and direction (all_gather_rows).
 """
 from typing import Dict, Optional, Tuple
 
@@ -77,6 +78,14 @@ def all_gather_frames(local: torch.Tensor, n_frames: int) -> torch.Tensor:
     if all(c == cmax for c in counts):
         return gathered
     return torch.cat([gathered[r * cmax:r * cmax + c] for r, c in enumerate(counts)])
+
+
+def all_gather_rows(buf: torch.Tensor, group=None) -> torch.Tensor:
+    """buf (world, ...) with this rank's row written -> every rank's row, in rank order, in place (the list form of
+    all_gather: NCCL, and gloo's CUDA allgather).  The SyncBatchNorm records' exchange (dense_train.bn_stats_module)."""
+    rows = list(buf.unbind(0))
+    dist.all_gather(rows, rows[dist.get_rank(group)], group=group)
+    return buf
 
 
 class PeerFrameBuffer:
