@@ -49,6 +49,10 @@ TmapEncodeFn tmap_encode_fn();
 // of 64 channels x box_w x box_h pixels, every `estride`-th column and row
 CUresult encode_act_5d(CUtensorMap* m, const void* plane, int cstride, int W, int H, int T, int B, int box_w, int box_h,
                        int estride);
+// The channel window [0, n_ch) of a channels-last bf16 output plane (n_img, Ho, Wo, cstride) that starts at `plane`, as
+// a 4-D map with the same swizzle: box of 64 channels x box_w x box_h pixels.  A store through it writes neither the
+// channels beyond n_ch nor the pixels outside the map
+CUresult encode_out_4d(CUtensorMap* m, void* plane, int cstride, int n_ch, int Wo, int Ho, int n_img, int box_w, int box_h);
 // Packed weights, `rows` rows of 64 bf16, as a 2-D map with the same swizzle: box of box_rows rows
 CUresult encode_rows_2d(CUtensorMap* m, const void* w, long long rows, int box_rows);
 // multiprocessor count of the current device (cached per device and host thread)

@@ -51,6 +51,9 @@ static_assert(kProducerRegs + 2 * kMmaRegs + 2 * kEpiRegs <= 5 * kLaunchRegs, "s
 // 1..4 are the epilogue's column-half pairs): "full" (MMA arrive, epilogue sync) and "free" (the reverse)
 constexpr int kBarAccFull = 5, kBarAccFree = 6;
 constexpr int kHandoverThreads = (kMmaWarps + kEpiWarps) * 32;
+// the epilogue threads alone: every row of the staging tile is written, its TMA stores may start
+constexpr int kBarEpi = 7;
+constexpr int kEpiThreads = kEpiWarps * 32;
 constexpr int kSubH = 8, kTileW = 16;           // one tile = 8 x 16 pixels = 128 accumulator rows
 constexpr int kBK = 64;                         // channels per K step (one 128-byte swizzle row of bf16)
 constexpr int kMaxTaps = 49;
@@ -96,10 +99,11 @@ struct ConvParams {
   const __nv_bfloat16* res_hi;
   const __nv_bfloat16* res_lo;
   int res_cstride, res_coff;
-  __nv_bfloat16* out_hi;    // channels-last (n_img, Ho, Wo, out_cstride), may be null when out_f32 is used
-  __nv_bfloat16* out_lo;
-  int out_cstride, out_coff, n_store;
-  int vec256;               // bit 0: output rows / windows are 32-byte aligned (256-bit stores), bit 1: residual likewise
+  // hi/lo destinations (channels-last (n_img, Ho, Wo, cstride)) are written through the kernel's output tensor maps,
+  // which start at the destination's channel offset and end after its n_store channels
+  int out_hl;               // 0: no hi/lo output (out_f32 or a fused head only)
+  int n_store;              // channels of the primary destination
+  int vec256;               // bit 1: residual rows / windows are 32-byte aligned (256-bit loads)
   float* out_f32;           // optional (n_img, n_valid, Ho, Wo) fp32, the reference's NCHW layout
   int n_valid;
   int f32_nhwc;             // out_f32 is channels-last (n_img, Ho, Wo, n_valid): 16 channels of a pixel = two 32-byte stores
@@ -115,9 +119,7 @@ struct ConvParams {
   int head_sigmoid_mask;    // bit k: sigmoid on output k
   // second destination (BN = 128): output columns [64, 128) go to another tensor with their own activation flag -- two
   // 64-column convolutions that read the same input run as one launch and read it once
-  __nv_bfloat16* out2_hi;
-  __nv_bfloat16* out2_lo;
-  int out2_cstride, out2_coff, n_store2, relu2;
+  int out2, relu2;
   // per-image column sums of the activated output (the consumer's pooling branches need sum over H*W): every epilogue
   // warp keeps running sums of its pixels in registers and writes one partial row per (CTA, row quarter, image) --
   // plain stores, fixed order: deterministic.  BN = 64 only.  sum_part: [gridDim.x][4][n_img][BN], zeroed by the host.
@@ -132,15 +134,26 @@ struct ConvParams {
 // columns c and b_rows + c on their way to the shared accumulator tile, which has BN columns either way.
 template <int BN>
 struct ConvSmem {
-  static constexpr int kAccStride = BN + 4;                            // floats per row of the shared accumulator tile
   // the tail behind the operand rings (or the resident weights), byte offsets from its start
   static constexpr int bias = 0;                                       // fp32 [n_nblk * BN]: the blocks beyond the first
                                                                        // lie over the head weights (n_nblk > 1: no head)
   static constexpr int head = bias + BN * 4;                           // fp32 [kMaxHeadOut][BN] fused head weights
   static constexpr int hx = head + kMaxHeadOut * BN * 4;               // fp32 [kMaxHeadOut][128] head partials handed between column halves
   static constexpr int wb = hx + kMaxHeadOut * 128 * 4;                // fp32 [kEpiWarps][64] per-image bias slice of each epilogue warp
-  static constexpr int acc = wb + kEpiWarps * 64 * 4;                  // fp32 [128][kAccStride] accumulator tile
-  static constexpr int bars = acc + 128 * kAccStride * 4;              // A ring, B ring, resident-weights barrier
+  // fp32 [128][BN] accumulator tile, which the epilogue turns into the staging tile of the hi/lo output stores in
+  // place: [BN / 64 channel planes][hi, lo part][128 pixels][64 bf16], each part 128-byte swizzled like the TMA loads
+  // (1024-byte aligned: the tail starts on a 1024-byte boundary)
+  static constexpr int acc = (wb + kEpiWarps * 64 * 4 + 1023) / 1024 * 1024;
+  static constexpr int kStagePart = 128 * 128;                         // bytes of one (plane, part)
+  static constexpr int bars = acc + BN / 64 * 2 * kStagePart;          // A ring, B ring, resident-weights barrier
+  // Byte offset of accumulator (row, col).  Of the 16 columns of a chunk (col / 16), columns 0..7 lie in the hi part
+  // and 8..15 in the lo part, each 8 in the two 16-byte slots of the row that the chunk's 8 hi (lo) bf16 outputs take
+  // (slot s of row r at s ^ (r % 8)): the epilogue thread of a row overwrites exactly the accumulators it has read.
+  static __device__ __forceinline__ int acc_off(int row, int col) {
+    const int k = col & 15;
+    const int slot = ((col & 63) >> 4) * 2 + ((k >> 2) & 1);
+    return ((col >> 6) * 2 + (k >> 3)) * kStagePart + row * 128 + ((slot ^ (row & 7)) << 4) + (k & 3) * 4;
+  }
   static constexpr size_t tail_bytes() { return bars + (2 * kMaxAStages + 2 * kMaxBStages + 8) * 8; }
 };
 
@@ -154,14 +167,6 @@ __device__ __forceinline__ bool group_is_padding(const ConvParams& p, int grp, i
   const int xlo = ox0 * p.stride + p.tap[tap0][2];
   const int xhi = (ox0 + kTileW - 1) * p.stride + p.tap[tap0][2];
   return t < 0 || t >= p.T_total || yhi < 0 || ylo >= p.H || xhi < 0 || xlo >= p.W;
-}
-
-__device__ __forceinline__ void ld_acc16(const float* src, uint32_t (&r)[16]) {   // 16 consecutive fp32, 16-byte aligned
-#pragma unroll
-  for (int g = 0; g < 4; ++g) {
-    const uint4 v = *reinterpret_cast<const uint4*>(src + 4 * g);
-    r[4 * g] = v.x; r[4 * g + 1] = v.y; r[4 * g + 2] = v.z; r[4 * g + 3] = v.w;
-  }
 }
 
 // Persistent, warp-specialised implicit-GEMM convolution.
@@ -181,7 +186,9 @@ __device__ __forceinline__ void ld_acc16(const float* src, uint32_t (&r)[16]) { 
 template <int BN, bool STACK, bool FULLK>
 __global__ void __launch_bounds__(kConvThreads, 1)
 conv_igemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ CUtensorMap tm_a_lo,
-                  const __grid_constant__ CUtensorMap tm_w, const ConvParams p) {
+                  const __grid_constant__ CUtensorMap tm_w, const __grid_constant__ CUtensorMap tm_o_hi,
+                  const __grid_constant__ CUtensorMap tm_o_lo, const __grid_constant__ CUtensorMap tm_o2_hi,
+                  const __grid_constant__ CUtensorMap tm_o2_lo, const ConvParams p) {
   using S = ConvSmem<BN>;
   static_assert(!STACK || BN == 64, "stacked weight operand: BN = 64 only");
   constexpr int kAccRegs = (STACK ? 2 * BN : BN) / 2;   // accumulator registers per thread (64 rows x columns per warpgroup)
@@ -200,7 +207,7 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
   float* s_head = reinterpret_cast<float*>(tail + S::head);
   float* s_hx = reinterpret_cast<float*>(tail + S::hx);
   float* s_wb = reinterpret_cast<float*>(tail + S::wb);
-  float* s_acc = reinterpret_cast<float*>(tail + S::acc);
+  unsigned char* s_acc = tail + S::acc;
   uint64_t* bars = reinterpret_cast<uint64_t*>(tail + S::bars);
   Ring ra{bars, bars + kMaxAStages, p.na_stages};
   Ring rb{bars + 2 * kMaxAStages, bars + 2 * kMaxAStages + kMaxBStages, p.nb_stages};   // no slots: resident weights
@@ -220,6 +227,8 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
   ptx::griddep_launch_dependents();
   if (warp == kProducerWarp && lane == 0) {
     ptx::prefetch_tmap(&tm_a_hi); ptx::prefetch_tmap(&tm_a_lo); ptx::prefetch_tmap(&tm_w);
+    if (p.out_hl) { ptx::prefetch_tmap(&tm_o_hi); ptx::prefetch_tmap(&tm_o_lo); }
+    if (p.out2) { ptx::prefetch_tmap(&tm_o2_hi); ptx::prefetch_tmap(&tm_o2_lo); }
     ra.init(2); rb.init(2);
     ptx::mbar_init(bres_bar, 1);
     ptx::fence_mbar_init();
@@ -369,7 +378,7 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
             const int row = row0 + 8 * ((i >> 1) & 1);
             float2 v = make_float2(accr[i], accr[i + 1]);
             if constexpr (kLo > 0) { v.x += accr[i + kLo]; v.y += accr[i + 1 + kLo]; }
-            *reinterpret_cast<float2*>(s_acc + (size_t)row * S::kAccStride + col) = v;
+            *reinterpret_cast<float2*>(s_acc + S::acc_off(row, col)) = v;
           }
         }
       };
@@ -397,16 +406,16 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
     constexpr int kColsPerWarp = BN / 2;
     const int col0 = half * kColsPerWarp;
     const int r = q * 32 + lane;                 // row of the tile = output pixel
-    // destination of this warp's columns (the upper column half may belong to a second tensor)
-    const bool second = BN == 128 && half == 1 && p.out2_hi != nullptr;
-    __nv_bfloat16* const d_hi = second ? p.out2_hi : p.out_hi;
-    __nv_bfloat16* const d_lo = second ? p.out2_lo : p.out_lo;
-    const int d_cstride = second ? p.out2_cstride : p.out_cstride;
-    const int d_coff = second ? p.out2_coff - 64 : p.out_coff;          // d_coff + column = channel in the destination
-    const int d_nstore = second ? 64 + p.n_store2 : p.n_store;
+    // activation of this warp's columns (the upper column half may belong to a second tensor)
+    const bool second = BN == 128 && half == 1 && p.out2;
     const bool d_relu = (second ? p.relu2 : p.relu) != 0;
     const bool d_swish = !second && p.swish != 0;
-    const bool d_vec = ((p.vec256 >> (second ? 2 : 0)) & 1) != 0;
+    const bool store_hl = p.out_hl != 0;
+    // the hi/lo outputs leave through the staging tile (the accumulator tile, overwritten chunk by chunk): one thread
+    // stores the tile's box of each plane part with TMA (pixels outside the map and channels outside the destination's
+    // window are clipped by the tensor maps) and waits until the stores have read the tile before it releases the
+    // accumulator tile to the MMA warpgroups
+    const bool store_issuer = e == 0 && lane == 0;
     constexpr bool kSums = BN == 64;              // column sums need kColsPerWarp (= 32) accumulators per thread
     float sacc[kSums ? 32 : 1];
 #pragma unroll
@@ -433,7 +442,9 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
     };
     ptx::griddep_wait();                          // residual / per-image bias reads and every global write come after
     for (int item = cta; item < n_items; item += n_cta) {
-      ptx::bar_arrive(kBarAccFree, kHandoverThreads);   // done with the previous item's accumulators (if any)
+      // done with the previous item's accumulators (if any), and the TMA stores with its staging tile
+      if (store_issuer) ptx::bulk_wait_read0();
+      ptx::bar_arrive(kBarAccFree, kHandoverThreads);
       const int tile = item / p.n_nblk;
       const int cblk = (item % p.n_nblk) * BN;          // first column of this item's block in the whole convolution
       const int img = tile / tiles_per_img, rem = tile % tiles_per_img;
@@ -444,7 +455,7 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
       }
       // latency hiding: the residual of the first chunk and this warp's slice of the per-image bias are requested
       // before waiting for the accumulator; every later residual chunk as soon as the previous one has been added
-      uint32_t nh[8], nl[8];
+      uint32_t nh[8] = {}, nl[8] = {};          // stay zero for pixels outside the map
       auto request_residual = [&](int j) {
         const int oy = oy_t + (r >> 4);
         if (oy < p.Ho && ox < p.Wo) {
@@ -484,65 +495,65 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
         float hacc[kMaxHeadOut];
 #pragma unroll
         for (int k = 0; k < kMaxHeadOut; ++k) hacc[k] = 0.f;
-        const float* acc_row = s_acc + (size_t)r * S::kAccStride + col0;
 #pragma unroll 1
         for (int j = 0; j < kColsPerWarp / 16; ++j) {
           const int cb = col0 + j * 16;              // first column of this chunk in the block,
           const int cg = cblk + cb;                  // in the convolution
+          // the chunk's four 16-byte slots of this row: hi part columns 0..3, 4..7, lo part columns 8..11, 12..15
+          uint4* const s_hi0 = reinterpret_cast<uint4*>(s_acc + S::acc_off(r, cb));
+          uint4* const s_hi1 = reinterpret_cast<uint4*>(s_acc + S::acc_off(r, cb + 4));
+          uint4* const s_lo0 = reinterpret_cast<uint4*>(s_acc + S::acc_off(r, cb + 8));
+          uint4* const s_lo1 = reinterpret_cast<uint4*>(s_acc + S::acc_off(r, cb + 12));
           uint32_t acc[16];
           const bool computed = cb < p.n_mma;        // columns beyond n_mma: zero weights, never multiplied
           if (computed) {
-            ld_acc16(acc_row + j * 16, acc);
+            const uint4 a0 = *s_hi0, a1 = *s_hi1, a2 = *s_lo0, a3 = *s_lo1;
+            acc[0] = a0.x; acc[1] = a0.y; acc[2] = a0.z; acc[3] = a0.w;
+            acc[4] = a1.x; acc[5] = a1.y; acc[6] = a1.z; acc[7] = a1.w;
+            acc[8] = a2.x; acc[9] = a2.y; acc[10] = a2.z; acc[11] = a2.w;
+            acc[12] = a3.x; acc[13] = a3.y; acc[14] = a3.z; acc[15] = a3.w;
           } else {
 #pragma unroll
             for (int i = 0; i < 16; ++i) acc[i] = 0u;
           }
+          // every row, pixels outside the map too: the hi/lo stores clip them
+          float v[16];
+#pragma unroll
+          for (int g = 0; g < 4; ++g) {            // bias: per-image slice (conv bias already folded in) or the conv's own
+            const float4 b4 = *reinterpret_cast<const float4*>(bsrc + cb + 4 * g);
+            v[4 * g + 0] = __uint_as_float(acc[4 * g + 0]) + b4.x;
+            v[4 * g + 1] = __uint_as_float(acc[4 * g + 1]) + b4.y;
+            v[4 * g + 2] = __uint_as_float(acc[4 * g + 2]) + b4.z;
+            v[4 * g + 3] = __uint_as_float(acc[4 * g + 3]) + b4.w;
+          }
+          if (p.res_mode) {
+#pragma unroll
+            for (int e2 = 0; e2 < 8; ++e2) {
+              const float2 r = ptx::join_hilo(nh[e2], nl[e2]);
+              float& a0 = v[e2 * 2], &a1 = v[e2 * 2 + 1];
+              if (p.res_mode == 1) { a0 += r.x; a1 += r.y; if (d_relu) { a0 = fmaxf(a0, 0.f); a1 = fmaxf(a1, 0.f); } }
+              else { if (d_relu) { a0 = fmaxf(a0, 0.f); a1 = fmaxf(a1, 0.f); } a0 += r.x; a1 += r.y; }
+            }
+            // the next chunk's residual is in flight while this chunk is finished (one buffer of residual registers)
+            if (j + 1 < kColsPerWarp / 16) request_residual(j + 1);
+          } else if (d_relu) {
+#pragma unroll
+            for (int i = 0; i < 16; ++i) v[i] = fmaxf(v[i], 0.f);
+          }
+          if (d_swish) {                           // after a res_mode 1 residual, like ReLU; swish launches take no res_mode 2
+#pragma unroll
+            for (int i = 0; i < 16; ++i) v[i] = v[i] / (1.f + __expf(-v[i]));
+          }
+          if (store_hl) {
+            uint32_t hw[8], lw[8];
+#pragma unroll
+            for (int e2 = 0; e2 < 8; ++e2) ptx::split_hilo(v[e2 * 2], v[e2 * 2 + 1], hw[e2], lw[e2]);
+            *s_hi0 = make_uint4(hw[0], hw[1], hw[2], hw[3]);
+            *s_hi1 = make_uint4(hw[4], hw[5], hw[6], hw[7]);
+            *s_lo0 = make_uint4(lw[0], lw[1], lw[2], lw[3]);
+            *s_lo1 = make_uint4(lw[4], lw[5], lw[6], lw[7]);
+          }
           if (valid) {
-            float v[16];
-#pragma unroll
-            for (int g = 0; g < 4; ++g) {          // bias: per-image slice (conv bias already folded in) or the conv's own
-              const float4 b4 = *reinterpret_cast<const float4*>(bsrc + cb + 4 * g);
-              v[4 * g + 0] = __uint_as_float(acc[4 * g + 0]) + b4.x;
-              v[4 * g + 1] = __uint_as_float(acc[4 * g + 1]) + b4.y;
-              v[4 * g + 2] = __uint_as_float(acc[4 * g + 2]) + b4.z;
-              v[4 * g + 3] = __uint_as_float(acc[4 * g + 3]) + b4.w;
-            }
-            if (p.res_mode) {
-#pragma unroll
-              for (int e2 = 0; e2 < 8; ++e2) {
-                const float2 r = ptx::join_hilo(nh[e2], nl[e2]);
-                float& a0 = v[e2 * 2], &a1 = v[e2 * 2 + 1];
-                if (p.res_mode == 1) { a0 += r.x; a1 += r.y; if (d_relu) { a0 = fmaxf(a0, 0.f); a1 = fmaxf(a1, 0.f); } }
-                else { if (d_relu) { a0 = fmaxf(a0, 0.f); a1 = fmaxf(a1, 0.f); } a0 += r.x; a1 += r.y; }
-              }
-              // the next chunk's residual is in flight while this chunk is stored (one buffer of residual registers)
-              if (j + 1 < kColsPerWarp / 16) request_residual(j + 1);
-            } else if (d_relu) {
-#pragma unroll
-              for (int i = 0; i < 16; ++i) v[i] = fmaxf(v[i], 0.f);
-            }
-            if (d_swish) {                         // after a res_mode 1 residual, like ReLU; swish launches take no res_mode 2
-#pragma unroll
-              for (int i = 0; i < 16; ++i) v[i] = v[i] / (1.f + __expf(-v[i]));
-            }
-            if (d_hi && cg < d_nstore) {
-              __nv_bfloat16* ohp = d_hi + pix * d_cstride + d_coff + cg;
-              __nv_bfloat16* olp = d_lo + pix * d_cstride + d_coff + cg;
-              uint32_t hw[8], lw[8];
-#pragma unroll
-              for (int e2 = 0; e2 < 8; ++e2) ptx::split_hilo(v[e2 * 2], v[e2 * 2 + 1], hw[e2], lw[e2]);
-              if (d_vec && cg + 16 <= d_nstore) {               // one full 32-byte sector per plane and lane
-                ptx::st_global_v8(ohp, hw);
-                ptx::st_global_v8(olp, lw);
-              } else {
-                reinterpret_cast<uint4*>(ohp)[0] = make_uint4(hw[0], hw[1], hw[2], hw[3]);
-                reinterpret_cast<uint4*>(olp)[0] = make_uint4(lw[0], lw[1], lw[2], lw[3]);
-                if (cg + 8 < d_nstore) {
-                  reinterpret_cast<uint4*>(ohp)[1] = make_uint4(hw[4], hw[5], hw[6], hw[7]);
-                  reinterpret_cast<uint4*>(olp)[1] = make_uint4(lw[4], lw[5], lw[6], lw[7]);
-                }
-              }
-            }
             if (p.out_f32 && p.f32_nhwc) {
               const int c0 = cg;
               float* dst = p.out_f32 + pix * p.n_valid + c0;
@@ -590,6 +601,25 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
             }
           }
         }
+        if (store_hl) {
+          ptx::fence_proxy_async();                 // the generic-proxy writes are visible to the TMA stores
+          ptx::bar_sync(kBarEpi, kEpiThreads);      // every row of the staging tile is written
+          if (store_issuer) {
+            const int ox0 = (rem % p.tiles_x) * kTileW;
+#pragma unroll
+            for (int pl = 0; pl < BN / 64; ++pl) {
+              const uint32_t src = ptx::smem_u32(s_acc + pl * 2 * S::kStagePart);
+              if (BN == 128 && pl == 1 && p.out2) {
+                ptx::tma_store_4d(&tm_o2_hi, src, 0, ox0, oy_t, img);
+                ptx::tma_store_4d(&tm_o2_lo, src + S::kStagePart, 0, ox0, oy_t, img);
+              } else if (cblk + pl * 64 < p.n_store) {
+                ptx::tma_store_4d(&tm_o_hi, src, cblk + pl * 64, ox0, oy_t, img);
+                ptx::tma_store_4d(&tm_o_lo, src + S::kStagePart, cblk + pl * 64, ox0, oy_t, img);
+              }
+            }
+            ptx::bulk_commit();
+          }
+        }
         if (p.head_ko) {
           // the two column halves of a pixel live in two warps of the same lane quarter: the upper half hands its
           // partial dot products over through shared memory (named barrier of the 64 threads involved)
@@ -613,6 +643,7 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
       }
     }
     if (kSums && p.sum_part && sum_img >= 0) flush_sums(sum_img);
+    if (store_issuer) ptx::bulk_wait0();            // the staging tile is read and the last tile's outputs are written
   }
 }
 
@@ -652,10 +683,11 @@ int launch_col_sum_reduce(const float* part, int n_part, int n_img, float* out, 
 
 template <int BN, bool STACK, bool FULLK>
 static int launch_conv(const ConvParams& p, const CUtensorMap& tm_hi, const CUtensorMap& tm_lo, const CUtensorMap& tm_w,
-                       size_t smem_bytes, unsigned grid, cudaStream_t stream) {
+                       const CUtensorMap (&tm_o)[4], size_t smem_bytes, unsigned grid, cudaStream_t stream) {
   constexpr auto kern = conv_igemm_kernel<BN, STACK, FULLK>;
   STP3_CUDA_OK(set_max_dynamic_smem<kern>((int)kSmemCap));
-  STP3_CUDA_OK(launch_pdl(kPdlConv, kern, dim3(grid), dim3(kConvThreads), smem_bytes, stream, tm_hi, tm_lo, tm_w, p));
+  STP3_CUDA_OK(launch_pdl(kPdlConv, kern, dim3(grid), dim3(kConvThreads), smem_bytes, stream, tm_hi, tm_lo, tm_w,
+                          tm_o[0], tm_o[1], tm_o[2], tm_o[3], p));
   return STP3_OK;
 }
 
@@ -841,17 +873,38 @@ extern "C" int stp3_conv_fwd(const stp3_conv_desc* d, const void* x_hi, const vo
   p.swish = d->swish; p.w_img_rows = d->w_img_stride / 64;
   p.res_hi = static_cast<const __nv_bfloat16*>(res_hi); p.res_lo = static_cast<const __nv_bfloat16*>(res_lo);
   p.res_cstride = d->res_cstride; p.res_coff = d->res_coff;
-  p.out_hi = static_cast<__nv_bfloat16*>(y_hi); p.out_lo = static_cast<__nv_bfloat16*>(y_lo);
-  p.out_cstride = d->out_cstride; p.out_coff = d->out_coff; p.n_store = n_store;
-  p.out2_hi = static_cast<__nv_bfloat16*>(d->y2_hi); p.out2_lo = static_cast<__nv_bfloat16*>(d->y2_lo);
-  p.out2_cstride = d->out2_cstride; p.out2_coff = d->out2_coff; p.relu2 = d->relu2;
-  p.n_store2 = d->n_store2 > 0 ? d->n_store2 : 64;
+  p.out_hl = y_hi != nullptr; p.n_store = n_store;
+  p.out2 = d->y2_hi != nullptr; p.relu2 = d->relu2;
+  const int n_store2 = d->n_store2 > 0 ? d->n_store2 : 64;
   if (d->y2_hi) {
     STP3_CHECK_ARG(d->bn == 128 && d->y2_lo && y_hi && !d->res_mode && !head && !y_f32 && !d->col_sums,
                    "second destination: 128-column convolutions with plain hi/lo outputs only");
-    STP3_CHECK_ARG(n_store <= 64 && p.n_store2 % 8 == 0 && p.n_store2 <= 64 && d->out2_cstride % 8 == 0 &&
-                   d->out2_coff % 8 == 0 && d->out2_coff + p.n_store2 <= d->out2_cstride,
+    STP3_CHECK_ARG(n_store <= 64 && n_store2 % 8 == 0 && n_store2 <= 64 && d->out2_cstride % 8 == 0 &&
+                   d->out2_coff % 8 == 0 && d->out2_coff + n_store2 <= d->out2_cstride,
                    "second destination: channel window does not fit");
+  }
+  // output maps: primary hi, lo, second destination hi, lo.  Each starts at its destination's channel offset and
+  // spans its stored channels, so a tile's TMA store writes nothing outside that window
+  CUtensorMap tm_o[4] = {};
+  {
+    auto al16 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; };
+    auto enc = [&](CUtensorMap* m, void* plane, int cstride, int coff, int n_ch) {
+      return encode_out_4d(m, static_cast<__nv_bfloat16*>(plane) + coff, cstride, n_ch, d->Wo, d->Ho, p.n_img, kTileW, kSubH);
+    };
+    if (y_hi) {
+      STP3_CHECK_ARG(al16(y_hi) && al16(y_lo), "hi/lo output planes must be 16-byte aligned");
+      const CUresult r1 = enc(&tm_o[0], y_hi, d->out_cstride, d->out_coff, n_store);
+      const CUresult r2 = enc(&tm_o[1], y_lo, d->out_cstride, d->out_coff, n_store);
+      if (r1 != CUDA_SUCCESS || r2 != CUDA_SUCCESS)
+        return set_error(STP3_ECUDA, "cuTensorMapEncodeTiled(output) failed: %d %d", (int)r1, (int)r2);
+    }
+    if (d->y2_hi) {
+      STP3_CHECK_ARG(al16(d->y2_hi) && al16(d->y2_lo), "second destination planes must be 16-byte aligned");
+      const CUresult r1 = enc(&tm_o[2], d->y2_hi, d->out2_cstride, d->out2_coff, n_store2);
+      const CUresult r2 = enc(&tm_o[3], d->y2_lo, d->out2_cstride, d->out2_coff, n_store2);
+      if (r1 != CUDA_SUCCESS || r2 != CUDA_SUCCESS)
+        return set_error(STP3_ECUDA, "cuTensorMapEncodeTiled(second output) failed: %d %d", (int)r1, (int)r2);
+    }
   }
   p.out_f32 = y_f32; p.n_valid = d->n_valid; p.sigmoid = d->sigmoid;
   p.f32_nhwc = d->f32_layout;
@@ -875,19 +928,17 @@ extern "C" int stp3_conv_fwd(const stp3_conv_desc* d, const void* x_hi, const vo
   }
   // every column block starts a multiple of 64 channels further: one alignment answer for all of them
   auto al32 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 31) == 0; };
-  p.vec256 = (y_hi && d->out_cstride % 16 == 0 && d->out_coff % 16 == 0 && al32(y_hi) && al32(y_lo) ? 1 : 0) |
-             (d->res_mode && d->res_cstride % 16 == 0 && d->res_coff % 16 == 0 && al32(res_hi) && al32(res_lo) ? 2 : 0) |
-             (d->y2_hi && d->out2_cstride % 16 == 0 && d->out2_coff % 16 == 0 && al32(d->y2_hi) && al32(d->y2_lo) ? 4 : 0);
+  p.vec256 = d->res_mode && d->res_cstride % 16 == 0 && d->res_coff % 16 == 0 && al32(res_hi) && al32(res_lo) ? 2 : 0;
   int rc;
   if (t.bn_blk == 64 && t.stack)
-    rc = t.full_k ? launch_conv<64, true, true>(p, tm_hi, tm_lo, tm_w, t.smem_bytes, t.grid, stream)
-                  : launch_conv<64, true, false>(p, tm_hi, tm_lo, tm_w, t.smem_bytes, t.grid, stream);
+    rc = t.full_k ? launch_conv<64, true, true>(p, tm_hi, tm_lo, tm_w, tm_o, t.smem_bytes, t.grid, stream)
+                  : launch_conv<64, true, false>(p, tm_hi, tm_lo, tm_w, tm_o, t.smem_bytes, t.grid, stream);
   else if (t.bn_blk == 64)
-    rc = t.full_k ? launch_conv<64, false, true>(p, tm_hi, tm_lo, tm_w, t.smem_bytes, t.grid, stream)
-                  : launch_conv<64, false, false>(p, tm_hi, tm_lo, tm_w, t.smem_bytes, t.grid, stream);
+    rc = t.full_k ? launch_conv<64, false, true>(p, tm_hi, tm_lo, tm_w, tm_o, t.smem_bytes, t.grid, stream)
+                  : launch_conv<64, false, false>(p, tm_hi, tm_lo, tm_w, tm_o, t.smem_bytes, t.grid, stream);
   else
-    rc = t.full_k ? launch_conv<128, false, true>(p, tm_hi, tm_lo, tm_w, t.smem_bytes, t.grid, stream)
-                  : launch_conv<128, false, false>(p, tm_hi, tm_lo, tm_w, t.smem_bytes, t.grid, stream);
+    rc = t.full_k ? launch_conv<128, false, true>(p, tm_hi, tm_lo, tm_w, tm_o, t.smem_bytes, t.grid, stream)
+                  : launch_conv<128, false, false>(p, tm_hi, tm_lo, tm_w, tm_o, t.smem_bytes, t.grid, stream);
   if (rc) return rc;
   STP3_CUDA_OK(cudaGetLastError());
   if (p.sum_part) {

@@ -31,6 +31,17 @@ CUresult encode_act_5d(CUtensorMap* m, const void* plane, int cstride, int W, in
              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
 }
 
+CUresult encode_out_4d(CUtensorMap* m, void* plane, int cstride, int n_ch, int Wo, int Ho, int n_img, int box_w, int box_h) {
+  const TmapEncodeFn enc = tmap_encode_fn();
+  if (!enc) return CUDA_ERROR_NOT_FOUND;
+  const cuuint64_t dims[4] = {(cuuint64_t)n_ch, (cuuint64_t)Wo, (cuuint64_t)Ho, (cuuint64_t)n_img};
+  const cuuint64_t strides[3] = {(cuuint64_t)cstride * 2, (cuuint64_t)Wo * cstride * 2, (cuuint64_t)Ho * Wo * cstride * 2};
+  const cuuint32_t box[4] = {64, (cuuint32_t)box_w, (cuuint32_t)box_h, 1};
+  const cuuint32_t es[4] = {1, 1, 1, 1};
+  return enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, plane, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
+             CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+}
+
 CUresult encode_rows_2d(CUtensorMap* m, const void* w, long long rows, int box_rows) {
   const TmapEncodeFn enc = tmap_encode_fn();
   if (!enc) return CUDA_ERROR_NOT_FOUND;

@@ -136,6 +136,19 @@ __device__ __forceinline__ void tma_load_5d(void* dst, const CUtensorMap* m, uin
       : "memory");
 }
 
+// shared::cta -> global tensor store of one box (4-D map), tracked by the issuing thread's bulk groups.  Elements of
+// the box outside the map's bounds are not written.
+__device__ __forceinline__ void tma_store_4d(const CUtensorMap* m, uint32_t src, int c0, int c1, int c2, int c3) {
+  asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];" ::"l"(m),
+               "r"(src), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
+               : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// every bulk group of this thread has finished reading its shared-memory source (the buffer may be overwritten)
+__device__ __forceinline__ void bulk_wait_read0() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+// every bulk group of this thread has completed, its global writes included
+__device__ __forceinline__ void bulk_wait0() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
+
 // warpgroup register reallocation (every warp of the warpgroup executes it): lower / raise this warpgroup's per-thread
 // register count to N
 template <int N>

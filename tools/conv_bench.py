@@ -3,7 +3,8 @@ builds the model): the temporal model's and the decoder's calls of one eval forw
 heads' calls first.  Each recorded call is replayed alone under the tiling the autotuner chose for it, as a CUDA graph,
 with L2 flushed before every repetition.  Per layer: taps x Cin -> Cout, output map, tiles, microseconds and the
 tensor-bound fraction (3 bf16 products per MAC at the data-sheet rate, scaled to the SM clock sampled during the
-timed loop).
+timed loop), and the HBM traffic the call cannot avoid (input window read once, every output stored once) over its
+time.
 
     python tools/conv_bench.py [--heads] [--reps 100] [--blocks 128|64s|64p] [--save DIR | --compare DIR] [--lib PATH]
     python tools/conv_bench.py --count-only [--sms 132]     # host counts of the decoder's 25x25 / 50x50 layers, no GPU
@@ -154,8 +155,21 @@ def layer_info(a, k):
     n_img = B * T
     cin = (pc.k_hi - pc.k_lo) if pc.k_hi else pc.cin_p
     macs = n_img * Ho * Wo * len(pc.taps) * cin * pc.cout
+    # bytes: hi + lo bf16 (4 B) per channel of the input frames the taps reach and of every stored output channel
+    frames_in = min(x.hi.shape[1], T + max(0, -min(t[0] for t in pc.taps)))
+    stored = 0
+    if k.get("store", True) and (k.get("out") is not None or k.get("out_f32") is None and k.get("head") is None):
+        stored += 4 * (k.get("n_store") or pc.bn)
+    if k.get("out2") is not None:
+        stored += 4 * (k.get("n_store2") or 64)
+    if k.get("out_f32") is not None:
+        stored += 4 * k["n_valid"]
+    if k.get("head") is not None:
+        stored += 4 * len(k["head"]["outs"])
+    nbytes = B * frames_in * H * W * pc.cin_p * 4 + n_img * Ho * Wo * stored
     return {"layer": f"{len(pc.taps)}x{cin}->{pc.cout}" + (f" s{pc.stride}" if pc.stride > 1 else ""),
-            "map": f"{n_img}x{Ho}x{Wo}", "tiles": n_img * -(-Ho // 8) * -(-Wo // 16), "flop": 3 * 2 * macs}
+            "map": f"{n_img}x{Ho}x{Wo}", "tiles": n_img * -(-Ho // 8) * -(-Wo // 16), "flop": 3 * 2 * macs,
+            "bytes": nbytes}
 
 
 def time_calls(calls, reps, dev):
@@ -224,7 +238,7 @@ def main():
     for i, ((a, k, tiling, dig), t) in enumerate(zip(calls, us)):
         info = layer_info(a, k)
         bound_us = info["flop"] / (FLOP_PER_CLK_SM * n_sm * mhz * 1e6) * 1e6 if mhz else None
-        row = dict(i=i, **info, tiling=tiling, us=round(t, 2),
+        row = dict(i=i, **info, tiling=tiling, us=round(t, 2), gb_per_s=round(info["bytes"] / (t * 1e3), 1),
                    tensor_bound_fraction=round(bound_us / t, 3) if bound_us else None)
         if ref:
             r = ref["calls"][i]
