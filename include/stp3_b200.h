@@ -271,6 +271,22 @@ int stp3_conv_fwd(const stp3_conv_desc* desc, const void* x_hi, const void* x_lo
                   const float* img_bias, const void* res_hi, const void* res_lo, void* y_hi, void* y_lo,
                   float* y_f32, const stp3_conv_head* head /* may be NULL */, void* stream);
 
+/* Operand kinds of the train-mode convolutions.  HILO: fp32 carried as bf16 hi/lo planes, three MMAs per product (what
+ * stp3_conv_fwd, stp3_conv_wgrad and stp3_conv3d_wgrad do).  BF16 / F16: ONE 16-bit plane per operand and one MMA per
+ * product, fp32 accumulation -- the convolutions of a training step under torch.autocast(dtype=torch.bfloat16 /
+ * torch.float16).  Every fp32 -> 16-bit conversion of this library rounds to nearest even, overflows to +-inf and
+ * passes NaN through; nothing saturates, so a loss scaler sees an overflowed gradient as inf / NaN. */
+#define STP3_OPERAND_HILO 0
+#define STP3_OPERAND_BF16 1
+#define STP3_OPERAND_F16 2
+/* stp3_conv_fwd with one-plane operands (operand BF16 or F16): x (B, T_total, H, W, in_cstride) is one plane of that
+ * kind (padding channels zero) and w is [ntaps][cin/64][bn][64] of the same kind (one plane instead of two per K block).
+ * Each K step issues one MMA; the stacked operand (tune_group +8) does not apply and is ignored.  Output: y_f32 only
+ * (required), with n_valid / f32_layout / sigmoid and the optional img_bias as in stp3_conv_fwd.  The descriptor rules
+ * of stp3_conv_fwd hold, and it must carry no residual, second destination, col_sums, swish or per-image weights. */
+int stp3_conv_fwd_plane(const stp3_conv_desc* desc, int operand, const void* x, const void* w, const float* bias,
+                        const float* img_bias, float* y_f32, void* stream);
+
 /* ---------------------------------------------------------------------------------------------------------
  * ASPP branches + projection of a DeepLabHead as ONE back-to-back tensor-core kernel (stp3/layers/convolutions.py:242-270):
  *   y = relu(BN(project.0(cat_b relu(BN(conv_b(x))))))   for the spatial branches b (1x1 and the dilated 3x3s); the
@@ -341,6 +357,10 @@ int stp3_block_fused_fwd(const stp3_block_desc* desc, const void* mid_hi, const 
  * Used where a foreign fp32 tensor enters a drop-in module (e.g. TemporalModel.forward, temporal_model.py:50). */
 int stp3_f32_to_hilo(const float* x, int channels_last, int n_img, int C, int H, int W, int cp, void* hi, void* lo,
                      void* stream);
+/* The one-plane counterpart: fp32 -> ONE plane (n_img,H,W,cp) of kind `operand` (STP3_OPERAND_BF16 or _F16), rounded
+ * to nearest even (overflow to +-inf, NaN passes through), padding channels 0.  Same layouts and limits. */
+int stp3_f32_to_plane(const float* x, int channels_last, int n_img, int C, int H, int W, int cp, int operand, void* out,
+                      void* stream);
 /* hi/lo (n_img,H,W,cstride) channels [c_off, c_off+C) -> fp32 (n_img,C,H,W): module outputs in the reference layout */
 int stp3_hilo_to_f32(const void* hi, const void* lo, int n_img, int H, int W, int cstride, int c_off, int C, float* out,
                      void* stream);
@@ -399,6 +419,17 @@ int stp3_conv_wgrad(const float* x, int n_img, int H, int W, int x_cstride, int 
 size_t stp3_conv3d_wgrad_scratch_bytes(int B, int T, int H, int W, int cout, int cin, int kt, int kh, int kw);
 int stp3_conv3d_wgrad(const float* x, int B, int T, int H, int W, int x_cstride, int cin, const float* g, int g_cstride,
                       int cout, int kt, int kh, int kw, void* scratch, size_t scratch_bytes, float* dw, void* stream);
+/* One-product weight gradients: stp3_conv_wgrad / stp3_conv3d_wgrad on ONE 16-bit plane per operand (operand BF16 or
+ * F16; x and g hold values of that kind, e.g. the planes the forward convolution and the input gradient read), one MMA
+ * per 16-pixel k-slice instead of three.  Same arguments, layouts, argument checks and scratch queries
+ * (stp3_conv_wgrad_scratch_bytes / stp3_conv3d_wgrad_scratch_bytes); the same K split, per-stage fp32 add into the
+ * accumulator and ordered reduction, so two calls give bitwise-identical dw. */
+int stp3_conv_wgrad_plane(int operand, const void* x, int n_img, int H, int W, int x_cstride, int cin, const void* g,
+                          int Ho, int Wo, int g_cstride, int cout, int kh, int kw, int stride, int pad, int dilation,
+                          void* scratch, size_t scratch_bytes, float* dw, void* stream);
+int stp3_conv3d_wgrad_plane(int operand, const void* x, int B, int T, int H, int W, int x_cstride, int cin,
+                            const void* g, int g_cstride, int cout, int kt, int kh, int kw, void* scratch,
+                            size_t scratch_bytes, float* dw, void* stream);
 /* BatchNorm batch statistics over n_pix rows (two passes: mean, then the centred sum of squares; fp64 partials):
  * mean[C], var[C] (biased; may be NULL), invstd = 1/sqrt(var + eps); when running_mean/var are given they are updated
  * like nn.BatchNorm2d: r = (1 - momentum) r + momentum b, with the unbiased variance var * n/(n-1).
@@ -420,6 +451,14 @@ int stp3_bn_apply(const float* x, long long n_pix, int C, int x_cstride, const f
                   const float* gamma, const float* beta, const float* res, int res_cstride, int relu, float dropout_p,
                   unsigned long long seed, unsigned long long offset, float* y, int y_cstride, void* y_hi, void* y_lo,
                   int hl_cstride, void* stream);
+/* stp3_bn_apply emitting ONE plane of kind `operand` (STP3_OPERAND_BF16 or _F16) instead of the hi/lo pair: y_plane
+ * (n_pix, plane_cstride) receives the fp32 result y rounded to nearest even (overflow to +-inf, NaN passes through),
+ * channels [C, plane_cstride) as zeros.  Same values of y, same dropout bits, same argument rules (y_plane follows the
+ * rules of y_hi). */
+int stp3_bn_apply_plane(const float* x, long long n_pix, int C, int x_cstride, const float* mean, const float* invstd,
+                        const float* gamma, const float* beta, const float* res, int res_cstride, int relu,
+                        float dropout_p, unsigned long long seed, unsigned long long offset, float* y, int y_cstride,
+                        void* y_plane, int plane_cstride, int operand, void* stream);
 /* sum_g[c] = sum_p g'[p][c] (= dbeta, or a conv bias gradient when x is NULL) and sum_gxhat[c] = sum_p g' xhat (= dgamma),
  * g' = g where y > 0 (the ReLU mask of the BN's activated output y; y NULL = no mask), xhat = (x - mean) * invstd. */
 int stp3_bn_bwd_reduce(const float* g, int g_cstride, const float* y, int y_cstride, const float* x, int x_cstride,

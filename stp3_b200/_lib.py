@@ -96,6 +96,7 @@ SIGNATURES = {
     "stp3_lift_splat_workspace_bytes": (_SZ, [_LSD]),
     "stp3_lift_splat_workspace_init": (_I, [_V, _SZ, _V]),
     "stp3_f32_to_hilo": (_I, [_V, _I, _I, _I, _I, _I, _I, _V, _V, _V]),
+    "stp3_f32_to_plane": (_I, [_V, _I, _I, _I, _I, _I, _I, _I, _V, _V]),
     "stp3_hilo_to_f32": (_I, [_V, _V, _I, _I, _I, _I, _I, _I, _V, _V]),
     "stp3_spatial_sum": (_I, [_V, _V, _I, _I, _I, _V, _V]),
     "stp3_pool_bias": (_I, [_V, _I, _I, _I, _I, _F, _I, _V, _I, _V, _V, _I, _V, _I, _V, _V, _I, _I, _V]),
@@ -109,6 +110,7 @@ SIGNATURES = {
     "stp3_lift_splat_bwd_cl": (_I, [_LSD, _V, _V, _V, _V, _SZ, _V, _V, _V]),
     "stp3_bev_discount": (_I, [_V, _I, _I, _I, _I, _I, _F, _V, _V, _V]),
     "stp3_conv_fwd": (_I, [ctypes.POINTER(ConvDesc), _V, _V, _V, _V, _V, _V, _V, _V, _V, _V, ctypes.POINTER(ConvHead), _V]),
+    "stp3_conv_fwd_plane": (_I, [ctypes.POINTER(ConvDesc), _I, _V, _V, _V, _V, _V, _V]),
     "stp3_lift_splat_fwd": (_I, [_LSD, _V, _V, _V, _V, _V, _SZ, _V, _I, _I, ctypes.POINTER(_V), _V]),
     "stp3_lift_splat_plan": (_I, [_LSD, _V, _V, _I, _I, ctypes.POINTER(LiftSplatPlan)]),
     # train mode of the decoder and the DeepLab head
@@ -117,6 +119,7 @@ SIGNATURES = {
     "stp3_bn_scratch_bytes": (_SZ, [_LL, _I]),
     "stp3_bn_stats": (_I, [_V, _LL, _I, _I, _F, _F, _V, _V, _V, _V, _V, _V, _SZ, _V]),
     "stp3_bn_apply": (_I, [_V, _LL, _I, _I, _V, _V, _V, _V, _V, _I, _I, _F, _ULL, _ULL, _V, _I, _V, _V, _I, _V]),
+    "stp3_bn_apply_plane": (_I, [_V, _LL, _I, _I, _V, _V, _V, _V, _V, _I, _I, _F, _ULL, _ULL, _V, _I, _V, _I, _I, _V]),
     "stp3_image_channel_sums_scratch_bytes": (_SZ, [_I, _LL, _I]),
     "stp3_image_channel_sums": (_I, [_V, _I, _LL, _I, _I, _V, _V, _SZ, _V]),
     "stp3_bn_bwd_reduce": (_I, [_V, _I, _V, _I, _V, _I, _V, _V, _LL, _I, _V, _V, _V, _SZ, _V]),
@@ -135,6 +138,9 @@ SIGNATURES = {
     # train mode of the TemporalBlocks
     "stp3_conv3d_wgrad_scratch_bytes": (_SZ, [_I, _I, _I, _I, _I, _I, _I, _I, _I]),
     "stp3_conv3d_wgrad": (_I, [_V, _I, _I, _I, _I, _I, _I, _V, _I, _I, _I, _I, _I, _V, _SZ, _V, _V]),
+    # one-plane (autocast) train mode: operand STP3_OPERAND_BF16 / STP3_OPERAND_F16
+    "stp3_conv_wgrad_plane": (_I, [_I, _V, _I, _I, _I, _I, _I, _V, _I, _I, _I, _I, _I, _I, _I, _I, _I, _V, _SZ, _V, _V]),
+    "stp3_conv3d_wgrad_plane": (_I, [_I, _V, _I, _I, _I, _I, _I, _I, _V, _I, _I, _I, _I, _I, _V, _SZ, _V, _V]),
     "stp3_temporal_pair_mean": (_I, [_V, _I, _I, _I, _I, _V, _V]),
     # EfficientNet trunk
     "stp3_effnet_stem": (_I, [_V, _I, _I, _I, _I, _I, _I, _I, _V, _V, _I, _I, _V, _V, _V]),
@@ -143,6 +149,10 @@ SIGNATURES = {
     "stp3_se_proj_weight_elems": (_LL, [_I, _I]),
     "stp3_se_gate": (_I, [_V, _I, _I, _I, _F, _V, _V, _I, _V, _V, _V, _I, _V, _V, _V]),
 }
+
+
+# operand kinds of the train-mode convolutions (STP3_OPERAND_* of include/stp3_b200.h)
+OPERAND_HILO, OPERAND_BF16, OPERAND_F16 = 0, 1, 2
 
 
 def build(verbose: bool = False) -> str:

@@ -12,11 +12,12 @@ __device__ __forceinline__ float join_bf16(__nv_bfloat16 h, __nv_bfloat16 l) {
   return __bfloat162float(h) + __bfloat162float(l);
 }
 
-// fp32 (n_img, C, H*W) [NCHW] or (n_img, H*W, C) [NHWC] -> hi/lo (n_img, H*W, cp), zero padding channels.
+// fp32 (n_img, C, H*W) [NCHW] or (n_img, H*W, C) [NHWC] -> hi/lo (n_img, H*W, cp) (OP 0), or one 16-bit plane (OP 1 =
+// bf16, 2 = fp16, in `hi`), zero padding channels.
 // 32 pixels x 32 channels per block through shared memory so that both sides are coalesced.
-__global__ void __launch_bounds__(256)
-f32_to_hilo_kernel(const float* __restrict__ x, int channels_last, int C, int HW, int cp,
-                   __nv_bfloat16* __restrict__ hi, __nv_bfloat16* __restrict__ lo) {
+template <int OP, typename Out>
+__device__ __forceinline__ void f32_to_planes(const float* __restrict__ x, int channels_last, int C, int HW, int cp,
+                                              Out* __restrict__ hi, Out* __restrict__ lo) {
   __shared__ float tile[32][33];
   const int img = blockIdx.z;
   const int p0 = blockIdx.x * 32, c0 = blockIdx.y * 32;
@@ -39,12 +40,29 @@ f32_to_hilo_kernel(const float* __restrict__ x, int channels_last, int C, int HW
   for (int k = 0; k < 4; ++k) {
     const int px = p0 + ty + 8 * k, c = c0 + tx;
     if (px < HW && c < cp) {
-      __nv_bfloat16 h, l;
-      ptx::split_hilo(tile[tx][ty + 8 * k], h, l);
-      hi[((size_t)img * HW + px) * cp + c] = h;
-      lo[((size_t)img * HW + px) * cp + c] = l;
+      if constexpr (OP == 0) {
+        __nv_bfloat16 h, l;
+        ptx::split_hilo(tile[tx][ty + 8 * k], h, l);
+        hi[((size_t)img * HW + px) * cp + c] = h;
+        lo[((size_t)img * HW + px) * cp + c] = l;
+      } else {
+        hi[((size_t)img * HW + px) * cp + c] = ptx::plane16<OP>(tile[tx][ty + 8 * k]);
+      }
     }
   }
+}
+
+__global__ void __launch_bounds__(256)
+f32_to_hilo_kernel(const float* __restrict__ x, int channels_last, int C, int HW, int cp,
+                   __nv_bfloat16* __restrict__ hi, __nv_bfloat16* __restrict__ lo) {
+  f32_to_planes<0>(x, channels_last, C, HW, cp, hi, lo);
+}
+
+// the one-plane counterpart (stp3_f32_to_plane): OP 1 = bf16, 2 = fp16
+template <int OP>
+__global__ void __launch_bounds__(256)
+f32_to_plane_kernel(const float* __restrict__ x, int channels_last, int C, int HW, int cp, uint16_t* __restrict__ out) {
+  f32_to_planes<OP>(x, channels_last, C, HW, cp, out, static_cast<uint16_t*>(nullptr));
 }
 
 // hi/lo (n_img, H*W, cstride) channels [c_off, c_off+C) -> fp32 (n_img, C, H*W)
@@ -248,6 +266,22 @@ extern "C" int stp3_f32_to_hilo(const float* x, int channels_last, int n_img, in
   const int HW = H * W;
   dim3 grid(ceil_div(HW, 32), ceil_div(cp, 32), n_img), block(32, 8);
   f32_to_hilo_kernel<<<grid, block, 0, (cudaStream_t)stream>>>(x, channels_last, C, HW, cp, (bf16*)hi, (bf16*)lo);
+  STP3_CUDA_OK(cudaGetLastError());
+  return STP3_OK;
+}
+
+extern "C" int stp3_f32_to_plane(const float* x, int channels_last, int n_img, int C, int H, int W, int cp, int operand,
+                                 void* out, void* stream) {
+  STP3_CHECK_ARG(x && out && n_img > 0 && C > 0 && H > 0 && W > 0 && cp >= C, "stp3_f32_to_plane: bad argument");
+  STP3_CHECK_ARG(operand == STP3_OPERAND_BF16 || operand == STP3_OPERAND_F16,
+                 "stp3_f32_to_plane: operand must be STP3_OPERAND_BF16 or STP3_OPERAND_F16");
+  STP3_CHECK_ARG(n_img <= 65535, "stp3_f32_to_plane: more than 65535 images");
+  const int HW = H * W;
+  dim3 grid(ceil_div(HW, 32), ceil_div(cp, 32), n_img), block(32, 8);
+  if (operand == STP3_OPERAND_F16)
+    f32_to_plane_kernel<2><<<grid, block, 0, (cudaStream_t)stream>>>(x, channels_last, C, HW, cp, (uint16_t*)out);
+  else
+    f32_to_plane_kernel<1><<<grid, block, 0, (cudaStream_t)stream>>>(x, channels_last, C, HW, cp, (uint16_t*)out);
   STP3_CUDA_OK(cudaGetLastError());
   return STP3_OK;
 }

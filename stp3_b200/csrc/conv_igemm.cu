@@ -183,7 +183,9 @@ __device__ __forceinline__ bool group_is_padding(const ConvParams& p, int grp, i
 // FULLK: every K = 16 step of every K block carries data (ks_first == 0, ks_end == 4).  Then a tap is a branch-free run
 // of wgmma with N fixed at compile time (BN, 2 * BN for the stacked operand), which ptxas pipelines; any branch around
 // the MMAs (skipped K steps, an N chosen at run time) makes it serialise them.
-template <int BN, bool STACK, bool FULLK>
+// OP: operand kind.  0 = bf16 hi/lo planes, three MMAs per product (fp32-equivalent); 1 = one bf16 plane, 2 = one fp16
+// plane (autocast training): the activation stage and the weight tile hold one plane and each K step is one MMA.
+template <int BN, bool STACK, bool FULLK, int OP = 0>
 __global__ void __launch_bounds__(kConvThreads, 1)
 conv_igemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ CUtensorMap tm_a_lo,
                   const __grid_constant__ CUtensorMap tm_w, const __grid_constant__ CUtensorMap tm_o_hi,
@@ -191,6 +193,8 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
                   const __grid_constant__ CUtensorMap tm_o2_lo, const ConvParams p) {
   using S = ConvSmem<BN>;
   static_assert(!STACK || BN == 64, "stacked weight operand: BN = 64 only");
+  static_assert(OP == 0 || !STACK, "one-plane operands: no stacked weight operand");
+  constexpr int kPlanes = OP == 0 ? 2 : 1;             // planes per activation stage and per weight tile
   constexpr int kAccRegs = (STACK ? 2 * BN : BN) / 2;   // accumulator registers per thread (64 rows x columns per warpgroup)
   const int kBRows = p.b_rows;
   const int cta = (int)blockIdx.x, n_cta = (int)gridDim.x;
@@ -199,7 +203,7 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
   unsigned char* smem = smem_raw + ((1024u - (ptx::smem_u32(smem_raw) & 1023u)) & 1023u);
   const int k_iters = p.ntaps * p.kblocks;
   const bool resident = p.b_resident != 0;
-  const int a_stage_bytes = 2 * p.a_plane_bytes;
+  const int a_stage_bytes = kPlanes * p.a_plane_bytes;
   unsigned char* a_ring = smem;
   unsigned char* b_ring = a_ring + (size_t)p.na_stages * a_stage_bytes;            // ring, or the resident weights
   unsigned char* tail = b_ring + (size_t)(resident ? k_iters : p.nb_stages) * p.b_tile_bytes;
@@ -226,7 +230,7 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
   // weights) are read before griddep_wait().
   ptx::griddep_launch_dependents();
   if (warp == kProducerWarp && lane == 0) {
-    ptx::prefetch_tmap(&tm_a_hi); ptx::prefetch_tmap(&tm_a_lo); ptx::prefetch_tmap(&tm_w);
+    ptx::prefetch_tmap(&tm_a_hi); if constexpr (OP == 0) ptx::prefetch_tmap(&tm_a_lo); ptx::prefetch_tmap(&tm_w);
     if (p.out_hl) { ptx::prefetch_tmap(&tm_o_hi); ptx::prefetch_tmap(&tm_o_lo); }
     if (p.out2) { ptx::prefetch_tmap(&tm_o2_hi); ptx::prefetch_tmap(&tm_o2_lo); }
     ra.init(2); rb.init(2);
@@ -248,9 +252,9 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
     // ===================== TMA producer (whole warp walks the loops; one elected lane issues) =====================
     // load_b: the weight tile of K step `it` into `dst` (called by the elected lane; transaction bytes on `bar`)
     auto load_b = [&](unsigned char* dst, int it, uint64_t* bar, int img_w, int nb) {
-      const int row_hi = (int)((it * 2) * p.w_rows + nb * BN + img_w * p.w_img_rows), row_lo = row_hi + p.w_rows;
+      const int row_hi = (int)((it * kPlanes) * p.w_rows + nb * BN + img_w * p.w_img_rows), row_lo = row_hi + p.w_rows;
       ptx::tma_load_2d(dst, &tm_w, bar, 0, row_hi);                       // [W_hi; W_lo], also the stacked operand
-      ptx::tma_load_2d(dst + kBRows * kBK * 2, &tm_w, bar, 0, row_lo);
+      if constexpr (OP == 0) ptx::tma_load_2d(dst + kBRows * kBK * 2, &tm_w, bar, 0, row_lo);
     };
     if (resident && ptx::elect_one_sync()) {
       ptx::mbar_arrive_expect_tx(bres_bar, (uint32_t)(k_iters * p.b_load_bytes));
@@ -274,7 +278,7 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
             unsigned char* sa = a_ring + (size_t)s * a_stage_bytes;
             const int c = p.cin_off + kb * kBK;
             ptx::tma_load_5d(sa, &tm_a_hi, bar, c, x, y, t, bidx);
-            ptx::tma_load_5d(sa + p.a_plane_bytes, &tm_a_lo, bar, c, x, y, t, bidx);
+            if constexpr (OP == 0) ptx::tma_load_5d(sa + p.a_plane_bytes, &tm_a_lo, bar, c, x, y, t, bidx);
           });
           if (!resident) {
             for (int j = 0; j < gsz; ++j) {
@@ -329,7 +333,9 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
               for (int k = 0; k < kBK / 16; ++k) {
                 const uint64_t koff = (uint64_t)((k * 16 * 2) >> 4);   // advance 16 bf16 = 32 bytes along K
                 const uint32_t acc0 = accumulate | (uint32_t)(k > 0);
-                if constexpr (STACK) {
+                if constexpr (OP != 0) {
+                  wg::mma_plane<OP, BN>(accr, da_hi + koff, db_hi + koff, acc0);
+                } else if constexpr (STACK) {
                   wg::mma_bf16<2 * BN>(accr, da_hi + koff, db_hi + koff, acc0);                // A_hi x [W_hi; W_lo]
                   wg::mma_bf16<BN>(accr, da_lo + koff, db_lo + koff, 1);                       // A_lo x W_hi
                 } else {
@@ -342,7 +348,9 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
                 if (k < k_begin || k >= k_end) continue;               // K steps of pure channel padding
                 const uint64_t koff = (uint64_t)((k * 16 * 2) >> 4);
                 const uint32_t acc0 = accumulate | (uint32_t)(k > k_begin);
-                if constexpr (STACK) {
+                if constexpr (OP != 0) {
+                  wg::mma_plane_n<OP, BN>(p.n_mma, accr, da_hi + koff, db_hi + koff, acc0);
+                } else if constexpr (STACK) {
                   wg::mma_bf16_n<2 * BN>(2 * p.n_mma, accr, da_hi + koff, db_hi + koff, acc0);
                   wg::mma_bf16_n<2 * BN>(p.n_mma, accr, da_lo + koff, db_lo + koff, 1);
                 } else {
@@ -681,10 +689,10 @@ int launch_col_sum_reduce(const float* part, int n_part, int n_img, float* out, 
   return STP3_OK;
 }
 
-template <int BN, bool STACK, bool FULLK>
+template <int BN, bool STACK, bool FULLK, int OP = 0>
 static int launch_conv(const ConvParams& p, const CUtensorMap& tm_hi, const CUtensorMap& tm_lo, const CUtensorMap& tm_w,
                        const CUtensorMap (&tm_o)[4], size_t smem_bytes, unsigned grid, cudaStream_t stream) {
-  constexpr auto kern = conv_igemm_kernel<BN, STACK, FULLK>;
+  constexpr auto kern = conv_igemm_kernel<BN, STACK, FULLK, OP>;
   STP3_CUDA_OK(set_max_dynamic_smem<kern>((int)kSmemCap));
   STP3_CUDA_OK(launch_pdl(kPdlConv, kern, dim3(grid), dim3(kConvThreads), smem_bytes, stream, tm_hi, tm_lo, tm_w,
                           tm_o[0], tm_o[1], tm_o[2], tm_o[3], p));
@@ -703,7 +711,8 @@ struct ConvPlan {
 };
 
 // Checks every rule of the descriptor that needs no tensor pointer and fills the geometry, tiling and ring fields of p.
-static int plan_conv(const stp3_conv_desc* d, bool has_head, int n_sm, ConvParams& p, ConvPlan& t) {
+// operand: STP3_OPERAND_* (one-plane operands halve the activation stage and the weight tile and never stack).
+static int plan_conv(const stp3_conv_desc* d, bool has_head, int n_sm, ConvParams& p, ConvPlan& t, int operand = 0) {
   STP3_CHECK_ARG(d->B > 0 && d->T > 0 && d->H > 0 && d->W > 0 && d->Ho > 0 && d->Wo > 0, "non-positive dimension");
   const int T_total = d->T_total > 0 ? d->T_total : d->T;
   STP3_CHECK_ARG(d->t0 >= 0 && d->t0 + d->T <= T_total, "frame window [t0, t0+T) outside the input tensor");
@@ -739,7 +748,7 @@ static int plan_conv(const stp3_conv_desc* d, bool has_head, int n_sm, ConvParam
   const bool stream_weights = (want_group_raw & 4) != 0 || d->w_img_stride != 0 || p.n_nblk > 1;
   // +8: stacked [W_hi; W_lo] operand (64-column blocks only).  Untuned (tune_group == 0) multi-tap layers in 64-column
   // blocks use it: it reads the activation tile twice instead of three times
-  t.stack = t.bn_blk == 64 && ((want_group_raw & 8) != 0 || (want_group_raw == 0 && d->ntaps > 1));
+  t.stack = operand == 0 && t.bn_blk == 64 && ((want_group_raw & 8) != 0 || (want_group_raw == 0 && d->ntaps > 1));
   // taps that can share one activation load: runs (<= 4) of consecutive taps with the same (dt, dx) and dy advancing
   // by the stride
   p.n_groups = 0; p.gmax = 1;
@@ -786,10 +795,11 @@ static int plan_conv(const stp3_conv_desc* d, bool has_head, int n_sm, ConvParam
 
   // ring depths beside this block width's shared-memory tail
   const size_t tail = t.bn_blk == 64 ? ConvSmem<64>::tail_bytes() : ConvSmem<128>::tail_bytes();
-  const size_t a_stage = 2 * (size_t)p.a_plane_bytes;
+  const int planes = operand == 0 ? 2 : 1;
+  const size_t a_stage = planes * (size_t)p.a_plane_bytes;
   p.b_rows = t.full_k ? t.bn_blk : n_mma;
-  p.b_tile_bytes = 2 * p.b_rows * kBK * 2;
-  p.b_load_bytes = 2 * n_mma * kBK * 2;
+  p.b_tile_bytes = planes * p.b_rows * kBK * 2;
+  p.b_load_bytes = planes * n_mma * kBK * 2;
   const size_t avail = kSmemCap - 1024 - tail;
   const size_t wbytes = (size_t)t.k_iters * (size_t)p.b_tile_bytes;
   // small weight tensors stay resident in smem next to >= 2 activation stages
@@ -831,12 +841,10 @@ extern "C" int stp3_conv_tiling(const stp3_conv_desc* d, int n_sm, stp3_conv_til
   return STP3_OK;
 }
 
-extern "C" int stp3_conv_fwd(const stp3_conv_desc* d, const void* x_hi, const void* x_lo, const void* w,
-                             const float* bias, const float* img_bias, const void* res_hi, const void* res_lo,
-                             void* y_hi, void* y_lo, float* y_f32, const stp3_conv_head* head, void* stream_) {
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  STP3_CHECK_ARG(d && x_hi && x_lo && w && bias, "stp3_conv_fwd: null pointer argument");
-  STP3_CHECK_ARG((y_hi && y_lo) || y_f32 || head, "stp3_conv_fwd: no output tensor");
+// stp3_conv_fwd and stp3_conv_fwd_plane (operand != 0: x_lo, the residual, the hi/lo outputs and the head are absent)
+static int conv_fwd(const stp3_conv_desc* d, int operand, const void* x_hi, const void* x_lo, const void* w,
+                    const float* bias, const float* img_bias, const void* res_hi, const void* res_lo, void* y_hi,
+                    void* y_lo, float* y_f32, const stp3_conv_head* head, cudaStream_t stream) {
   if (head) {
     STP3_CHECK_ARG(head->n_out >= 1 && head->n_out <= kMaxHeadOut && head->w && head->b, "bad fused head");
     STP3_CHECK_ARG(d->bn <= 128, "a fused head needs bn <= 128");
@@ -844,7 +852,7 @@ extern "C" int stp3_conv_fwd(const stp3_conv_desc* d, const void* x_hi, const vo
   }
   ConvParams p;
   ConvPlan t;
-  if (const int rc = plan_conv(d, head != nullptr, num_sms(), p, t)) return rc;
+  if (const int rc = plan_conv(d, head != nullptr, num_sms(), p, t, operand)) return rc;
   const int n_store = d->n_store > 0 ? d->n_store : d->bn;
   if (y_hi) STP3_CHECK_ARG(d->out_cstride % 8 == 0 && d->out_coff % 8 == 0 && d->out_coff + n_store <= d->out_cstride,
                            "output channel window does not fit the output tensor");
@@ -857,13 +865,16 @@ extern "C" int stp3_conv_fwd(const stp3_conv_desc* d, const void* x_hi, const vo
   {
     const int box_w = (kTileW - 1) * d->stride + 1, box_rows = (t.box_h - 1) * d->stride + 1;
     const CUresult r1 = encode_act_5d(&tm_hi, x_hi, d->in_cstride, d->W, d->H, p.T_total, d->B, box_w, box_rows, d->stride);
-    const CUresult r2 = encode_act_5d(&tm_lo, x_lo, d->in_cstride, d->W, d->H, p.T_total, d->B, box_w, box_rows, d->stride);
+    const CUresult r2 = operand ? r1 : encode_act_5d(&tm_lo, x_lo, d->in_cstride, d->W, d->H, p.T_total, d->B, box_w,
+                                                     box_rows, d->stride);
+    if (operand) tm_lo = tm_hi;
     if (r1 != CUDA_SUCCESS || r2 != CUDA_SUCCESS)
       return set_error(STP3_ECUDA, "cuTensorMapEncodeTiled(activation) failed: %d %d", (int)r1, (int)r2);
   }
   {
+    const int planes = operand ? 1 : 2;
     const long long rows = d->w_img_stride ? (long long)(d->B * d->T - 1) * (d->w_img_stride / 64) + (long long)t.k_iters * 2 * d->bn
-                                           : (long long)t.k_iters * 2 * d->bn;
+                                           : (long long)t.k_iters * planes * d->bn;
     const CUresult r = encode_rows_2d(&tm_w, w, rows, p.n_mma);
     if (r != CUDA_SUCCESS) return set_error(STP3_ECUDA, "cuTensorMapEncodeTiled(weights) failed: %d", (int)r);
   }
@@ -930,7 +941,19 @@ extern "C" int stp3_conv_fwd(const stp3_conv_desc* d, const void* x_hi, const vo
   auto al32 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 31) == 0; };
   p.vec256 = d->res_mode && d->res_cstride % 16 == 0 && d->res_coff % 16 == 0 && al32(res_hi) && al32(res_lo) ? 2 : 0;
   int rc;
-  if (t.bn_blk == 64 && t.stack)
+  if (operand == STP3_OPERAND_BF16 && t.bn_blk == 64)
+    rc = t.full_k ? launch_conv<64, false, true, 1>(p, tm_hi, tm_lo, tm_w, tm_o, t.smem_bytes, t.grid, stream)
+                  : launch_conv<64, false, false, 1>(p, tm_hi, tm_lo, tm_w, tm_o, t.smem_bytes, t.grid, stream);
+  else if (operand == STP3_OPERAND_BF16)
+    rc = t.full_k ? launch_conv<128, false, true, 1>(p, tm_hi, tm_lo, tm_w, tm_o, t.smem_bytes, t.grid, stream)
+                  : launch_conv<128, false, false, 1>(p, tm_hi, tm_lo, tm_w, tm_o, t.smem_bytes, t.grid, stream);
+  else if (operand == STP3_OPERAND_F16 && t.bn_blk == 64)
+    rc = t.full_k ? launch_conv<64, false, true, 2>(p, tm_hi, tm_lo, tm_w, tm_o, t.smem_bytes, t.grid, stream)
+                  : launch_conv<64, false, false, 2>(p, tm_hi, tm_lo, tm_w, tm_o, t.smem_bytes, t.grid, stream);
+  else if (operand == STP3_OPERAND_F16)
+    rc = t.full_k ? launch_conv<128, false, true, 2>(p, tm_hi, tm_lo, tm_w, tm_o, t.smem_bytes, t.grid, stream)
+                  : launch_conv<128, false, false, 2>(p, tm_hi, tm_lo, tm_w, tm_o, t.smem_bytes, t.grid, stream);
+  else if (t.bn_blk == 64 && t.stack)
     rc = t.full_k ? launch_conv<64, true, true>(p, tm_hi, tm_lo, tm_w, tm_o, t.smem_bytes, t.grid, stream)
                   : launch_conv<64, true, false>(p, tm_hi, tm_lo, tm_w, tm_o, t.smem_bytes, t.grid, stream);
   else if (t.bn_blk == 64)
@@ -946,4 +969,24 @@ extern "C" int stp3_conv_fwd(const stp3_conv_desc* d, const void* x_hi, const vo
                             (const float*)p.sum_part, (int)t.grid * 4, p.n_img, 64, static_cast<float*>(d->col_sums)));
   }
   return STP3_OK;
+}
+
+extern "C" int stp3_conv_fwd(const stp3_conv_desc* d, const void* x_hi, const void* x_lo, const void* w,
+                             const float* bias, const float* img_bias, const void* res_hi, const void* res_lo,
+                             void* y_hi, void* y_lo, float* y_f32, const stp3_conv_head* head, void* stream) {
+  STP3_CHECK_ARG(d && x_hi && x_lo && w && bias, "stp3_conv_fwd: null pointer argument");
+  STP3_CHECK_ARG((y_hi && y_lo) || y_f32 || head, "stp3_conv_fwd: no output tensor");
+  return conv_fwd(d, STP3_OPERAND_HILO, x_hi, x_lo, w, bias, img_bias, res_hi, res_lo, y_hi, y_lo, y_f32, head,
+                  reinterpret_cast<cudaStream_t>(stream));
+}
+
+extern "C" int stp3_conv_fwd_plane(const stp3_conv_desc* d, int operand, const void* x, const void* w,
+                                   const float* bias, const float* img_bias, float* y_f32, void* stream) {
+  STP3_CHECK_ARG(d && x && w && bias && y_f32, "stp3_conv_fwd_plane: null pointer argument");
+  STP3_CHECK_ARG(operand == STP3_OPERAND_BF16 || operand == STP3_OPERAND_F16,
+                 "stp3_conv_fwd_plane: operand must be STP3_OPERAND_BF16 or STP3_OPERAND_F16");
+  STP3_CHECK_ARG(!d->res_mode && !d->y2_hi && !d->col_sums && !d->swish && !d->w_img_stride,
+                 "stp3_conv_fwd_plane: no residual, second destination, col_sums, swish or per-image weights");
+  return conv_fwd(d, operand, x, nullptr, w, bias, img_bias, nullptr, nullptr, nullptr, nullptr, y_f32, nullptr,
+                  reinterpret_cast<cudaStream_t>(stream));
 }

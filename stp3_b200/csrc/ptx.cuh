@@ -16,6 +16,22 @@ __device__ __forceinline__ uint32_t pack_bf16x2(float a, float b) {
   return r;
 }
 
+// two fp32 -> packed f16x2 (round to nearest even; overflow gives +-inf, NaN stays NaN): low half = a, high half = b
+__device__ __forceinline__ uint32_t pack_f16x2(float a, float b) {
+  uint32_t r;
+  asm("cvt.rn.f16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(b), "f"(a));
+  return r;
+}
+// the one-plane formats of the autocast train path (OP 1 = bf16, 2 = fp16), rounded to nearest even, never saturated
+template <int OP>
+__device__ __forceinline__ uint32_t pack_plane16x2(float a, float b) {
+  static_assert(OP == 1 || OP == 2, "one-plane kind: 1 = bf16, 2 = fp16");
+  if constexpr (OP == 2) return pack_f16x2(a, b);
+  else return pack_bf16x2(a, b);
+}
+template <int OP>
+__device__ __forceinline__ uint16_t plane16(float x) { return (uint16_t)(pack_plane16x2<OP>(x, 0.f) & 0xFFFFu); }
+
 // The hi/lo plane format of every fp32 tensor: hi = bf16(x), lo = bf16(x - hi), both rounded to nearest even.
 // A pair (x0, x1) -> packed bf16x2 words, x0 in the low halves.
 __device__ __forceinline__ void split_hilo(float x0, float x1, uint32_t& hi, uint32_t& lo) {

@@ -6,6 +6,7 @@
 // (no float atomics), and the block decomposition depends only on the problem shape, so two calls on the same inputs
 // return bitwise-identical results.
 #include <climits>
+#include <type_traits>
 
 #include <cuda_bf16.h>
 
@@ -70,11 +71,29 @@ __device__ __forceinline__ void load8_split(const float* row, int c0, int C, boo
   lo = make_uint4(l[0], l[1], l[2], l[3]);
 }
 
+// 8 consecutive 16-bit channels [c0, c0 + 8) of row `row` (NULL row = zeros), one 16-byte chunk
+__device__ __forceinline__ uint4 load8_plane(const uint16_t* row, int c0, int C, bool vec) {
+  if (row && vec && c0 + 8 <= C) return *reinterpret_cast<const uint4*>(row + c0);
+  uint32_t h[4];
+#pragma unroll
+  for (int e = 0; e < 4; ++e) {
+    const uint32_t a = (row && c0 + 2 * e < C) ? row[c0 + 2 * e] : 0u;
+    const uint32_t b = (row && c0 + 2 * e + 1 < C) ? row[c0 + 2 * e + 1] : 0u;
+    h[e] = a | (b << 16);
+  }
+  return make_uint4(h[0], h[1], h[2], h[3]);
+}
+
+// OP 0: x and g fp32, split into hi / lo on the way in, three products per pair.  OP 1 / 2 (the one-product mode of
+// stp3_conv_wgrad_plane): x and g are one bf16 / fp16 plane each, staged as they are, one product per pair.
+template <int OP>
 __global__ void __launch_bounds__(128, 1)
-wgrad_partial_kernel(const float* __restrict__ x, const float* __restrict__ g, WgradShape s, long long px_per_split,
-                     int vec_x, int vec_g, float* __restrict__ part) {
+wgrad_partial_kernel(const std::conditional_t<OP == 0, float, uint16_t>* __restrict__ x,
+                     const std::conditional_t<OP == 0, float, uint16_t>* __restrict__ g, WgradShape s,
+                     long long px_per_split, int vec_x, int vec_g, float* __restrict__ part) {
+  using In = std::conditional_t<OP == 0, float, uint16_t>;
   extern __shared__ uint8_t wg_smem_raw[];
-  // four 8 KB planes, 1024-byte aligned (the swizzle atom): A hi, A lo (g), B hi, B lo (x)
+  // four 8 KB planes, 1024-byte aligned (the swizzle atom): A hi, A lo (g), B hi, B lo (x); OP != 0: A (g), B (x)
   uint8_t* sm = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(wg_smem_raw) + 1023) & ~uintptr_t(1023));
   const int co_tiles = (s.cout + kWgTile - 1) / kWgTile, ci_tiles = (s.cin + kWgTile - 1) / kWgTile;
   int t = blockIdx.y;
@@ -105,8 +124,8 @@ wgrad_partial_kernel(const float* __restrict__ x, const float* __restrict__ g, W
       const int idx = tid + 128 * k;
       const int r = idx >> 3, c = idx & 7;
       const long long p = p0 + r;
-      const float* grow = nullptr;
-      const float* xrow = nullptr;
+      const In* grow = nullptr;
+      const In* xrow = nullptr;
       if (p < p_end) {
         const int ox = (int)(p % s.Wo);
         const long long q = p / s.Wo;
@@ -117,14 +136,19 @@ wgrad_partial_kernel(const float* __restrict__ x, const float* __restrict__ g, W
         if (iy >= 0 && iy < s.H && ix >= 0 && ix < s.W && it >= 0)
           xrow = x + (((img + dt) * s.H + iy) * s.W + ix) * s.x_cstride + ci0;
       }
-      uint4 gh, gl, xh, xl;
-      load8_split(grow, c * 8, s.cout - co0, vec_g, gh, gl);
-      load8_split(xrow, c * 8, s.cin - ci0, vec_x, xh, xl);
       const int off = r * 128 + ((c ^ (r & 7)) << 4);
-      *reinterpret_cast<uint4*>(sm + 0 * kWgTileBytes + off) = gh;
-      *reinterpret_cast<uint4*>(sm + 1 * kWgTileBytes + off) = gl;
-      *reinterpret_cast<uint4*>(sm + 2 * kWgTileBytes + off) = xh;
-      *reinterpret_cast<uint4*>(sm + 3 * kWgTileBytes + off) = xl;
+      if constexpr (OP == 0) {
+        uint4 gh, gl, xh, xl;
+        load8_split(grow, c * 8, s.cout - co0, vec_g, gh, gl);
+        load8_split(xrow, c * 8, s.cin - ci0, vec_x, xh, xl);
+        *reinterpret_cast<uint4*>(sm + 0 * kWgTileBytes + off) = gh;
+        *reinterpret_cast<uint4*>(sm + 1 * kWgTileBytes + off) = gl;
+        *reinterpret_cast<uint4*>(sm + 2 * kWgTileBytes + off) = xh;
+        *reinterpret_cast<uint4*>(sm + 3 * kWgTileBytes + off) = xl;
+      } else {
+        *reinterpret_cast<uint4*>(sm + 0 * kWgTileBytes + off) = load8_plane(grow, c * 8, s.cout - co0, vec_g);
+        *reinterpret_cast<uint4*>(sm + 1 * kWgTileBytes + off) = load8_plane(xrow, c * 8, s.cin - ci0, vec_x);
+      }
     }
     ptx::fence_proxy_async();                          // generic-proxy stores -> visible to the wgmma (async proxy)
     __syncthreads();
@@ -132,6 +156,11 @@ wgrad_partial_kernel(const float* __restrict__ x, const float* __restrict__ g, W
 #pragma unroll
     for (int ks = 0; ks < kWgK / 16; ++ks) {
       const uint32_t koff = ks * 16 * 128;
+      if constexpr (OP != 0) {
+        wg::mma_plane_mn64<OP>(stage, wg::desc_mn_sw128(s_base + 0 * kWgTileBytes + koff, 1024),
+                               wg::desc_mn_sw128(s_base + 1 * kWgTileBytes + koff, 1024), ks > 0);
+        continue;
+      }
       const uint64_t a_hi = wg::desc_mn_sw128(s_base + 0 * kWgTileBytes + koff, 1024);
       const uint64_t a_lo = wg::desc_mn_sw128(s_base + 1 * kWgTileBytes + koff, 1024);
       const uint64_t b_hi = wg::desc_mn_sw128(s_base + 2 * kWgTileBytes + koff, 1024);
@@ -384,6 +413,8 @@ __device__ __forceinline__ uint32_t dropout_keep8(unsigned long long seed, unsig
 // y = relu?((x - mean) * invstd * gamma + beta (+ res)) [* keep / (1 - p)]; one thread = one pixel x 8 channels (two
 // 128-bit loads); groups of 8 channels in [C, y_cs) of the bf16 planes are written as zeros (padding of the next conv's
 // K blocks).  Dropout (p > 0): the keep bit of element (pixel, c) depends only on (seed, offset + pixel * C + c).
+// OP != 0 (stp3_bn_apply_plane): yh receives ONE bf16 (1) / fp16 (2) plane instead of the hi/lo pair
+template <int OP>
 __global__ void __launch_bounds__(256)
 bn_apply_kernel(const float* __restrict__ x, int x_cs, const float* __restrict__ mean, const float* __restrict__ invstd,
                 const float* __restrict__ gamma, const float* __restrict__ beta, const float* __restrict__ res, int res_cs,
@@ -428,11 +459,18 @@ bn_apply_kernel(const float* __restrict__ x, int x_cs, const float* __restrict__
     for (int k = 0; k < 8; ++k) v[k] = 0.f;
   }
   if (yh && c0 < hl_cs) {
-    uint32_t oh[4], ol[4];
+    if constexpr (OP == 0) {
+      uint32_t oh[4], ol[4];
 #pragma unroll
-    for (int e = 0; e < 4; ++e) ptx::split_hilo(v[2 * e], v[2 * e + 1], oh[e], ol[e]);
-    *reinterpret_cast<uint4*>(yh + p * hl_cs + c0) = make_uint4(oh[0], oh[1], oh[2], oh[3]);
-    *reinterpret_cast<uint4*>(yl + p * hl_cs + c0) = make_uint4(ol[0], ol[1], ol[2], ol[3]);
+      for (int e = 0; e < 4; ++e) ptx::split_hilo(v[2 * e], v[2 * e + 1], oh[e], ol[e]);
+      *reinterpret_cast<uint4*>(yh + p * hl_cs + c0) = make_uint4(oh[0], oh[1], oh[2], oh[3]);
+      *reinterpret_cast<uint4*>(yl + p * hl_cs + c0) = make_uint4(ol[0], ol[1], ol[2], ol[3]);
+    } else {
+      uint32_t o[4];
+#pragma unroll
+      for (int e = 0; e < 4; ++e) o[e] = ptx::pack_plane16x2<OP>(v[2 * e], v[2 * e + 1]);
+      *reinterpret_cast<uint4*>(yh + p * hl_cs + c0) = make_uint4(o[0], o[1], o[2], o[3]);
+    }
   }
 }
 
@@ -488,6 +526,7 @@ __device__ __forceinline__ bool dropout_keep1(unsigned long long seed, unsigned 
 
 // bn_apply_kernel for any C and row stride (channel windows at odd offsets, C % 8 != 0): one thread = one element of
 // the n_cols = max(C, hl_cs) columns; the same arithmetic per element as the vector kernel
+template <int OP>
 __global__ void __launch_bounds__(256)
 bn_apply_scalar_kernel(const float* __restrict__ x, int x_cs, const float* __restrict__ mean,
                        const float* __restrict__ invstd, const float* __restrict__ gamma, const float* __restrict__ beta,
@@ -506,7 +545,11 @@ bn_apply_scalar_kernel(const float* __restrict__ x, int x_cs, const float* __res
     if (drop_p > 0.f) v = dropout_keep1(seed, offset + (unsigned long long)p * C + c, drop_p) ? v * (1.f / (1.f - drop_p)) : 0.f;
     if (y) y[p * y_cs + c] = v;
   }
-  if (yh && c < hl_cs) ptx::split_hilo(v, yh[p * hl_cs + c], yl[p * hl_cs + c]);
+  if constexpr (OP == 0) {
+    if (yh && c < hl_cs) ptx::split_hilo(v, yh[p * hl_cs + c], yl[p * hl_cs + c]);
+  } else {
+    if (yh && c < hl_cs) reinterpret_cast<uint16_t*>(yh)[p * hl_cs + c] = ptx::plane16<OP>(v);
+  }
 }
 
 // bn_bwd_apply_kernel for any C and row stride: one thread = one element
@@ -702,8 +745,9 @@ extern "C" size_t stp3_conv_wgrad_scratch_bytes(int n_img, int Ho, int Wo, int c
   return (size_t)wgrad_splits(s) * kh * kw * (size_t)cout * cin * sizeof(float);
 }
 
-// the partial GEMMs and the ordered reduction of one (validated) weight gradient
-static int launch_wgrad(const WgradShape& s, const float* x, const float* g, float* scratch, float* dw, cudaStream_t st,
+// the partial GEMMs and the ordered reduction of one (validated) weight gradient (OP: operand kind, STP3_OPERAND_*)
+template <int OP = 0, typename In = float>
+static int launch_wgrad(const WgradShape& s, const In* x, const In* g, float* scratch, float* dw, cudaStream_t st,
                         const char* what) {
   const int n_split = wgrad_splits(s);
   const long long P = wgrad_pixels(s);
@@ -712,11 +756,12 @@ static int launch_wgrad(const WgradShape& s, const float* x, const float* g, flo
   const int ntaps = s.kt * s.kh * s.kw;
   const long long tiles = (long long)ntaps * ceil_div(s.cout, kWgTile) * ceil_div(s.cin, kWgTile);
   if (tiles >= 65536) return stp3::set_error(STP3_EINVAL, "%s: too many output tiles", what);
-  // float4 loads need 16-byte aligned rows
-  const int vec_x = s.x_cstride % 4 == 0 && (reinterpret_cast<uintptr_t>(x) & 15) == 0;
-  const int vec_g = s.g_cstride % 4 == 0 && (reinterpret_cast<uintptr_t>(g) & 15) == 0;
-  const size_t smem = 4 * kWgTileBytes + 1024;
-  wgrad_partial_kernel<<<dim3(n_split, (unsigned)tiles), 128, smem, st>>>(x, g, s, per, vec_x, vec_g, scratch);
+  // 16-byte loads need 16-byte aligned rows
+  constexpr int kPerChunk = 16 / sizeof(In);
+  const int vec_x = s.x_cstride % kPerChunk == 0 && (reinterpret_cast<uintptr_t>(x) & 15) == 0;
+  const int vec_g = s.g_cstride % kPerChunk == 0 && (reinterpret_cast<uintptr_t>(g) & 15) == 0;
+  const size_t smem = (OP == 0 ? 4 : 2) * kWgTileBytes + 1024;
+  wgrad_partial_kernel<OP><<<dim3(n_split, (unsigned)tiles), 128, smem, st>>>(x, g, s, per, vec_x, vec_g, scratch);
   STP3_CUDA_OK(cudaGetLastError());
   const long long n = (long long)ntaps * s.cout * s.cin;
   wgrad_reduce_kernel<<<blocks_for(n), 256, 0, st>>>(scratch, n_split, ntaps, s.cout, s.cin, dw);
@@ -763,6 +808,51 @@ extern "C" int stp3_conv3d_wgrad(const float* x, int B, int T, int H, int W, int
   return launch_wgrad(s, x, g, (float*)scratch, dw, (cudaStream_t)stream, "stp3_conv3d_wgrad");
 }
 
+static int launch_wgrad_plane(int operand, const WgradShape& s, const void* x, const void* g, void* scratch, float* dw,
+                              void* stream, const char* what) {
+  const uint16_t* xs = static_cast<const uint16_t*>(x);
+  const uint16_t* gs = static_cast<const uint16_t*>(g);
+  if (operand == STP3_OPERAND_F16)
+    return launch_wgrad<STP3_OPERAND_F16>(s, xs, gs, (float*)scratch, dw, (cudaStream_t)stream, what);
+  return launch_wgrad<STP3_OPERAND_BF16>(s, xs, gs, (float*)scratch, dw, (cudaStream_t)stream, what);
+}
+
+extern "C" int stp3_conv_wgrad_plane(int operand, const void* x, int n_img, int H, int W, int x_cstride, int cin,
+                                     const void* g, int Ho, int Wo, int g_cstride, int cout, int kh, int kw, int stride,
+                                     int pad, int dilation, void* scratch, size_t scratch_bytes, float* dw,
+                                     void* stream) {
+  STP3_CHECK_ARG(operand == STP3_OPERAND_BF16 || operand == STP3_OPERAND_F16,
+                 "stp3_conv_wgrad_plane: operand must be STP3_OPERAND_BF16 or STP3_OPERAND_F16");
+  STP3_CHECK_ARG(x && g && dw && scratch, "stp3_conv_wgrad_plane: null pointer argument");
+  STP3_CHECK_ARG(n_img > 0 && H > 0 && W > 0 && Ho > 0 && Wo > 0 && cin > 0 && cout > 0 && kh > 0 && kw > 0 && pad >= 0,
+                 "stp3_conv_wgrad_plane: non-positive dimension");
+  STP3_CHECK_ARG(stride == 1 || stride == 2, "stp3_conv_wgrad_plane: stride must be 1 or 2");
+  STP3_CHECK_ARG(dilation >= 1, "stp3_conv_wgrad_plane: dilation must be >= 1");
+  STP3_CHECK_ARG(cin <= x_cstride && cout <= g_cstride, "stp3_conv_wgrad_plane: channel count exceeds the row stride");
+  const size_t need = stp3_conv_wgrad_scratch_bytes(n_img, Ho, Wo, cout, cin, kh, kw, dilation);
+  STP3_CHECK_ARG(scratch_bytes >= need, "stp3_conv_wgrad_plane: scratch smaller than stp3_conv_wgrad_scratch_bytes()");
+  WgradShape s{n_img, H, W, x_cstride, cin, Ho, Wo, g_cstride, cout, stride, kh, kw, pad, dilation};
+  return launch_wgrad_plane(operand, s, x, g, scratch, dw, stream, "stp3_conv_wgrad_plane");
+}
+
+extern "C" int stp3_conv3d_wgrad_plane(int operand, const void* x, int B, int T, int H, int W, int x_cstride, int cin,
+                                       const void* g, int g_cstride, int cout, int kt, int kh, int kw, void* scratch,
+                                       size_t scratch_bytes, float* dw, void* stream) {
+  STP3_CHECK_ARG(operand == STP3_OPERAND_BF16 || operand == STP3_OPERAND_F16,
+                 "stp3_conv3d_wgrad_plane: operand must be STP3_OPERAND_BF16 or STP3_OPERAND_F16");
+  STP3_CHECK_ARG(x && g && dw && scratch, "stp3_conv3d_wgrad_plane: null pointer argument");
+  STP3_CHECK_ARG(B > 0 && T > 0 && H > 0 && W > 0 && cin > 0 && cout > 0 && kt > 0 && kh > 0 && kw > 0,
+                 "stp3_conv3d_wgrad_plane: non-positive dimension");
+  STP3_CHECK_ARG((long long)B * T <= INT_MAX, "stp3_conv3d_wgrad_plane: too many frames");
+  STP3_CHECK_ARG(kh == kw && kh % 2 == 1, "stp3_conv3d_wgrad_plane: the spatial kernel must be square and odd");
+  STP3_CHECK_ARG(cin <= x_cstride && cout <= g_cstride, "stp3_conv3d_wgrad_plane: channel count exceeds the row stride");
+  const size_t need = stp3_conv3d_wgrad_scratch_bytes(B, T, H, W, cout, cin, kt, kh, kw);
+  STP3_CHECK_ARG(scratch_bytes >= need, "stp3_conv3d_wgrad_plane: scratch smaller than stp3_conv3d_wgrad_scratch_bytes()");
+  WgradShape s{B * T, H, W, x_cstride, cin, H, W, g_cstride, cout, 1, kh, kw, (kh - 1) / 2, 1};
+  s.T = T; s.kt = kt;
+  return launch_wgrad_plane(operand, s, x, g, scratch, dw, stream, "stp3_conv3d_wgrad_plane");
+}
+
 extern "C" size_t stp3_bn_scratch_bytes(long long n_pix, int C) {
   if (n_pix <= 0 || C <= 0) return 0;
   return (size_t)red_parts(n_pix) * 2 * C * sizeof(double);
@@ -790,25 +880,26 @@ extern "C" int stp3_bn_stats(const float* x, long long n_pix, int C, int x_cstri
   return STP3_OK;
 }
 
-extern "C" int stp3_bn_apply(const float* x, long long n_pix, int C, int x_cstride, const float* mean,
-                             const float* invstd, const float* gamma, const float* beta, const float* res,
-                             int res_cstride, int relu, float dropout_p, unsigned long long seed,
-                             unsigned long long offset, float* y, int y_cstride, void* y_hi, void* y_lo, int hl_cstride,
-                             void* stream) {
+// stp3_bn_apply (OP 0: y_hi / y_lo) and stp3_bn_apply_plane (OP 1 / 2: one plane in y_hi, y_lo NULL)
+template <int OP>
+static int bn_apply(const float* x, long long n_pix, int C, int x_cstride, const float* mean, const float* invstd,
+                    const float* gamma, const float* beta, const float* res, int res_cstride, int relu, float dropout_p,
+                    unsigned long long seed, unsigned long long offset, float* y, int y_cstride, void* y_hi, void* y_lo,
+                    int hl_cstride, void* stream) {
   STP3_CHECK_ARG(x && mean && invstd && gamma && beta && (y || y_hi) && n_pix > 0 && C > 0, "stp3_bn_apply: bad argument");
   STP3_CHECK_ARG(dropout_p >= 0.f && dropout_p < 1.f, "stp3_bn_apply: dropout p must be in [0, 1)");
-  STP3_CHECK_ARG((y_hi == nullptr) == (y_lo == nullptr), "stp3_bn_apply: give both bf16 planes or neither");
+  if (OP == 0) STP3_CHECK_ARG((y_hi == nullptr) == (y_lo == nullptr), "stp3_bn_apply: give both bf16 planes or neither");
   STP3_CHECK_ARG(C <= x_cstride, "stp3_bn_apply: C exceeds the row stride");
   STP3_CHECK_ARG(!res || C <= res_cstride, "stp3_bn_apply: bad residual");
   STP3_CHECK_ARG(!y || C <= y_cstride, "stp3_bn_apply: bad fp32 output");
-  STP3_CHECK_ARG(!y_hi || (hl_cstride % 8 == 0 && C <= hl_cstride && al16(y_hi) && al16(y_lo)),
+  STP3_CHECK_ARG(!y_hi || (hl_cstride % 8 == 0 && C <= hl_cstride && al16(y_hi) && (OP != 0 || al16(y_lo))),
                  "stp3_bn_apply: bad bf16 planes");
   // 8 channels per thread with 128-bit accesses when every row allows it, else one element per thread
   const bool vec = C % 8 == 0 && x_cstride % 4 == 0 && al16(x) && (!res || (res_cstride % 4 == 0 && al16(res))) &&
                    (!y || (y_cstride % 4 == 0 && al16(y)));
   if (!vec) {
     const int n_cols = (y_hi && hl_cstride > C) ? hl_cstride : C;
-    bn_apply_scalar_kernel<<<blocks_for(n_pix * n_cols), 256, 0, (cudaStream_t)stream>>>(
+    bn_apply_scalar_kernel<OP><<<blocks_for(n_pix * n_cols), 256, 0, (cudaStream_t)stream>>>(
         x, x_cstride, mean, invstd, gamma, beta, res, res_cstride, relu, dropout_p, seed, offset, n_pix, C, n_cols, y,
         y_cstride, (__nv_bfloat16*)y_hi, (__nv_bfloat16*)y_lo, y_hi ? hl_cstride : 0);
     STP3_CUDA_OK(cudaGetLastError());
@@ -816,12 +907,35 @@ extern "C" int stp3_bn_apply(const float* x, long long n_pix, int C, int x_cstri
   }
   const int groups = ((y_hi && hl_cstride > C) ? hl_cstride : C) / 8;
   const long long total = n_pix * groups;
-  bn_apply_kernel<<<blocks_for(total), 256, 0, (cudaStream_t)stream>>>(
+  bn_apply_kernel<OP><<<blocks_for(total), 256, 0, (cudaStream_t)stream>>>(
       x, x_cstride, mean, invstd, gamma, beta, res, res_cstride, relu, dropout_p, seed, offset, n_pix, C, y, y_cstride,
       (__nv_bfloat16*)y_hi,
       (__nv_bfloat16*)y_lo, y_hi ? hl_cstride : 0);
   STP3_CUDA_OK(cudaGetLastError());
   return STP3_OK;
+}
+
+extern "C" int stp3_bn_apply(const float* x, long long n_pix, int C, int x_cstride, const float* mean,
+                             const float* invstd, const float* gamma, const float* beta, const float* res,
+                             int res_cstride, int relu, float dropout_p, unsigned long long seed,
+                             unsigned long long offset, float* y, int y_cstride, void* y_hi, void* y_lo, int hl_cstride,
+                             void* stream) {
+  return bn_apply<0>(x, n_pix, C, x_cstride, mean, invstd, gamma, beta, res, res_cstride, relu, dropout_p, seed, offset,
+                     y, y_cstride, y_hi, y_lo, hl_cstride, stream);
+}
+
+extern "C" int stp3_bn_apply_plane(const float* x, long long n_pix, int C, int x_cstride, const float* mean,
+                                   const float* invstd, const float* gamma, const float* beta, const float* res,
+                                   int res_cstride, int relu, float dropout_p, unsigned long long seed,
+                                   unsigned long long offset, float* y, int y_cstride, void* y_plane,
+                                   int plane_cstride, int operand, void* stream) {
+  STP3_CHECK_ARG(operand == STP3_OPERAND_BF16 || operand == STP3_OPERAND_F16,
+                 "stp3_bn_apply_plane: operand must be STP3_OPERAND_BF16 or STP3_OPERAND_F16");
+  if (operand == STP3_OPERAND_F16)
+    return bn_apply<2>(x, n_pix, C, x_cstride, mean, invstd, gamma, beta, res, res_cstride, relu, dropout_p, seed,
+                       offset, y, y_cstride, y_plane, nullptr, plane_cstride, stream);
+  return bn_apply<1>(x, n_pix, C, x_cstride, mean, invstd, gamma, beta, res, res_cstride, relu, dropout_p, seed, offset,
+                     y, y_cstride, y_plane, nullptr, plane_cstride, stream);
 }
 
 extern "C" int stp3_bn_bwd_reduce(const float* g, int g_cstride, const float* y, int y_cstride, const float* x,

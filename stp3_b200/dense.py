@@ -29,9 +29,10 @@ def out_tile(c: int) -> int:
 
 @dataclass
 class HL:
-    """(B, T, H, W, Cp) fp32 tensor carried as bf16 hi/lo planes; `c` = number of real channels."""
+    """(B, T, H, W, Cp) fp32 tensor carried as bf16 hi/lo planes; `c` = number of real channels.  lo None: ONE 16-bit
+    plane (hi.dtype torch.bfloat16 or torch.float16), the operand of the autocast train path (dense_train)."""
     hi: torch.Tensor
-    lo: torch.Tensor
+    lo: Optional[torch.Tensor]
     c: int
 
     @property
@@ -81,6 +82,23 @@ class PackedConv:
     k_lo: int = 0              # input channels [k_lo, k_hi) of the window carry weights (multiples of 16)
     k_hi: int = 0
     uid: int = 0               # identity of this packing for the autotune cache (a data_ptr can be reused after a repack)
+    plane: Optional[torch.dtype] = None   # None: w holds hi/lo planes; torch.bfloat16 / torch.float16: w is
+                                          # [ntaps][cin_p/64][bn][64] of that type (stp3_conv_fwd_plane)
+
+
+PLANE_OPERAND = {torch.bfloat16: _lib.OPERAND_BF16, torch.float16: _lib.OPERAND_F16}
+
+
+def pack_planes(m: torch.Tensor, plane: Optional[torch.dtype] = None) -> torch.Tensor:
+    """Tap matrices m (ntaps, bn, cin_p) fp32 -> the weight operand of stp3_conv_fwd: [tap][K block][hi, lo][bn][64] bf16,
+    or with plane (torch.bfloat16 / torch.float16) one plane [tap][K block][bn][64] of m rounded to that type."""
+    nt, bn, cin_p = m.shape
+    kbs = cin_p // KB
+    if plane is not None:
+        return m.to(plane).view(nt, bn, kbs, KB).permute(0, 2, 1, 3).contiguous()
+    hi, lo = split_hilo(m)
+    packed = torch.stack([hi.view(nt, bn, kbs, KB), lo.view(nt, bn, kbs, KB)], dim=0)   # (2, nt, bn, kbs, 64)
+    return packed.permute(1, 3, 0, 2, 4).contiguous()                                   # (nt, kbs, 2, bn, 64)
 
 
 _PACK_COUNTER = 0
@@ -89,10 +107,12 @@ _PACK_COUNTER = 0
 def pack_conv(weight: torch.Tensor, bias: torch.Tensor, *, stride: int = 1, dilation: int = 1,
               padding: Optional[int] = None, causal_time: bool = True, cin_p: Optional[int] = None,
               bn: Optional[int] = None, prune_extent: Optional[Tuple[int, int]] = None,
-              in_layout: Optional[Sequence[Tuple[int, int, int]]] = None) -> PackedConv:
+              in_layout: Optional[Sequence[Tuple[int, int, int]]] = None,
+              plane: Optional[torch.dtype] = None) -> PackedConv:
     """weight: (Cout, Cin, kh, kw) or (Cout, Cin, kt, kh, kw), already BN-folded; bias (Cout).
     Taps are (dt, dy, dx) input offsets: dy = ky*dilation - padding (padding defaults to 'same'); for 3-D kernels
-    dt = kt_index - (kt - 1) (causal: the reference pads time on the left only, temporal.py:256-262)."""
+    dt = kt_index - (kt - 1) (causal: the reference pads time on the left only, temporal.py:256-262).
+    plane (torch.bfloat16 / torch.float16): one plane of the weights rounded to that type (pack_planes)."""
     if weight.dim() == 4:
         weight = weight.unsqueeze(2)
     cout, cin, kt, kh, kw = weight.shape
@@ -120,12 +140,7 @@ def pack_conv(weight: torch.Tensor, bias: torch.Tensor, *, stride: int = 1, dila
                 for src, n, off in in_layout:
                     m[:cout, off:off + n] = weight[:, src:src + n, it, iy, ix]
                 mats.append(m)
-    w = torch.stack(mats)                                            # (ntaps, bn, cin_p)
-    hi, lo = split_hilo(w)
-    nt = len(taps)
-    kbs = cin_p // KB
-    packed = torch.stack([hi.view(nt, bn, kbs, KB), lo.view(nt, bn, kbs, KB)], dim=0)   # (2, nt, bn, kbs, 64)
-    packed = packed.permute(1, 3, 0, 2, 4).contiguous()              # (nt, kbs, 2, bn, 64)
+    packed = pack_planes(torch.stack(mats), plane)                   # mats: (ntaps, bn, cin_p)
     b = torch.zeros(bn, dtype=torch.float32, device=dev)
     b[:cout] = bias
     k_lo = min(off for _, _, off in in_layout) // 16 * 16
@@ -134,7 +149,7 @@ def pack_conv(weight: torch.Tensor, bias: torch.Tensor, *, stride: int = 1, dila
         k_lo, k_hi = 0, cin_p
     global _PACK_COUNTER
     _PACK_COUNTER += 1
-    return PackedConv(packed, b, taps, cin_p, bn, cout, stride, k_lo, k_hi, _PACK_COUNTER)
+    return PackedConv(packed, b, taps, cin_p, bn, cout, stride, k_lo, k_hi, _PACK_COUNTER, plane)
 
 
 # ------------------------------------------------------------------------------------------------ autotuner
@@ -264,6 +279,13 @@ def conv(x: HL, pc: PackedConv, *, cin_off: int = 0, out: Optional[HL] = None, o
         d.col_sums, d.col_sums_scratch, d.col_sums_scratch_bytes = col_sums.data_ptr(), scratch.data_ptr(), nbytes
     if img_bias is not None:
         assert img_bias.shape == (B * T, pc.bn) and img_bias.dtype == torch.float32 and img_bias.is_contiguous()
+    operand = PLANE_OPERAND[x.hi.dtype] if x.lo is None else _lib.OPERAND_HILO
+    if operand != _lib.OPERAND_HILO:      # one-plane operands: fp32 output only (stp3_conv_fwd_plane)
+        assert pc.plane == x.hi.dtype, (pc.plane, x.hi.dtype)
+        assert out_f32 is not None and out is None and out2 is None and residual is None and hd is None and \
+            scratch is None and not swish and not w_img_stride
+    else:
+        assert pc.plane is None, "one-plane weights need a one-plane input"
     dev = x.hi.device
     ptr = lambda t: t.data_ptr() if t is not None else None
 
@@ -273,6 +295,12 @@ def conv(x: HL, pc: PackedConv, *, cin_off: int = 0, out: Optional[HL] = None, o
         d.tune_n_sub, d.tune_group = n_sub, group & ~BLOCKS64
         d.tune_bn = 64 if group & BLOCKS64 and not one_block else 0
         with torch.cuda.device(dev):
+            if operand != _lib.OPERAND_HILO:
+                code = _lib.lib().stp3_conv_fwd_plane(
+                    ctypes.byref(d), operand, x.hi.data_ptr(), pc.w.data_ptr(), pc.bias.data_ptr(), ptr(img_bias),
+                    out_f32.data_ptr(), torch.cuda.current_stream(dev).cuda_stream)
+                _lib.check(code, "stp3_conv_fwd_plane")
+                return
             code = _lib.lib().stp3_conv_fwd(
                 ctypes.byref(d), x.hi.data_ptr(), x.lo.data_ptr(), pc.w.data_ptr(), pc.bias.data_ptr(), ptr(img_bias),
                 ptr(residual.hi if residual is not None else None), ptr(residual.lo if residual is not None else None),
@@ -286,7 +314,7 @@ def conv(x: HL, pc: PackedConv, *, cin_off: int = 0, out: Optional[HL] = None, o
     if cfg is None and _AUTOTUNE and not torch.cuda.is_current_stream_capturing():
         desc = f"{len(pc.taps)}tap cin{pc.cin_p} bn{pc.bn} s{pc.stride} {B * T}x{Ho}x{Wo}"
         # the tuner launches the layer many times: an output that aliases an input would be corrupted silently
-        ins = {x.hi.data_ptr(), x.lo.data_ptr()} | ({residual.hi.data_ptr(), residual.lo.data_ptr()} if residual is not None else set())
+        ins = {x.hi.data_ptr()} | ({x.lo.data_ptr()} if x.lo is not None else set()) | ({residual.hi.data_ptr(), residual.lo.data_ptr()} if residual is not None else set())
         outs = {t.data_ptr() for t in ((out.hi, out.lo) if out is not None else ()) + ((out2.hi, out2.lo) if out2 is not None else ())}
         assert not (ins & outs), "stp3_b200.dense.conv: output aliases an input (in-place convolution is not supported)"
         cfg = _tune(key, desc, launch, [c for c in tune_candidates(pc, per_image=w_img_stride > 0)

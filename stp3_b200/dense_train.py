@@ -7,6 +7,13 @@ the pyramid-pooling branch, and the bilinear x2 pair (dense, and on a channel wi
 
 Tensors are fp32 channels-last (N, H, W, C) contiguous; the inputs of the tensor-core convolutions are the usual
 bf16 hi/lo planes (dense.HL with T = 1).  Nothing here falls back to ATen convolutions or F.batch_norm.
+
+Autocast: a train-mode forward run under torch.autocast("cuda", dtype=torch.float16 / torch.bfloat16) takes its
+precision `mode` from amp_mode() and records it; the convolutions, input gradients and weight gradients of that step
+(forward and backward) then read ONE 16-bit plane per operand (dense.HL with lo None, weights rounded to the same type,
+as autocast rounds the operands of F.conv2d) and issue one MMA per product, accumulating in fp32.  mode None (outside
+autocast) is the fp32-equivalent hi/lo path, bit for bit.  BatchNorm statistics, running statistics and the BatchNorm
+backward stay fp32 in every mode, and so do the tensors the functions return.
 """
 from dataclasses import dataclass
 from typing import List, Optional, Tuple
@@ -41,10 +48,56 @@ def _row_stride(t: torch.Tensor) -> int:
     return cs
 
 
-def to_hl(x: torch.Tensor, cp: Optional[int] = None) -> dense.HL:
-    """(N, H, W, C) fp32 -> HL (N, 1, H, W, cp) bf16 hi/lo planes, padding channels zero."""
+def amp_mode() -> Optional[torch.dtype]:
+    """The precision mode of a train-mode forward: torch.float16 / torch.bfloat16 inside a CUDA autocast region of that
+    type, None (fp32-equivalent hi/lo operands) outside one."""
+    if not torch.is_autocast_enabled("cuda"):
+        return None
+    dt = torch.get_autocast_dtype("cuda")
+    return dt if dt in dense.PLANE_OPERAND else None
+
+
+def amp_kw(mode: Optional[torch.dtype]) -> dict:
+    """The keyword arguments that select `mode` in to_hl, bn_apply, conv_dgrad and conv_wgrad: none outside autocast,
+    so the fp32 path makes exactly the calls it always made.  That is a contract, not a style: the launch-by-launch
+    contract suites (tests/test_train_contract_gpu.py, tests/test_aux_contract_gpu.py) replace these functions with
+    recorders of their fp32 signatures while a train step runs, and a `mode=None` argument would break them."""
+    return {} if mode is None else {"mode": mode}
+
+
+def operand(t: torch.Tensor, mode: Optional[torch.dtype]):
+    """What conv_dgrad / conv_wgrad read: t itself outside autocast; under a mode, ONE plane of t (to_hl), so a
+    gradient that feeds both the input and the weight gradient is converted once.  A one-plane HL passes through."""
+    if mode is None or isinstance(t, dense.HL):
+        return t
+    return to_hl(t.reshape(-1, *t.shape[-3:]).contiguous(), mode=mode)
+
+
+def _dims(t) -> Tuple[int, int, int, int, int]:
+    """(images, H, W, channels, row stride) of an fp32 (N, H, W, C) / (B, T, H, W, C) tensor or a one-plane HL"""
+    if isinstance(t, dense.HL):
+        return t.hi.shape[0] * t.hi.shape[1], t.hi.shape[2], t.hi.shape[3], t.c, t.hi.shape[-1]
+    return t.numel() // (t.shape[-3] * t.shape[-2] * t.shape[-1]), t.shape[-3], t.shape[-2], t.shape[-1], t.shape[-1]
+
+
+def _plane_empty(N: int, H: int, W: int, cp: int, mode: torch.dtype, dev) -> dense.HL:
+    return dense.HL(torch.empty((N, 1, H, W, cp), dtype=mode, device=dev), None, 0)
+
+
+def to_hl(x: torch.Tensor, cp: Optional[int] = None, mode: Optional[torch.dtype] = None) -> dense.HL:
+    """(N, H, W, C) fp32 -> HL (N, 1, H, W, cp) bf16 hi/lo planes, padding channels zero.  mode (torch.float16 /
+    torch.bfloat16): ONE plane of that type instead (lo None), x rounded to nearest even, overflow to +-inf
+    (stp3_f32_to_plane)."""
     _f32_cl(x)
     N, H, W, C = x.shape
+    if mode is not None:
+        out = _plane_empty(N, H, W, cp or dense.pad_to(C), mode, x.device)
+        out.c = C
+        with torch.cuda.device(x.device):
+            code = _lib.lib().stp3_f32_to_plane(x.data_ptr(), 1, N, C, H, W, out.hi.shape[-1], dense.PLANE_OPERAND[mode],
+                                                out.hi.data_ptr(), _stream(x.device))
+        _lib.check(code, "stp3_f32_to_plane")
+        return out
     out = dense.HL.empty(N, 1, H, W, C, x.device, cp=cp)
     with torch.cuda.device(x.device):
         code = _lib.lib().stp3_f32_to_hilo(x.data_ptr(), 1, N, C, H, W, out.hi.shape[-1], out.hi.data_ptr(),
@@ -54,22 +107,20 @@ def to_hl(x: torch.Tensor, cp: Optional[int] = None) -> dense.HL:
 
 
 # ------------------------------------------------------------------------------------------------ convolutions
-def _pack_taps(mats: List[torch.Tensor], taps: List[Tuple[int, ...]], cin: int, cout: int) -> dense.PackedConv:
+def _pack_taps(mats: List[torch.Tensor], taps: List[Tuple[int, ...]], cin: int, cout: int,
+               plane: Optional[torch.dtype] = None) -> dense.PackedConv:
     """Weight matrices (cout, cin) of arbitrary (dy, dx) or (dt, dy, dx) taps -> the tap-major / K-major layout of
-    stp3_conv_fwd."""
+    stp3_conv_fwd (plane: one plane of that 16-bit type, stp3_conv_fwd_plane)."""
     cin_p, bn = dense.pad_to(cin), dense.out_tile(cout)
     dev = mats[0].device
     m = torch.zeros((len(mats), bn, cin_p), dtype=torch.float32, device=dev)
     for i, w in enumerate(mats):
         m[i, :cout, :cin] = w
-    hi, lo = dense.split_hilo(m)
-    nt, kbs = len(mats), cin_p // dense.KB
-    packed = torch.stack([hi.view(nt, bn, kbs, dense.KB), lo.view(nt, bn, kbs, dense.KB)], dim=0)
-    packed = packed.permute(1, 3, 0, 2, 4).contiguous()
+    packed = dense.pack_planes(m, plane)
     bias = torch.zeros(bn, dtype=torch.float32, device=dev)
     dense._PACK_COUNTER += 1
     return dense.PackedConv(packed, bias, [tuple(t) if len(t) == 3 else (0, *t) for t in taps], cin_p, bn, cout, 1, 0,
-                            cin_p, dense._PACK_COUNTER)
+                            cin_p, dense._PACK_COUNTER, plane)
 
 
 def dgrad_taps(kh: int, kw: int, stride: int, pad: int, dilation: int = 1):
@@ -103,16 +154,16 @@ def dgrad_taps_3d(kt: int, kh: int, kw: int):
     return [(it, ky, kx, kt - 1 - it, pad - ky, pad - kx) for it in range(kt) for ky in range(kh) for kx in range(kw)]
 
 
-def pack_dgrad3d(weight: torch.Tensor) -> dense.PackedConv:
+def pack_dgrad3d(weight: torch.Tensor, plane: Optional[torch.dtype] = None) -> dense.PackedConv:
     """weight (cout, cin, kt, kh, kw) of a causal 3-D convolution -> the transposed (cin x cout) tap matrices with the
     anti-causal taps of dgrad_taps_3d, for stp3_conv_fwd on the output gradient."""
     w = weight.detach().float()
     cout, cin, kt, kh, kw = w.shape
     taps = dgrad_taps_3d(kt, kh, kw)
-    return _pack_taps([w[:, :, it, ky, kx].t() for it, ky, kx, _, _, _ in taps], [t[3:] for t in taps], cout, cin)
+    return _pack_taps([w[:, :, it, ky, kx].t() for it, ky, kx, _, _, _ in taps], [t[3:] for t in taps], cout, cin, plane)
 
 
-def pack_dgrad(weight: torch.Tensor, stride: int, pad: int, dilation: int = 1):
+def pack_dgrad(weight: torch.Tensor, stride: int, pad: int, dilation: int = 1, plane: Optional[torch.dtype] = None):
     """weight (cout, cin, kh, kw) -> [((py, px), PackedConv or None)]: the transposed (cin x cout) tap matrices of every
     phase, for stp3_conv_fwd on the output gradient."""
     w = weight.detach().float()
@@ -123,7 +174,7 @@ def pack_dgrad(weight: torch.Tensor, stride: int, pad: int, dilation: int = 1):
             out.append((ph, None))
             continue
         mats = [w[:, :, ky, kx].t() for ky, kx, _, _ in taps]
-        out.append((ph, _pack_taps(mats, [(ey, ex) for _, _, ey, ex in taps], cout, cin)))
+        out.append((ph, _pack_taps(mats, [(ey, ex) for _, _, ey, ex in taps], cout, cin, plane)))
     return out
 
 
@@ -134,10 +185,12 @@ def conv_raw(x: dense.HL, weight: torch.Tensor, stride: int, bias: Optional[torc
     stp3_conv_fwd: (N, Ho, Wo, cout) fp32 channels-last, or (N, cout, Ho, Wo) with nchw (the reference's logits layout,
     optional sigmoid), N = B*T images of x (B, T, H, W, .).  A 5-D weight (cout, cin, kt, kh, kw) is the causal 3-D
     convolution of the TemporalBlocks (time padded on the left, stride 1).  img_bias (N, out_tile(cout)) replaces the
-    bias per image."""
+    bias per image.  A one-plane x (to_hl / bn_apply with a mode) runs the one-product convolution on the weights
+    rounded to x's type."""
     cout = weight.shape[0]
     b = bias.detach().float() if bias is not None else torch.zeros(cout, device=weight.device)
-    pc = dense.pack_conv(weight.detach().float(), b, stride=stride, dilation=dilation)
+    plane = x.hi.dtype if x.lo is None else None
+    pc = dense.pack_conv(weight.detach().float(), b, stride=stride, dilation=dilation, plane=plane)
     B, T, H, W, _ = x.hi.shape
     N = B * T
     Ho, Wo = (H + stride - 1) // stride, (W + stride - 1) // stride
@@ -151,29 +204,33 @@ def conv_raw(x: dense.HL, weight: torch.Tensor, stride: int, bias: Optional[torc
 
 
 def conv_dgrad(g: torch.Tensor, weight: torch.Tensor, stride: int, H: int, W: int,
-               packed=None, dilation: int = 1, img_bias: Optional[torch.Tensor] = None, T: int = 1) -> torch.Tensor:
+               packed=None, dilation: int = 1, img_bias: Optional[torch.Tensor] = None, T: int = 1,
+               mode: Optional[torch.dtype] = None) -> torch.Tensor:
     """dL/dx (N, H, W, cin) of a 'same'-padded convolution from g = dL/dy (N, Ho, Wo, cout).  Stride 1 only: img_bias
     (N, out_tile(cin)) is added to every pixel of image n (a spatially constant gradient term, for free).  A 5-D weight
     (cout, cin, kt, kh, kw) is the causal 3-D convolution of conv_raw on N = B*T frames (T given): its input gradient is
-    one stp3_conv_fwd with the anti-causal taps of dgrad_taps_3d."""
-    _f32_cl(g)
+    one stp3_conv_fwd with the anti-causal taps of dgrad_taps_3d.  mode (the forward's amp_mode()): g and the weights
+    as one plane of that type, one product each; g may then be its plane already (operand())."""
+    if isinstance(g, dense.HL):
+        assert mode is not None and g.lo is None and g.hi.dtype == mode
+    else:
+        _f32_cl(g)
+    N, cout, dev = _dims(g)[0], _dims(g)[3], (g.hi if isinstance(g, dense.HL) else g).device
     if weight.dim() == 5:
-        N, _, _, cout = g.shape
         cin = weight.shape[1]
         assert N % T == 0 and stride == 1 and dilation == 1
-        pc = packed if packed is not None else pack_dgrad3d(weight)
-        g_hl = to_hl(g)
-        g_hl = dense.HL(g_hl.hi.view(N // T, T, *g_hl.hi.shape[2:]), g_hl.lo.view(N // T, T, *g_hl.lo.shape[2:]), cout)
-        out = torch.empty((N, H, W, cin), dtype=torch.float32, device=g.device)
+        pc = packed if packed is not None else pack_dgrad3d(weight, mode)
+        g_hl = operand(g, mode) if mode is not None else to_hl(g)
+        g_hl = dense.HL(g_hl.hi.view(N // T, T, *g_hl.hi.shape[2:]),
+                        g_hl.lo.view(N // T, T, *g_hl.lo.shape[2:]) if g_hl.lo is not None else None, cout)
+        out = torch.empty((N, H, W, cin), dtype=torch.float32, device=dev)
         dense.conv(g_hl, pc, out_f32=out, n_valid=cin, out_f32_nhwc=True, out_hw=(H, W), store=False, tune=(0, 0),
                    img_bias=img_bias)
         return out
     cout, cin, kh, kw = weight.shape
     pad = (kh - 1) * dilation // 2
-    N = g.shape[0]
-    packed = packed if packed is not None else pack_dgrad(weight, stride, pad, dilation)
-    g_hl = to_hl(g)
-    dev = g.device
+    packed = packed if packed is not None else pack_dgrad(weight, stride, pad, dilation, mode)
+    g_hl = operand(g, mode) if mode is not None else to_hl(g)
     if stride == 1:
         out = torch.empty((N, H, W, cin), dtype=torch.float32, device=dev)
         dense.conv(g_hl, packed[0][1], out_f32=out, n_valid=cin, out_f32_nhwc=True, out_hw=(H, W), store=False,
@@ -205,10 +262,14 @@ def phase_interleave(phases: List[Optional[torch.Tensor]], H: int, W: int) -> to
 
 
 def conv_wgrad(x: torch.Tensor, g: torch.Tensor, kh: int, kw: int, stride: int, dilation: int = 1,
-               kt: Optional[int] = None) -> torch.Tensor:
+               kt: Optional[int] = None, mode: Optional[torch.dtype] = None) -> torch.Tensor:
     """dL/dW (cout, cin, kh, kw) of a 'same'-padded convolution: x (N, H, W, cin) its input, g (N, Ho, Wo, cout).
     x and g 5-D (B, T, H, W, .) with kt: the causal 3-D convolution of conv_raw, dL/dW (cout, cin, kt, kh, kw)
-    (stp3_conv3d_wgrad)."""
+    (stp3_conv3d_wgrad).  mode (the forward's amp_mode()): the one-product weight gradient on x and g rounded to one
+    plane of that type (stp3_conv_wgrad_plane / stp3_conv3d_wgrad_plane); either may then be its plane already
+    (operand(), or the plane the forward convolution read), of N = B*T images for the 3-D one."""
+    if mode is not None:
+        return _conv_wgrad_plane(x, g, kh, kw, stride, dilation, kt, mode)
     L = _lib.lib()
     if x.dim() == 5:
         assert kt is not None and stride == 1 and dilation == 1 and x.shape[:4] == g.shape[:4]
@@ -234,6 +295,41 @@ def conv_wgrad(x: torch.Tensor, g: torch.Tensor, kh: int, kw: int, stride: int, 
                                  (kh - 1) * dilation // 2, dilation, scratch.data_ptr(), nbytes, dw.data_ptr(),
                                  _stream(x.device))
     _lib.check(code, "stp3_conv_wgrad")
+    return dw
+
+
+def _conv_wgrad_plane(x, g, kh: int, kw: int, stride: int, dilation: int, kt: Optional[int],
+                      mode: torch.dtype) -> torch.Tensor:
+    L = _lib.lib()
+    op = dense.PLANE_OPERAND[mode]
+    fp32 = [t for t in (x, g) if not isinstance(t, dense.HL)]
+    B_T = fp32[0].shape[:2] if fp32 and fp32[0].dim() == 5 else None
+    xp, gp = operand(x, mode), operand(g, mode)
+    for t in (xp, gp):
+        assert t.lo is None and t.hi.dtype == mode, "one-plane operands of the autocast type"
+    N, H, W, cin, xcs = _dims(xp)
+    Ng, Ho, Wo, cout, gcs = _dims(gp)
+    assert N == Ng
+    dev = xp.hi.device
+    if kt is not None:
+        assert B_T is not None and stride == 1 and dilation == 1 and (Ho, Wo) == (H, W), "3-D: x or g (B, T, H, W, C)"
+        B, T = B_T
+        nbytes = L.stp3_conv3d_wgrad_scratch_bytes(B, T, H, W, cout, cin, kt, kh, kw)
+        scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+        dw = torch.empty((cout, cin, kt, kh, kw), dtype=torch.float32, device=dev)
+        with torch.cuda.device(dev):
+            code = L.stp3_conv3d_wgrad_plane(op, xp.hi.data_ptr(), B, T, H, W, xcs, cin, gp.hi.data_ptr(), gcs, cout,
+                                             kt, kh, kw, scratch.data_ptr(), nbytes, dw.data_ptr(), _stream(dev))
+        _lib.check(code, "stp3_conv3d_wgrad_plane")
+        return dw
+    nbytes = L.stp3_conv_wgrad_scratch_bytes(N, Ho, Wo, cout, cin, kh, kw, dilation)
+    scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+    dw = torch.empty((cout, cin, kh, kw), dtype=torch.float32, device=dev)
+    with torch.cuda.device(dev):
+        code = L.stp3_conv_wgrad_plane(op, xp.hi.data_ptr(), N, H, W, xcs, cin, gp.hi.data_ptr(), Ho, Wo, gcs, cout,
+                                       kh, kw, stride, (kh - 1) * dilation // 2, dilation, scratch.data_ptr(), nbytes,
+                                       dw.data_ptr(), _stream(dev))
+    _lib.check(code, "stp3_conv_wgrad_plane")
     return dw
 
 
@@ -361,10 +457,12 @@ def _bn_stats_sync(x: torch.Tensor, bn: nn.SyncBatchNorm, group) -> BNStats:
 
 def bn_apply(x: torch.Tensor, st: BNStats, gamma: torch.Tensor, beta: torch.Tensor, relu: bool,
              res: Optional[torch.Tensor] = None, hl: bool = True, dropout: Tuple[float, int, int] = (0.0, 0, 0),
-             y_out: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, Optional[dense.HL]]:
+             y_out: Optional[torch.Tensor] = None,
+             mode: Optional[torch.dtype] = None) -> Tuple[torch.Tensor, Optional[dense.HL]]:
     """y = relu?(xhat * gamma + beta (+ res)) [* keep / (1 - p)] -> (fp32 (N, H, W, C), HL planes for the next
     convolution or None).  dropout = (p, seed, offset): the keep bits of stp3_bn_apply.  y_out: where y goes (default a
-    new tensor; a channel slice of a wider channels-last tensor is fine)."""
+    new tensor; a channel slice of a wider channels-last tensor is fine).  mode (torch.float16 / torch.bfloat16): the
+    planes are ONE plane of that type (stp3_bn_apply_plane), y and the dropout bits unchanged."""
     _f32_cl(x)
     N, H, W, C = x.shape
     dev = x.device
@@ -372,12 +470,23 @@ def bn_apply(x: torch.Tensor, st: BNStats, gamma: torch.Tensor, beta: torch.Tens
     assert y.shape == x.shape
     y_cs = _row_stride(y)
     p, seed, offset = dropout
-    out = dense.HL.empty(N, 1, H, W, C, dev) if hl else None
+    if hl and mode is not None:
+        out = _plane_empty(N, H, W, dense.pad_to(C), mode, dev)
+        out.c = C
+    else:
+        out = dense.HL.empty(N, 1, H, W, C, dev) if hl else None
     g, b = gamma.detach().float().contiguous(), beta.detach().float().contiguous()
     if res is not None:
         _f32_cl(res)
         assert res.shape == x.shape
     with torch.cuda.device(dev):
+        if out is not None and out.lo is None:
+            code = _lib.lib().stp3_bn_apply_plane(x.data_ptr(), N * H * W, C, C, st.mean.data_ptr(), st.invstd.data_ptr(),
+                                                  g.data_ptr(), b.data_ptr(), _p(res), C, int(relu), float(p), int(seed),
+                                                  int(offset), y.data_ptr(), y_cs, out.hi.data_ptr(), out.hi.shape[-1],
+                                                  dense.PLANE_OPERAND[mode], _stream(dev))
+            _lib.check(code, "stp3_bn_apply_plane")
+            return y, out
         code = _lib.lib().stp3_bn_apply(x.data_ptr(), N * H * W, C, C, st.mean.data_ptr(), st.invstd.data_ptr(),
                                         g.data_ptr(), b.data_ptr(), _p(res), C, int(relu), float(p), int(seed),
                                         int(offset), y.data_ptr(), y_cs,

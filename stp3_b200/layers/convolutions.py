@@ -184,7 +184,8 @@ class DeepLabHead(nn.Sequential, PackedModule):
         N, cin, H, W = x.shape
         dev = x.device
         x_cl = x.detach().permute(0, 2, 3, 1).contiguous()
-        x_hl = dense_train.to_hl(x_cl)
+        mode = dense_train.amp_mode()
+        x_hl = dense_train.to_hl(x_cl, **dense_train.amp_kw(mode))
         # the nb spatial branches write their activated outputs side by side: the projection's input
         cat = torch.empty((N, H, W, nb * h), dtype=torch.float32, device=dev)
         branches = []
@@ -206,41 +207,47 @@ class DeepLabHead(nn.Sequential, PackedModule):
         w_proj = proj.weight.detach().float().reshape(h, (nb + 1) * h)
         pbias = torch.zeros((N, dense.out_tile(h)), dtype=torch.float32, device=dev)
         dense.small_linear(v.view(N, h), w_proj[:, nb * h:].contiguous(), pbias, False)
-        praw = dense_train.conv_raw(dense_train.to_hl(cat), w_proj[:, :nb * h].reshape(h, nb * h, 1, 1), 1,
+        praw = dense_train.conv_raw(dense_train.to_hl(cat, **dense_train.amp_kw(mode)), w_proj[:, :nb * h].reshape(h, nb * h, 1, 1), 1,
                                     img_bias=pbias)
         proj_st = dense_train.bn_stats_module(praw, proj_bn)
         p = float(drop.p) if drop.training else 0.0
         seed = int(torch.randint(0, 2 ** 63 - 1, (1,)).item()) if p > 0 else 0     # torch.manual_seed reproduces it
-        z, z_hl = dense_train.bn_apply(praw, proj_st, proj_bn.weight, proj_bn.bias, relu=True, dropout=(p, seed, 0))
+        z, z_hl = dense_train.bn_apply(praw, proj_st, proj_bn.weight, proj_bn.bias, relu=True, dropout=(p, seed, 0),
+                                       **dense_train.amp_kw(mode))
         raw3 = dense_train.conv_raw(z_hl, self[1].weight, 1)
         st3 = dense_train.bn_stats_module(raw3, self[2])
-        y3, y3_hl = dense_train.bn_apply(raw3, st3, self[2].weight, self[2].bias, relu=True)
+        y3, y3_hl = dense_train.bn_apply(raw3, st3, self[2].weight, self[2].bias, relu=True, **dense_train.amp_kw(mode))
         out = dense_train.conv_raw(y3_hl, self[4].weight, 1, bias=self[4].bias, nchw=True)
-        tape = {"x": x_cl, "cat": cat, "branches": branches, "mean": mean, "v_raw": v_raw, "pst": pst, "v": v,
-                "praw": praw, "proj_st": proj_st, "p": p, "z": z, "raw3": raw3, "st3": st3, "y3": y3}
+        # x: what the branches' weight gradients read (under autocast the plane they multiplied, not an fp32 copy)
+        tape = {"x": x_cl if mode is None else x_hl, "shape": (N, H, W, cin), "cat": cat, "branches": branches, "mean": mean, "v_raw": v_raw, "pst": pst, "v": v,
+                "praw": praw, "proj_st": proj_st, "p": p, "z": z, "raw3": raw3, "st3": st3, "y3": y3, "mode": mode}
         return out, tape
 
     def _train_backward(self, tape, g_out: torch.Tensor, need_x: bool):
         """Reverse walk of _train_forward -> (dL/dx (N, Cin, H, W) or None, {parameter: gradient})."""
         aspp: ASPP = self[0]
         h, nb = self.hidden, 1 + len(aspp.rates)
-        x_cl = tape["x"]
-        N, H, W, cin = x_cl.shape
-        dev = x_cl.device
+        x_op = tape["x"]
+        N, H, W, cin = tape["shape"]
+        dev = tape["cat"].device
         grads = {}
+        mode = tape["mode"]       # the spatial convolutions' precision; the pooling branch's products stay fp32
+        op = lambda t: dense_train.operand(t, mode)     # noqa: E731  (one plane per gradient under autocast)
         conv3, bn3, cls = self[1], self[2], self[4]
         g = g_out.float().permute(0, 2, 3, 1).contiguous()
         grads[cls.bias] = dense_train.channel_sums(g)
-        grads[cls.weight] = dense_train.conv_wgrad(tape["y3"], g, 1, 1, 1)
-        g = dense_train.conv_dgrad(g, cls.weight, 1, H, W)
+        g_op = op(g)
+        grads[cls.weight] = dense_train.conv_wgrad(tape["y3"], g_op, 1, 1, 1, **dense_train.amp_kw(mode))
+        g = dense_train.conv_dgrad(g_op, cls.weight, 1, H, W, **dense_train.amp_kw(mode))
         g, grads[bn3.weight], grads[bn3.bias], _ = dense_train.bn_backward(g, tape["raw3"], tape["st3"], bn3.weight,
                                                                           tape["y3"])
-        grads[conv3.weight] = dense_train.conv_wgrad(tape["z"], g, 3, 3, 1)
+        g_op = op(g)
+        grads[conv3.weight] = dense_train.conv_wgrad(tape["z"], g_op, 3, 3, 1, **dense_train.amp_kw(mode))
         # dropout: z > 0 marks the kept positive elements (the projection BN's mask below); the 1 / (1 - p) factor of
         # the kept ones rides on the transposed 3x3 weights
         p = tape["p"]
         w3 = conv3.weight.detach().float() * (1.0 / (1.0 - p)) if p > 0 else conv3.weight
-        g = dense_train.conv_dgrad(g, w3, 1, H, W)
+        g = dense_train.conv_dgrad(g_op, w3, 1, H, W, **dense_train.amp_kw(mode))
         proj, proj_bn = aspp.project[0], aspp.project[1]
         g, grads[proj_bn.weight], grads[proj_bn.bias], _ = dense_train.bn_backward(g, tape["praw"], tape["proj_st"],
                                                                                   proj_bn.weight, tape["z"])
@@ -248,7 +255,9 @@ class DeepLabHead(nn.Sequential, PackedModule):
         w_proj = proj.weight.detach().float().reshape(h, (nb + 1) * h)
         gsum = dense_train.image_channel_sums(g)
         dw_pool = dense_train.conv_wgrad(tape["v"], gsum.view(N, 1, 1, h), 1, 1, 1)
-        grads[proj.weight] = torch.cat([dense_train.conv_wgrad(tape["cat"], g, 1, 1, 1), dw_pool], dim=1)
+        g_op = op(g)
+        grads[proj.weight] = torch.cat([dense_train.conv_wgrad(tape["cat"], g_op, 1, 1, 1, **dense_train.amp_kw(mode)),
+                                        dw_pool], dim=1)
         g_v = torch.empty((N, 1, 1, h), dtype=torch.float32, device=dev)
         dense.small_linear(gsum, w_proj[:, nb * h:].t().contiguous(), g_v.view(N, h), False)
         pconv, pbn = aspp.convs[nb][1], aspp.convs[nb][2]
@@ -264,14 +273,15 @@ class DeepLabHead(nn.Sequential, PackedModule):
             dense.small_linear(g_v.view(N, h), w1t.contiguous(), gx_pool, False)
         for i, (conv, bn, raw, st) in enumerate(tape["branches"]):
             sl = slice(i * h, (i + 1) * h)
-            gb = dense_train.conv_dgrad(g, w_proj[:, sl].reshape(h, h, 1, 1), 1, H, W)
+            gb = dense_train.conv_dgrad(g_op, w_proj[:, sl].reshape(h, h, 1, 1), 1, H, W, **dense_train.amp_kw(mode))
             gb, grads[bn.weight], grads[bn.bias], _ = dense_train.bn_backward(gb, raw, st, bn.weight,
                                                                              tape["cat"][..., sl])
             k, d = conv.kernel_size[0], conv.dilation[0]
-            grads[conv.weight] = dense_train.conv_wgrad(x_cl, gb, k, k, 1, dilation=d)
+            gb_op = op(gb)
+            grads[conv.weight] = dense_train.conv_wgrad(x_op, gb_op, k, k, 1, dilation=d, **dense_train.amp_kw(mode))
             if need_x:
-                gxi = dense_train.conv_dgrad(gb, conv.weight, 1, H, W, dilation=d,
-                                             img_bias=gx_pool if i == 0 else None)
+                gxi = dense_train.conv_dgrad(gb_op, conv.weight, 1, H, W, dilation=d,
+                                             img_bias=gx_pool if i == 0 else None, **dense_train.amp_kw(mode))
                 gx = gxi if gx is None else gx.add_(gxi)
         return (gx.permute(0, 3, 1, 2).contiguous() if need_x else None), grads
 
@@ -408,34 +418,41 @@ class UpsamplingConcat(PackedModule):
         cat[..., :cf].copy_(x.detach().permute(0, 2, 3, 1))
         dense_train.upsample2x_into(x_up.detach().permute(0, 2, 3, 1).contiguous(), cat, cf)
         conv0, bn0, conv1, bn1 = self.conv[0], self.conv[1], self.conv[3], self.conv[4]
-        raw0 = dense_train.conv_raw(dense_train.to_hl(cat), conv0.weight, 1)
+        mode = dense_train.amp_mode()
+        cat_hl = dense_train.to_hl(cat, **dense_train.amp_kw(mode))
+        raw0 = dense_train.conv_raw(cat_hl, conv0.weight, 1)
         st0 = dense_train.bn_stats_module(raw0, bn0)
-        y0, y0_hl = dense_train.bn_apply(raw0, st0, bn0.weight, bn0.bias, relu=True)
+        y0, y0_hl = dense_train.bn_apply(raw0, st0, bn0.weight, bn0.bias, relu=True, **dense_train.amp_kw(mode))
         raw1 = dense_train.conv_raw(y0_hl, conv1.weight, 1)
         st1 = dense_train.bn_stats_module(raw1, bn1)
         y1, _ = dense_train.bn_apply(raw1, st1, bn1.weight, bn1.bias, relu=True, hl=False)
-        tape = {"cat": cat, "cf": cf, "raw0": raw0, "st0": st0, "y0": y0, "raw1": raw1, "st1": st1, "y1": y1}
+        # cat: what conv0's weight gradient reads (under autocast the plane it multiplied, not an fp32 copy)
+        tape = {"cat": cat if mode is None else cat_hl, "shape": tuple(cat.shape), "cf": cf, "raw0": raw0, "st0": st0,
+                "y0": y0, "raw1": raw1, "st1": st1, "y1": y1, "mode": mode}
         return (y1 if channels_last else y1.permute(0, 3, 1, 2).contiguous()), tape
 
     def _train_backward(self, tape, g_out: torch.Tensor, channels_last: bool, need_up: bool, need_x: bool):
         """Reverse walk of _train_forward -> (dL/dx_to_upsample or None, dL/dx or None (both NCHW), {parameter: gradient})."""
         conv0, bn0, conv1, bn1 = self.conv[0], self.conv[1], self.conv[3], self.conv[4]
         cat, cf = tape["cat"], tape["cf"]
-        N, H, W, ccat = cat.shape
+        N, H, W, ccat = tape["shape"]
         grads = {}
         g = g_out.float().contiguous() if channels_last else g_out.float().permute(0, 2, 3, 1).contiguous()
         g, grads[bn1.weight], grads[bn1.bias], _ = dense_train.bn_backward(g, tape["raw1"], tape["st1"], bn1.weight,
                                                                           tape["y1"])
-        grads[conv1.weight] = dense_train.conv_wgrad(tape["y0"], g, 3, 3, 1)
-        g = dense_train.conv_dgrad(g, conv1.weight, 1, H, W)
+        mode = tape["mode"]
+        g_op = dense_train.operand(g, mode)                # one plane for both products under autocast
+        grads[conv1.weight] = dense_train.conv_wgrad(tape["y0"], g_op, 3, 3, 1, **dense_train.amp_kw(mode))
+        g = dense_train.conv_dgrad(g_op, conv1.weight, 1, H, W, **dense_train.amp_kw(mode))
         g, grads[bn0.weight], grads[bn0.bias], _ = dense_train.bn_backward(g, tape["raw0"], tape["st0"], bn0.weight,
                                                                           tape["y0"])
-        grads[conv0.weight] = dense_train.conv_wgrad(cat, g, 3, 3, 1)
+        g_op = dense_train.operand(g, mode)
+        grads[conv0.weight] = dense_train.conv_wgrad(cat, g_op, 3, 3, 1, **dense_train.amp_kw(mode))
         g_up = g_x = None
         if need_up or need_x:
             # the concat gradient splits: the fine map's channels as they are, the coarse map's through the adjoint of
             # the upsample, read from their window
-            g_cat = dense_train.conv_dgrad(g, conv0.weight, 1, H, W)
+            g_cat = dense_train.conv_dgrad(g_op, conv0.weight, 1, H, W, **dense_train.amp_kw(mode))
             if need_x:
                 g_x = g_cat[..., :cf].permute(0, 3, 1, 2).contiguous()
             if need_up:

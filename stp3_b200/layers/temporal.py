@@ -346,7 +346,8 @@ class TemporalBlock(PackedModule):
         h, cout = self.half_channels, self.out_channels
         dev = x.device
         TT = dense_train
-        x_hl = TT.to_hl(x)
+        mode = TT.amp_mode()
+        x_hl = TT.to_hl(x, **TT.amp_kw(mode))
 
         def x_conv(conv):                  # 1x1x1 convolution of x; the constant channels enter as a per-image bias
             w = conv.weight.detach().float().reshape(conv.out_channels, -1)
@@ -364,9 +365,10 @@ class TemporalBlock(PackedModule):
             raw = x_conv(e.conv)
             st = TT.bn_stats_module(raw, e.norm)
             if i < 2:
-                y, y_hl = TT.bn_apply(raw, st, e.norm.weight, e.norm.bias, relu=True)
+                y, y_hl = TT.bn_apply(raw, st, e.norm.weight, e.norm.bias, relu=True, **TT.amp_kw(mode))
                 cc = path[1]
-                y_hl = dense.HL(y_hl.hi.view(B, T, *y_hl.hi.shape[2:]), y_hl.lo.view(B, T, *y_hl.lo.shape[2:]), h)
+                y_hl = dense.HL(y_hl.hi.view(B, T, *y_hl.hi.shape[2:]),
+                                y_hl.lo.view(B, T, *y_hl.lo.shape[2:]) if y_hl.lo is not None else None, h)
                 raw2 = TT.conv_raw(y_hl, cc.conv.weight, 1)
                 st2 = TT.bn_stats_module(raw2, cc.norm)
                 TT.bn_apply(raw2, st2, cc.norm.weight, cc.norm.bias, relu=True, hl=False, y_out=cat[..., i * h:(i + 1) * h])
@@ -377,7 +379,10 @@ class TemporalBlock(PackedModule):
             entry.append((e, raw, st, y))
         agg = self.aggregation[0]
         wg = agg.conv.weight.detach().float().reshape(cout, -1)
-        tape = {"x": x, "const": const, "B": B, "T": T, "cat": cat, "entry": entry, "mids": mids}
+        # x: what the 1x1x1 convolutions' weight gradient reads (under autocast the plane they multiplied, not the fp32
+        # block input)
+        tape = {"x": x if mode is None else x_hl, "shape": (N, H, W, cs), "const": const, "B": B, "T": T, "cat": cat,
+                "entry": entry, "mids": mids, "mode": mode}
         pbias = None
         if self.use_pyramid_pooling:
             # per-frame means -> temporal pair mean (AvgPool3d with count_include_pad=False: T + 1 frames) -> 1x1x1 ->
@@ -403,7 +408,7 @@ class TemporalBlock(PackedModule):
             pbias = torch.zeros((N, dense.out_tile(cout)), dtype=torch.float32, device=dev)
             dense.small_linear(v.view(N, red), wg[:, 3 * h:].contiguous(), pbias, False)
             tape.update(m=m, v_raw=v_raw, pst=pst, v_full=v_full, v=v)
-        araw = TT.conv_raw(TT.to_hl(cat), wg[:, :3 * h].reshape(cout, 3 * h, 1, 1).contiguous(), 1, img_bias=pbias)
+        araw = TT.conv_raw(TT.to_hl(cat, **TT.amp_kw(mode)), wg[:, :3 * h].reshape(cout, 3 * h, 1, 1).contiguous(), 1, img_bias=pbias)
         ast = TT.bn_stats_module(araw, agg.norm)
         ya, _ = TT.bn_apply(araw, ast, agg.norm.weight, agg.norm.bias, relu=True, hl=False)
         tape.update(araw=araw, ast=ast, ya=ya)
@@ -423,10 +428,12 @@ class TemporalBlock(PackedModule):
         None, {parameter: gradient}).  No gradient reaches the constant channels (host-derived input data)."""
         TT = dense_train
         x, const, B, T, cat = tape["x"], tape["const"], tape["B"], tape["T"], tape["cat"]
-        N, H, W, cs = x.shape
+        mode = tape["mode"]       # the spatial convolutions' precision; the pooling branch's products stay fp32
+        op = lambda t: TT.operand(t, mode)     # noqa: E731  (one plane per gradient under autocast)
+        N, H, W, cs = tape["shape"]
         nc = 0 if const is None else const.shape[1]
         h, cout = self.half_channels, self.out_channels
-        dev = x.device
+        dev = cat.device
         grads = {}
         convs = self._x_convs()
         K = 3 * h + (cout if self.projection is not None else 0)
@@ -441,8 +448,9 @@ class TemporalBlock(PackedModule):
         wg = agg.conv.weight.detach().float().reshape(cout, -1)
         ga, grads[agg.norm.weight], grads[agg.norm.bias], _ = TT.bn_backward(g, tape["araw"], tape["ast"],
                                                                             agg.norm.weight, tape["ya"])
-        dw_agg = TT.conv_wgrad(cat, ga, 1, 1, 1).reshape(cout, 3 * h)
-        g_cat = TT.conv_dgrad(ga, wg[:, :3 * h].reshape(cout, 3 * h, 1, 1), 1, H, W)
+        ga_op = op(ga)
+        dw_agg = TT.conv_wgrad(cat, ga_op, 1, 1, 1, **TT.amp_kw(mode)).reshape(cout, 3 * h)
+        g_cat = TT.conv_dgrad(ga_op, wg[:, :3 * h].reshape(cout, 3 * h, 1, 1), 1, H, W, **TT.amp_kw(mode))
         gx_pool = None
         if self.use_pyramid_pooling:
             pcbr = self.pyramid_pooling.features[0].conv_bn_relu
@@ -477,11 +485,13 @@ class TemporalBlock(PackedModule):
                 g2, grads[cc.norm.weight], grads[cc.norm.bias], _ = TT.bn_backward(gi, raw2, st2, cc.norm.weight,
                                                                                   cat[..., sl])
                 kt = cc.conv.kernel_size[0]
-                grads[cc.conv.weight] = TT.conv_wgrad(y.view(B, T, H, W, h), g2.view(B, T, H, W, h), 3, 3, 1, kt=kt)
-                gi = TT.conv_dgrad(g2, cc.conv.weight, 1, H, W, T=T)
+                g2_op = op(g2) if mode is not None else g2.view(B, T, H, W, h)
+                grads[cc.conv.weight] = TT.conv_wgrad(y.view(B, T, H, W, h), g2_op, 3, 3, 1, kt=kt, **TT.amp_kw(mode))
+                gi = TT.conv_dgrad(g2 if mode is None else g2_op, cc.conv.weight, 1, H, W, T=T, **TT.amp_kw(mode))
             _, grads[e.norm.weight], grads[e.norm.bias], _ = TT.bn_backward(gi, raw, st, e.norm.weight, y,
                                                                             dx_out=graw[..., sl])
-        dw_x = TT.conv_wgrad(x, graw, 1, 1, 1).reshape(K, cs)
+        graw_op = op(graw)
+        dw_x = TT.conv_wgrad(x, graw_op, 1, 1, 1, **TT.amp_kw(mode)).reshape(K, cs)
         if nc:
             # the constant channels' columns: sum over images of (per-image sums of the pre-BN gradient) x const
             gs = TT.image_channel_sums(graw)
@@ -493,7 +503,8 @@ class TemporalBlock(PackedModule):
         gx = None
         if need_x:
             w_x = torch.cat([conv.weight.detach().float().reshape(conv.out_channels, -1)[:, :cs] for conv in convs], 0)
-            gx = TT.conv_dgrad(graw, w_x.reshape(K, cs, 1, 1).contiguous(), 1, H, W, img_bias=gx_pool)
+            gx = TT.conv_dgrad(graw_op, w_x.reshape(K, cs, 1, 1).contiguous(), 1, H, W, img_bias=gx_pool,
+                               **TT.amp_kw(mode))
             if self.projection is None:
                 gx.add_(g)
         return gx, grads

@@ -195,12 +195,13 @@ class Decoder(PackedModule):
         return out
 
     @staticmethod
-    def _cbn(inp, inp_hl, conv, bn, relu, res=None, hl=True):
+    def _cbn(inp, inp_hl, conv, bn, relu, res=None, hl=True, mode=None):
         """conv (no bias) -> BatchNorm with batch statistics (running ones updated) -> (+ res) -> relu?"""
         raw = dense_train.conv_raw(inp_hl, conv.weight, conv.stride[0])
         st = dense_train.bn_stats_module(raw, bn)
-        y, y_hl = dense_train.bn_apply(raw, st, bn.weight, bn.bias, relu, res, hl=hl)
-        return y, y_hl, {"inp": inp, "conv": conv, "bn": bn, "raw": raw, "st": st, "y": y, "relu": relu}
+        y, y_hl = dense_train.bn_apply(raw, st, bn.weight, bn.bias, relu, res, hl=hl, **dense_train.amp_kw(mode))
+        return y, y_hl, {"inp": inp, "hw": tuple(inp.shape[1:3]), "conv": conv, "bn": bn, "raw": raw, "st": st, "y": y,
+                         "relu": relu, "mode": mode}
 
     @staticmethod
     def _cbn_backward(rec, g, grads, need_input=True, want_masked=False):
@@ -210,11 +211,12 @@ class Decoder(PackedModule):
                                                            rec["y"] if rec["relu"] else None, want_masked)
         grads[bn.weight], grads[bn.bias] = dgamma, dbeta
         kh, kw = conv.kernel_size
-        grads[conv.weight] = dense_train.conv_wgrad(rec["inp"], g_raw, kh, kw, conv.stride[0])
+        mode = rec["mode"]
+        g_op = dense_train.operand(g_raw, mode)           # one plane for both products under autocast
+        grads[conv.weight] = dense_train.conv_wgrad(rec["inp"], g_op, kh, kw, conv.stride[0], **dense_train.amp_kw(mode))
         gin = None
         if need_input:
-            H, W = rec["inp"].shape[1:3]
-            gin = dense_train.conv_dgrad(g_raw, conv.weight, conv.stride[0], H, W)
+            gin = dense_train.conv_dgrad(g_op, conv.weight, conv.stride[0], *rec["hw"], **dense_train.amp_kw(mode))
         return gin, gm
 
     def _train_forward(self, x: torch.Tensor):
@@ -222,18 +224,23 @@ class Decoder(PackedModule):
         B, S, C, H, W = x.shape
         N = B * S
         x_cl = x.detach().permute(0, 1, 3, 4, 2).reshape(N, H, W, C).contiguous()
-        x_hl = dense_train.to_hl(x_cl)
-        tape = {"shape": (B, S, C, H, W), "x": x_cl, "blocks": [], "ups": [], "heads": []}
-        y, y_hl, tape["first"] = self._cbn(x_cl, x_hl, self.first_conv, self.bn1, relu=True)
+        mode = dense_train.amp_mode()
+        x_hl = dense_train.to_hl(x_cl, **dense_train.amp_kw(mode))
+        tape = {"shape": (B, S, C, H, W), "x": x_cl, "blocks": [], "ups": [], "heads": [], "mode": mode}
+        y, y_hl, tape["first"] = self._cbn(x_cl, x_hl, self.first_conv, self.bn1, relu=True, mode=mode)
+        if mode is not None:      # only the first convolution's weight gradient reads the input: keep its plane
+            tape["first"]["inp"] = x_hl
+            tape["x"] = None
         skips = []
         for name in ("layer1", "layer2", "layer3"):
             for blk in getattr(self, name):
                 r1 = r2 = rd = None
-                y1, y1_hl, r1 = self._cbn(y, y_hl, blk.conv1, blk.bn1, relu=True)
+                y1, y1_hl, r1 = self._cbn(y, y_hl, blk.conv1, blk.bn1, relu=True, mode=mode)
                 res = y
                 if blk.downsample is not None:
-                    res, _, rd = self._cbn(y, y_hl, blk.downsample[0], blk.downsample[1], relu=False, hl=False)
-                y, y_hl, r2 = self._cbn(y1, y1_hl, blk.conv2, blk.bn2, relu=True, res=res)
+                    res, _, rd = self._cbn(y, y_hl, blk.downsample[0], blk.downsample[1], relu=False, hl=False,
+                                           mode=mode)
+                y, y_hl, r2 = self._cbn(y1, y1_hl, blk.conv2, blk.bn2, relu=True, res=res, mode=mode)
                 tape["blocks"].append((name, r1, r2, rd))
             skips.append(y)
         # UpsamplingAdd: BN(conv1x1(up(x))) + skip == BN_{stats of up(conv1x1(x))}(up(conv1x1(x))) + skip: the 1x1 runs
@@ -243,7 +250,7 @@ class Decoder(PackedModule):
             low = dense_train.conv_raw(y_hl, conv.weight, 1)
             raw = dense_train.upsample2x(low)
             st = dense_train.bn_stats_module(raw, bn)
-            out, y_hl = dense_train.bn_apply(raw, st, bn.weight, bn.bias, relu=False, res=skip)
+            out, y_hl = dense_train.bn_apply(raw, st, bn.weight, bn.bias, relu=False, res=skip, **dense_train.amp_kw(mode))
             tape["ups"].append({"inp": y, "conv": conv, "bn": bn, "raw": raw, "st": st})
             y = out
         outs = []
@@ -255,8 +262,9 @@ class Decoder(PackedModule):
                 inp = y.view(B, S, Hh, Wh, c)[:, t_present].contiguous()
                 cp = y_hl.hi.shape[-1]
                 inp_hl = dense.HL(y_hl.hi.view(B, S, 1, Hh, Wh, cp)[:, t_present].contiguous(),
-                                  y_hl.lo.view(B, S, 1, Hh, Wh, cp)[:, t_present].contiguous(), y_hl.c)
-            z, z_hl, rec = self._cbn(inp, inp_hl, h[0], h[1], relu=True)
+                                  y_hl.lo.view(B, S, 1, Hh, Wh, cp)[:, t_present].contiguous() if y_hl.lo is not None
+                                  else None, y_hl.c)
+            z, z_hl, rec = self._cbn(inp, inp_hl, h[0], h[1], relu=True, mode=mode)
             sig = len(h) > 4
             o = dense_train.conv_raw(z_hl, h[3].weight, 1, bias=h[3].bias, sigmoid=sig, nchw=True)
             tape["heads"].append({"rec": rec, "conv": h[3], "z": z, "out": o, "sigmoid": sig, "present": present})
@@ -267,6 +275,7 @@ class Decoder(PackedModule):
     def _train_backward(self, tape, grads_out, need_x):
         """Reverse walk of _train_forward -> (dL/dx (B, S, C, H, W) or None, {parameter: gradient})."""
         B, S, C, H, W = tape["shape"]
+        mode = tape["mode"]
         grads = {}
         y = tape["y"]
         g = torch.zeros_like(y)
@@ -278,8 +287,9 @@ class Decoder(PackedModule):
             g_cl = go.permute(0, 2, 3, 1).contiguous()                      # (n, H, W, ko)
             conv = hd["conv"]
             grads[conv.bias] = dense_train.channel_sums(g_cl)
-            grads[conv.weight] = dense_train.conv_wgrad(hd["z"], g_cl, 1, 1, 1)
-            gz = dense_train.conv_dgrad(g_cl, conv.weight, 1, *hd["z"].shape[1:3])
+            g_op = dense_train.operand(g_cl, mode)
+            grads[conv.weight] = dense_train.conv_wgrad(hd["z"], g_op, 1, 1, 1, **dense_train.amp_kw(mode))
+            gz = dense_train.conv_dgrad(g_op, conv.weight, 1, *hd["z"].shape[1:3], **dense_train.amp_kw(mode))
             gin, _ = self._cbn_backward(hd["rec"], gz, grads)
             if hd["present"]:
                 g.view(B, S, *g.shape[1:])[:, t_present] += gin
@@ -292,9 +302,10 @@ class Decoder(PackedModule):
             g_raw, dgamma, dbeta, _ = dense_train.bn_backward(g, u["raw"], u["st"], bn.weight, None)
             grads[bn.weight], grads[bn.bias] = dgamma, dbeta
             g_low = dense_train.upsample2x_backward(g_raw)
-            grads[conv.weight] = dense_train.conv_wgrad(u["inp"], g_low, 1, 1, 1)
+            g_op = dense_train.operand(g_low, mode)
+            grads[conv.weight] = dense_train.conv_wgrad(u["inp"], g_op, 1, 1, 1, **dense_train.amp_kw(mode))
             skip_grads.append(g)                                             # + skip: identity
-            g = dense_train.conv_dgrad(g_low, conv.weight, 1, *u["inp"].shape[1:3])
+            g = dense_train.conv_dgrad(g_op, conv.weight, 1, *u["inp"].shape[1:3], **dense_train.amp_kw(mode))
         # skip_grads: up1 (skip = the decoder input), up2 (skip = out of layer1), up3 (skip = out of layer2)
         g_x = skip_grads[0]
         stage_skip = {"layer3": skip_grads[2], "layer2": skip_grads[1]}
