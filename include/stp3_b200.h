@@ -140,6 +140,33 @@ typedef struct stp3_lift_splat_kernel_plan {
 int stp3_lift_splat_plan(const stp3_lift_splat_desc* desc, const float* feat, const float* depth_logits, int out_layout,
                          int n_peers, stp3_lift_splat_kernel_plan* plan);
 
+/* Deterministic form of stp3_lift_splat_fwd (torch.use_deterministic_algorithms; DESIGN.md §3.14).  Same arguments,
+ * rules, frame-sharded and peer modes, and the scatter and finalize kernels stp3_lift_splat_plan reports, in their
+ * 64-bit fixed-point form:
+ *   - a pre-pass finds m_f, the largest finite |feature| of every frame f (all cameras and channels);
+ *   - every flushed fp32 partial of frame f is rounded to a multiple of 2^-k_f, k_f = 62 - (ceil(log2 m_f) +
+ *     ceil(log2(N*D*Hf*Wf))) (0 for an all-zero frame), and added as int64 (red.global.add.u64).  Probabilities are
+ *     <= 1, so no pillar sum reaches 2^63; integer addition is associative, so the sum does not depend on the order in
+ *     which CTAs and warps arrive;
+ *   - the finalize converts each int64 v to fp32 as __double2float_rn((double)v * 2^-k_f), then runs the unchanged
+ *     discount recurrence, hi/lo split and pool partials; the pool slices are added in a fixed order.
+ * Result: bitwise identical for the same inputs, build and GPU model.  A frame's values depend on that frame's inputs
+ * only (and, through the recurrence, on the earlier frames of its sample): not on the batch it sits in, on
+ * f_begin / f_count, or on the rank that computed it.  Within one fp32 ulp of the exact sum of the grid-rounded
+ * partials; the rounding adds at most 2^-(k_f+1) per partial.
+ * Non-finite values: a NaN or +-inf partial marks its pillar in a per-frame poison bitmap instead of being added; the
+ * finalize writes NaN into EVERY channel of a poisoned pillar in that frame, and the recurrence carries it into later
+ * frames.  Per-channel fidelity is given up on purpose: a loss scaler only needs to see the NaN.  Non-finite features
+ * are left out of m_f.
+ * Memory: the int64 grid is twice the fp32 one (perceive at B = 4: 246 MB instead of 123 MB; B = 8, S = 5, 400 x 400,
+ * C = 128: 6.6 GB instead of 3.3 GB).  The workspace holds >= stp3_lift_splat_det_workspace_bytes(desc) bytes, which
+ * is never less than stp3_lift_splat_workspace_bytes(desc); it obeys the same all-zero rule, so one zeroed workspace
+ * serves both entry points, in any interleaving. */
+size_t stp3_lift_splat_det_workspace_bytes(const stp3_lift_splat_desc* desc);
+int stp3_lift_splat_fwd_det(const stp3_lift_splat_desc* desc, const float* feat, const float* depth_logits,
+                            int32_t* ranks_out, float* pool_sum, void* workspace, size_t workspace_bytes,
+                            float* out, int out_layout, int n_peers, void* const* peer_out, void* stream);
+
 /* Backward of stp3_lift_splat_fwd (training through the drop-in, SURVEY.md row f2): given grad_out = dLoss/d out
  * (B,S,C,nx,ny) fp32 it returns grad_feat (B,S,N,C,Hf,Wf) and grad_depth_logits (B,S,N,D,Hf,Wf; may be NULL, and is not
  * written when use_depth_distribution == 0).  Replaces the autograd chain of the reference:
@@ -366,6 +393,13 @@ int stp3_hilo_to_f32(const void* hi, const void* lo, int n_img, int H, int W, in
                      void* stream);
 /* sums[img][c] = sum over the H*W pixels (fp32, (n_img, cstride)); cstride <= 1024 */
 int stp3_spatial_sum(const void* hi, const void* lo, int n_img, int HW, int cstride, float* sums, void* stream);
+/* stp3_spatial_sum in a fixed order (the deterministic mode): per image and channel, fp64 partial sums of hi + lo over
+ * fixed pixel ranges, added in range order and rounded once to fp32 -- the two passes of stp3_image_channel_sums.
+ * The result depends on the input values and shape only.  Same arguments and limits (n_img <= 65535, cstride <= 1024);
+ * scratch: stp3_spatial_sum_det_scratch_bytes(n_img, HW, cstride) bytes of device memory (no invariant). */
+size_t stp3_spatial_sum_det_scratch_bytes(int n_img, int HW, int cstride);
+int stp3_spatial_sum_det(const void* hi, const void* lo, int n_img, int HW, int cstride, float* sums, void* scratch,
+                         size_t scratch_bytes, void* stream);
 /* Spatially constant branches folded to a per-image bias of the consuming 1x1 convolution:
  *   m[c] = sums[c] * inv_hw for the C - n_const spatial channels, const_vals[img][c - (C - n_const)] for the trailing
  *       n_const spatially constant ones (their mean is the value); temporal != 0: averaged with the previous frame of

@@ -113,6 +113,11 @@ SIGNATURES = {
     "stp3_conv_fwd_plane": (_I, [ctypes.POINTER(ConvDesc), _I, _V, _V, _V, _V, _V, _V]),
     "stp3_lift_splat_fwd": (_I, [_LSD, _V, _V, _V, _V, _V, _SZ, _V, _I, _I, ctypes.POINTER(_V), _V]),
     "stp3_lift_splat_plan": (_I, [_LSD, _V, _V, _I, _I, ctypes.POINTER(LiftSplatPlan)]),
+    # deterministic mode (torch.use_deterministic_algorithms)
+    "stp3_lift_splat_det_workspace_bytes": (_SZ, [_LSD]),
+    "stp3_lift_splat_fwd_det": (_I, [_LSD, _V, _V, _V, _V, _V, _SZ, _V, _I, _I, ctypes.POINTER(_V), _V]),
+    "stp3_spatial_sum_det_scratch_bytes": (_SZ, [_I, _I, _I]),
+    "stp3_spatial_sum_det": (_I, [_V, _V, _I, _I, _I, _V, _V, _SZ, _V]),
     # train mode of the decoder and the DeepLab head
     "stp3_conv_wgrad_scratch_bytes": (_SZ, [_I, _I, _I, _I, _I, _I, _I, _I]),
     "stp3_conv_wgrad": (_I, [_V, _I, _I, _I, _I, _I, _V, _I, _I, _I, _I, _I, _I, _I, _I, _I, _V, _SZ, _V, _V]),

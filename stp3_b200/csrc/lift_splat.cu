@@ -21,6 +21,7 @@
 // Reference semantics: stp3/models/stp3.py:186-301, stp3/utils/geometry.py:299-318.
 #include <cuda_bf16.h>
 
+#include <algorithm>
 #include <cmath>
 #include <cstdint>
 #include <cstdlib>
@@ -61,10 +62,79 @@ struct LiftSplatParams {
   int32_t* ranks_out;
   float* grid;          // (B,S,nx*ny*nz,C) fp32, all-zero on entry
   unsigned char* occ;   // (B,S,nx*ny*nz) bytes, all-zero on entry; set to 1 where the grid was written
+  // fixed-point mode only (stp3_lift_splat_fwd_det), indexed by the frame's slot in this launch
+  long long* qgrid;         // (B,S,nx*ny*nz,C) int64 multiples of 2^-k_f, all-zero on entry
+  const unsigned* fmax;     // bits of m_f, the largest finite |feature| of the frame
+  unsigned* poison;         // per-frame bitmap of pillars that received a NaN or +-inf partial
+  int lp;                   // ceil(log2(N * D * Hf * Wf)): points per frame
 };
 
 __device__ __forceinline__ void red_add_v2(float* addr, float a, float b) {
   asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(addr), "f"(a), "f"(b) : "memory");
+}
+
+// ---- 64-bit fixed point (deterministic mode).  A frame's partials are rounded to multiples of 2^-k_f with
+// k_f = 62 - (ceil(log2 m_f) + ceil(log2 points)), so no pillar sum of the frame can reach 2^63 (every point adds at
+// most m_f: probabilities are <= 1), and summed as int64: integer addition is associative, so the result does not
+// depend on the order in which CTAs and warps arrive.
+__host__ __device__ inline int ceil_log2_f32(unsigned bits) {   // bits of a finite float > 0
+  const unsigned e = bits >> 23, m = bits & 0x7fffffu;
+  if (e == 0) {                                                // subnormal m * 2^-149: -149 + ceil(log2 m)
+    int c = 0;
+    while ((1u << c) < m) ++c;
+    return -149 + c;
+  }
+  return (int)e - 127 + (m != 0);
+}
+
+__host__ __device__ inline int frame_exponent(unsigned mbits, int lp) {
+  return mbits == 0 ? 0 : 62 - (ceil_log2_f32(mbits) + lp);
+}
+
+// k_f of the frame in launch slot `slot`: the one place the kernels look up a frame's scale
+__device__ __forceinline__ int slot_exponent(const unsigned* fmax, size_t slot, int lp) {
+  return frame_exponent(fmax[slot], lp);
+}
+
+__device__ __forceinline__ double pow2d(int k) { return __hiloint2double((k + 1023) << 20, 0); }   // |k| <= 1022
+
+__device__ __forceinline__ void red_add_u64(long long* addr, long long v) {
+  asm volatile("red.global.add.u64 [%0], %1;" ::"l"(addr), "l"(v) : "memory");
+}
+
+// where one frame's fixed-point partials go
+struct FxSink {
+  long long* grid;      // the frame's (pillar, C) int64 rows
+  unsigned* poison;     // the frame's poison bitmap
+  double scale;         // 2^k_f
+};
+
+__device__ __forceinline__ FxSink fx_sink(const LiftSplatParams& p, int bt, size_t nvox) {
+  FxSink s;
+  s.grid = p.qgrid + (size_t)bt * nvox * p.C;
+  s.poison = p.poison + (size_t)bt * ((nvox + 31) / 32);
+  s.scale = pow2d(slot_exponent(p.fmax, bt, p.lp));
+  return s;
+}
+
+__device__ __forceinline__ void fx_add(const FxSink& s, int rank, long long* dst, float a) {
+  if (isfinite(a)) {
+    const long long q = __double2ll_rn((double)a * s.scale);
+    if (q != 0) red_add_u64(dst, q);
+  } else {
+    atomicOr(s.poison + (rank >> 5), 1u << (rank & 31));
+  }
+}
+
+// fixed-point counterpart of flush_segment
+__device__ __forceinline__ void fx_flush(const FxSink& s, unsigned char* obase, int rank, int C, int c, bool mark,
+                                         float a0, float a1) {
+  if (c < C) {
+    long long* dst = s.grid + (size_t)rank * C + c;
+    fx_add(s, rank, dst, a0);
+    if (c + 1 < C) fx_add(s, rank, dst + 1, a1);
+  }
+  if (mark) obase[rank] = 1;
 }
 
 // shared-memory row of channel (c0 + cl) in the feature tile: the two channels of a lane (2*lane, 2*lane+1) live in
@@ -104,7 +174,8 @@ __device__ __forceinline__ void mma_bf16_m16n8k16(float (&c)[4], const uint32_t 
 //                            of pixels at one depth into one pillar), -1 if the whole column is masked,
 //                            -2 if the column spans several pillars (segmented slow path)
 //   s_feat [64][npix|1] f32  context features of 64 channels, row permuted by feat_row()
-template <int TW>
+// FX: fixed-point accumulation (see FxSink) instead of fp32 red.add.
+template <int TW, bool FX>
 __global__ void __launch_bounds__(kScatterThreads, 2)
 lift_splat_scatter_kernel(const LiftSplatParams p) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -258,6 +329,8 @@ lift_splat_scatter_kernel(const LiftSplatParams p) {
   float* gbase = p.grid + (size_t)bt * nvox * C;
   unsigned char* obase = p.occ + (size_t)bt * nvox;
   const bool vec_ok = (C % 2) == 0;
+  FxSink fx;
+  if constexpr (FX) fx = fx_sink(p, bt, nvox);
   for (int i = tid; i < kCChunk * (fstride - npix); i += nthr)     // zero padding of the feature rows (once)
     s_feat[(i / (fstride - npix)) * fstride + npix + i % (fstride - npix)] = 0.f;
   for (int c0 = 0; c0 < C; c0 += kCChunk) {
@@ -319,7 +392,8 @@ lift_splat_scatter_kernel(const LiftSplatParams p) {
                 a0 = fmaf(q.w, f0[4 * j4 + 3], a0); a1 = fmaf(q.w, f1[4 * j4 + 3], a1);
               }
             }
-            flush_segment(gbase, obase, col, C, c, vec_ok, mark, a0, a1);
+            if constexpr (FX) fx_flush(fx, obase, col, C, c, mark, a0, a1);
+            else flush_segment(gbase, obase, col, C, c, vec_ok, mark, a0, a1);
           } else {
             // slow path: segmented reduction over equal ranks along the column
             const int* rk = s_rank + (d * TW + wl) * HP + h0;
@@ -330,7 +404,10 @@ lift_splat_scatter_kernel(const LiftSplatParams p) {
               if (h0 + j < Hf) {
                 const int r = rk[j];
                 if (r != cur) {                      // warp-uniform: segment boundary
-                  if (cur >= 0) flush_segment(gbase, obase, cur, C, c, vec_ok, mark, a0, a1);
+                  if (cur >= 0) {
+                    if constexpr (FX) fx_flush(fx, obase, cur, C, c, mark, a0, a1);
+                    else flush_segment(gbase, obase, cur, C, c, vec_ok, mark, a0, a1);
+                  }
                   cur = r; a0 = 0.f; a1 = 0.f;
                 }
                 const float q = pr[j];
@@ -338,7 +415,10 @@ lift_splat_scatter_kernel(const LiftSplatParams p) {
                 a1 = fmaf(q, f1[j], a1);
               }
             }
-            if (cur >= 0) flush_segment(gbase, obase, cur, C, c, vec_ok, mark, a0, a1);
+            if (cur >= 0) {
+              if constexpr (FX) fx_flush(fx, obase, cur, C, c, mark, a0, a1);
+              else flush_segment(gbase, obase, cur, C, c, vec_ok, mark, a0, a1);
+            }
           }
         }
       }
@@ -393,6 +473,7 @@ struct LiftSplatTmaMaps {
   CUtensorMap feat;    // NCHW: (Wf, Hf, C * n_img) fp32 ; NHWC: (C, Wf, Hf * n_img) fp32
 };
 
+template <bool FX>
 __global__ void __launch_bounds__(kScatterThreads, 2)
 lift_splat_scatter_tma_kernel(const __grid_constant__ LiftSplatTmaMaps maps, const LiftSplatParams p) {
   extern __shared__ unsigned char smem_dyn[];
@@ -582,7 +663,9 @@ lift_splat_scatter_tma_kernel(const __grid_constant__ LiftSplatTmaMaps maps, con
   const size_t nvox = (size_t)p.nx * p.ny * p.nz;
   float* gbase = p.grid + (size_t)bt * nvox * C;
   unsigned char* obase = p.occ + (size_t)bt * nvox;
-  constexpr int KS = 2;                                          // k-steps of 16 image rows: Hf <= 32 (host-checked)
+  FxSink fx;
+  if constexpr (FX) fx = fx_sink(p, bt, nvox);
+  constexpr int KS = 2;                                         // k-steps of 16 image rows: Hf <= 32 (host-checked)
   const int n_mt = (D + 15) >> 4;
   const bool col_ok = w0 + wl < Wf;
   const int cmax = s_cinfo[wl];                                  // 0: nothing of this column lands in the grid
@@ -651,8 +734,19 @@ lift_splat_scatter_tma_kernel(const __grid_constant__ LiftSplatTmaMaps maps, con
             }
             // c0, c1 = (row g, columns 2tg, 2tg+1); c2, c3 = (row g+8, same columns)
             const int c = c0 + nhalf * 32 + nt * 8 + 2 * tg;
-            if (seg_lo >= 0) red_add_v2(gbase + (size_t)seg_lo * C + c, acc[0], acc[1]);
-            if (seg_hi >= 0) red_add_v2(gbase + (size_t)seg_hi * C + c, acc[2], acc[3]);
+            if constexpr (FX) {
+              if (seg_lo >= 0) {
+                fx_add(fx, seg_lo, fx.grid + (size_t)seg_lo * C + c, acc[0]);
+                fx_add(fx, seg_lo, fx.grid + (size_t)seg_lo * C + c + 1, acc[1]);
+              }
+              if (seg_hi >= 0) {
+                fx_add(fx, seg_hi, fx.grid + (size_t)seg_hi * C + c, acc[2]);
+                fx_add(fx, seg_hi, fx.grid + (size_t)seg_hi * C + c + 1, acc[3]);
+              }
+            } else {
+              if (seg_lo >= 0) red_add_v2(gbase + (size_t)seg_lo * C + c, acc[0], acc[1]);
+              if (seg_hi >= 0) red_add_v2(gbase + (size_t)seg_hi * C + c, acc[2], acc[3]);
+            }
           }
           if (c0 == 0 && nhalf == 0 && tg == 0) {
             if (seg_lo >= 0) obase[seg_lo] = 1;
@@ -681,7 +775,10 @@ lift_splat_scatter_tma_kernel(const __grid_constant__ LiftSplatTmaMaps maps, con
             for (int k = 0; k < kSegPasses; ++k) skip |= (r == ex[k]);
             if (skip) continue;                             // warp-uniform
             if (r != cur) {
-              if (cur >= 0) flush_segment(gbase, obase, cur, C, c, true, lane == 0 && c0 == 0, a0, a1);
+              if (cur >= 0) {
+                if constexpr (FX) fx_flush(fx, obase, cur, C, c, lane == 0 && c0 == 0, a0, a1);
+                else flush_segment(gbase, obase, cur, C, c, true, lane == 0 && c0 == 0, a0, a1);
+              }
               cur = r; a0 = 0.f; a1 = 0.f;
             }
             float f0, f1;
@@ -696,7 +793,10 @@ lift_splat_scatter_tma_kernel(const __grid_constant__ LiftSplatTmaMaps maps, con
             a0 = fmaf(q, f0, a0);
             a1 = fmaf(q, f1, a1);
           }
-          if (cur >= 0) flush_segment(gbase, obase, cur, C, c, true, lane == 0 && c0 == 0, a0, a1);
+          if (cur >= 0) {
+            if constexpr (FX) fx_flush(fx, obase, cur, C, c, lane == 0 && c0 == 0, a0, a1);
+            else flush_segment(gbase, obase, cur, C, c, true, lane == 0 && c0 == 0, a0, a1);
+          }
         }
       }
     }
@@ -713,10 +813,29 @@ lift_splat_scatter_tma_kernel(const __grid_constant__ LiftSplatTmaMaps maps, con
 // shared memory or barrier is needed.  Only occupied (frame, pillar) rows of the scatter grid are read; they are
 // zeroed again and their occupancy byte cleared, which leaves the workspace clean for the next call.
 // pool_sum (B,S,C) += sum over cells (optional).
-template <bool VEC, int SMAX>
+// Fixed-point finalize (stp3_lift_splat_fwd_det): what the FX kernels read instead of the fp32 grid.
+struct FxGrid {
+  long long* grid;          // int64 scatter grid, same layout as the fp32 one
+  const unsigned* fmax;     // per-frame bits of m_f
+  const unsigned* poison;   // per-frame pillar bitmaps
+  int lp;
+};
+
+// one int64 grid value of frame scale 2^-k as fp32 (the conversion the deterministic mode defines)
+__device__ __forceinline__ float fx_value(long long q, double inv_scale) {
+  return __double2float_rn((double)q * inv_scale);
+}
+
+__device__ __forceinline__ bool fx_poisoned(const FxGrid& fx, size_t frame, int nvox, int pcell) {
+  const size_t words = ((size_t)nvox + 31) / 32;
+  return (fx.poison[frame * words + (pcell >> 5)] >> (pcell & 31)) & 1u;
+}
+
+template <bool VEC, int SMAX, bool FX>
 __global__ void __launch_bounds__(256)
 bev_finalize_kernel(float* __restrict__ grid, unsigned char* __restrict__ occ, float* __restrict__ out,
-                    float* __restrict__ pool_sum, int S, int C, int nvox, float discount, int out_nhwc) {
+                    float* __restrict__ pool_sum, int S, int C, int nvox, float discount, int out_nhwc,
+                    const FxGrid fx) {
   const int b = blockIdx.y;
   const int lane = threadIdx.x;
   const int pcell = blockIdx.x * 32 + lane;
@@ -734,7 +853,17 @@ bev_finalize_kernel(float* __restrict__ grid, unsigned char* __restrict__ occ, f
   for (int t = 0; t < SMAX; ++t) {
 #pragma unroll
     for (int i = 0; i < 8; ++i) v[t][i] = 0.f;
-    if (occ_bits & (1u << t)) {
+    if constexpr (FX) {
+      if (occ_bits & (1u << t)) {
+        const size_t frame = (size_t)b * S + t;
+        const long long* src = fx.grid + (frame * nvox + pcell) * C + c0;
+        const double inv = pow2d(-slot_exponent(fx.fmax, frame, fx.lp));
+        const bool nan = fx_poisoned(fx, frame, nvox, pcell);
+#pragma unroll
+        for (int i = 0; i < 8; ++i)
+          if (VEC || c0 + i < C) v[t][i] = nan ? __int_as_float(0x7fffffff) : fx_value(__ldcs(src + i), inv);
+      }
+    } else if (occ_bits & (1u << t)) {
       const float* src = grid + (((size_t)b * S + t) * nvox + pcell) * C + c0;
       if (VEC) {
         const float4 lo = __ldcs(reinterpret_cast<const float4*>(src));
@@ -801,7 +930,13 @@ bev_finalize_kernel(float* __restrict__ grid, unsigned char* __restrict__ occ, f
   // warp of the CTA has read them)
 #pragma unroll
   for (int t = 0; t < SMAX; ++t) {
-    if (occ_bits & (1u << t)) {
+    if constexpr (FX) {
+      if (occ_bits & (1u << t)) {
+        long long* src = fx.grid + (((size_t)b * S + t) * nvox + pcell) * C + c0;
+#pragma unroll
+        for (int i = 0; i < 8; ++i) if (VEC || c0 + i < C) src[i] = 0;
+      }
+    } else if (occ_bits & (1u << t)) {
       float* src = grid + (((size_t)b * S + t) * nvox + pcell) * C + c0;
       if (VEC) {
         const float4 z = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -838,11 +973,11 @@ struct PeerOut {
   int first_slot;
 };
 
-template <int LPP, int SMAX, bool PEERS>
+template <int LPP, int SMAX, bool PEERS, bool FX>
 __global__ void __launch_bounds__(256)
 bev_finalize_cl_kernel(float* __restrict__ grid, unsigned char* __restrict__ occ, float* __restrict__ out,
                        float* __restrict__ pool_sum, int S, int nvox, float discount, int out_layout,
-                       const __grid_constant__ PeerOut peers) {
+                       const __grid_constant__ PeerOut peers, const FxGrid fx) {
   constexpr int C = LPP * 16, PPB = 256 / LPP;
   __shared__ float s_pool[8][SMAX][C];
   const int b = blockIdx.y;
@@ -860,7 +995,20 @@ bev_finalize_cl_kernel(float* __restrict__ grid, unsigned char* __restrict__ occ
   for (int t = 0; t < SMAX; ++t) {
 #pragma unroll
     for (int i = 0; i < 16; ++i) v[t][i] = 0u;
-    if (occ_bits & (1u << t)) {
+    if constexpr (FX) {
+      if (occ_bits & (1u << t)) {
+        const size_t frame = (size_t)b * S + t;
+        const longlong2* src = reinterpret_cast<const longlong2*>(fx.grid + (frame * nvox + pcell) * C + c0);
+        const double inv = pow2d(-slot_exponent(fx.fmax, frame, fx.lp));
+        const bool nan = fx_poisoned(fx, frame, nvox, pcell);
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+          const longlong2 q = __ldcs(src + i);
+          v[t][2 * i] = nan ? 0x7fffffffu : __float_as_uint(fx_value(q.x, inv));
+          v[t][2 * i + 1] = nan ? 0x7fffffffu : __float_as_uint(fx_value(q.y, inv));
+        }
+      }
+    } else if (occ_bits & (1u << t)) {
       const float* src = grid + (((size_t)b * S + t) * nvox + pcell) * C + c0;
       uint32_t a[8], c[8];
       ptx::ld_global_v8(src, a);
@@ -945,9 +1093,15 @@ bev_finalize_cl_kernel(float* __restrict__ grid, unsigned char* __restrict__ occ
 #pragma unroll
   for (int t = 0; t < SMAX; ++t) {
     if (occ_bits & (1u << t)) {
-      float* src = grid + (((size_t)b * S + t) * nvox + pcell) * C + c0;
-      ptx::st_global_v8(src, z);
-      ptx::st_global_v8(src + 8, z);
+      if constexpr (FX) {
+        long long* src = fx.grid + (((size_t)b * S + t) * nvox + pcell) * C + c0;
+#pragma unroll
+        for (int i = 0; i < 4; ++i) ptx::st_global_v8(src + 4 * i, z);
+      } else {
+        float* src = grid + (((size_t)b * S + t) * nvox + pcell) * C + c0;
+        ptx::st_global_v8(src, z);
+        ptx::st_global_v8(src + 8, z);
+      }
     }
   }
   __syncthreads();
@@ -968,7 +1122,10 @@ bev_finalize_cl_kernel(float* __restrict__ grid, unsigned char* __restrict__ occ
 // pool_sum[b,t,c] += sum over a slice of the finalize CTAs' partials (B, nblk, S, C); grid (B*S, kPoolSlices),
 // block (32, 8).  All loads of a thread are issued before the partials are zeroed again (the whole workspace stays
 // all-zero between calls); pool_sum is cleared by the caller (cudaMemsetAsync in stp3_lift_splat_fwd).
+// ORDERED (deterministic mode): each slice stores its sum to slices (B*S, kPoolSlices, C) instead of adding it to out;
+// pool_slices_kernel then adds the slices in order.
 constexpr int kPoolSlices = 16;
+template <bool ORDERED>
 __global__ void pool_reduce_kernel(float* __restrict__ part, int nblk, int S, int C, float* __restrict__ out) {
   __shared__ float sm[8][33];
   const int b = blockIdx.x / S, t = blockIdx.x % S;
@@ -1000,9 +1157,53 @@ __global__ void pool_reduce_kernel(float* __restrict__ part, int nblk, int S, in
       float tot = 0.f;
 #pragma unroll
       for (int r = 0; r < 8; ++r) tot += sm[r][threadIdx.x];
-      atomicAdd(out + (size_t)blockIdx.x * C + c, tot);
+      if constexpr (ORDERED) out[((size_t)blockIdx.x * kPoolSlices + blockIdx.y) * C + c] = tot;
+      else atomicAdd(out + (size_t)blockIdx.x * C + c, tot);
     }
     __syncthreads();
+  }
+}
+
+// pool_sum[f, c] = sum of the kPoolSlices slices of frame f in slice order; re-zeroes the slices
+__global__ void pool_slices_kernel(float* __restrict__ slices, int n, int C, float* __restrict__ out) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;     // (frame, channel)
+  if (i >= n) return;
+  const int f = i / C, c = i % C;
+  float* s = slices + (size_t)f * kPoolSlices * C + c;
+  float v[kPoolSlices];
+#pragma unroll
+  for (int k = 0; k < kPoolSlices; ++k) v[k] = s[(size_t)k * C];
+  float a = 0.f;
+#pragma unroll
+  for (int k = 0; k < kPoolSlices; ++k) { a += v[k]; s[(size_t)k * C] = 0.f; }
+  out[i] = a;
+}
+
+// fmax[slot] = bits of the largest finite |x| over the frame's n_per_frame features, for slots blockIdx.y,
+// blockIdx.y + gridDim.y, ... < n_frames; the maximum of non-negative float bit patterns is order-independent, so the
+// atomicMax is deterministic
+__global__ void __launch_bounds__(256)
+frame_absmax_kernel(const float* __restrict__ feat, size_t n_per_frame, int n_frames, int vec4,
+                    unsigned* __restrict__ fmax) {
+  for (int slot = blockIdx.y; slot < n_frames; slot += gridDim.y) {
+    const float* x = feat + (size_t)slot * n_per_frame;
+    unsigned m = 0;
+    auto take = [&](float v) {
+      const unsigned b = __float_as_uint(v) & 0x7fffffffu;
+      if (b < 0x7f800000u) m = max(m, b);
+    };
+    const size_t stride = (size_t)gridDim.x * blockDim.x;
+    if (vec4) {
+      const float4* x4 = reinterpret_cast<const float4*>(x);
+      for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n_per_frame / 4; i += stride) {
+        const float4 v = __ldg(x4 + i);
+        take(v.x); take(v.y); take(v.z); take(v.w);
+      }
+    } else {
+      for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n_per_frame; i += stride) take(__ldg(x + i));
+    }
+    m = __reduce_max_sync(0xffffffffu, m);
+    if ((threadIdx.x & 31) == 0 && m != 0) atomicMax(fmax + slot, m);
   }
 }
 
@@ -1034,6 +1235,41 @@ extern "C" size_t stp3_lift_splat_workspace_bytes(const stp3_lift_splat_desc* de
   if (!desc || desc->f_count < 0) return 0;
   const bool raw = desc->f_count > 0;
   return workspace_bytes_for(raw ? desc->f_count : desc->B, raw ? 1 : desc->S, desc->C, desc->nx, desc->ny);
+}
+
+// Workspace of stp3_lift_splat_fwd_det, byte offsets:
+//   int64 scatter grid | occupancy | pool partials | m_f bits (per frame) | poison bitmaps | pool slices
+// The grid alone is twice the fp32 one, so the total is above stp3_lift_splat_workspace_bytes and one zeroed buffer
+// serves both modes.
+namespace {
+struct DetLayout {
+  size_t occ, part, fmax, poison, slices, total;
+};
+
+DetLayout det_layout(int B, int S, int C, int nx, int ny) {
+  auto al = [](size_t x) { return (x + 255) & ~(size_t)255; };
+  const size_t frames = (size_t)B * S, nvox = (size_t)nx * ny;
+  DetLayout L;
+  size_t o = al(frames * nvox * C * sizeof(long long));
+  L.occ = o;    o += occ_bytes(B, S, nx, ny);
+  L.part = o;   o += al((size_t)B * ceil_div(nx * ny, 32) * S * C * sizeof(float));
+  L.fmax = o;   o += al(frames * sizeof(unsigned));
+  L.poison = o; o += al(frames * ((nvox + 31) / 32) * sizeof(unsigned));
+  L.slices = o; o += al(frames * kPoolSlices * C * sizeof(float));
+  L.total = o;
+  return L;
+}
+
+DetLayout det_layout(const stp3_lift_splat_desc* d) {
+  const bool raw = d->f_count > 0;
+  return det_layout(raw ? d->f_count : d->B, raw ? 1 : d->S, d->C, d->nx, d->ny);
+}
+}  // namespace
+
+extern "C" size_t stp3_lift_splat_det_workspace_bytes(const stp3_lift_splat_desc* desc) {
+  if (!desc || desc->f_count < 0 || desc->B <= 0 || desc->S <= 0 || desc->C <= 0 || desc->nx <= 0 || desc->ny <= 0)
+    return 0;
+  return det_layout(desc).total;
 }
 
 extern "C" int stp3_lift_splat_workspace_init(void* workspace, size_t workspace_bytes, void* stream) {
@@ -1183,13 +1419,16 @@ extern "C" int stp3_lift_splat_plan(const stp3_lift_splat_desc* desc, const floa
 // f_count == 0: all B*S frames, discount recurrence over each sample's S frames.  f_count > 0: frame-sharded call --
 // only the flat frames f_begin + [0, f_count) are splatted and written RAW (no recurrence), one (nx, ny, C) grid per
 // frame, to `out` or to every peer's gathered buffer; the caller all-gathers them and applies stp3_bev_discount.
-extern "C" int stp3_lift_splat_fwd(const stp3_lift_splat_desc* desc, const float* feat, const float* depth_logits,
-                                   int32_t* ranks_out, float* pool_sum, void* workspace, size_t workspace_bytes,
-                                   float* out, int out_layout, int n_peers, void* const* peer_out, void* stream_) {
+// det: the fixed-point form (stp3_lift_splat_fwd_det) -- the same plan's kernels with FX set, after the m_f pre-pass,
+// and the pool slices added in order.
+static int lift_splat_fwd(bool det, const char* fn, const stp3_lift_splat_desc* desc, const float* feat,
+                          const float* depth_logits, int32_t* ranks_out, float* pool_sum, void* workspace,
+                          size_t workspace_bytes, float* out, int out_layout, int n_peers, void* const* peer_out,
+                          void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   BevQuant q;
   LiftLaunch L;
-  if (const int rc = plan_lift_splat("stp3_lift_splat_fwd", desc, feat, depth_logits, out_layout, n_peers, q, L))
+  if (const int rc = plan_lift_splat(fn, desc, feat, depth_logits, out_layout, n_peers, q, L))
     return rc;
   const stp3_lift_splat_kernel_plan& P = L.plan;
   const int nx = desc->nx, ny = desc->ny, nz = desc->nz;
@@ -1198,7 +1437,7 @@ extern "C" int stp3_lift_splat_fwd(const stp3_lift_splat_desc* desc, const float
   const float discount = raw ? 0.f : desc->discount;
   const int Bw = raw ? desc->f_count : B, Sw = raw ? 1 : S;     // shape of the scatter grid / finalize launch
   STP3_CHECK_ARG(n_peers == 0 || peer_out, "n_peers must be in [0, %d], with peer_out when it is not 0", kMaxPeers);
-  STP3_CHECK_ARG((out || n_peers > 0) && workspace, "stp3_lift_splat_fwd: null pointer argument");
+  STP3_CHECK_ARG((out || n_peers > 0) && workspace, "%s: null pointer argument", fn);
   STP3_CHECK_ARG(!raw || (!ranks_out && !pool_sum), "frame mode writes no ranks_out or pool_sum");
   PeerOut po;
   po.n = n_peers; po.first_slot = desc->f_begin;
@@ -1206,7 +1445,7 @@ extern "C" int stp3_lift_splat_fwd(const stp3_lift_splat_desc* desc, const float
   for (int i = 0; i < n_peers; ++i)
     STP3_CHECK_ARG(po.ptr[i] && (reinterpret_cast<uintptr_t>(po.ptr[i]) & 31) == 0, "peer buffer %d is null or not 32-byte aligned", i);
   STP3_CHECK_ARG((reinterpret_cast<uintptr_t>(workspace) & 255) == 0, "workspace must be 256-byte aligned");
-  const size_t need = stp3_lift_splat_workspace_bytes(desc);
+  const size_t need = det ? stp3_lift_splat_det_workspace_bytes(desc) : stp3_lift_splat_workspace_bytes(desc);
   if (workspace_bytes < need) return set_error(STP3_ENOSPC, "workspace too small: %zu < %zu", workspace_bytes, need);
 
   LiftSplatParams p;
@@ -1224,49 +1463,93 @@ extern "C" int stp3_lift_splat_fwd(const stp3_lift_splat_desc* desc, const float
   p.tiles_w = ceil_div(Wf, P.scatter_tw);
   const long long nblk = (long long)Bw * Sw * N * p.tiles_w;
   STP3_CHECK_ARG(nblk < (1ll << 31), "grid too large");
+  unsigned char* ws = static_cast<unsigned char*>(workspace);
+  const DetLayout DL = det_layout(desc);
+  FxGrid fx;
+  memset(&fx, 0, sizeof(fx));
+  p.qgrid = nullptr; p.fmax = nullptr; p.poison = nullptr; p.lp = 0;
+  if (det) {
+    const long long points = (long long)N * D * Hf * Wf;
+    while ((1ll << p.lp) < points) ++p.lp;
+    p.grid = nullptr;
+    p.qgrid = reinterpret_cast<long long*>(ws);
+    p.occ = ws + DL.occ;
+    p.fmax = reinterpret_cast<unsigned*>(ws + DL.fmax);
+    p.poison = reinterpret_cast<unsigned*>(ws + DL.poison);
+    fx.grid = p.qgrid; fx.fmax = p.fmax; fx.poison = p.poison; fx.lp = p.lp;
+    // m_f of every frame of the launch (its features are one contiguous block in both layouts)
+    const size_t per_frame = (size_t)N * C * Hf * Wf;
+    const int vec4 = per_frame % 4 == 0 && (reinterpret_cast<uintptr_t>(feat) & 15) == 0;
+    const size_t work = vec4 ? per_frame / 4 : per_frame;
+    const unsigned gx = (unsigned)std::max<size_t>(1, std::min<size_t>(1024, (work + 2047) / 2048));
+    const int frames = Bw * Sw;     // grid.y is capped at 65535; the kernel loops over the frames beyond
+    frame_absmax_kernel<<<dim3(gx, std::min(frames, 65535)), 256, 0, stream>>>(
+        feat + (size_t)desc->f_begin * per_frame, per_frame, frames, vec4, reinterpret_cast<unsigned*>(ws + DL.fmax));
+    STP3_CUDA_OK(cudaGetLastError());
+  }
 
   if (P.scatter) {
-    STP3_CUDA_OK(cudaFuncSetAttribute(lift_splat_scatter_tma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                      (int)L.smem_tma));
-    lift_splat_scatter_tma_kernel<<<(unsigned)nblk, kScatterThreads, L.smem_tma, stream>>>(L.maps, p);
+    auto tma = det ? lift_splat_scatter_tma_kernel<true> : lift_splat_scatter_tma_kernel<false>;
+    STP3_CUDA_OK(cudaFuncSetAttribute(tma, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L.smem_tma));
+    tma<<<(unsigned)nblk, kScatterThreads, L.smem_tma, stream>>>(L.maps, p);
   } else {
     auto launch = [&](auto kernel) -> int {
       STP3_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L.smem));
       kernel<<<(unsigned)nblk, kScatterThreads, L.smem, stream>>>(p);
       return STP3_OK;
     };
-    const int rc = P.scatter_tw == 4 ? launch(lift_splat_scatter_kernel<4>)
-                 : P.scatter_tw == 2 ? launch(lift_splat_scatter_kernel<2>) : launch(lift_splat_scatter_kernel<1>);
+    int rc;
+    if (det)
+      rc = P.scatter_tw == 4 ? launch(lift_splat_scatter_kernel<4, true>)
+         : P.scatter_tw == 2 ? launch(lift_splat_scatter_kernel<2, true>) : launch(lift_splat_scatter_kernel<1, true>);
+    else
+      rc = P.scatter_tw == 4 ? launch(lift_splat_scatter_kernel<4, false>)
+         : P.scatter_tw == 2 ? launch(lift_splat_scatter_kernel<2, false>) : launch(lift_splat_scatter_kernel<1, false>);
     if (rc != STP3_OK) return rc;
   }
   STP3_CUDA_OK(cudaGetLastError());
 
   const int nvox = nx * ny * nz;
-  float* pool_part = pool_sum ? reinterpret_cast<float*>(p.occ + occ_bytes(Bw, Sw, nx, ny)) : nullptr;
+  float* pool_part = pool_sum ? reinterpret_cast<float*>(det ? ws + DL.part : p.occ + occ_bytes(Bw, Sw, nx, ny)) : nullptr;
   int pool_blocks = ceil_div(nvox, 32);
   if (P.finalize) {
     pool_blocks = ceil_div(nvox, 256 / P.finalize_lpp);
     dim3 cgrid(pool_blocks, Bw);
-#define STP3_FIN_CL(LPP_, PEERS_) \
-    bev_finalize_cl_kernel<LPP_, 4, PEERS_><<<cgrid, 256, 0, stream>>>(p.grid, p.occ, out, pool_part, Sw, nvox, discount, out_layout, po)
-    if (po.n > 0) {
-      if (P.finalize_lpp == 2) STP3_FIN_CL(2, true); else if (P.finalize_lpp == 4) STP3_FIN_CL(4, true); else STP3_FIN_CL(8, true);
-    } else {
-      if (P.finalize_lpp == 2) STP3_FIN_CL(2, false); else if (P.finalize_lpp == 4) STP3_FIN_CL(4, false); else STP3_FIN_CL(8, false);
-    }
+#define STP3_FIN_CL(LPP_, PEERS_, FX_) \
+    bev_finalize_cl_kernel<LPP_, 4, PEERS_, FX_><<<cgrid, 256, 0, stream>>>(p.grid, p.occ, out, pool_part, Sw, nvox, discount, out_layout, po, fx)
+#define STP3_FIN_CL_LPP(PEERS_, FX_) \
+    do { \
+      if (P.finalize_lpp == 2) STP3_FIN_CL(2, PEERS_, FX_); else if (P.finalize_lpp == 4) STP3_FIN_CL(4, PEERS_, FX_); \
+      else STP3_FIN_CL(8, PEERS_, FX_); \
+    } while (0)
+    if (det) { if (po.n > 0) STP3_FIN_CL_LPP(true, true); else STP3_FIN_CL_LPP(false, true); }
+    else     { if (po.n > 0) STP3_FIN_CL_LPP(true, false); else STP3_FIN_CL_LPP(false, false); }
+#undef STP3_FIN_CL_LPP
 #undef STP3_FIN_CL
   } else {
     dim3 fgrid(pool_blocks, Bw, P.channel_groups), fblock(32, C >= 64 ? 8 : ceil_div(C, 8));
-#define STP3_FINALIZE(VEC, SMAX) \
-  bev_finalize_kernel<VEC, SMAX><<<fgrid, fblock, 0, stream>>>(p.grid, p.occ, out, pool_part, Sw, C, nvox, discount, out_layout)
-    if (P.finalize_vec) { if (P.finalize_smax == 4) STP3_FINALIZE(true, 4); else STP3_FINALIZE(true, 8); }
-    else                { if (P.finalize_smax == 4) STP3_FINALIZE(false, 4); else STP3_FINALIZE(false, 8); }
+#define STP3_FINALIZE(VEC, SMAX, FX_) \
+  bev_finalize_kernel<VEC, SMAX, FX_><<<fgrid, fblock, 0, stream>>>(p.grid, p.occ, out, pool_part, Sw, C, nvox, discount, out_layout, fx)
+#define STP3_FINALIZE_ANY(FX_) \
+    do { \
+      if (P.finalize_vec) { if (P.finalize_smax == 4) STP3_FINALIZE(true, 4, FX_); else STP3_FINALIZE(true, 8, FX_); } \
+      else                { if (P.finalize_smax == 4) STP3_FINALIZE(false, 4, FX_); else STP3_FINALIZE(false, 8, FX_); } \
+    } while (0)
+    if (det) STP3_FINALIZE_ANY(true); else STP3_FINALIZE_ANY(false);
+#undef STP3_FINALIZE_ANY
 #undef STP3_FINALIZE
   }
   STP3_CUDA_OK(cudaGetLastError());
-  if (pool_sum) {
+  if (pool_sum && det) {
+    float* slices = reinterpret_cast<float*>(ws + DL.slices);
+    pool_reduce_kernel<true><<<dim3(Bw * Sw, kPoolSlices), dim3(32, 8), 0, stream>>>(pool_part, pool_blocks, Sw, C, slices);
+    STP3_CUDA_OK(cudaGetLastError());
+    const int n = Bw * Sw * C;
+    pool_slices_kernel<<<ceil_div(n, 256), 256, 0, stream>>>(slices, n, C, pool_sum);
+    STP3_CUDA_OK(cudaGetLastError());
+  } else if (pool_sum) {
     STP3_CUDA_OK(cudaMemsetAsync(pool_sum, 0, (size_t)Bw * Sw * C * sizeof(float), stream));
-    pool_reduce_kernel<<<dim3(Bw * Sw, kPoolSlices), dim3(32, 8), 0, stream>>>(pool_part, pool_blocks, Sw, C, pool_sum);
+    pool_reduce_kernel<false><<<dim3(Bw * Sw, kPoolSlices), dim3(32, 8), 0, stream>>>(pool_part, pool_blocks, Sw, C, pool_sum);
     STP3_CUDA_OK(cudaGetLastError());
   }
   if (P.channel_groups > 1) {
@@ -1274,7 +1557,23 @@ extern "C" int stp3_lift_splat_fwd(const stp3_lift_splat_desc* desc, const float
     clear_bytes_kernel<<<(unsigned)((nocc / 16 + 255) / 256), 256, 0, stream>>>(p.occ, nocc);
     STP3_CUDA_OK(cudaGetLastError());
   }
+  if (det)   // the m_f bits and the poison bitmaps: everything else was re-zeroed by the kernels that read it
+    STP3_CUDA_OK(cudaMemsetAsync(ws + DL.fmax, 0, DL.slices - DL.fmax, stream));
   return STP3_OK;
+}
+
+extern "C" int stp3_lift_splat_fwd(const stp3_lift_splat_desc* desc, const float* feat, const float* depth_logits,
+                                   int32_t* ranks_out, float* pool_sum, void* workspace, size_t workspace_bytes,
+                                   float* out, int out_layout, int n_peers, void* const* peer_out, void* stream) {
+  return lift_splat_fwd(false, "stp3_lift_splat_fwd", desc, feat, depth_logits, ranks_out, pool_sum, workspace,
+                        workspace_bytes, out, out_layout, n_peers, peer_out, stream);
+}
+
+extern "C" int stp3_lift_splat_fwd_det(const stp3_lift_splat_desc* desc, const float* feat, const float* depth_logits,
+                                       int32_t* ranks_out, float* pool_sum, void* workspace, size_t workspace_bytes,
+                                       float* out, int out_layout, int n_peers, void* const* peer_out, void* stream) {
+  return lift_splat_fwd(true, "stp3_lift_splat_fwd_det", desc, feat, depth_logits, ranks_out, pool_sum, workspace,
+                        workspace_bytes, out, out_layout, n_peers, peer_out, stream);
 }
 
 namespace stp3 {

@@ -210,10 +210,19 @@ constexpr int kRedParts = 128;
 
 inline int red_parts(long long n_pix) { return (int)(n_pix < kRedParts ? n_pix : kRedParts); }
 
+// Loaders of `a`: fp32 rows, or bf16 hi/lo rows read as hi + lo (stp3_spatial_sum_det).  a + n moves both.
+struct HiLoRows {
+  const __nv_bfloat16* hi;
+  const __nv_bfloat16* lo;
+  __device__ float operator[](long long i) const { return __bfloat162float(hi[i]) + __bfloat162float(lo[i]); }
+  __device__ HiLoRows& operator+=(long long n) { hi += n; lo += n; return *this; }
+};
+
 // mode 0: sum x;  mode 1: sum (x - mean)^2;  mode 2: sum g' and sum g' * xhat (two outputs), g' = g masked by y > 0
 // when y is given, xhat = (x - mean) * invstd (x may be NULL in mode 2: only sum g')
+template <class Rows>
 __global__ void __launch_bounds__(256)
-chan_partial_kernel(int mode, const float* __restrict__ a, int a_cs, const float* __restrict__ y, int y_cs,
+chan_partial_kernel(int mode, Rows a, int a_cs, const float* __restrict__ y, int y_cs,
                     const float* __restrict__ x, int x_cs, const float* __restrict__ mean,
                     const float* __restrict__ invstd, long long n_pix, int C, double* __restrict__ part) {
   __shared__ double red[2][8][33];
@@ -975,6 +984,32 @@ extern "C" int stp3_image_channel_sums(const float* x, int n_img, long long hw, 
                                                                                  nullptr, nullptr, hw, C, part);
   STP3_CUDA_OK(cudaGetLastError());
   sums_finalize_kernel<<<dim3(ceil_div(C, 128), n_img), 128, 0, st>>>(part, parts, C, sums, nullptr);
+  STP3_CUDA_OK(cudaGetLastError());
+  return STP3_OK;
+}
+
+// stp3_spatial_sum's result with stp3_image_channel_sums' two passes: every pixel's hi + lo, fp64 partials over fixed
+// pixel ranges, added in range order
+extern "C" size_t stp3_spatial_sum_det_scratch_bytes(int n_img, int HW, int cstride) {
+  if (HW <= 0 || cstride <= 0) return 0;
+  return stp3_image_channel_sums_scratch_bytes(n_img, HW, cstride);
+}
+
+extern "C" int stp3_spatial_sum_det(const void* hi, const void* lo, int n_img, int HW, int cstride, float* sums,
+                                    void* scratch, size_t scratch_bytes, void* stream) {
+  STP3_CHECK_ARG(hi && lo && sums && scratch && n_img > 0 && HW > 0 && cstride > 0 && cstride <= 1024,
+                 "stp3_spatial_sum_det: bad argument");
+  STP3_CHECK_ARG(n_img <= 65535, "stp3_spatial_sum_det: more than 65535 images");
+  STP3_CHECK_ARG(scratch_bytes >= stp3_spatial_sum_det_scratch_bytes(n_img, HW, cstride),
+                 "stp3_spatial_sum_det: scratch smaller than stp3_spatial_sum_det_scratch_bytes()");
+  cudaStream_t st = (cudaStream_t)stream;
+  const int parts = red_parts(HW);
+  double* part = (double*)scratch;
+  const HiLoRows rows{(const __nv_bfloat16*)hi, (const __nv_bfloat16*)lo};
+  chan_partial_kernel<<<dim3(ceil_div(cstride, 32), parts, n_img), dim3(32, 8), 0, st>>>(
+      0, rows, cstride, nullptr, 0, nullptr, 0, nullptr, nullptr, HW, cstride, part);
+  STP3_CUDA_OK(cudaGetLastError());
+  sums_finalize_kernel<<<dim3(ceil_div(cstride, 128), n_img), 128, 0, st>>>(part, parts, cstride, sums, nullptr);
   STP3_CUDA_OK(cudaGetLastError());
   return STP3_OK;
 }

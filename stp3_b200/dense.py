@@ -158,7 +158,9 @@ def pack_conv(weight: torch.Tensor, bias: torch.Tensor, *, stride: int = 1, dila
 # 128 / 256 columns).  Which combination wins depends on the layer (K depth, N width, image size, whether the weights
 # are smem-resident), so the first eager call of every (layer, shape) times the candidates back to back and the winner
 # is cached; CUDA-graph capture then records the tuned launches.  STP3_CONV_AUTOTUNE=0 disables it (kernel heuristics,
-# and untuned_blocks() for the column blocks).
+# and untuned_blocks() for the column blocks).  So does torch.use_deterministic_algorithms: tilings do not all give the
+# same bits, and one picked by timing can differ between processes.  The mode is part of the cache key, so a tiling
+# timed with the flag off is never reused with it on.
 import os as _os
 
 _TUNED = {}
@@ -308,10 +310,12 @@ def conv(x: HL, pc: PackedConv, *, cin_off: int = 0, out: Optional[HL] = None, o
                 ctypes.byref(hd) if hd is not None else None, torch.cuda.current_stream(dev).cuda_stream)
         _lib.check(code, "stp3_conv_fwd")
 
+    det = torch.are_deterministic_algorithms_enabled()
     key = (pc.uid, B, T, H, W, cs, cin_off, Ho, Wo, t0, int(relu), residual is not None, out_f32 is not None,
-           hd is not None, out2 is not None, int(swish), int(w_img_stride))
+           hd is not None, out2 is not None, int(swish), int(w_img_stride), det)
     cfg = tune if tune is not None else _TUNED.get(key)
-    if cfg is None and _AUTOTUNE and not torch.cuda.is_current_stream_capturing():
+    autotune = _AUTOTUNE and not det
+    if cfg is None and autotune and not torch.cuda.is_current_stream_capturing():
         desc = f"{len(pc.taps)}tap cin{pc.cin_p} bn{pc.bn} s{pc.stride} {B * T}x{Ho}x{Wo}"
         # the tuner launches the layer many times: an output that aliases an input would be corrupted silently
         ins = {x.hi.data_ptr()} | ({x.lo.data_ptr()} if x.lo is not None else set()) | ({residual.hi.data_ptr(), residual.lo.data_ptr()} if residual is not None else set())
@@ -319,7 +323,7 @@ def conv(x: HL, pc: PackedConv, *, cin_off: int = 0, out: Optional[HL] = None, o
         assert not (ins & outs), "stp3_b200.dense.conv: output aliases an input (in-place convolution is not supported)"
         cfg = _tune(key, desc, launch, [c for c in tune_candidates(pc, per_image=w_img_stride > 0)
                                         if not (one_block and c[1] & BLOCKS64)])
-    elif cfg is None and not _AUTOTUNE and not one_block and pc.bn >= 128:
+    elif cfg is None and not autotune and not one_block and pc.bn >= 128:
         tiles = B * T * -(-Ho // 8) * -(-Wo // 16)
         cfg = _TUNED[key] = (0, untuned_blocks(pc, tiles, torch.cuda.get_device_properties(dev).multi_processor_count))
         TUNE_LOG.append((f"{len(pc.taps)}tap cin{pc.cin_p} bn{pc.bn} s{pc.stride} {B * T}x{Ho}x{Wo}", {cfg: float("nan")}))
@@ -529,12 +533,22 @@ def to_f32(x: HL, c_off: int = 0, c: Optional[int] = None) -> torch.Tensor:
 
 
 def spatial_sum(x: HL) -> torch.Tensor:
-    """(B*T, cstride) fp32 sums over the H*W pixels of every image."""
+    """(B*T, cstride) fp32 sums over the H*W pixels of every image.  Under torch.use_deterministic_algorithms the sums
+    are added in a fixed order (stp3_spatial_sum_det) instead of with float atomics."""
     B, T, H, W, cs = x.hi.shape
-    out = torch.empty((B * T, cs), dtype=torch.float32, device=x.hi.device)
-    with torch.cuda.device(x.hi.device):
-        code = _lib.lib().stp3_spatial_sum(x.hi.data_ptr(), x.lo.data_ptr(), B * T, H * W, cs, out.data_ptr(),
-                                           _stream(x.hi.device))
+    dev = x.hi.device
+    out = torch.empty((B * T, cs), dtype=torch.float32, device=dev)
+    L = _lib.lib()
+    if torch.are_deterministic_algorithms_enabled():
+        nbytes = L.stp3_spatial_sum_det_scratch_bytes(B * T, H * W, cs)
+        scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+        with torch.cuda.device(dev):
+            code = L.stp3_spatial_sum_det(x.hi.data_ptr(), x.lo.data_ptr(), B * T, H * W, cs, out.data_ptr(),
+                                          scratch.data_ptr(), nbytes, _stream(dev))
+        _lib.check(code, "stp3_spatial_sum_det")
+        return out
+    with torch.cuda.device(dev):
+        code = L.stp3_spatial_sum(x.hi.data_ptr(), x.lo.data_ptr(), B * T, H * W, cs, out.data_ptr(), _stream(dev))
     _lib.check(code, "stp3_spatial_sum")
     return out
 

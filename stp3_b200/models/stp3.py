@@ -434,6 +434,11 @@ class GraphedPerception:
             self.graph = torch.cuda.CUDAGraph()
             with torch.cuda.graph(self.graph):
                 self.out = self._fwd(**self.static)
+            # ... and the lift-splat workspace it splats into: a later eager call may replace model._ws's buffer by a
+            # larger one (another batch, or the deterministic mode's int64 grid), and the graph must not replay into
+            # freed memory
+            if model._ws.buf is not None:
+                self._keepalive.append(model._ws.buf)
 
     def check_weights_unchanged(self):
         """Raises if a parameter or buffer the captured kernels read was modified (load_state_dict, optimizer step,

@@ -81,19 +81,24 @@ def _lift_desc(feat, depth_logits, cam_M, cam_t, ego_R, ego_t, xs, ys, ds, bev_o
 
 def _lift_fwd(desc, feat, depth_logits, workspace: Optional[Workspace], out, out_layout: int, ranks=None, psum=None,
               peer_ptrs=None):
-    """stp3_lift_splat_fwd on the current stream; the workspace is re-initialised when the call fails."""
+    """stp3_lift_splat_fwd on the current stream -- or, when torch.are_deterministic_algorithms_enabled() (warn_only
+    included), its fixed-point form stp3_lift_splat_fwd_det, whose results are bitwise repeatable.  A CUDA graph
+    replays the mode it was captured in.  The workspace is re-initialised when the call fails."""
     L = _lib.lib()
     dev = feat.device
     workspace = workspace or _default_ws
-    ws = workspace.get(L.stp3_lift_splat_workspace_bytes(desc), dev)
+    det = torch.are_deterministic_algorithms_enabled()
+    name = "stp3_lift_splat_fwd_det" if det else "stp3_lift_splat_fwd"
+    nbytes = L.stp3_lift_splat_det_workspace_bytes(desc) if det else L.stp3_lift_splat_workspace_bytes(desc)
+    ws = workspace.get(nbytes, dev)
     peers = (ctypes.c_void_p * len(peer_ptrs))(*[int(x) for x in peer_ptrs]) if peer_ptrs is not None else None
     with torch.cuda.device(dev):
-        code = L.stp3_lift_splat_fwd(desc, feat.data_ptr(), _ptr(depth_logits), _ptr(ranks), _ptr(psum), ws.data_ptr(),
-                                     ws.numel(), _ptr(out), out_layout, len(peer_ptrs or ()), peers,
-                                     torch.cuda.current_stream(dev).cuda_stream)
+        code = getattr(L, name)(desc, feat.data_ptr(), _ptr(depth_logits), _ptr(ranks), _ptr(psum), ws.data_ptr(),
+                                ws.numel(), _ptr(out), out_layout, len(peer_ptrs or ()), peers,
+                                torch.cuda.current_stream(dev).cuda_stream)
     if code != 0:
         workspace.reset()
-    _lib.check(code, "stp3_lift_splat_fwd")
+    _lib.check(code, name)
 
 
 def lift_splat(feat, depth_logits, cam_M, cam_t, ego_R, ego_t, xs, ys, ds, bev_off, bev_res, bev_dim,
