@@ -313,6 +313,10 @@ int stp3_conv_fwd(const stp3_conv_desc* desc, const void* x_hi, const void* x_lo
  * of stp3_conv_fwd hold, and it must carry no residual, second destination, col_sums, swish or per-image weights. */
 int stp3_conv_fwd_plane(const stp3_conv_desc* desc, int operand, const void* x, const void* w, const float* bias,
                         const float* img_bias, float* y_f32, void* stream);
+/* stp3_conv_tiling for an operand kind: how stp3_conv_fwd (HILO) or stp3_conv_fwd_plane (BF16 / F16) would run desc.
+ * A one-plane operand halves the activation stage and the weight tile, so it may keep weights resident or pick ring
+ * depths that the hi/lo pair does not, and it never stacks.  operand HILO answers exactly as stp3_conv_tiling. */
+int stp3_conv_tiling_op(const stp3_conv_desc* desc, int n_sm, int operand, stp3_conv_tiling_info* out);
 
 /* ---------------------------------------------------------------------------------------------------------
  * ASPP branches + projection of a DeepLabHead as ONE back-to-back tensor-core kernel (stp3/layers/convolutions.py:242-270):

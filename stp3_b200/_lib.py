@@ -111,6 +111,7 @@ SIGNATURES = {
     "stp3_bev_discount": (_I, [_V, _I, _I, _I, _I, _I, _F, _V, _V, _V]),
     "stp3_conv_fwd": (_I, [ctypes.POINTER(ConvDesc), _V, _V, _V, _V, _V, _V, _V, _V, _V, _V, ctypes.POINTER(ConvHead), _V]),
     "stp3_conv_fwd_plane": (_I, [ctypes.POINTER(ConvDesc), _I, _V, _V, _V, _V, _V, _V]),
+    "stp3_conv_tiling_op": (_I, [ctypes.POINTER(ConvDesc), _I, _I, ctypes.POINTER(ConvTilingInfo)]),
     "stp3_lift_splat_fwd": (_I, [_LSD, _V, _V, _V, _V, _V, _SZ, _V, _I, _I, ctypes.POINTER(_V), _V]),
     "stp3_lift_splat_plan": (_I, [_LSD, _V, _V, _I, _I, ctypes.POINTER(LiftSplatPlan)]),
     # deterministic mode (torch.use_deterministic_algorithms)

@@ -832,10 +832,16 @@ extern "C" size_t stp3_conv_col_sums_scratch_bytes(int n_img, int bn) {
 }
 
 extern "C" int stp3_conv_tiling(const stp3_conv_desc* d, int n_sm, stp3_conv_tiling_info* out) {
+  return stp3_conv_tiling_op(d, n_sm, STP3_OPERAND_HILO, out);
+}
+
+extern "C" int stp3_conv_tiling_op(const stp3_conv_desc* d, int n_sm, int operand, stp3_conv_tiling_info* out) {
   STP3_CHECK_ARG(d && out && n_sm > 0, "stp3_conv_tiling: null pointer argument or no SM");
+  STP3_CHECK_ARG(operand == STP3_OPERAND_HILO || operand == STP3_OPERAND_BF16 || operand == STP3_OPERAND_F16,
+                 "stp3_conv_tiling_op: operand must be STP3_OPERAND_HILO, _BF16 or _F16");
   ConvParams p;
   ConvPlan t;
-  if (const int rc = plan_conv(d, false, n_sm, p, t)) return rc;
+  if (const int rc = plan_conv(d, false, n_sm, p, t, operand)) return rc;
   out->bn_blk = t.bn_blk; out->stacked = t.stack; out->tiles = p.n_tiles; out->items = p.n_tiles * p.n_nblk;
   out->ctas = (int)t.grid; out->a_stages = p.na_stages; out->b_stages = p.nb_stages; out->resident = p.b_resident;
   return STP3_OK;

@@ -59,9 +59,9 @@ def amp_mode() -> Optional[torch.dtype]:
 
 def amp_kw(mode: Optional[torch.dtype]) -> dict:
     """The keyword arguments that select `mode` in to_hl, bn_apply, conv_dgrad and conv_wgrad: none outside autocast,
-    so the fp32 path makes exactly the calls it always made.  That is a contract, not a style: the launch-by-launch
-    contract suites (tests/test_train_contract_gpu.py, tests/test_aux_contract_gpu.py) replace these functions with
-    recorders of their fp32 signatures while a train step runs, and a `mode=None` argument would break them."""
+    so the fp32 path makes exactly the calls it always made, and a function that has no `mode` parameter is never
+    handed one.  The launch-by-launch contract suites replace to_hl, bn_apply and conv_wgrad with recorders that take
+    `mode` as a keyword and record fp32 and autocast steps alike."""
     return {} if mode is None else {"mode": mode}
 
 

@@ -176,6 +176,16 @@ def f32_to_hilo(x: torch.Tensor, channels_last: int, n_img: int, C: int, H: int,
     return torch.cat([hi, z], -1), torch.cat([lo, z], -1)
 
 
+def f32_to_plane(x: torch.Tensor, channels_last: int, n_img: int, C: int, H: int, W: int, cp: int,
+                 mode: torch.dtype) -> torch.Tensor:
+    """x fp32 (n_img, C, H, W) or (n_img, H, W, C) -> ONE plane (n_img, H, W, cp) of `mode` (torch.float16 /
+    torch.bfloat16): torch's own rounding (to nearest even, overflow to +-inf, NaN kept), channels [C, cp) +0: bit-exact
+    except for the NaN payloads"""
+    x = x.reshape(n_img, H, W, C) if channels_last else x.reshape(n_img, C, H, W).permute(0, 2, 3, 1)
+    z = torch.zeros((n_img, H, W, cp - C), dtype=mode, device=x.device)
+    return torch.cat([x.to(mode), z], -1)
+
+
 def hilo_to_f32(hi: torch.Tensor, lo: torch.Tensor, n_img: int, H: int, W: int, cstride: int, c_off: int, C: int):
     """planes (n_img, H, W, cstride), channels [c_off, c_off + C) -> (n_img, C, H, W) fp32 hi + lo, summed in fp32:
     bit-exact"""

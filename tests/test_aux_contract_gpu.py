@@ -8,7 +8,10 @@ perceive forward with the fused and the unfused TemporalBlock tail, the stress s
 train steps of the decoder, the DeepLab head, the TemporalModel and the encoder heads -- and built synthetically for what
 the model never passes (stem widths and pads, channel windows inside wider strides, one-pixel maps, squeeze-excite
 projections whose last chunk is exactly 64 or 128 wide, rounding edge cases of the hi/lo split, multi-slice pooling
-rows, 8-mod-16 upsample windows).
+rows, 8-mod-16 upsample windows).  stp3_f32_to_plane (the one 16-bit plane of an autocast train step) is recorded from
+the same train steps with their forward under torch.autocast in float16 and in bfloat16 (dense_train.to_hl with a
+mode), and run synthetically in both layouts at the rounding edges of both types; every plane must be bitwise torch's
+own .to(mode) of the input (NaN where torch has NaN), its padding +0.
 
 Each launch is replayed twice through _lib.lib() into outputs filled with a sentinel (NaN for fp32, the bf16 NaN 0x7FA5
 for planes) followed by a guard; scratch is 0xFF bytes (NaN), and the input channels a kernel must not read are NaN.
@@ -159,6 +162,16 @@ def to_hilo_case(x, cl, n, C, H, W, cp, tag, extra=()):
     return Case("to_hilo", dict(x=x.reshape(-1), cl=int(cl), n=n, C=C, H=H, W=W, cp=cp), tag, features=f)
 
 
+def to_plane_case(x, cl, n, C, H, W, cp, mode, tag, extra=()):
+    name = "f16" if mode == torch.float16 else "bf16"
+    f = {"f32_to_plane", f"f32_to_plane {name}", f"f32_to_plane {'NHWC' if cl else 'NCHW'}"} | set(extra)
+    if cp > C:
+        f.add("f32_to_plane cp > C")
+    if C > 32:
+        f.add("f32_to_plane several channel tiles")
+    return Case("to_plane", dict(x=x.reshape(-1), cl=int(cl), n=n, C=C, H=H, W=W, cp=cp, mode=mode), tag, features=f)
+
+
 def to_f32_case(hi, lo, n, H, W, c_off, C, tag):
     cs = hi.shape[-1]
     hi, lo = _poison(hi.reshape(n, H, W, cs), lo.reshape(n, H, W, cs), slice(c_off, c_off + C))
@@ -266,6 +279,11 @@ def run(case: Case) -> dict:
         code = L.stp3_f32_to_hilo(a["x"].data_ptr(), a["cl"], a["n"], a["C"], a["H"], a["W"], a["cp"], yh.data_ptr(),
                                   yl.data_ptr(), _stream())
         outs = {"hi": yh, "lo": yl}
+    elif k == "to_plane":
+        o = torch.full((a["n"] * a["H"] * a["W"] * a["cp"] + GUARD,), SENT16, dtype=torch.int16, device=DEV).view(a["mode"])
+        code = L.stp3_f32_to_plane(a["x"].data_ptr(), a["cl"], a["n"], a["C"], a["H"], a["W"], a["cp"],
+                                   dense.PLANE_OPERAND[a["mode"]], o.data_ptr(), _stream())
+        outs = {"plane": o}
     elif k == "to_f32":
         o = _f32_out(a["n"] * a["C"] * a["H"] * a["W"])
         code = L.stp3_hilo_to_f32(a["hi"].data_ptr(), a["lo"].data_ptr(), a["n"], a["H"], a["W"], a["cs"], a["c_off"],
@@ -303,6 +321,8 @@ def run(case: Case) -> dict:
 def windows(case: Case, outs: dict) -> dict:
     """the elements the launch writes, per output, in the layout the recorder clones production's into"""
     a, k = case.a, case.kind
+    if k == "to_plane":
+        return {"plane": outs["plane"][:a["n"] * a["H"] * a["W"] * a["cp"]]}
     if k in ("stem", "to_hilo"):
         n = a["n"] * (a["Ho"] * a["Wo"] * a["ocs"] if k == "stem" else a["H"] * a["W"] * a["cp"])
         return {"hi": outs["hi"][:n], "lo": outs["lo"][:n]}
@@ -342,7 +362,7 @@ def _ulps(got, ref, mag):
 
 def _guard_ok(t):
     g = t[-GUARD:]
-    return bool(_is_sent(g).all()) if t.dtype == torch.bfloat16 else bool(torch.isnan(g).all())
+    return bool(_is_sent(g).all()) if t.element_size() == 2 else bool(torch.isnan(g).all())
 
 
 def _plane_checks(res, hi, lo, name=""):
@@ -406,6 +426,12 @@ def check(case: Case) -> dict:
     elif k == "to_hilo":
         hi, lo = R.f32_to_hilo(a["x"], a["cl"], a["n"], a["C"], a["H"], a["W"], a["cp"])
         res["bitwise"] = torch.equal(_bits(win["hi"]), _bits(hi)) and torch.equal(_bits(win["lo"]), _bits(lo))
+    elif k == "to_plane":
+        ref = R.f32_to_plane(a["x"], a["cl"], a["n"], a["C"], a["H"], a["W"], a["cp"], a["mode"]).reshape(-1)
+        got = win["plane"]
+        nan = torch.isnan(ref)
+        res["nan"] = torch.equal(torch.isnan(got), nan)
+        res["bitwise"] = torch.equal(_bits(got)[~nan], _bits(ref)[~nan])
     elif k == "to_f32":
         ref = R.hilo_to_f32(a["hi"], a["lo"], a["n"], a["H"], a["W"], a["cs"], a["c_off"], a["C"])
         res["bitwise"] = torch.equal(_bits(win["out"]), _bits(ref))
@@ -518,10 +544,14 @@ class Recorder:
         return f
 
     def _to_hl(self, orig):
-        def f(x, cp=None):
+        def f(x, cp=None, mode=None):
             xs = x.clone()
-            out = orig(x, cp)
+            out = orig(x, cp, **dense_train.amp_kw(mode))
             N, H, W, C = xs.shape
+            if mode is not None:
+                self._add(to_plane_case(xs, 1, N, C, H, W, out.hi.shape[-1], mode, f"to_hl {tuple(xs.shape)} {mode}",
+                                        ("to_hl plane",)), {"plane": out.hi.reshape(-1)})
+                return out
             self._add(to_hilo_case(xs, 1, N, C, H, W, out.hi.shape[-1], f"to_hl {tuple(xs.shape)}", ("to_hl",)),
                       {"hi": out.hi.reshape(-1), "lo": out.lo.reshape(-1)})
             return out
@@ -634,6 +664,14 @@ def rec_encoder_heads():
     return r.cases
 
 
+def rec_amp(mode, step, *args):
+    """a train step of tests/test_train_contract_gpu.py with its forward under torch.autocast(dtype=mode)"""
+    from tests import test_train_contract_gpu as TC
+    with Recorder(f"{step} {mode}") as r:
+        getattr(TC, step)(*args, mode=mode)
+    return r.cases
+
+
 def rec_train(name, fn, *args):
     """a train step of the model of tests/test_train_contract_gpu.py (its own recorder runs too, unused)"""
     from tests import test_train_contract_gpu as TC
@@ -736,6 +774,33 @@ def synth_hilo():
     return cases
 
 
+def _plane_specials(mode):
+    """fp32 values at the rounding edges of `mode`: ties to even, subnormals and values below half the smallest one,
+    the largest finite value and the first values that round past it, -0.0, NaN and +-inf"""
+    inf, nan = float("inf"), float("nan")
+    both = [0.0, -0.0, nan, inf, -inf, 1.0, -1.0, 3.0e-39, -1e-45]
+    if mode == torch.float16:
+        v = [1 + 2 ** -11, 1 + 3 * 2 ** -11, -(1 + 2 ** -11), 2 ** -24, 3 * 2 ** -25, 2 ** -25, 2 ** -25 * (1 + 2 ** -20),
+             -2 ** -26, 2 ** -26, 5 * 2 ** -26, 2 ** -14 - 2 ** -25, 65504.0, 65519.0, 65520.0, -65520.0, 1e6, 2.0 ** -15]
+    else:
+        v = [1 + 2 ** -8, 1 + 3 * 2 ** -8, -(1 + 2 ** -8), 1e-45, -3e-42, 1e-39, 9.2e-41, 1.1754942e-38,
+             3.3895314e38, -3.3895314e38, 3.3961e38, 3.3962e38, -3.4e38, 3.4028235e38, 1.0 + 2 ** -8 + 2 ** -20]
+    return torch.tensor(both + v, dtype=torch.float32)
+
+
+def synth_plane():
+    cases = []
+    for mode in (torch.float16, torch.bfloat16):
+        sp = _plane_specials(mode)
+        for i, (n, C, H, W, cp, cl) in enumerate([(2, 37, 5, 7, 64, 0), (2, 37, 5, 7, 64, 1), (3, 64, 4, 8, 64, 0),
+                                                  (1, 100, 9, 13, 192, 1), (1, 100, 9, 13, 128, 0), (1, 8, 1, 1, 64, 1)]):
+            x = rnd(n * C * H * W, seed=1400 + i, scale=30.0)
+            x[::2] = sp.repeat(-(-x[::2].numel() // sp.numel()))[:x[::2].numel()].to(DEV)
+            cases.append(to_plane_case(x, cl, n, C, H, W, cp, mode, f"{'NHWC' if cl else 'NCHW'} n{n} C{C} {H}x{W} "
+                                       f"cp{cp} {mode}", ("f32_to_plane edge values",)))
+    return cases
+
+
 def synth_small():
     cases = []
     for i, (B, T, C, R_, CO, nc, temporal, with_bias, acc, extra) in enumerate([
@@ -787,7 +852,14 @@ SOURCES = {
     "synthetic_se": synth_se,
     "synthetic_hilo": synth_hilo,
     "synthetic_small": synth_small,
+    "synthetic_plane": synth_plane,
 }
+for _m, _nm in ((torch.float16, "fp16"), (torch.bfloat16, "bf16")):
+    SOURCES.update({
+        f"amp_decoder_{_nm}": lambda m=_m: rec_amp(m, "decoder_step", (2, 3, 64, 48, 64), GATES_ALL),
+        f"amp_deeplab_{_nm}": lambda m=_m: rec_amp(m, "deeplab_step", 64, 64, 128, 6, 48, 64),
+        f"amp_temporal_{_nm}": lambda m=_m: rec_amp(m, "temporal_step", 70, 6, 3, 2, 48, 64),
+        f"amp_encoder_heads_{_nm}": lambda m=_m: rec_amp(m, "encoder_heads_step", "feat")})
 
 _RUNS = {}
 
@@ -826,7 +898,9 @@ def test_aux_launches_against_the_fp64_contract(name):
 
 
 REQUIRED = (["recorded"] + [f"recorded {k}" for k in ("stem", "dw", "se", "to_hilo", "to_f32", "ssum", "pool", "lin", "up")]
-            + ["to_hl"]
+            + ["to_hl", "to_hl plane", "recorded to_plane"]
+            + [f"f32_to_plane {k}" for k in ("f16", "bf16", "NCHW", "NHWC", "cp > C", "several channel tiles",
+                                              "edge values")]
             + [f"stem pad ({a},{b})" for a in range(3) for b in range(3)]
             + [f"stem cout {c}" for c in (1, 8, 24, 32, 40, 63, 64)]
             + ["stem ragged grid", "stem one-pixel output", "stem odd H or W", "stem out_cstride 128",

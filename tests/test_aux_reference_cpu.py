@@ -147,6 +147,21 @@ def test_layout_conversions(cl):
     _close(s["sums"], (hi.double() + lo.double()).sum((1, 2)).reshape(n, cp))
 
 
+@pytest.mark.parametrize("mode", [torch.float16, torch.bfloat16])
+@pytest.mark.parametrize("cl", [0, 1])
+def test_f32_to_plane_layouts(mode, cl):
+    """both layouts land channels-last with +0 padding; the values are torch's rounding, -0.0 kept"""
+    n, C, H, W, cp = 2, 37, 3, 11, 64
+    x = _rand(n, C, H, W, seed=17) * 1e3
+    x[0, 1, 2, 3] = -0.0
+    src = x.permute(0, 2, 3, 1).contiguous() if cl else x
+    p = R.f32_to_plane(src, cl, n, C, H, W, cp, mode)
+    assert p.dtype == mode and p.shape == (n, H, W, cp)
+    assert torch.equal(p[..., :C].view(torch.int16), x.permute(0, 2, 3, 1).to(mode).view(torch.int16))
+    assert not p[..., C:].view(torch.int16).any()
+    assert torch.signbit(p[0, 2, 3, 1].float())
+
+
 # ------------------------------------------------------------------------------------------------ small dense layers
 @pytest.mark.parametrize("temporal,n_const,accumulate,with_bias", [(True, 0, False, True), (True, 2, True, True),
                                                                    (False, 3, False, False), (True, 0, False, False)])
@@ -278,13 +293,14 @@ WRAPPERS = {"stp3_effnet_stem": "effnet_stem", "stp3_dw_fwd": "dw_conv", "stp3_s
 
 
 def aux_calls_outside_the_wrappers():
-    """Uses of the nine entry points anywhere in the package except inside their dense.py wrapper (and
-    stp3_f32_to_hilo inside dense_train.to_hl), and imports of a wrapper by name: each would launch a kernel the
+    """Uses of the nine entry points and of stp3_f32_to_plane anywhere in the package except inside their dense.py
+    wrapper (and stp3_f32_to_hilo / stp3_f32_to_plane inside dense_train.to_hl), and imports of a wrapper by name: each would launch a kernel the
     recorder does not see.  (A bare call inside the wrapper's own module resolves the module attribute the recorder
     replaces, so it is recorded.)"""
     pkg = os.path.dirname(os.path.abspath(dense.__file__))
     allowed = {(os.path.abspath(dense.__file__), fn, sym) for sym, fn in WRAPPERS.items()}
-    allowed.add((os.path.abspath(dense_train.__file__), "to_hl", "stp3_f32_to_hilo"))
+    allowed |= {(os.path.abspath(dense_train.__file__), "to_hl", sym) for sym in ("stp3_f32_to_hilo", "stp3_f32_to_plane")}
+    symbols = set(WRAPPERS) | {"stp3_f32_to_plane"}
     wrappers = set(WRAPPERS.values())
     bad = []
     for root, _, files in os.walk(pkg):
@@ -303,7 +319,7 @@ def aux_calls_outside_the_wrappers():
                     for n in ast.walk(fn):
                         owner.setdefault(id(n), fn.name)     # the outermost function wins (ast.walk is breadth first)
             for n in ast.walk(tree):
-                if isinstance(n, ast.Attribute) and n.attr in WRAPPERS:
+                if isinstance(n, ast.Attribute) and n.attr in symbols:
                     if (path, owner.get(id(n)), n.attr) not in allowed:
                         bad.append(f"{f}:{n.lineno} {n.attr} in {owner.get(id(n))}")
     return bad

@@ -118,3 +118,56 @@ def test_dgrad_phase_packs_match_conv2d_input(k, stride, hw):
         else:
             out[:, py::2, px::2] = ph
     assert rel(out, ref.permute(0, 2, 3, 1)) < TOL
+
+
+@pytest.mark.parametrize("mode", [torch.float16, torch.bfloat16])
+@pytest.mark.parametrize("cin,cout,k,stride,dil,hw", [(64, 64, 3, 1, 1, (13, 11)), (35, 40, 3, 1, 2, (9, 14)),
+                                                      (64, 128, 3, 2, 1, (13, 10)), (64, 64, 7, 2, 1, (15, 12)),
+                                                      (130, 8, 1, 1, 1, (5, 6))])
+def test_plane_tap_sum_matches_conv2d_of_rounded_operands(mode, cin, cout, k, stride, dil, hw):
+    """one-plane weights and input: the tap sum is the fp64 convolution of the operands rounded to the plane type, and
+    `absolute` is that of their magnitudes"""
+    H, W = hw
+    x = torch.randn(2, cin, H, W, generator=torch.Generator().manual_seed(11)) * 3
+    w = torch.randn(cout, cin, k, k, generator=torch.Generator().manual_seed(12)) * 0.1
+    pc = dense.pack_conv(w, torch.zeros(cout), stride=stride, dilation=dil, plane=mode)
+    assert pc.w.dtype == mode and pc.w.shape == (len(pc.taps), pc.cin_p // 64, pc.bn, 64)
+    xp = torch.zeros(2, 1, H, W, pc.cin_p, dtype=mode)
+    xp[..., :cin] = x.permute(0, 2, 3, 1).unsqueeze(1).to(mode)
+    xr, wr = x.to(mode).double(), w.to(mode).double()
+    kw = dict(stride=stride, padding=(k - 1) * dil // 2, dilation=dil)
+    ref = F.conv2d(xr, wr, **kw).permute(0, 2, 3, 1)
+    mag = F.conv2d(xr.abs(), wr.abs(), **kw).permute(0, 2, 3, 1)
+    got = R.tap_sum(xp, None, pc)
+    assert rel(got[..., :cout], ref) < TOL
+    assert float(got[..., cout:].abs().max() if pc.bn > cout else 0.0) == 0.0
+    assert torch.equal(R.tap_sum(xp, None, pc, model=True), got)
+    assert rel(R.tap_sum(xp, None, pc, absolute=True)[..., :cout], mag) < TOL
+    with pytest.raises(AssertionError):
+        R.tap_sum(xp, xp, pc)
+
+
+@pytest.mark.parametrize("mode", [torch.float16, torch.bfloat16])
+def test_plane_tap_sum_matches_causal_conv3d_and_dgrad_phases(mode):
+    """the TemporalBlocks' causal (2, 3, 3) forward over a frame window, and the stride-2 input-gradient phases, as
+    one-plane tap sums"""
+    B, T, C, H, W = 2, 3, 35, 9, 12
+    x = torch.randn(B, C, T, H, W, generator=torch.Generator().manual_seed(13))
+    w = torch.randn(40, C, 2, 3, 3, generator=torch.Generator().manual_seed(14)) * 0.1
+    pc = dense.pack_conv(w, torch.zeros(40), plane=mode)
+    xp = torch.zeros(B, T, H, W, pc.cin_p, dtype=mode)
+    xp[..., :C] = x.permute(0, 2, 3, 4, 1).to(mode)
+    ref = F.conv3d(F.pad(x.to(mode).double(), (1, 1, 1, 1, 1, 0)), w.to(mode).double()).permute(0, 2, 3, 4, 1)
+    assert rel(R.tap_sum(xp, None, pc).view(B, T, H, W, -1)[..., :40], ref) < TOL
+    assert rel(R.tap_sum(xp, None, pc, frames=(1, 2)).view(B, 2, H, W, -1)[..., :40], ref[:, 1:]) < TOL
+    # input gradient of a 3x3 stride-2 convolution, phase by phase
+    Hi, Wi, cin, cout = 9, 8, 40, 64
+    wg = torch.randn(cout, cin, 3, 3, generator=torch.Generator().manual_seed(15)) * 0.1
+    g = torch.randn(2, cout, 5, 4, generator=torch.Generator().manual_seed(16))
+    ref = torch.nn.grad.conv2d_input((2, cin, Hi, Wi), wg.to(mode).double(), g.to(mode).double(), stride=2, padding=1)
+    gp = g.permute(0, 2, 3, 1).unsqueeze(1).to(mode).contiguous()
+    out = torch.zeros(2, Hi, Wi, cin, dtype=torch.float64)
+    for (py, px), ph in dense_train.pack_dgrad(wg, 2, 1, plane=mode):
+        Hp, Wp = (Hi - py + 1) // 2, (Wi - px + 1) // 2
+        out[:, py::2, px::2] = R.tap_sum(gp, None, ph, out_hw=(Hp, Wp))[..., :cin]
+    assert rel(out, ref.permute(0, 2, 3, 1)) < TOL

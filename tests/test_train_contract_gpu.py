@@ -17,6 +17,14 @@ planes with their padding), inputs placed in NaN-filled rows (a read outside the
     hi/lo split of the stored fp32 output; the dropout mask bit for bit the header's Philox-4x32-10; g_masked bitwise
     where(y > 0, g, 0); phase_interleave an exact copy;
   - the two replays bitwise equal, and equal to what the production launch wrote.
+One-plane (autocast) launches: the same modules run steps with the forward under torch.autocast in float16 and in
+bfloat16 (one of them at 200 x 200, so the weight gradient's pixels per split reach the thousands), and synthetic calls
+cover what they never produce.  stp3_conv_wgrad_plane / stp3_conv3d_wgrad_plane are replayed on the plane bytes
+production read (the forward's kept plane or the operand() plane, at its row stride; an fp32 operand as the plane
+stp3_f32_to_plane makes of it, torch's rounding, which tests/test_aux_contract_gpu.py holds it to bit for bit), in rows
+whose channels outside [0, cin) are a NaN of the plane type, and held to the fp64 product of the plane values within
+wgrad_bar(per) of its max; stp3_bn_apply_plane must store y bitwise as stp3_bn_apply does on the same arguments, the
+plane bitwise torch's rounding of y with padding channels +0, and the dropout bits of the Philox reference.
 The last test asserts that the replays reached every entry point and path."""
 import ast
 import inspect
@@ -81,6 +89,43 @@ class In:
 
     def aligned(self):
         return self.cs % 4 == 0 and (self.shift + self.coff) % 4 == 0
+
+
+NAN16 = 0x7FFF          # a NaN of both fp16 and bf16
+SENT16 = 0x7FA5         # sentinel of one-plane outputs (also a NaN of both types)
+
+
+@dataclass
+class PIn:
+    """A one-plane (fp16 / bf16) input of n rows x C channels at row stride cs, the storage shifted by `shift` elements
+    (shift % 8 != 0: not 16-byte aligned); every element outside channels [0, C) is NaN of the plane type."""
+    vals: torch.Tensor                 # (n, C) fp16 / bf16
+    cs: int = 0
+    shift: int = 0
+    coff = 0
+
+    def __post_init__(self):
+        self.vals = self.vals.detach().reshape(-1, self.vals.shape[-1]).to(DEV).clone()
+        n, C = self.vals.shape
+        self.cs = self.cs or C
+        self.store = torch.full((self.shift + n * self.cs + 16,), NAN16, dtype=torch.int16, device=DEV).view(self.vals.dtype)
+        self.store[self.shift:self.shift + n * self.cs].view(n, self.cs)[:, :C] = self.vals
+
+    def ptr(self):
+        return self.store.data_ptr() + 2 * self.shift
+
+    def aligned(self):
+        return self.cs % 8 == 0 and self.shift % 8 == 0
+
+
+def _plane_operand(t, mode):
+    """(plane values (rows, C), row stride, (H, W), (B, T) or None) of what dense_train.conv_wgrad reads under `mode`:
+    a one-plane HL as it is, an fp32 tensor as operand() converts it (cp = pad_to(C))"""
+    if isinstance(t, dense.HL):
+        B, T, H, W, cs = t.hi.shape
+        return t.hi.reshape(-1, cs)[:, :t.c], cs, (H, W), None
+    C = t.shape[-1]
+    return t.reshape(-1, C).to(mode), dense.pad_to(C), tuple(t.shape[-3:-1]), tuple(t.shape[:2]) if t.dim() == 5 else None
 
 
 def In_of(t: torch.Tensor) -> In:
@@ -158,7 +203,19 @@ def run(case: Case):
         x, g = a["x"], a["g"]
         shape = (a["cout"], a["cin"], a["kt"], a["kh"], a["kw"])
         dw = out("dw", _dense_out(shape))
-        if a["is3d"]:
+        op = dense.PLANE_OPERAND[a["mode"]] if a["mode"] is not None else None
+        if op is not None and a["is3d"]:
+            nb = L.stp3_conv3d_wgrad_scratch_bytes(a["B"], a["T"], a["H"], a["W"], a["cout"], a["cin"], a["kt"], a["kh"], a["kw"])
+            sc = _scratch(nb)
+            code = L.stp3_conv3d_wgrad_plane(op, x.ptr(), a["B"], a["T"], a["H"], a["W"], x.cs, a["cin"], g.ptr(), g.cs,
+                                             a["cout"], a["kt"], a["kh"], a["kw"], sc.data_ptr(), nb, dw, _stream())
+        elif op is not None:
+            nb = L.stp3_conv_wgrad_scratch_bytes(a["n_img"], a["Ho"], a["Wo"], a["cout"], a["cin"], a["kh"], a["kw"], a["dil"])
+            sc = _scratch(nb)
+            code = L.stp3_conv_wgrad_plane(op, x.ptr(), a["n_img"], a["H"], a["W"], x.cs, a["cin"], g.ptr(), a["Ho"],
+                                           a["Wo"], g.cs, a["cout"], a["kh"], a["kw"], a["stride"], a["pad"], a["dil"],
+                                           sc.data_ptr(), nb, dw, _stream())
+        elif a["is3d"]:
             nb = L.stp3_conv3d_wgrad_scratch_bytes(a["B"], a["T"], a["H"], a["W"], a["cout"], a["cin"], a["kt"], a["kh"], a["kw"])
             sc = _scratch(nb)
             code = L.stp3_conv3d_wgrad(x.ptr(), a["B"], a["T"], a["H"], a["W"], x.cs, a["cin"], g.ptr(), g.cs, a["cout"],
@@ -179,6 +236,17 @@ def run(case: Case):
                                rv.data_ptr() if rv is not None else None, *ptrs, sc.data_ptr(), nb, _stream())
         if rm is not None:
             outs["run_mean"], outs["run_var"] = (None, rm, None), (None, rv, None)
+    elif k == "bn_apply" and a["mode"] is not None:
+        C, n, hl = a["C"], a["n"], a["hl_cs"]
+        yp = out("y", a["y"])
+        plane = torch.full((n * hl + 8,), SENT16, dtype=torch.int16, device=DEV).view(a["mode"])
+        outs["plane"] = (None, plane, None)
+        res = a["res"]
+        code = L.stp3_bn_apply_plane(a["x"].ptr(), n, C, a["x"].cs, a["mean"].data_ptr(), a["invstd"].data_ptr(),
+                                     a["gamma"].data_ptr(), a["beta"].data_ptr(), res.ptr() if res else None,
+                                     res.cs if res else 0, int(a["relu"]), a["p"], a["seed"], a["offset"], yp, a["y"].cs,
+                                     plane.data_ptr() + 2 * a["plane_shift"], hl, dense.PLANE_OPERAND[a["mode"]],
+                                     _stream())
     elif k == "bn_apply":
         C, n, hl = a["C"], a["n"], a["hl_cs"]
         yp = out("y", a["y"]) if a["y"] is not None else None
@@ -268,7 +336,10 @@ def check(case: Case):
         x = a["x"].vals.view(a["n_img"], a["H"], a["W"], a["cin"])
         g = a["g"].vals.view(a["n_img"], a["Ho"], a["Wo"], a["cout"])
         args = (a["kh"], a["kw"], a["stride"], a["pad"], a["dil"], a["kt"], a["T"])
-        exact, model = R.wgrad(x, g, *args), R.wgrad(x, g, *args, model=True)
+        if a["mode"] is not None:       # one product of the plane values: the exact result is the model
+            exact = model = R.wgrad(x, g, *args, plane=a["mode"])
+        else:
+            exact, model = R.wgrad(x, g, *args), R.wgrad(x, g, *args, model=True)
         dw = got["dw"].reshape(exact.shape).double()
         scale = max(float(exact.abs().max()), 1e-30)
         res["exact"] = float((dw - exact).abs().max()) / scale
@@ -290,6 +361,24 @@ def check(case: Case):
             mag_v = (1 - m) * a["rv"].double().abs() + m * ref["var"].abs() * 2
             ratios["run_mean"] = _ulps(got["run_mean"], ref["run_mean"], mag_m, 4)
             ratios["run_var"] = _ulps(got["run_var"], ref["run_var"], mag_v, 6)
+    elif k == "bn_apply" and a["mode"] is not None:
+        n, C, hl, sh = a["n"], a["C"], a["hl_cs"], a["plane_shift"]
+        ref = R.bn_apply(a["x"].vals, a["mean"], a["invstd"], a["gamma"], a["beta"],
+                         a["res"].vals if a["res"] else None, a["relu"], a["p"], a["seed"], a["offset"])
+        y = got["y"]
+        # y exactly as stp3_bn_apply stores it on the same arguments
+        twin, _ = run(Case("bn_apply", dict(a, mode=None, hl_cs=0)))
+        res["y_as_bn_apply"] = torch.equal(y.contiguous().view(torch.int32), twin["y"].contiguous().view(torch.int32))
+        pl = got["plane"][sh:sh + n * hl].view(n, hl)
+        want = R.bn_apply_plane(y.contiguous(), hl, a["mode"])
+        res["plane_is_rounded_y"] = torch.equal(pl.view(torch.int16), want.view(torch.int16))
+        res["padding +0"] = not bool(pl[:, C:].view(torch.int16).any())
+        bits = got["plane"].view(torch.int16)
+        res["guard"] = bool((bits[:sh] == SENT16).all() and (bits[sh + n * hl:] == SENT16).all())
+        ratios["y"] = _ulps(y, ref["y"], ref["mag"], 8)
+        if ref["keep"] is not None:
+            res["dropped_zero"] = not bool(y[~ref["keep"]].any())
+            res["keep_bits"] = not bool(((y == 0) & (ref["y"].abs() > 8 * ULP * ref["mag"])).any())
     elif k == "bn_apply":
         ref = R.bn_apply(a["x"].vals, a["mean"], a["invstd"], a["gamma"], a["beta"],
                          a["res"].vals if a["res"] else None, a["relu"], a["p"], a["seed"], a["offset"])
@@ -355,11 +444,12 @@ def passed(res):
 
 
 # ------------------------------------------------------------------------------------------------ case constructors
-def wgrad_case(x: In, g: In, n_img, H, W, cin, Ho, Wo, cout, kh, kw, stride=1, pad=None, dil=1, kt=1, B=None, T=1,
-               is3d=False, tag=""):
+def wgrad_case(x, g, n_img, H, W, cin, Ho, Wo, cout, kh, kw, stride=1, pad=None, dil=1, kt=1, B=None, T=1,
+               is3d=False, tag="", mode=None):
+    """x, g: In (fp32), or PIn of the plane type `mode` (stp3_conv_wgrad_plane / stp3_conv3d_wgrad_plane)"""
     pad = (kh - 1) * dil // 2 if pad is None else pad
     a = dict(x=x, g=g, n_img=n_img, H=H, W=W, cin=cin, Ho=Ho, Wo=Wo, cout=cout, kh=kh, kw=kw, stride=stride, pad=pad,
-             dil=dil, kt=kt, T=T, B=B if B is not None else n_img // T, is3d=is3d)
+             dil=dil, kt=kt, T=T, B=B if B is not None else n_img // T, is3d=is3d, mode=mode)
     P = n_img * Ho * Wo
     n, per = R.wgrad_split(P, kt * kh * kw, cout, cin)
     a["per"], a["n_split"] = per, n
@@ -385,14 +475,25 @@ def wgrad_case(x: In, g: In, n_img, H, W, cin, Ho, Wo, cout, kh, kw, stride=1, p
             for kx in range(kw):
                 if not (live(ky * dil - pad, Ho, H) and live(kx * dil - pad, Wo, W) and kt - 1 - it < T):
                     f.add("dead tap")
+    if mode is not None:
+        f = {f"plane {v}" for v in f} | {f"plane wgrad {PLANE_NAMES[mode]}"}
+        if P % 64 in (1, 63):
+            f.add("plane P = 64k +- 1")
+        if P < 64:
+            f.add("plane P < 64")
     return Case("wgrad", a, tag, features=f)
 
 
+PLANE_NAMES = {torch.float16: "fp16", torch.bfloat16: "bf16"}
+
+
 def bn_apply_case(x: In, C, mean, invstd, gamma, beta, res=None, relu=False, p=0.0, seed=0, offset=0, y=None, hl_cs=0,
-                  tag=""):
+                  tag="", mode=None, plane_shift=0):
+    """mode (torch.float16 / torch.bfloat16): stp3_bn_apply_plane, one plane of rows of hl_cs channels starting
+    plane_shift elements into its storage"""
     n = x.vals.shape[0]
     a = dict(x=x, n=n, C=C, mean=mean, invstd=invstd, gamma=gamma, beta=beta, res=res, relu=relu, p=float(p), seed=seed,
-             offset=offset, y=y, hl_cs=hl_cs)
+             offset=offset, y=y, hl_cs=hl_cs, mode=mode, plane_shift=plane_shift)
     vec = C % 8 == 0 and x.aligned() and (res is None or res.aligned()) and (y is None or y.aligned())
     f = {"bn_apply vector" if vec else "bn_apply scalar"}
     if p > 0:
@@ -403,6 +504,12 @@ def bn_apply_case(x: In, C, mean, invstd, gamma, beta, res=None, relu=False, p=0
         f.add("bf16 padding" if not vec else "bf16 padding, vector")
     if y is not None and y.cs > C:
         f.add("bn_apply window")
+    if mode is not None:
+        f = {f"plane {v}" for v in f if "bf16 padding" not in v} | {"bn_apply_plane", f"bn_apply_plane {PLANE_NAMES[mode]}"}
+        if hl_cs > C:
+            f.add("plane padding" + (", vector" if vec and hl_cs - C >= 8 else ""))
+        if hl_cs % 64:
+            f.add("plane plane_cstride not a multiple of 64")
     return Case("bn_apply", a, tag, features=f)
 
 
@@ -457,7 +564,7 @@ class Recorder:
     def _add(self, case, prod):
         case.tag = f"{self.source}: {case.tag}"
         case.prod = {k: v.detach().clone() for k, v in prod.items()}
-        case.features.add("recorded")
+        case.features.add("plane recorded" if case.a.get("mode") is not None else "recorded")
         self.cases.append(case)
 
     def _wrap(self, nm, orig):
@@ -471,10 +578,23 @@ class Recorder:
         return wrapper
 
     # each _<name>(args, _after=None): called before the call (returns what must be cloned first) and after it
-    def _conv_wgrad(self, x, g, kh, kw, stride, dilation=1, kt=None, _after=None):
+    def _conv_wgrad(self, x, g, kh, kw, stride, dilation=1, kt=None, mode=None, _after=None):
         if _after is None:
             return None
         dw = _after[1]
+        if mode is not None:
+            (xv, xcs, (H, W), bt_x), (gv, gcs, (Ho, Wo), bt_g) = _plane_operand(x, mode), _plane_operand(g, mode)
+            cin, cout, N = xv.shape[-1], gv.shape[-1], xv.shape[0] // (H * W)
+            name = PLANE_NAMES[mode]
+            if kt is not None:
+                B, T = bt_x or bt_g
+                c = wgrad_case(PIn(xv, xcs), PIn(gv, gcs), N, H, W, cin, H, W, cout, kh, kw, 1, (kh - 1) // 2, 1, kt, B,
+                               T, True, f"wgrad3d {name} ({kt},{kh},{kw}) {cin}->{cout} {B}x{T}x{H}x{W}", mode)
+            else:
+                c = wgrad_case(PIn(xv, xcs), PIn(gv, gcs), N, H, W, cin, Ho, Wo, cout, kh, kw, stride, None, dilation,
+                               tag=f"wgrad {name} {kh}x{kw} s{stride} d{dilation} {cin}->{cout} {N}x{H}x{W}", mode=mode)
+            self._add(c, {"dw": dw.reshape(-1)})
+            return
         if x.dim() == 5:
             B, T, H, W, cin = x.shape
             cout = g.shape[-1]
@@ -500,7 +620,8 @@ class Recorder:
             prod.update(run_mean=running_mean, run_var=running_var)
         self._add(c, prod)
 
-    def _bn_apply(self, x, st, gamma, beta, relu, res=None, hl=True, dropout=(0.0, 0, 0), y_out=None, _after=None):
+    def _bn_apply(self, x, st, gamma, beta, relu, res=None, hl=True, dropout=(0.0, 0, 0), y_out=None, mode=None,
+                  _after=None):
         if _after is None:
             return None
         y, planes = _after[1]
@@ -510,9 +631,12 @@ class Recorder:
         p, seed, offset = dropout
         c = bn_apply_case(In_of(x), C, _vec(st.mean), _vec(st.invstd), _vec(gamma), _vec(beta),
                           In_of(res) if res is not None else None, relu, p, int(seed), int(offset), ys,
-                          planes.hi.shape[-1] if planes is not None else 0, f"bn_apply C{C} n{N * H * W} p{p}")
+                          planes.hi.shape[-1] if planes is not None else 0, f"bn_apply C{C} n{N * H * W} p{p}",
+                          mode if planes is not None else None)
         prod = {"y": y.reshape(-1, C)}
-        if planes is not None:
+        if planes is not None and mode is not None:
+            prod["plane"] = planes.hi.reshape(-1)
+        elif planes is not None:
             prod.update(hi=planes.hi.reshape(-1), lo=planes.lo.reshape(-1))
         self._add(c, prod)
 
@@ -609,7 +733,7 @@ def train_entry_points_called_outside_dense_train():
     names = {"stp3_conv_wgrad", "stp3_conv3d_wgrad", "stp3_bn_stats", "stp3_bn_apply", "stp3_bn_bwd_reduce",
              "stp3_bn_bwd_apply", "stp3_image_channel_sums", "stp3_temporal_pair_mean", "stp3_upsample2x_f32",
              "stp3_upsample2x_bwd", "stp3_upsample2x_window_f32", "stp3_upsample2x_window_bwd", "stp3_phase_interleave",
-             "stp3_sigmoid_bwd"}
+             "stp3_sigmoid_bwd", "stp3_conv_wgrad_plane", "stp3_conv3d_wgrad_plane", "stp3_bn_apply_plane"}
     pkg = os.path.dirname(os.path.abspath(dense_train.__file__))
     bad = []
     for root, _, files in os.walk(pkg):
@@ -618,11 +742,23 @@ def train_entry_points_called_outside_dense_train():
                 with open(os.path.join(root, f)) as fh:
                     tree = ast.parse(fh.read())
                 bad += [f"{f}:{n.lineno}" for n in ast.walk(tree) if isinstance(n, ast.Attribute) and n.attr in names]
-    # inside dense_train.py every entry point is called from the function the Recorder wraps
+    # inside dense_train.py every entry point is called from the function the Recorder wraps, or from
+    # _conv_wgrad_plane provided the wrapped conv_wgrad is its only caller
     tree = ast.parse(inspect.getsource(dense_train))
     wrapped = set(Recorder.NAMES)
+    helper = "_conv_wgrad_plane"
+    callers = {fn.name for fn in tree.body if isinstance(fn, ast.FunctionDef)
+               for n in ast.walk(fn) if isinstance(n, ast.Name) and n.id == helper}
+    if callers != {"conv_wgrad"}:
+        bad.append(f"dense_train.{helper} referenced from {sorted(callers)}, not only from conv_wgrad")
+    for root, _, files in os.walk(pkg):
+        for f in files:
+            if f.endswith(".py") and os.path.join(root, f) != os.path.abspath(dense_train.__file__):
+                with open(os.path.join(root, f)) as fh:
+                    bad += [f"{f}:{n.lineno}" for n in ast.walk(ast.parse(fh.read()))
+                            if isinstance(n, (ast.Attribute, ast.Name)) and getattr(n, "attr", getattr(n, "id", "")) == helper]
     for fn in tree.body:
-        if isinstance(fn, ast.FunctionDef) and fn.name not in wrapped:
+        if isinstance(fn, ast.FunctionDef) and fn.name not in wrapped | {helper}:
             bad += [f"dense_train.{fn.name}:{n.lineno}" for n in ast.walk(fn) if isinstance(n, ast.Attribute) and n.attr in names]
     return bad
 
@@ -632,34 +768,34 @@ def gauss(shape, seed):
     return TD.exact_gauss(shape, torch.Generator().manual_seed(seed))
 
 
-def _step(fwd, seed):
-    """run fwd() -> outputs, then backward of sum(out * G) with G from `seed`"""
-    out = fwd()
+def _step(fwd, seed, mode=None):
+    """run fwd() -> outputs, then backward of sum(out * G) with G from `seed`.  mode (torch.float16 / torch.bfloat16):
+    the forward under torch.autocast of that type and the backward outside it, as a precision-16 trainer runs a step"""
+    with torch.autocast("cuda", dtype=mode or torch.float16, enabled=mode is not None):
+        out = fwd()
     outs = [v for v in (out.values() if isinstance(out, dict) else [out]) if v is not None]
     gen = torch.Generator().manual_seed(seed)
-    sum((v * torch.randn(v.shape, generator=gen).to(DEV)).sum() for v in outs).backward()
+    sum((v.float() * torch.randn(v.shape, generator=gen).to(DEV)).sum() for v in outs).backward()
 
 
-def rec_decoder(shape, gates, name):
+# One train step of each module; the rec_* functions record it with this file's Recorder, and the convolution and
+# helper suites run the same steps (under autocast too) inside their own recorders.
+def decoder_step(shape, gates, mode=None):
     from stp3_b200.models.decoder import Decoder
     dec = TD.init_exact(Decoder(64, 2, 3, 2, gates), seed=2).train().to(DEV)
     x = gauss(shape, 6).to(DEV).requires_grad_(True)
-    with Recorder(name) as r:
-        _step(lambda: dec(x), 9)
-    return r.cases
+    _step(lambda: dec(x), 9, mode)
 
 
-def rec_deeplab(cin, ncls, hidden, N, H, W, name):
+def deeplab_step(cin, ncls, hidden, N, H, W, mode=None):
     from stp3_b200.layers.convolutions import DeepLabHead
     head = TD.init_exact(DeepLabHead(cin, ncls, hidden_channel=hidden), seed=3).train().to(DEV)
     x = gauss((N, cin, H, W), 4).to(DEV).requires_grad_(True)
     torch.manual_seed(5)
-    with Recorder(name) as r:
-        _step(lambda: head(x), 6)
-    return r.cases
+    _step(lambda: head(x), 6, mode)
 
 
-def rec_temporal(cin, nc, S, B, H, W, name):
+def temporal_step(cin, nc, S, B, H, W, mode=None):
     from stp3_b200.models.temporal_model import TemporalModel
     tm = TD.init_exact(TemporalModel(cin, S, (H, W), start_out_channels=64), seed=3)
     tm.model[0].n_const = nc
@@ -667,20 +803,40 @@ def rec_temporal(cin, nc, S, B, H, W, name):
     x = gauss((B, S, cin - nc, H, W), 5).to(DEV).requires_grad_(True)
     const = gauss((B * S, nc), 6).to(DEV) if nc else None
     torch.manual_seed(7)
-    with Recorder(name) as r:
-        _step(lambda: tm(x, const=const), 8)
-    return r.cases
+    _step(lambda: tm(x, const=const), 8, mode)
 
 
-def rec_encoder_heads(name):
+def encoder_heads_step(name, mode=None):
     from oracle import make_golden_encoder_train as MG
     from stp3_b200.layers import convolutions as CV
     head, up, mods = MG.make_modules(CV, name)
     mods.to(DEV)
     r_lo, r_hi = (t.to(DEV).requires_grad_(True) for t in MG.endpoints())
     torch.manual_seed(17)
+    _step(lambda: up(head(r_hi) if head is not None else r_hi, r_lo), 18, mode)
+
+
+def rec_decoder(shape, gates, name):
+    with Recorder(name) as r:
+        decoder_step(shape, gates)
+    return r.cases
+
+
+def rec_deeplab(cin, ncls, hidden, N, H, W, name):
+    with Recorder(name) as r:
+        deeplab_step(cin, ncls, hidden, N, H, W)
+    return r.cases
+
+
+def rec_temporal(cin, nc, S, B, H, W, name):
+    with Recorder(name) as r:
+        temporal_step(cin, nc, S, B, H, W)
+    return r.cases
+
+
+def rec_encoder_heads(name):
     with Recorder(f"encoder heads {name}") as r:
-        _step(lambda: up(head(r_hi) if head is not None else r_hi, r_lo), 18)
+        encoder_heads_step(name)
     return r.cases
 
 
@@ -768,6 +924,72 @@ def synth_bn():
     return cases
 
 
+def synth_wgrad_plane():
+    """plane weight gradients (both types) the modules never launch: odd row strides and pointers off 16 bytes (the
+    scalar loads), channel counts 1 to 200, P < 64 and P = 64k +- 1, one-row / one-column maps, 7x7 and 3x3 stride 2 on
+    odd and even maps, dilations with dead taps, empty trailing splits, 3-D with T = 1, T < kt and (2, 1, 1)"""
+    cases = []
+    for mode in PLANE_NAMES:
+        def add(n_img, H, W, cin, cout, k, stride=1, dil=1, x_cs=0, g_cs=0, x_shift=0, g_shift=0, tag="", kt=1, T=1):
+            s = len(cases)
+            Ho, Wo = (H + stride - 1) // stride, (W + stride - 1) // stride
+            x = PIn(_r(n_img * H * W, cin, seed=3000 + 2 * s).to(mode), x_cs or dense.pad_to(cin), x_shift)
+            g = PIn(_r(n_img * Ho * Wo, cout, seed=3001 + 2 * s).to(mode), g_cs or dense.pad_to(cout), g_shift)
+            tag = f"{PLANE_NAMES[mode]} {tag}"
+            if kt > 1 or T > 1:
+                cases.append(wgrad_case(x, g, n_img, H, W, cin, H, W, cout, k, k, 1, (k - 1) // 2, 1, kt, n_img // T, T,
+                                        True, tag, mode))
+            else:
+                cases.append(wgrad_case(x, g, n_img, H, W, cin, Ho, Wo, cout, k, k, stride, None, dil, tag=tag, mode=mode))
+        add(2, 9, 11, 35, 40, 3, x_cs=37, g_cs=41, tag="row strides 37 / 41 (scalar loads)")
+        add(1, 8, 9, 64, 64, 3, x_shift=1, g_shift=3, tag="pointers off by 2 / 6 bytes (scalar loads)")
+        for cin in (1, 8, 63, 65, 129, 200):
+            add(1, 10, 12, cin, 24, 3, tag=f"cin {cin}")
+        add(1, 5, 7, 16, 16, 3, tag="P = 35 < 64")
+        add(1, 5, 13, 16, 16, 3, tag="P = 65 = 64 + 1")
+        add(1, 127, 65, 16, 16, 1, tag="P = 64k - 1, several stages")
+        add(2, 1, 77, 24, 40, 3, tag="1 x W")
+        add(2, 61, 1, 24, 40, 3, tag="H x 1")
+        add(2, 37, 29, 64, 48, 7, 2, tag="7x7 stride 2 odd")
+        add(1, 40, 30, 32, 64, 7, 2, tag="7x7 stride 2 even")
+        add(1, 21, 15, 64, 64, 3, 2, tag="3x3 stride 2 odd")
+        add(1, 20, 14, 64, 64, 3, 2, tag="3x3 stride 2 even")
+        add(1, 19, 43, 64, 64, 3, 1, 12, tag="dilation 12, taps partly in padding")
+        add(1, 11, 7, 40, 40, 3, 1, 36, tag="dilation 36 > H, W: only the centre tap lives")
+        add(2, 130, 130, 128, 128, 1, tag="empty trailing splits")
+        add(1, 9, 10, 35, 35, 3, kt=2, T=1, tag="3-D T = 1, kt = 2 (dead time tap)")
+        add(2, 6, 5, 35, 35, 3, kt=3, T=2, tag="3-D T < kt")
+        add(6, 14, 12, 64, 64, 1, kt=2, T=3, tag="3-D (2,1,1), B = 2")
+    return cases
+
+
+def synth_bn_plane():
+    """stp3_bn_apply_plane (both types): C = 1, 7, 33, 64, 1030, input and output windows, residuals, dropout offsets
+    at and past 2^32, plane row strides that are not multiples of 64, a plane starting 16 bytes into its storage"""
+    cases = []
+    for mode in PLANE_NAMES:
+        for C, n, xcs, coff, shift, p, seed, off, relu, res, hl, psh in [
+                (1, 300, 1, 0, 0, 0.0, 0, 0, True, False, 8, 0),
+                (7, 1000, 9, 1, 0, 0.3, (5 << 32) | 11, 2 ** 32 - 3000, True, True, 16, 8),
+                (33, 127, 40, 3, 1, 0.0, 0, 0, False, True, 40, 0),
+                (1030, 129, 1030, 0, 0, 0.5, 77, 2 ** 33 + 5, True, False, 1088, 0),
+                (64, 100, 64, 0, 0, 0.1, (1 << 40) + 3, 2 ** 32 - 64 * 50, True, True, 72, 8),
+                (64, 5000, 72, 8, 0, 0.0, 0, 0, True, True, 128, 0),
+                (40, 300, 40, 0, 0, 0.2, 5, 2 ** 32 + 7, True, False, 64, 0),
+                (64, 200, 64, 0, 0, 0.0, 0, 0, False, False, 128, 8)]:
+            k = len(cases)
+            x = In(_r(n, C, seed=4000 + k, scale=3.0) + 0.5, xcs, coff, shift)
+            mean = _r(C, seed=4100 + k).to(DEV)
+            invstd = (_r(C, seed=4200 + k).abs() + 0.2).to(DEV)
+            gamma, beta = _r(C, seed=4300 + k).to(DEV), _r(C, seed=4400 + k, scale=0.3).to(DEV)
+            r = In(_r(n, C, seed=4500 + k), xcs + 1, 1) if res else None
+            y = Out(n, C, xcs + 3, 2, shift) if k % 2 and k % 8 < 6 else Out(n, C)
+            cases.append(bn_apply_case(x, C, mean, invstd, gamma, beta, r, relu, p, seed, off, y, hl,
+                                       f"bn_apply_plane {PLANE_NAMES[mode]} C{C} n{n} cs{xcs}@{coff}+{shift} p{p} "
+                                       f"off{off:#x} plane cs{hl}+{psh}", mode, psh))
+    return cases
+
+
 def synth_small():
     cases = []
     for n_img, h, w, C, cs, coff, shift in [(2, 5, 7, 12, 40, 4, 0), (1, 1, 9, 8, 8, 0, 0), (3, 6, 1, 5, 9, 3, 0),
@@ -806,7 +1028,27 @@ SOURCES = {
     "synthetic_wgrad": synth_wgrad,
     "synthetic_bn": synth_bn,
     "synthetic_small": synth_small,
+    "synthetic_wgrad_plane": synth_wgrad_plane,
+    "synthetic_bn_plane": synth_bn_plane,
 }
+
+
+def rec_amp(mode, step, *args):
+    """a step of one module with its forward under torch.autocast(dtype=mode)"""
+    with Recorder(f"{step} {args[-1] if isinstance(args[-1], str) else args} {PLANE_NAMES[mode]}") as r:
+        globals()[step](*args, mode=mode)
+    return r.cases
+
+
+for _m, _nm in PLANE_NAMES.items():
+    SOURCES.update({
+        f"amp_decoder_48x64_{_nm}": lambda m=_m: rec_amp(m, "decoder_step", (2, 3, 64, 48, 64), GATES_ALL),
+        f"amp_deeplab_temporal_48x64_{_nm}": lambda m=_m: rec_amp(m, "deeplab_step", 64, 64, 128, 6, 48, 64),
+        f"amp_deeplab_encoder_14x30_{_nm}": lambda m=_m: rec_amp(m, "deeplab_step", 160, 160, 64, 18, 14, 30),
+        f"amp_temporal_48x64_{_nm}": lambda m=_m: rec_amp(m, "temporal_step", 70, 6, 3, 2, 48, 64),
+        f"amp_encoder_heads_feat_{_nm}": lambda m=_m: rec_amp(m, "encoder_heads_step", "feat"),
+        f"amp_encoder_heads_uc_{_nm}": lambda m=_m: rec_amp(m, "encoder_heads_step", "uc")})
+SOURCES["amp_temporal_200x200_fp16"] = lambda: rec_amp(torch.float16, "temporal_step", 70, 6, 3, 2, 200, 200)
 
 _RUNS = {}
 
@@ -858,6 +1100,12 @@ REQUIRED = ["recorded", "wgrad 2-D", "wgrad 3-D", "wgrad scalar loads", "dead ta
             "temporal_pair_mean adjoint 0", "temporal_pair_mean adjoint 1", "upsample vector", "upsample scalar",
             "upsample window", "upsample_bwd vector", "upsample_bwd scalar", "upsample_bwd window", "phase_interleave",
             "NULL phase", "sigmoid_bwd"]
+REQUIRED += ["plane recorded", "plane wgrad fp16", "plane wgrad bf16", "plane wgrad 2-D", "plane wgrad 3-D",
+             "plane wgrad scalar loads", "plane dead tap", "plane empty split", "plane stride 2", "plane dilation",
+             "plane time taps", "plane sample boundaries", "plane P = 64k +- 1", "plane P < 64", "bn_apply_plane fp16",
+             "bn_apply_plane bf16", "plane bn_apply vector", "plane bn_apply scalar", "plane dropout",
+             "plane dropout offset >= 2^32", "plane bn_apply window", "plane padding", "plane padding, vector",
+             "plane plane_cstride not a multiple of 64"]
 
 
 def test_every_entry_point_and_path_is_replayed():
@@ -870,4 +1118,14 @@ def test_every_entry_point_and_path_is_replayed():
     print("weight gradients by pixels per split: per, worst model excess, exact error (of max |exact|)")
     for per, m, e, tag in wg:
         print(f"  {per:6d}  {m:.2e}  {e:.2e}  {tag}")
+    print("one-plane weight gradients, worst per `per` (of max |model|): fp16 / bf16 (bar wgrad_bar(per))")
+    worst = {}
+    for r in rows:
+        for nm in PLANE_NAMES.values():
+            if f"plane wgrad {nm}" in r["features"]:
+                k = (r["res"]["per"], nm)
+                worst[k] = max(worst.get(k, 0.0), r["res"]["model"])
+    for per in sorted({p for p, _ in worst}):
+        print(f"  {per:6d}  " + "  ".join(f"{nm} {worst[(per, nm)]:.2e}" if (per, nm) in worst else f"{nm}    -    "
+                                          for nm in PLANE_NAMES.values()) + f"  (bar {wgrad_bar(per):.1e})")
     assert all(counts.values()), [f for f, c in counts.items() if not c]

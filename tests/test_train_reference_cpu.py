@@ -63,6 +63,52 @@ def test_wgrad_model_is_three_bf16_products():
     _close(model, by_hand, 1e-15)
 
 
+@pytest.mark.parametrize("mode", [torch.float16, torch.bfloat16])
+@pytest.mark.parametrize("H,W,cin,cout,k,stride,dil", [(9, 7, 5, 3, 3, 1, 1), (8, 10, 4, 6, 7, 2, 1), (9, 8, 3, 4, 3, 2, 1),
+                                                       (6, 11, 3, 2, 3, 1, 4)])
+def test_plane_wgrad_matches_conv2d_weight_of_rounded_operands(mode, H, W, cin, cout, k, stride, dil):
+    """2-D, stride 2 (odd and even) and dilated: the plane weight gradient is torch.nn.grad.conv2d_weight of x and g
+    rounded to the plane type, whether they arrive as fp32 or as planes"""
+    pad = (k - 1) * dil // 2
+    x = _rand(2, H, W, cin, seed=21) * 3
+    Ho, Wo = (H + stride - 1) // stride, (W + stride - 1) // stride
+    g = _rand(2, Ho, Wo, cout, seed=22)
+    ref = torch.nn.grad.conv2d_weight(x.to(mode).double().permute(0, 3, 1, 2), (cout, cin, k, k),
+                                      g.to(mode).double().permute(0, 3, 1, 2), stride=stride, padding=pad, dilation=dil)
+    got = R.wgrad(x, g, k, k, stride, pad, dil, plane=mode)
+    _close(got[:, :, 0], ref)
+    assert torch.equal(R.wgrad(x.to(mode), g.to(mode), k, k, stride, pad, dil, plane=mode), got)
+    assert not torch.equal(got, R.wgrad(x, g, k, k, stride, pad, dil))       # the rounding is there
+
+
+@pytest.mark.parametrize("mode", [torch.float16, torch.bfloat16])
+@pytest.mark.parametrize("B,T,kt,k", [(2, 3, 2, 3), (1, 1, 2, 3), (2, 2, 3, 1)])
+def test_plane_wgrad_3d_matches_causal_conv3d_autograd(mode, B, T, kt, k):
+    H, W, cin, cout = 5, 6, 3, 4
+    x = _rand(B, T, H, W, cin, seed=23)
+    g = _rand(B, T, H, W, cout, seed=24)
+    w = torch.zeros(cout, cin, kt, k, k, dtype=torch.float64, requires_grad=True)
+    xin = F.pad(x.to(mode).double().permute(0, 4, 1, 2, 3), (0, 0, 0, 0, kt - 1, 0))
+    (F.conv3d(xin, w, padding=(0, k // 2, k // 2)) * g.to(mode).double().permute(0, 4, 1, 2, 3)).sum().backward()
+    got = R.wgrad(x.reshape(B * T, H, W, cin), g.reshape(B * T, H, W, cout), k, k, 1, k // 2, 1, kt=kt, T=T, plane=mode)
+    _close(got, w.grad)
+
+
+@pytest.mark.parametrize("mode", [torch.float16, torch.bfloat16])
+def test_bn_apply_plane_is_the_rounded_fp32_output(mode):
+    """the plane reference is torch's rounding of the fp32 bn_apply output (overflow to inf, -0.0 kept) with +0
+    padding channels"""
+    x = _rand(50, 7, seed=25) * 4
+    mean, invstd, gamma, beta = _rand(7, seed=26), _rand(7, seed=27).abs() + 0.5, _rand(7, seed=28), _rand(7, seed=29)
+    y = R.bn_apply(x, mean, invstd, gamma, beta)["y"].float()
+    y[0, 0], y[1, 1] = -0.0, 1e6
+    pl = R.bn_apply_plane(y, 16, mode)
+    assert pl.dtype == mode and pl.shape == (50, 16)
+    assert torch.equal(pl[:, :7].view(torch.int16), y.to(mode).view(torch.int16))
+    assert not pl[:, 7:].view(torch.int16).any() and torch.signbit(pl[0, 0].float())
+    assert torch.isinf(pl[1, 1].float()) == (mode == torch.float16)
+
+
 def test_wgrad_split_plan():
     assert R.wgrad_split(240000, 18, 35, 35) == (30, 8000)            # causal (2,3,3) 35 -> 35, B = 2, T = 3, 200x200
     assert R.wgrad_split(2 * 48 * 64, 9, 64, 64) == (24, 256)

@@ -7,7 +7,9 @@ Tensors are dense channels-last; the callers cut channel windows out of wider ro
 Besides the exact value, most functions return the magnitude the kernel's fp32 rounding is measured against: the sum of
 the absolute values of the terms (an elementwise bar of a few ulps of that is what a correct fp32 evaluation meets), and
 for the weight gradient the "model" value: the three bf16 products g_hi x_hi + g_hi x_lo + g_lo x_hi the tensor cores
-issue, with the planes split like ptx::split_hilo (round to nearest, then the remainder to nearest)."""
+issue, with the planes split like ptx::split_hilo (round to nearest, then the remainder to nearest).  The one-plane
+(autocast) kernels read fp16 / bf16 values exactly and issue one product each, so their fp64 product of the rounded
+values is both the exact result and the model (wgrad with `plane`)."""
 from typing import List, Optional, Sequence
 
 import numpy as np
@@ -46,13 +48,17 @@ def _shift(x: torch.Tensor, dy: int, dx: int, dt: int, stride: int, Ho: int, Wo:
 
 
 def wgrad(x: torch.Tensor, g: torch.Tensor, kh: int, kw: int, stride: int = 1, pad: int = 0, dil: int = 1,
-          kt: int = 1, T: int = 1, model: bool = False) -> torch.Tensor:
+          kt: int = 1, T: int = 1, model: bool = False, plane: Optional[torch.dtype] = None) -> torch.Tensor:
     """dw (cout, cin, kt, kh, kw) of stp3_conv_wgrad (kt = T = 1) or stp3_conv3d_wgrad (n_img = B * T frames,
     frame-major within a sample; time tap it reads frame t + it - (kt - 1)): x (n_img, H, W, cin) and g (n_img, Ho, Wo,
-    cout) fp32.  model: the three bf16 products of the kernel instead of the exact product of the fp32 values."""
+    cout) fp32.  model: the three bf16 products of the kernel instead of the exact product of the fp32 values.
+    plane (torch.float16 / torch.bfloat16): stp3_conv_wgrad_plane / stp3_conv3d_wgrad_plane, the product of x and g
+    rounded to that type (torch's rounding, as stp3_f32_to_plane; a plane passed in stays as it is)."""
     n, Ho, Wo, cout = g.shape
     cin = x.shape[-1]
-    if model:
+    if plane is not None:
+        pairs = [(g.to(plane), x.to(plane))]
+    elif model:
         (xh, xl), (gh, gl) = dense.split_hilo(x.float()), dense.split_hilo(g.float())
         pairs = [(gh, xh), (gh, xl), (gl, xh)]
     else:
@@ -144,6 +150,15 @@ def bn_apply(x, mean, invstd, gamma, beta, res=None, relu=False, p=0.0, seed=0, 
         s = dropout_scale(p)
         y, mag = torch.where(keep, y * s, torch.zeros_like(y)), mag * s
     return {"y": y, "keep": keep, "mag": mag}
+
+
+def bn_apply_plane(y: torch.Tensor, cs: int, mode: torch.dtype) -> torch.Tensor:
+    """the plane of stp3_bn_apply_plane: y (n_pix, C) fp32 as stp3_bn_apply stores it, rounded by torch's .to(mode),
+    in rows of cs channels whose channels [C, cs) are +0"""
+    n, C = y.shape
+    out = torch.zeros((n, cs), dtype=mode, device=y.device)
+    out[:, :C] = y.to(mode)
+    return out
 
 
 def _masked(g, y):
