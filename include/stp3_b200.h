@@ -605,6 +605,63 @@ int stp3_se_gate(const float* sums, int sums_stride, int n_img, int C, float inv
                  void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------
+ * EfficientNet trunk, train mode (EfficientNetTrunk(trainable=True).train()).  fp32 channels-last tensors with C
+ * channels per pixel row unless a stride says otherwise; the static pads are the eval kernels' (top / left from the
+ * nominal image size, zero past the bottom / right edge).  Reductions write per-block fp64 partials into caller scratch
+ * and add them in a fixed order: no atomics, bitwise repeatable.  1x1 convolutions, their gradients, the batch
+ * statistics and the BatchNorm backward are the decoder's train-mode entry points above.
+ *
+ * stp3_effnet_stem_raw: y (n_img, Ho, Wo, cout) = 3x3 stride-2 conv of the NCHW images x (n_img, 3, H, W) with
+ * w [cout][3][3][3], no bias, no activation.  cout <= 64.
+ * stp3_effnet_stem_wgrad: dw [cout][3][3][3] = sum over images and output pixels of g (n_img, Ho, Wo, cout) times the
+ * input tap the forward read (zero outside the image), through stp3_effnet_stem_wgrad_scratch_bytes() of scratch. */
+int stp3_effnet_stem_raw(const float* x, int n_img, int H, int W, int Ho, int Wo, int pad_t, int pad_l, const float* w,
+                         int cout, float* y, void* stream);
+size_t stp3_effnet_stem_wgrad_scratch_bytes(int n_img, int Ho, int Wo, int cout);
+int stp3_effnet_stem_wgrad(const float* x, int n_img, int H, int W, int Ho, int Wo, int pad_t, int pad_l, const float* g,
+                           int cout, float* dw, void* scratch, size_t scratch_bytes, void* stream);
+/* Depthwise k x k (3 / 5), stride 1 / 2, on fp32 tensors described by stp3_dw_desc with in_cstride / out_cstride in
+ * fp32 elements (>= C, any C):
+ * stp3_dw_fwd_raw: y (n_img, Ho, Wo, .) = the convolution of x (n_img, H, W, .) with w [k*k][C], no bias, no activation.
+ * stp3_dw_dgrad: dx (n_img, H, W, .) = its exact adjoint applied to g (n_img, Ho, Wo, .): every input pixel gets the taps
+ * that read it; pixels no output read (past the bottom / right edge) get zero.
+ * stp3_dw_wgrad: dw [k*k][C] = sum over images and output pixels of g times the input tap, through
+ * stp3_dw_wgrad_scratch_bytes(desc) of scratch. */
+int stp3_dw_fwd_raw(const stp3_dw_desc* desc, const float* x, const float* w, float* y, void* stream);
+int stp3_dw_dgrad(const stp3_dw_desc* desc, const float* g, const float* w, float* dx, void* stream);
+size_t stp3_dw_wgrad_scratch_bytes(const stp3_dw_desc* desc);
+int stp3_dw_wgrad(const stp3_dw_desc* desc, const float* x, const float* g, float* dw, void* scratch,
+                  size_t scratch_bytes, void* stream);
+/* stp3_trunk_bn_act: y = act(z) * mul[img][c] * scale[img] + res over x (n_pix, C), img = pixel / img_pix, with
+ * z = (x - mean) * invstd * gamma + beta (batch statistics of stp3_bn_stats; z = x when mean is NULL) and act swish
+ * (swish != 0) or the identity.  mul (n_img, C), scale (n_img), res (n_pix, C) are optional.  Writes y (n_pix, C) fp32
+ * and / or the hi/lo planes (n_pix, hl_cstride) of the next convolution, columns [C, hl_cstride) as zeros.
+ * The MBConv uses: _bn0 / _bn1 / stem + swish; the squeeze-excite gate (no statistics, mul = gate); _bn2 with the
+ * drop-connect scale and the identity skip.
+ * stp3_trunk_bn_act_bwd: out = (g * mul[img][c] + add[img][c]) * act'(z) * scale[img], z recomputed from x; the
+ * dL/dz stp3_bn_bwd_reduce / stp3_bn_bwd_apply (or their SyncBatchNorm forms) then take with no ReLU mask.  out must
+ * not alias g. */
+int stp3_trunk_bn_act(const float* x, long long n_pix, int C, long long img_pix, const float* mean, const float* invstd,
+                      const float* gamma, const float* beta, int swish, const float* mul, const float* scale,
+                      const float* res, float* y, void* y_hi, void* y_lo, int hl_cstride, void* stream);
+int stp3_trunk_bn_act_bwd(const float* g, const float* x, long long n_pix, int C, long long img_pix, const float* mean,
+                          const float* invstd, const float* gamma, const float* beta, int swish, const float* mul,
+                          const float* add, const float* scale, float* out, void* stream);
+/* stp3_image_channel_dot: out (n_img, C) = per image and channel, the sum over its hw pixels of a * b (a, b
+ * (n_img, hw, C)): the squeeze-excite gate gradient sum_p y * (W_proj^T dz). */
+size_t stp3_image_channel_dot_scratch_bytes(int n_img, long long hw, int C);
+int stp3_image_channel_dot(const float* a, const float* b, int n_img, long long hw, int C, float* out, void* scratch,
+                           size_t scratch_bytes, void* stream);
+/* stp3_se_bwd: one CTA per image, from dgate (n_img, C), the forward's gate (n_img, C) and spatial sums (n_img, C):
+ * m = sums * inv_hw, r = w_r m + b_r (w_r [R][C]), de = dgate * gate * (1 - gate) (n_img, C), sr = swish(r) (n_img, R),
+ * dr = (w_e^T de) * swish'(r) (n_img, R) (w_e [C][R]), dmean = (w_r^T dr) * inv_hw (n_img, C): the gradient of the
+ * squeeze-excite mean spread over each pixel.  The weight gradients are dW_e = de^T sr, dW_r = dr^T m and the bias
+ * gradients the column sums of de and dr. */
+int stp3_se_bwd(const float* dgate, const float* gate, const float* sums, int n_img, int C, float inv_hw,
+                const float* w_r, const float* b_r, int R, const float* w_e, float* de, float* sr, float* dr,
+                float* dmean, void* stream);
+
+/* ---------------------------------------------------------------------------------------------------------
  * Discount recurrence of the frame-sharded lift-splat (stp3_lift_splat_fwd with f_count > 0), after the all-gather */
 int stp3_bev_discount(const float* raw /*(B,S,nx,ny,C) fp32*/, int B, int S, int nx, int ny, int C, float discount,
                       void* out_hi, void* out_lo /*(B,S,nx,ny,C) bf16 each*/, void* stream);

@@ -154,6 +154,19 @@ SIGNATURES = {
     "stp3_dw_fwd": (_I, [ctypes.POINTER(DwDesc), _V, _V, _V, _V, _V, _V, _V, _V, _SZ, _V]),
     "stp3_se_proj_weight_elems": (_LL, [_I, _I]),
     "stp3_se_gate": (_I, [_V, _I, _I, _I, _F, _V, _V, _I, _V, _V, _V, _I, _V, _V, _V]),
+    # train mode of the EfficientNet trunk
+    "stp3_effnet_stem_raw": (_I, [_V, _I, _I, _I, _I, _I, _I, _I, _V, _I, _V, _V]),
+    "stp3_effnet_stem_wgrad_scratch_bytes": (_SZ, [_I, _I, _I, _I]),
+    "stp3_effnet_stem_wgrad": (_I, [_V, _I, _I, _I, _I, _I, _I, _I, _V, _I, _V, _V, _SZ, _V]),
+    "stp3_dw_fwd_raw": (_I, [ctypes.POINTER(DwDesc), _V, _V, _V, _V]),
+    "stp3_dw_dgrad": (_I, [ctypes.POINTER(DwDesc), _V, _V, _V, _V]),
+    "stp3_dw_wgrad_scratch_bytes": (_SZ, [ctypes.POINTER(DwDesc)]),
+    "stp3_dw_wgrad": (_I, [ctypes.POINTER(DwDesc), _V, _V, _V, _V, _SZ, _V]),
+    "stp3_trunk_bn_act": (_I, [_V, _LL, _I, _LL, _V, _V, _V, _V, _I, _V, _V, _V, _V, _V, _V, _I, _V]),
+    "stp3_trunk_bn_act_bwd": (_I, [_V, _V, _LL, _I, _LL, _V, _V, _V, _V, _I, _V, _V, _V, _V, _V]),
+    "stp3_image_channel_dot_scratch_bytes": (_SZ, [_I, _LL, _I]),
+    "stp3_image_channel_dot": (_I, [_V, _V, _I, _LL, _I, _V, _V, _SZ, _V]),
+    "stp3_se_bwd": (_I, [_V, _V, _V, _I, _I, _F, _V, _V, _I, _V, _V, _V, _V, _V, _V]),
 }
 
 

@@ -15,6 +15,7 @@ as autocast rounds the operands of F.conv2d) and issue one MMA per product, accu
 autocast) is the fp32-equivalent hi/lo path, bit for bit.  BatchNorm statistics, running statistics and the BatchNorm
 backward stay fp32 in every mode, and so do the tensors the functions return.
 """
+import ctypes
 from dataclasses import dataclass
 from typing import List, Optional, Tuple
 
@@ -657,3 +658,208 @@ def sigmoid_backward(g: torch.Tensor, s: torch.Tensor) -> torch.Tensor:
         code = _lib.lib().stp3_sigmoid_bwd(g.data_ptr(), s.data_ptr(), s.numel(), dz.data_ptr(), _stream(s.device))
     _lib.check(code, "stp3_sigmoid_bwd")
     return dz
+
+
+
+# ------------------------------------------------------------------------------------------------ EfficientNet trunk
+# Train mode of the native trunk (models/efficientnet.py, include/stp3_b200.h "EfficientNet trunk, train mode").
+def conv1x1_raw(x: dense.HL, weight: torch.Tensor) -> torch.Tensor:
+    """conv_raw of a 1x1 convolution with any number of output channels: more than 256 (the trunk's expand
+    convolutions) run as column chunks of at most 256 whose fp32 outputs are concatenated."""
+    cout = weight.shape[0]
+    if cout <= 256:
+        return conv_raw(x, weight, 1)
+    return torch.cat([conv_raw(x, weight[n0:n0 + 256], 1) for n0 in range(0, cout, 256)], dim=-1)
+
+
+def conv1x1_dgrad(g: torch.Tensor, weight: torch.Tensor) -> torch.Tensor:
+    """conv_dgrad of a 1x1 convolution with any number of input channels (the trunk's projections): g is converted to
+    hi/lo once, and more than 256 input channels run as chunks whose fp32 outputs are concatenated."""
+    _f32_cl(g)
+    N, H, W, _ = g.shape
+    cin = weight.shape[1]
+    g_hl = to_hl(g)
+    outs = []
+    for c0 in range(0, cin, 256):
+        w = weight[:, c0:c0 + 256]
+        out = torch.empty((N, H, W, w.shape[1]), dtype=torch.float32, device=g.device)
+        dense.conv(g_hl, pack_dgrad(w, 1, 0)[0][1], out_f32=out, n_valid=w.shape[1], out_f32_nhwc=True, store=False,
+                   tune=(0, 0))
+        outs.append(out)
+    return outs[0] if len(outs) == 1 else torch.cat(outs, dim=-1)
+
+
+def stem_raw(x: torch.Tensor, weight: torch.Tensor, out_hw: Tuple[int, int], pad: int) -> torch.Tensor:
+    """x (M, 3, H, W) fp32 NCHW images -> (M, Ho, Wo, cout) fp32: the 3x3 stride-2 stem convolution, no BatchNorm, no
+    activation (stp3_effnet_stem_raw); pad = the top / left static pad."""
+    assert x.dtype == torch.float32 and x.is_contiguous() and x.is_cuda and x.dim() == 4 and x.shape[1] == 3
+    M, _, H, W = x.shape
+    cout = weight.shape[0]
+    w = weight.detach().float().contiguous()
+    y = torch.empty((M, *out_hw, cout), dtype=torch.float32, device=x.device)
+    with torch.cuda.device(x.device):
+        code = _lib.lib().stp3_effnet_stem_raw(x.data_ptr(), M, H, W, out_hw[0], out_hw[1], pad, pad, w.data_ptr(), cout,
+                                               y.data_ptr(), _stream(x.device))
+    _lib.check(code, "stp3_effnet_stem_raw")
+    return y
+
+
+def stem_wgrad(x: torch.Tensor, g: torch.Tensor, pad: int) -> torch.Tensor:
+    """dL/dW (cout, 3, 3, 3) of stem_raw from its images x and g = dL/dy (M, Ho, Wo, cout) (stp3_effnet_stem_wgrad)."""
+    _f32_cl(g)
+    M, _, H, W = x.shape
+    _, Ho, Wo, cout = g.shape
+    L = _lib.lib()
+    nbytes = L.stp3_effnet_stem_wgrad_scratch_bytes(M, Ho, Wo, cout)
+    scratch = torch.empty(nbytes, dtype=torch.uint8, device=x.device)
+    dw = torch.empty((cout, 3, 3, 3), dtype=torch.float32, device=x.device)
+    with torch.cuda.device(x.device):
+        code = L.stp3_effnet_stem_wgrad(x.data_ptr(), M, H, W, Ho, Wo, pad, pad, g.data_ptr(), cout, dw.data_ptr(),
+                                        scratch.data_ptr(), nbytes, _stream(x.device))
+    _lib.check(code, "stp3_effnet_stem_wgrad")
+    return dw
+
+
+def _dw_desc(N: int, H: int, W: int, Ho: int, Wo: int, k: int, stride: int, pad: int, C: int):
+    return _lib.DwDesc(n_img=N, H=H, W=W, Ho=Ho, Wo=Wo, k=k, stride=stride, pad_t=pad, pad_l=pad, C=C, in_cstride=C,
+                       out_cstride=C)
+
+
+def _dw_taps(weight: torch.Tensor) -> torch.Tensor:
+    """depthwise weight (C, 1, k, k) -> the kernels' [k*k][C] layout"""
+    C, k = weight.shape[0], weight.shape[-1]
+    return weight.detach().float().reshape(C, k * k).t().contiguous()
+
+
+def dw_raw(x: torch.Tensor, weight: torch.Tensor, stride: int, pad: int, out_hw: Tuple[int, int]) -> torch.Tensor:
+    """Depthwise convolution of x (N, H, W, C) with weight (C, 1, k, k), top / left pad `pad`, zero past the bottom /
+    right edge -> (N, Ho, Wo, C) fp32, no BatchNorm, no activation (stp3_dw_fwd_raw)."""
+    _f32_cl(x)
+    N, H, W, C = x.shape
+    k = weight.shape[-1]
+    d = _dw_desc(N, H, W, *out_hw, k, stride, pad, C)
+    w = _dw_taps(weight)
+    y = torch.empty((N, *out_hw, C), dtype=torch.float32, device=x.device)
+    with torch.cuda.device(x.device):
+        code = _lib.lib().stp3_dw_fwd_raw(ctypes.byref(d), x.data_ptr(), w.data_ptr(), y.data_ptr(), _stream(x.device))
+    _lib.check(code, "stp3_dw_fwd_raw")
+    return y
+
+
+def dw_dgrad(g: torch.Tensor, weight: torch.Tensor, stride: int, pad: int, in_hw: Tuple[int, int]) -> torch.Tensor:
+    """dL/dx (N, H, W, C) of dw_raw from g = dL/dy (N, Ho, Wo, C): its exact adjoint (stp3_dw_dgrad)."""
+    _f32_cl(g)
+    N, Ho, Wo, C = g.shape
+    k = weight.shape[-1]
+    d = _dw_desc(N, *in_hw, Ho, Wo, k, stride, pad, C)
+    w = _dw_taps(weight)
+    dx = torch.empty((N, *in_hw, C), dtype=torch.float32, device=g.device)
+    with torch.cuda.device(g.device):
+        code = _lib.lib().stp3_dw_dgrad(ctypes.byref(d), g.data_ptr(), w.data_ptr(), dx.data_ptr(), _stream(g.device))
+    _lib.check(code, "stp3_dw_dgrad")
+    return dx
+
+
+def dw_wgrad(x: torch.Tensor, g: torch.Tensor, k: int, stride: int, pad: int) -> torch.Tensor:
+    """dL/dW (C, 1, k, k) of dw_raw from its input x (N, H, W, C) and g = dL/dy (N, Ho, Wo, C) (stp3_dw_wgrad)."""
+    _f32_cl(x), _f32_cl(g)
+    N, H, W, C = x.shape
+    _, Ho, Wo, _ = g.shape
+    d = _dw_desc(N, H, W, Ho, Wo, k, stride, pad, C)
+    L = _lib.lib()
+    nbytes = L.stp3_dw_wgrad_scratch_bytes(ctypes.byref(d))
+    scratch = torch.empty(nbytes, dtype=torch.uint8, device=x.device)
+    dw = torch.empty((k * k, C), dtype=torch.float32, device=x.device)
+    with torch.cuda.device(x.device):
+        code = L.stp3_dw_wgrad(ctypes.byref(d), x.data_ptr(), g.data_ptr(), dw.data_ptr(), scratch.data_ptr(), nbytes,
+                               _stream(x.device))
+    _lib.check(code, "stp3_dw_wgrad")
+    return dw.t().reshape(C, 1, k, k).contiguous()
+
+
+def _bn_vectors(st: Optional[BNStats], bn: Optional[nn.Module]):
+    if st is None:
+        return None, None, None, None
+    return st.mean, st.invstd, bn.weight.detach().float().contiguous(), bn.bias.detach().float().contiguous()
+
+
+def bn_act(x: torch.Tensor, st: Optional[BNStats], bn: Optional[nn.Module], swish: bool,
+           mul: Optional[torch.Tensor] = None, scale: Optional[torch.Tensor] = None, res: Optional[torch.Tensor] = None,
+           hl: bool = False, f32: bool = True) -> Tuple[Optional[torch.Tensor], Optional[dense.HL]]:
+    """y = act(BN(x)) * mul[img] * scale[img] + res on x (N, H, W, C) (stp3_trunk_bn_act): BN with the batch statistics
+    st and bn's gamma / beta (st None: no BatchNorm), act swish or the identity, mul (N, C) (the squeeze-excite gate),
+    scale (N,) (drop-connect), res (N, H, W, C) (identity skip) -> (fp32 y or None, hi/lo planes or None)."""
+    _f32_cl(x)
+    N, H, W, C = x.shape
+    dev = x.device
+    for t in (mul, scale):
+        assert t is None or (t.dtype == torch.float32 and t.is_contiguous() and t.numel() in (N, N * C))
+    if res is not None:
+        _f32_cl(res)
+        assert res.shape == x.shape
+    y = torch.empty_like(x) if f32 else None
+    out = dense.HL.empty(N, 1, H, W, C, dev) if hl else None
+    mean, invstd, gam, bet = _bn_vectors(st, bn)
+    with torch.cuda.device(dev):
+        code = _lib.lib().stp3_trunk_bn_act(x.data_ptr(), N * H * W, C, H * W, _p(mean), _p(invstd), _p(gam), _p(bet),
+                                            int(swish), _p(mul), _p(scale), _p(res), _p(y),
+                                            _p(out.hi if out else None), _p(out.lo if out else None),
+                                            out.hi.shape[-1] if out else 0, _stream(dev))
+    _lib.check(code, "stp3_trunk_bn_act")
+    return y, out
+
+
+def bn_act_grad(g: torch.Tensor, x: Optional[torch.Tensor], st: Optional[BNStats], bn: Optional[nn.Module],
+                swish: bool, mul: Optional[torch.Tensor] = None, add: Optional[torch.Tensor] = None,
+                scale: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """dL/dz = (g * mul[img] + add[img]) * act'(z) * scale[img], z = BN(x) recomputed from x and st
+    (stp3_trunk_bn_act_bwd): what bn_backward then takes, with no ReLU mask."""
+    _f32_cl(g)
+    N, H, W, C = g.shape
+    if x is not None:
+        assert x.shape == g.shape and x.is_contiguous()
+    mean, invstd, gam, bet = _bn_vectors(st, bn)
+    out = torch.empty_like(g)
+    with torch.cuda.device(g.device):
+        code = _lib.lib().stp3_trunk_bn_act_bwd(g.data_ptr(), _p(x), N * H * W, C, H * W, _p(mean), _p(invstd),
+                                                _p(gam), _p(bet), int(swish), _p(mul), _p(add), _p(scale),
+                                                out.data_ptr(), _stream(g.device))
+    _lib.check(code, "stp3_trunk_bn_act_bwd")
+    return out
+
+
+def image_channel_dot(a: torch.Tensor, b: torch.Tensor) -> torch.Tensor:
+    """(N, C) fp32: per image and channel, the sum over pixels of a * b (a, b (N, H, W, C)) in a fixed order
+    (stp3_image_channel_dot)."""
+    _f32_cl(a), _f32_cl(b)
+    assert a.shape == b.shape
+    N, H, W, C = a.shape
+    L = _lib.lib()
+    nbytes = L.stp3_image_channel_dot_scratch_bytes(N, H * W, C)
+    scratch = torch.empty(nbytes, dtype=torch.uint8, device=a.device)
+    out = torch.empty((N, C), dtype=torch.float32, device=a.device)
+    with torch.cuda.device(a.device):
+        code = L.stp3_image_channel_dot(a.data_ptr(), b.data_ptr(), N, H * W, C, out.data_ptr(), scratch.data_ptr(),
+                                        nbytes, _stream(a.device))
+    _lib.check(code, "stp3_image_channel_dot")
+    return out
+
+
+def se_backward(dgate: torch.Tensor, gate: torch.Tensor, sums: torch.Tensor, hw: int, w_r: torch.Tensor,
+                b_r: torch.Tensor, w_e: torch.Tensor):
+    """The squeeze-excite chain backward of every image (stp3_se_bwd): from dL/dgate, the forward's gate and spatial
+    sums (N, C) and the weights w_r (R, C), b_r (R), w_e (C, R) -> (de (N, C), swish(r) (N, R), dr (N, R),
+    dL/dmean / hw (N, C))."""
+    N, C = gate.shape
+    R = w_r.shape[0]
+    for t in (dgate, gate, sums, w_r, b_r, w_e):
+        assert t.dtype == torch.float32 and t.is_contiguous() and t.is_cuda
+    assert dgate.shape == sums.shape == (N, C) and w_r.shape == (R, C) and w_e.shape == (C, R) and b_r.numel() == R
+    de, dmean = (torch.empty((N, C), dtype=torch.float32, device=gate.device) for _ in range(2))
+    sr, dr = (torch.empty((N, R), dtype=torch.float32, device=gate.device) for _ in range(2))
+    with torch.cuda.device(gate.device):
+        code = _lib.lib().stp3_se_bwd(dgate.data_ptr(), gate.data_ptr(), sums.data_ptr(), N, C, 1.0 / hw,
+                                      w_r.data_ptr(), b_r.data_ptr(), R, w_e.data_ptr(), de.data_ptr(), sr.data_ptr(),
+                                      dr.data_ptr(), dmean.data_ptr(), _stream(gate.device))
+    _lib.check(code, "stp3_se_bwd")
+    return de, sr, dr, dmean

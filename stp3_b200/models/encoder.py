@@ -9,9 +9,11 @@ The heads -- DeepLabHead + UpsamplingConcat -- run on the wgmma kernels.  With t
 heads as hi/lo planes: block 9 writes reduction_3 straight into the heads' concat tensor.
 
 The heads also run in train mode (batch statistics, dropout, autograd; DeepLabHead.forward and
-UpsamplingConcat.forward on fp32 endpoints).  The native trunk is eval-only: with it the endpoints are computed under
-no_grad and train_heads() gives the frozen-trunk fine-tune; an injected torch trunk follows nn.Module.train() and
-receives the gradients of both endpoints through torch autograd."""
+UpsamplingConcat.forward on fp32 endpoints).  The default native trunk is eval-only: with it the endpoints are computed
+under no_grad and train_heads() gives the frozen-trunk fine-tune.  A native trunk built with
+EfficientNetTrunk(version, trainable=True) follows nn.Module.train(): in train mode its endpoints leave the trunk as fp32
+tensors with a grad_fn (channels-last memory, NCHW views) and receive the gradients of both heads.  An injected torch
+trunk follows nn.Module.train() and receives the gradients of both endpoints through torch autograd."""
 import math
 
 import torch
@@ -72,8 +74,8 @@ class Encoder(nn.Module):
         return modes.pop()
 
     def train_heads(self, mode: bool = True):
-        """Sets the four head modules' mode and leaves the trunk alone (the native trunk is eval-only):
-        model.eval(); model.encoder.train_heads() is the frozen-trunk recipe.  Returns self."""
+        """Sets the four head modules' mode and leaves the trunk alone: model.eval(); model.encoder.train_heads() is the
+        frozen-trunk recipe, for the default (eval-only) native trunk and a trainable one alike.  Returns self."""
         for m in self._head_modules():
             m.train(mode)
         return self
@@ -115,12 +117,22 @@ class Encoder(nn.Module):
     def native(self) -> bool:
         return isinstance(self.backbone, EfficientNetTrunk)
 
+    def trunk_training(self) -> bool:
+        """True when the native trunk is in train mode (a trunk built with trainable=True, after train())."""
+        return self.native and self.backbone.training
+
     def features_native(self, x: torch.Tensor, channels_last: bool = False):
         """(M,3,H,W) fp32 images -> heads_f32's outputs through the native trunk, hi/lo from the stem to the heads."""
         if self.heads_training():
-            with torch.no_grad():                 # the native trunk is frozen: fp32 endpoints, no graph behind them
-                r_lo, r_hi = self.backbone(x)
+            if self.trunk_training():
+                r_lo, r_hi = self.backbone(x)     # fp32 endpoints with a grad_fn: the trunk trains too
+            else:
+                with torch.no_grad():             # the native trunk is frozen: fp32 endpoints, no graph behind them
+                    r_lo, r_hi = self.backbone(x)
             return self.heads_train(r_lo, r_hi, channels_last)
+        if self.trunk_training():
+            raise RuntimeError("Encoder: the native trunk is in train mode but the heads are in eval mode, so no "
+                               "gradient could reach it -- call encoder.train_heads() as well, or backbone.eval()")
         M, _, H, W = x.shape
         ds = self.downsample
         index = int(math.log2(ds))

@@ -243,8 +243,13 @@ class STP3(nn.Module):
 
     def _check_encoder_train(self):
         """Train-mode encoder heads need a train-mode path behind them: only the train-mode TemporalBlocks take the
-        lift-splat through autograd, and the head and the decoder carry the gradient to them."""
+        lift-splat through autograd, and the head and the decoder carry the gradient to them.  A train-mode native
+        trunk needs train-mode heads behind it for the same reason."""
         if not self.encoder.heads_training():
+            if self.encoder.trunk_training():
+                raise RuntimeError("STP3: the native trunk is in train mode but the encoder heads are in eval mode, so "
+                                   "no gradient could reach it -- call model.encoder.train_heads() as well, or "
+                                   "model.encoder.backbone.eval()")
             return
         if not isinstance(self.temporal_model, TemporalModel):
             raise RuntimeError("STP3: the encoder heads are in train mode, which needs the temporal_block model (the "
@@ -271,6 +276,9 @@ class STP3(nn.Module):
         if self.encoder.heads_training():
             raise RuntimeError("frame-sharded forward: the encoder heads are in train mode; the sharded path runs the "
                                "inference forward only -- call model.encoder.train_heads(False)")
+        if self.encoder.trunk_training():
+            raise RuntimeError("frame-sharded forward: the native trunk is in train mode; the sharded path runs the "
+                               "inference forward only -- call model.encoder.backbone.eval()")
         h = {k: v.to(dev) for k, v in self.prepare_inputs(intrinsics, extrinsics, future_egomotion).items()}
         feat = feat[:, :S].contiguous()
         depth_logits = depth_logits[:, :S].contiguous() if depth_logits is not None else None
@@ -377,6 +385,10 @@ class GraphedPerception:
             raise RuntimeError("GraphedPerception: the encoder heads are in train mode (batch statistics, dropout, "
                                "autograd); a CUDA graph replays the inference forward only -- call "
                                "model.encoder.train_heads(False)")
+        if model.encoder.trunk_training():
+            raise RuntimeError("GraphedPerception: the native trunk is in train mode (batch statistics, drop-connect, "
+                               "autograd); a CUDA graph replays the inference forward only -- call "
+                               "model.encoder.backbone.eval()")
         self.model = model
         self.entry = entry
         dev = torch.device(device) if device is not None else next(model.parameters()).device
