@@ -666,6 +666,57 @@ int stp3_se_bwd(const float* dgate, const float* gate, const float* sums, int n_
 int stp3_bev_discount(const float* raw /*(B,S,nx,ny,C) fp32*/, int B, int S, int nx, int ny, int C, float discount,
                       void* out_hi, void* out_lo /*(B,S,nx,ny,C) bf16 each*/, void* stream);
 
+
+/* ---------------------------------------------------------------------------------------------------------
+ * Prediction stage (eval mode, N_FUTURE_FRAMES > 0): the per-pixel kernels between the stage's convolutions
+ *   DistributionModule / Bottleneck(downsample)   stp3/models/distributions.py, stp3/layers/convolutions.py:65-170
+ *   Dual_GRU, SpatialGRU                          stp3/layers/temporal.py:11-160
+ *   LayerNorm, Block (ConvNeXt), Bottleblock      stp3/layers/convolutions.py:283-380
+ *
+ * stp3_hl_slot: a channel slot of a channels-last bf16 hi/lo activation (B, t_total, H, W, cstride) -- channels
+ * [coff, coff + C) of frames [t0, t0 + T) of every sample, where a call processes B samples of T frames.  cstride and
+ * coff are multiples of 8 and both planes 16-byte aligned.  Each call reads and writes only its slots; channels outside
+ * them are untouched.  Every result is a fixed-order fp32 function of its inputs (no atomics): repeated launches are
+ * bitwise equal. */
+typedef struct {
+  void* hi;
+  void* lo;
+  int cstride, coff;
+  int t_total, t0;
+} stp3_hl_slot;
+
+/* out = (1 - sigmoid(r)) * h: the reset-gated state of a conv-GRU proposal (r is the raw reset-gate convolution) */
+int stp3_gru_gates(const stp3_hl_slot* r, const stp3_hl_slot* h, const stp3_hl_slot* out, int B, int T, long long HW,
+                   int C, void* stream);
+/* out [and out2 when not NULL] = (1 - s) * h + s * h_tilde, s = sigmoid(u) (u the raw update-gate convolution); out
+ * may be the slot of h itself */
+int stp3_gru_update(const stp3_hl_slot* u, const stp3_hl_slot* h, const stp3_hl_slot* h_tilde, const stp3_hl_slot* out,
+                    const stp3_hl_slot* out2, int B, int T, long long HW, int C, void* stream);
+/* out = act(LN(x)) + act_y(y), per pixel over its C <= 256 channels: LN with gamma / beta (C) fp32 and eps, biased
+ * variance (skipped when gamma and beta are NULL); act = exact GELU when gelu != 0; y optional (NULL: nothing added),
+ * act_y = exact GELU when gelu_y != 0.  out may be the slot of x. */
+int stp3_channel_norm_act(const stp3_hl_slot* x, const float* gamma, const float* beta, float eps, int gelu,
+                          const stp3_hl_slot* y, int gelu_y, const stp3_hl_slot* out, int B, int T, long long HW, int C,
+                          void* stream);
+/* out = LN(depthwise k x k convolution of x (zero padding k/2, stride 1) + bias): w (k*k, C) fp32 tap-major, 16-byte
+ * aligned, bias / gamma / beta (C) fp32, C <= 256; out's planes must not overlap x's (not even in other channels or
+ * frames of the same buffer: the call refuses any overlap of the two slots' address spans) */
+int stp3_dw_ln(const stp3_hl_slot* x, const float* w, const float* bias, int k, const float* gamma, const float* beta,
+               float eps, const stp3_hl_slot* out, int B, int T, int H, int W, int C, void* stream);
+/* The trusting gate's tail (temporal.py:110-115): z = w t (w (2, C) fp32, C <= 256), p = softmax(z),
+ * mix = s2 * p0 + s1 * p1, written to each of the n_dst (1..4) slots of dst (a host array) */
+int stp3_trust_mix(const stp3_hl_slot* t, const float* w, const stp3_hl_slot* s1, const stp3_hl_slot* s2,
+                   const stp3_hl_slot* dst, int n_dst, int B, int T, long long HW, int C, void* stream);
+/* out (ceil(H/2), ceil(W/2)) = MaxPool2d(2, 2) of x after an odd H / W was zero-padded by one row / column at the
+ * bottom / right (convolutions.py:160-164: the padded zeros take part in the max); the winning hi / lo bits are
+ * stored unchanged */
+int stp3_maxpool2_pad(const stp3_hl_slot* x, const stp3_hl_slot* out, int B, int T, int H, int W, int C, void* stream);
+/* dst = src (C channels of every pixel, both planes bit for bit) */
+int stp3_hl_copy(const stp3_hl_slot* src, const stp3_hl_slot* dst, int B, int T, long long HW, int C, void* stream);
+/* dst[img, pixel, c] = vec[img * vstride + c] (img = b * T + t): a per-image vector broadcast over H x W */
+int stp3_hl_broadcast(const float* vec, int vstride, const stp3_hl_slot* dst, int B, int T, long long HW, int C,
+                      void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -87,6 +87,13 @@ class ConvHead(ctypes.Structure):
                 ("sigmoid_mask", _I)]
 
 
+class HlSlot(ctypes.Structure):
+    """Mirror of stp3_hl_slot (include/stp3_b200.h)."""
+    _fields_ = [("hi", _V), ("lo", _V), ("cstride", _I), ("coff", _I), ("t_total", _I), ("t0", _I)]
+
+
+_HS = ctypes.POINTER(HlSlot)
+
 SIGNATURES = {
     "stp3_abi_version": (_I, []),
     "stp3_conv_col_sums_scratch_bytes": (_SZ, [_I, _I]),
@@ -167,6 +174,15 @@ SIGNATURES = {
     "stp3_image_channel_dot_scratch_bytes": (_SZ, [_I, _LL, _I]),
     "stp3_image_channel_dot": (_I, [_V, _V, _I, _LL, _I, _V, _V, _SZ, _V]),
     "stp3_se_bwd": (_I, [_V, _V, _V, _I, _I, _F, _V, _V, _I, _V, _V, _V, _V, _V, _V]),
+    # eval-mode prediction stage
+    "stp3_gru_gates": (_I, [_HS, _HS, _HS, _I, _I, _LL, _I, _V]),
+    "stp3_gru_update": (_I, [_HS, _HS, _HS, _HS, _HS, _I, _I, _LL, _I, _V]),
+    "stp3_channel_norm_act": (_I, [_HS, _V, _V, _F, _I, _HS, _I, _HS, _I, _I, _LL, _I, _V]),
+    "stp3_dw_ln": (_I, [_HS, _V, _V, _I, _V, _V, _F, _HS, _I, _I, _I, _I, _I, _V]),
+    "stp3_trust_mix": (_I, [_HS, _V, _HS, _HS, _HS, _I, _I, _I, _LL, _I, _V]),
+    "stp3_maxpool2_pad": (_I, [_HS, _HS, _I, _I, _I, _I, _I, _V]),
+    "stp3_hl_copy": (_I, [_HS, _HS, _I, _I, _LL, _I, _V]),
+    "stp3_hl_broadcast": (_I, [_V, _I, _HS, _I, _I, _LL, _I, _V]),
 }
 
 

@@ -66,6 +66,17 @@ PERCEPTION_OVERRIDES = {
     "PROBABILISTIC": {"ENABLED": False}, "PLANNING": {"ENABLED": False},
 }
 
+# stp3/configs/nuscenes/Prediction.yml (apply with get_cfg(PREDICTION_OVERRIDES, perception=False))
+PREDICTION_OVERRIDES = {
+    "TIME_RECEPTIVE_FIELD": 3, "N_FUTURE_FRAMES": 4,
+    "LIFT": {"GT_DEPTH": False},
+    "MODEL": {"ENCODER": {"NAME": 'efficientnet-b4', "USE_DEPTH_DISTRIBUTION": True},
+              "TEMPORAL_MODEL": {"NAME": 'temporal_block', "INPUT_EGOPOSE": True}, "BN_MOMENTUM": 0.05},
+    "SEMANTIC_SEG": {"PEDESTRIAN": {"ENABLED": False}, "HDMAP": {"ENABLED": False}},
+    "INSTANCE_FLOW": {"ENABLED": True},
+    "PROBABILISTIC": {"ENABLED": True, "METHOD": 'GAUSSIAN'}, "PLANNING": {"ENABLED": False},
+}
+
 
 def get_cfg(overrides=None, perception=True):
     """Reference defaults (+ the nuScenes perception YAML when perception=True) + overrides."""

@@ -683,3 +683,117 @@ def se_gate(sums: torch.Tensor, hw: int, C: int, w_r, b_r, w_e, b_e, w_proj: tor
                                        _stream(sums.device))
     _lib.check(code, "stp3_se_gate")
     return w_img
+
+
+# ------------------------------------------------------------------------------------------------ prediction stage
+# A slot is (HL, first channel, first frame): the channels [coff, coff + C) of frames [t0, t0 + T) of every sample of
+# an HL buffer, where the call processes T frames of each of the buffer's B samples (stp3_hl_slot).
+def _slot(v, C: int, T: int, bhw: Tuple[int, int, int]) -> "_lib.HlSlot":
+    """The stp3_hl_slot of v for a call over B samples of T frames of H x W pixels (bhw = (B, H, W)): the kernels index
+    every slot of a call with those dimensions, so each buffer must have them."""
+    x, coff, t0 = (v + (0, 0))[:3] if isinstance(v, tuple) else (v, 0, 0)
+    assert x.lo is not None and x.hi.is_contiguous() and x.lo.is_contiguous() and x.hi.dtype == torch.bfloat16
+    assert x.lo.shape == x.hi.shape and x.lo.dtype == torch.bfloat16
+    assert (x.hi.shape[0],) + tuple(x.hi.shape[2:4]) == tuple(bhw), (x.hi.shape, bhw)
+    assert coff + C <= x.hi.shape[-1] and t0 + T <= x.hi.shape[1], (coff, C, x.hi.shape, t0, T)
+    return _lib.HlSlot(x.hi.data_ptr(), x.lo.data_ptr(), x.hi.shape[-1], coff, x.hi.shape[1], t0)
+
+
+def _dims(v, T: Optional[int]):
+    x, t0 = (v[0], (v + (0, 0))[2]) if isinstance(v, tuple) else (v, 0)
+    B, Tt, H, W, _ = x.hi.shape
+    return B, (T if T is not None else Tt - t0), H, W, x.hi.device
+
+
+def gru_gates(r, h, out, C: int, T: Optional[int] = None):
+    """out = (1 - sigmoid(r)) * h over C channels (stp3_gru_gates); r, h, out are HLs or slots (HL, coff[, t0])."""
+    B, T, H, W, dev = _dims(r, T)
+    bhw = (B, H, W)
+    with torch.cuda.device(dev):
+        code = _lib.lib().stp3_gru_gates(_slot(r, C, T, bhw), _slot(h, C, T, bhw), _slot(out, C, T, bhw), B, T, H * W,
+                                         C, _stream(dev))
+    _lib.check(code, "stp3_gru_gates")
+
+
+def gru_update(u, h, h_tilde, out, C: int, out2=None, T: Optional[int] = None):
+    """out [, out2] = (1 - s) * h + s * h_tilde, s = sigmoid(u) (stp3_gru_update)."""
+    B, T, H, W, dev = _dims(u, T)
+    bhw = (B, H, W)
+    o2 = ctypes.byref(_slot(out2, C, T, bhw)) if out2 is not None else None
+    with torch.cuda.device(dev):
+        code = _lib.lib().stp3_gru_update(_slot(u, C, T, bhw), _slot(h, C, T, bhw), _slot(h_tilde, C, T, bhw),
+                                          _slot(out, C, T, bhw), o2, B, T, H * W, C, _stream(dev))
+    _lib.check(code, "stp3_gru_update")
+
+
+def channel_norm_act(x, out, C: int, ln: Optional[Tuple[torch.Tensor, torch.Tensor, float]] = None, gelu: bool = False,
+                     y=None, gelu_y: bool = False, T: Optional[int] = None):
+    """out = [gelu]([LN](x)) + [gelu](y) per pixel over C channels; ln = (gamma, beta, eps) (stp3_channel_norm_act)."""
+    B, T, H, W, dev = _dims(x, T)
+    bhw = (B, H, W)
+    g, b, eps = ln if ln is not None else (None, None, 0.0)
+    ys = ctypes.byref(_slot(y, C, T, bhw)) if y is not None else None
+    with torch.cuda.device(dev):
+        code = _lib.lib().stp3_channel_norm_act(_slot(x, C, T, bhw), g.data_ptr() if g is not None else None,
+                                                b.data_ptr() if b is not None else None, eps, int(gelu), ys,
+                                                int(gelu_y), _slot(out, C, T, bhw), B, T, H * W, C, _stream(dev))
+    _lib.check(code, "stp3_channel_norm_act")
+
+
+def dw_ln(x, w: torch.Tensor, b: torch.Tensor, k: int, ln: Tuple[torch.Tensor, torch.Tensor, float], out, C: int,
+          T: Optional[int] = None):
+    """out = LN(depthwise k x k (x) + b), w (k*k, C) fp32 (stp3_dw_ln)."""
+    B, T, H, W, dev = _dims(x, T)
+    bhw = (B, H, W)
+    g, beta, eps = ln
+    for t in (w, b, g, beta):
+        assert t.dtype == torch.float32 and t.is_contiguous() and t.is_cuda
+    assert w.shape == (k * k, C) and b.numel() == C
+    with torch.cuda.device(dev):
+        code = _lib.lib().stp3_dw_ln(_slot(x, C, T, bhw), w.data_ptr(), b.data_ptr(), k, g.data_ptr(), beta.data_ptr(),
+                                     eps, _slot(out, C, T, bhw), B, T, H, W, C, _stream(dev))
+    _lib.check(code, "stp3_dw_ln")
+
+
+def trust_mix(t, w: torch.Tensor, s1, s2, dsts, C: int, T: Optional[int] = None):
+    """p = softmax(w t), every slot of dsts = s2 * p0 + s1 * p1 (stp3_trust_mix); w (2, C) fp32."""
+    B, T, H, W, dev = _dims(t, T)
+    bhw = (B, H, W)
+    assert w.shape == (2, C) and w.dtype == torch.float32 and w.is_contiguous()
+    arr = (_lib.HlSlot * len(dsts))(*[_slot(d, C, T, bhw) for d in dsts])
+    with torch.cuda.device(dev):
+        code = _lib.lib().stp3_trust_mix(_slot(t, C, T, bhw), w.data_ptr(), _slot(s1, C, T, bhw), _slot(s2, C, T, bhw),
+                                         arr, len(dsts), B, T, H * W, C, _stream(dev))
+    _lib.check(code, "stp3_trust_mix")
+
+
+def maxpool2_pad(x: HL, out: Optional[HL] = None) -> HL:
+    """2x2 max pool of every channel after zero-padding an odd H / W by one (stp3_maxpool2_pad)."""
+    B, T, H, W, cs = x.hi.shape
+    if out is None:
+        out = HL.empty(B, T, (H + 1) // 2, (W + 1) // 2, x.c, x.hi.device, cp=cs)
+    assert out.hi.shape[:4] == (B, T, (H + 1) // 2, (W + 1) // 2)
+    o = _slot(out, cs, T, (B, (H + 1) // 2, (W + 1) // 2))
+    with torch.cuda.device(x.hi.device):
+        code = _lib.lib().stp3_maxpool2_pad(_slot(x, cs, T, (B, H, W)), o, B, T, H, W, cs, _stream(x.hi.device))
+    _lib.check(code, "stp3_maxpool2_pad")
+    return out
+
+
+def hl_copy(src, dst, C: int, T: Optional[int] = None):
+    """dst = src over C channels (stp3_hl_copy)."""
+    B, T, H, W, dev = _dims(src, T)
+    bhw = (B, H, W)
+    with torch.cuda.device(dev):
+        code = _lib.lib().stp3_hl_copy(_slot(src, C, T, bhw), _slot(dst, C, T, bhw), B, T, H * W, C, _stream(dev))
+    _lib.check(code, "stp3_hl_copy")
+
+
+def hl_broadcast(vec: torch.Tensor, dst, C: int, T: Optional[int] = None):
+    """dst[img, pixel, :C] = vec[img, :C] with vec (B*T, >= C) fp32 (stp3_hl_broadcast)."""
+    B, T, H, W, dev = _dims(dst, T)
+    bhw = (B, H, W)
+    assert vec.dtype == torch.float32 and vec.is_contiguous() and vec.shape[0] == B * T and vec.shape[1] >= C
+    with torch.cuda.device(dev):
+        code = _lib.lib().stp3_hl_broadcast(vec.data_ptr(), vec.shape[1], _slot(dst, C, T, bhw), B, T, H * W, C, _stream(dev))
+    _lib.check(code, "stp3_hl_broadcast")

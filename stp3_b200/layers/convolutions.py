@@ -8,8 +8,10 @@
                    runs in train() (batch statistics, dropout, autograd; dense_train.py).
   UpsamplingConcat : bilinear x2 of the coarse map into its channel window of the concat tensor, two 3x3 conv/BN/ReLU;
                    also in train().
+  Bottleneck / LayerNorm / Block / Bottleblock : the prediction stage's blocks, eval only (DESIGN.md §3.16).
 """
 import os
+from collections import OrderedDict
 from typing import Optional
 
 import torch
@@ -485,3 +487,203 @@ class _UpsamplingConcatTrainFn(torch.autograd.Function):
         g_up, g_x, grads = ctx.mod._train_backward(tape, g_out, ctx.channels_last, ctx.needs_input_grad[1],
                                                    ctx.needs_input_grad[2])
         return (None, g_up, g_x, None) + tuple(grads.get(p) for p in ctx.params)
+
+
+# ------------------------------------------------------------------------------------------------ prediction stage
+# Eval-only modules of the future-prediction stage (convolutions.py:65-170, 283-380).  Their convolutions run on
+# stp3_conv_fwd; LayerNorm, GELU, the depthwise 7x7 and the skip's max pool on the per-pixel kernels of
+# predict_kernels.cu.
+PREDICT_EVAL_ONLY = ("the prediction stage (N_FUTURE_FRAMES > 0) is eval-only on sm_90a: its gradients, the train-time "
+                     "noise and the probabilistic loss are not implemented -- call .eval()")
+
+
+class PredictModule(PackedModule):
+    def _require_eval(self):
+        if any(m.training for m in self.modules()):
+            raise NotImplementedError(f"{type(self).__name__}: {PREDICT_EVAL_ONLY}")
+
+    def forward(self, x):
+        """x (N, C, H, W) fp32 on the device -> (N, C_out, H, W') fp32 through forward_hl."""
+        y = self.forward_hl(dense.from_f32(x.unsqueeze(1)))
+        return dense.to_f32(y).squeeze(1)
+
+
+def _ln_params(ln):
+    return (ln.weight.detach().float().contiguous(), ln.bias.detach().float().contiguous(), float(ln.eps))
+
+
+class LayerNorm(nn.Module):
+    """The reference's LayerNorm (convolutions.py:283-306): parameters `weight` / `bias` over C channels, eps 1e-6,
+    biased variance.  Both data formats normalise each pixel's channel vector, which is what stp3_channel_norm_act and
+    stp3_dw_ln compute; inside Block and Bottleblock the parent runs it fused with its neighbours.  Called on its own it
+    runs stp3_channel_norm_act, eval only, for C <= 256 channels (a multiple of 8)."""
+
+    def __init__(self, normalized_shape, eps=1e-6, data_format="channels_last"):
+        super().__init__()
+        self.weight = nn.Parameter(torch.ones(normalized_shape))
+        self.bias = nn.Parameter(torch.zeros(normalized_shape))
+        self.eps = eps
+        self.data_format = data_format
+        if self.data_format not in ["channels_last", "channels_first"]:
+            raise NotImplementedError
+        self.normalized_shape = (normalized_shape,)
+
+    def forward(self, x):
+        """channels_first: x (N, C, H, W); channels_last: x (..., C); fp32 on the device, same shape out."""
+        if self.training:
+            raise NotImplementedError(f"LayerNorm: {PREDICT_EVAL_ONLY}")
+        C = self.normalized_shape[0]
+        if C % 8 != 0 or C > 256:
+            raise NotImplementedError(f"LayerNorm over {C} channels: stp3_channel_norm_act takes a multiple of 8, at "
+                                      "most 256")
+        if self.data_format == "channels_last":                     # one image of numel / C pixels
+            h = dense.from_f32(x.reshape(1, 1, -1, 1, C), channels_last=True)
+            dense.channel_norm_act(h, h, C, ln=_ln_params(self))
+            return dense.to_f32(h, 0, C)[0, 0, :, :, 0].t().reshape(x.shape)
+        h = dense.from_f32(x.reshape(1, -1, C, *x.shape[-2:]))      # N images
+        dense.channel_norm_act(h, h, C, ln=_ln_params(self))
+        return dense.to_f32(h, 0, C).reshape(x.shape)
+
+
+class Bottleneck(PredictModule):
+    """The reference's Bottleneck (convolutions.py:65-170) with downsample=True, the only form the Gaussian present
+    distribution builds: 1x1 -> BN -> ReLU -> 3x3 s2 -> BN -> ReLU -> 1x1 -> BN -> ReLU, plus the skip (zero-pad an odd
+    H / W, MaxPool 2x2, 1x1 -> BN).  The skip is the up-projection's residual, added after its ReLU."""
+
+    def __init__(self, in_channels, out_channels=None, kernel_size=3, dilation=1, groups=1, upsample=False,
+                 downsample=False, dropout=0.0):
+        super().__init__()
+        if not downsample or upsample or kernel_size != 3 or dilation != 1 or groups != 1:
+            raise NotImplementedError("Bottleneck: only the downsampling 3x3 form (the present distribution's) is built")
+        self._downsample = downsample
+        bottleneck_channels = int(in_channels / 2)
+        out_channels = out_channels or in_channels
+        self.in_channels, self.out_channels = in_channels, out_channels
+        self.layers = nn.Sequential(OrderedDict([
+            ('conv_down_project', nn.Conv2d(in_channels, bottleneck_channels, kernel_size=1, bias=False)),
+            ('abn_down_project', nn.Sequential(nn.BatchNorm2d(bottleneck_channels), nn.ReLU(inplace=True))),
+            ('conv', nn.Conv2d(bottleneck_channels, bottleneck_channels, kernel_size=3, bias=False, stride=2, padding=1)),
+            ('abn', nn.Sequential(nn.BatchNorm2d(bottleneck_channels), nn.ReLU(inplace=True))),
+            ('conv_up_project', nn.Conv2d(bottleneck_channels, out_channels, kernel_size=1, bias=False)),
+            ('abn_up_project', nn.Sequential(nn.BatchNorm2d(out_channels), nn.ReLU(inplace=True))),
+            ('dropout', nn.Dropout2d(p=dropout)),
+        ]))
+        self.projection = nn.Sequential(OrderedDict([
+            ('upsample_skip_proj', nn.MaxPool2d(kernel_size=2, stride=2)),
+            ('conv_skip_proj', nn.Conv2d(in_channels, out_channels, kernel_size=1, bias=False)),
+            ('bn_skip_proj', nn.BatchNorm2d(out_channels)),
+        ]))
+
+    def _pack(self):
+        L = self.layers
+        P = {}
+        for key, conv, bn in (("down", L.conv_down_project, L.abn_down_project[0]), ("conv", L.conv, L.abn[0]),
+                              ("up", L.conv_up_project, L.abn_up_project[0]),
+                              ("skip", self.projection.conv_skip_proj, self.projection.bn_skip_proj)):
+            w, b = dense.fold_bn(conv.weight, bn)
+            P[key] = dense.pack_conv(w, b, stride=conv.stride[0])
+        return P
+
+    def forward_hl(self, x: dense.HL) -> dense.HL:
+        """x: HL (B, T, H, W, >= in_channels) -> HL (B, T, ceil(H/2), ceil(W/2), 64-padded out_channels)."""
+        self._require_eval()
+        P = self.packed()
+        a = dense.conv(x, P["down"], relu=True)
+        a = dense.conv(a, P["conv"], relu=True)
+        skip = dense.conv(dense.maxpool2_pad(x), P["skip"])
+        return dense.conv(a, P["up"], relu=True, residual=skip, res_after_act=True)
+
+
+class Block(PredictModule):
+    """ConvNeXt Block (convolutions.py:308-345): depthwise 7x7 + bias -> LayerNorm -> Linear(C, 4C) -> GELU ->
+    Linear(4C, C) -> * gamma -> + input.  gamma folds into pwconv2's weight and bias; the input is the residual of that
+    convolution."""
+
+    def __init__(self, dim, drop_path=0., layer_scale_init_value=1e-6):
+        super().__init__()
+        if drop_path > 0.:
+            raise NotImplementedError("Block: drop_path > 0 is a training regulariser (no reference config uses it)")
+        self.dwconv = nn.Conv2d(dim, dim, kernel_size=7, padding=3, groups=dim)
+        self.norm = LayerNorm(dim, eps=1e-6)
+        self.pwconv1 = nn.Linear(dim, 4 * dim)
+        self.act = nn.GELU()
+        self.pwconv2 = nn.Linear(4 * dim, dim)
+        self.gamma = nn.Parameter(layer_scale_init_value * torch.ones((dim)),
+                                  requires_grad=True) if layer_scale_init_value > 0 else None
+        self.drop_path = nn.Identity()
+        self.dim = dim
+
+    def _pack(self):
+        C = self.dim
+        g = self.gamma.detach().float() if self.gamma is not None else torch.ones(C, device=self.pwconv2.weight.device)
+        w2 = self.pwconv2.weight.detach().float() * g[:, None]
+        b2 = self.pwconv2.bias.detach().float() * g
+        return {"dw_w": self.dwconv.weight.detach().float().reshape(C, 49).t().contiguous(),
+                "dw_b": self.dwconv.bias.detach().float().contiguous(), "ln": _ln_params(self.norm),
+                "pw1": dense.pack_conv(self.pwconv1.weight.detach().float().view(4 * C, C, 1, 1),
+                                       self.pwconv1.bias.detach().float()),
+                "pw2": dense.pack_conv(w2.view(C, 4 * C, 1, 1), b2)}
+
+    def forward_hl(self, x: dense.HL) -> dense.HL:
+        """x: HL (B, T, H, W, >= dim) -> HL (B, T, H, W, 64-padded dim)."""
+        self._require_eval()
+        P = self.packed()
+        B, T, H, W, _ = x.hi.shape
+        C = self.dim
+        t = (dense.HL.empty if C % dense.KB == 0 else dense.HL.zeros)(B, T, H, W, C, x.hi.device)   # padding feeds pw1
+        dense.dw_ln(x, P["dw_w"], P["dw_b"], 7, P["ln"], t, C)
+        y = dense.conv(t, P["pw1"])
+        dense.channel_norm_act(y, y, 4 * C, gelu=True)
+        return dense.conv(y, P["pw2"], residual=x)
+
+
+class Bottleblock(PredictModule):
+    """The trusting gate's block (convolutions.py:347-380): 7x7 -> LN -> GELU -> 1x1 -> LN -> GELU -> 3x3 -> LN -> GELU
+    (channels-first LayerNorms, no conv bias), plus GELU(1x1(x)) when the channel count changes (else x)."""
+
+    def __init__(self, in_channels, out_channels=None):
+        super().__init__()
+        bottleneck_channels = int(in_channels / 2)
+        out_channels = out_channels or in_channels
+        self.in_channels, self.out_channels, self.mid = in_channels, out_channels, bottleneck_channels
+        self.layers = nn.Sequential(
+            nn.Conv2d(in_channels, bottleneck_channels, kernel_size=7, bias=False, padding=3),
+            LayerNorm(bottleneck_channels, eps=1e-6, data_format='channels_first'),
+            nn.GELU(),
+            nn.Conv2d(bottleneck_channels, bottleneck_channels, kernel_size=1, bias=False),
+            LayerNorm(bottleneck_channels, eps=1e-6, data_format='channels_first'),
+            nn.GELU(),
+            nn.Conv2d(bottleneck_channels, out_channels, kernel_size=3, bias=False, padding=1),
+            LayerNorm(out_channels, eps=1e-6, data_format='channels_first'),
+            nn.GELU()
+        )
+        if out_channels == in_channels:
+            self.projection = None
+        else:
+            self.projection = nn.Sequential(nn.Conv2d(in_channels, out_channels, kernel_size=1, bias=False), nn.GELU())
+
+    def _pack(self):
+        L = self.layers
+        z = lambda c: torch.zeros(c.out_channels, device=c.weight.device)
+        P = {f"c{i}": dense.pack_conv(L[i].weight.detach().float(), z(L[i])) for i in (0, 3, 6)}
+        P.update({f"ln{i}": _ln_params(L[i]) for i in (1, 4, 7)})
+        if self.projection is not None:
+            P["proj"] = dense.pack_conv(self.projection[0].weight.detach().float(), z(self.projection[0]))
+        return P
+
+    def forward_hl(self, x: dense.HL) -> dense.HL:
+        """x: HL (B, T, H, W, >= in_channels) -> HL (B, T, H, W, 64-padded out_channels)."""
+        self._require_eval()
+        P = self.packed()
+        m, co = self.mid, self.out_channels
+        a = dense.conv(x, P["c0"])
+        dense.channel_norm_act(a, a, m, ln=P["ln1"], gelu=True)
+        a = dense.conv(a, P["c3"])
+        dense.channel_norm_act(a, a, m, ln=P["ln4"], gelu=True)
+        a = dense.conv(a, P["c6"])
+        if self.projection is not None:
+            y, gelu_y = dense.conv(x, P["proj"]), True
+        else:
+            y, gelu_y = x, False
+        dense.channel_norm_act(a, a, co, ln=P["ln7"], gelu=True, y=y, gelu_y=gelu_y)
+        return a

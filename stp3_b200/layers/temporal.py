@@ -10,6 +10,8 @@ TemporalBlock data flow on the device (channels-last hi/lo planes, o = half roun
 Spatially constant input channels (the broadcast ego-motion of stp3.py:145-152) are never materialised: they enter
 every 1x1x1 convolution that reads x as a per-image bias.
 
+SpatialGRU and Dual_GRU (bottom of the file) are the eval-only conv-GRUs of the prediction stage (DESIGN.md §3.16).
+
 Train mode (batch statistics, autograd) runs only inside TemporalModel, which wraps the whole block stack in one
 autograd node (temporal_model._TemporalBlocksTrainFn) built on _train_forward / _train_backward below; a block called
 on its own keeps refusing train().
@@ -23,6 +25,7 @@ import torch.nn as nn
 
 from .. import dense, dense_train
 from ._packing import PackedModule
+from .convolutions import Bottleblock, PredictModule
 
 
 def conv_1x1x1_norm_activated(in_channels, out_channels):
@@ -515,3 +518,163 @@ class TemporalBlock(PackedModule):
         assert self.n_const == 0
         y = self.forward_hl(dense.from_f32(x.permute(0, 2, 1, 3, 4)))
         return dense.to_f32(y, 0, self.out_channels).permute(0, 2, 1, 3, 4)
+
+
+# ------------------------------------------------------------------------------------------------ prediction stage
+def _gru_pack(conv_update, conv_reset, conv_tilde, input_size, hidden_size):
+    """The two convolutions of a conv-GRU cell over one buffer [h | x | (1 - r) * h] (64-channel slots; x at 64): the
+    update and reset gates as one 128-column convolution of channels [0, 128), the proposal as a convolution of
+    channels [64, 192).  The reference concatenates (x, h) in that order; in_layout maps its input channels."""
+    g_w = torch.cat([conv_update.weight, conv_reset.weight]).detach().float()
+    g_b = torch.cat([conv_update.bias, conv_reset.bias]).detach().float()
+    gate = dense.pack_conv(g_w, g_b, in_layout=[(0, input_size, 64), (input_size, hidden_size, 0)], cin_p=128)
+    prop = dense.pack_conv(conv_tilde.weight.detach().float(), conv_tilde.bias.detach().float(),
+                           in_layout=[(0, input_size, 0), (input_size, hidden_size, 64)], cin_p=128)
+    return gate, prop
+
+
+def _gru_step(buf: dense.HL, gate: dense.PackedConv, prop: dense.PackedConv, out2=None):
+    """One conv-GRU cell on buf = [h | x | scratch]: buf's h slot becomes (1 - u) * h + u * h_tilde (and out2 too).
+    The gates leave the convolution raw and the two per-pixel kernels apply the sigmoids: stp3_conv_fwd's sigmoid
+    exists only for its NCHW fp32 output (the instance-center head; the channels-last fp32 output refuses it and the
+    hi/lo output has none), and the kernels that consume the gates read channels-last hi/lo."""
+    g = dense.conv(buf, gate)                                   # raw [update | reset] gates, (B, 1, H, W, 128)
+    dense.gru_gates((g, 64), buf, (buf, 128), 64)
+    h_tilde = dense.conv(buf, prop, cin_off=64)
+    dense.gru_update(g, buf, h_tilde, buf, 64, out2=out2)
+
+
+class _PredictGRU(PredictModule):
+    @staticmethod
+    def _check_sizes(input_size, hidden_size):
+        if hidden_size != 64 or input_size > 64:
+            raise NotImplementedError(f"conv-GRU with input {input_size} / hidden {hidden_size}: the sm_90a cell keeps "
+                                      "64-channel slots (the reference's configs use hidden 64, inputs 32 and 64)")
+
+
+class SpatialGRU(_PredictGRU):
+    """Convolutional GRU over a sequence (temporal.py:11-58), eval only: gates sigmoid(conv3x3([x, h])), proposal
+    conv3x3([x, (1 - r) * h]), h = (1 - u) * h + u * h_tilde, and a 1x1 conv_decoder (no bias) on every state."""
+
+    def __init__(self, input_size, hidden_size, gru_bias_init=0.0):
+        super().__init__()
+        if gru_bias_init != 0.0:
+            raise NotImplementedError("SpatialGRU: gru_bias_init != 0 is not used by the reference")
+        self._check_sizes(input_size, hidden_size)
+        self.input_size = input_size
+        self.hidden_size = hidden_size
+        self.gru_bias_init = gru_bias_init
+        self.conv_update = nn.Conv2d(input_size + hidden_size, hidden_size, kernel_size=3, bias=True, padding=1)
+        self.conv_reset = nn.Conv2d(input_size + hidden_size, hidden_size, kernel_size=3, bias=True, padding=1)
+        self.conv_state_tilde = nn.Conv2d(input_size + hidden_size, hidden_size, kernel_size=3, bias=True, padding=1)
+        self.conv_decoder = nn.Conv2d(hidden_size, input_size, kernel_size=1, bias=False)
+
+    def _pack(self):
+        gate, prop = _gru_pack(self.conv_update, self.conv_reset, self.conv_state_tilde, self.input_size,
+                               self.hidden_size)
+        w = self.conv_decoder.weight.detach().float()
+        return {"gate": gate, "prop": prop, "dec": dense.pack_conv(w, torch.zeros(w.shape[0], device=w.device))}
+
+    def forward_hl(self, frames, state) -> dense.HL:
+        """frames: the input sequence as a list of (HL, frame index) -- frame t of every sample is x_t; state:
+        (HL, frame index) of the initial hidden state.  Returns HL (B, len(frames), H, W, 64): conv_decoder of every
+        state."""
+        self._require_eval()
+        P = self.packed()
+        x0 = frames[0][0]
+        B, _, H, W, _ = x0.hi.shape
+        dev = x0.hi.device
+        n = len(frames)
+        buf = dense.HL.zeros(B, 1, H, W, 192, dev, cp=192)         # [h | x | (1 - r) * h]
+        states = dense.HL.empty(B, n, H, W, 64, dev, cp=64)
+        dense.hl_copy((state[0], 0, state[1]), buf, 64, T=1)
+        for t, (src, f) in enumerate(frames):
+            dense.hl_copy((src, 0, f), (buf, 64), self.input_size + (-self.input_size) % 8, T=1)
+            _gru_step(buf, P["gate"], P["prop"], out2=(states, 0, t))
+        return dense.conv(states, P["dec"])
+
+    def forward(self, x, state=None):
+        """x (B, T, C, H, W) fp32, state (B, hidden, H, W) fp32 (zeros when None) -> (B, T, input_size, H, W) fp32."""
+        B, T = x.shape[:2]
+        xs = dense.from_f32(x)
+        h = dense.from_f32((state if state is not None else x.new_zeros(B, self.hidden_size, *x.shape[3:])).unsqueeze(1))
+        y = self.forward_hl([(xs, t) for t in range(T)], (h, 0))
+        return dense.to_f32(y, 0, self.input_size)
+
+
+class Dual_GRU(_PredictGRU):
+    """The future recurrence of FuturePrediction (temporal.py:60-160), eval only with mixture=True.  gru_cell_2 warms up
+    over the present states; each future step runs gru_cell_1 (input: the latent sample) and gru_cell_2 ->
+    conv_decoder_2, and the trusting gate mixes the two states: p = softmax(conv1x1(Bottleblock([s1, s2]))),
+    mix = s2 * p0 + s1 * p1, which becomes both recurrences' state and the step's output."""
+
+    def __init__(self, in_channels, latent_dim, n_future, mixture=True, gru_bias_init=0.0):
+        super().__init__()
+        if gru_bias_init != 0.0:
+            raise NotImplementedError("Dual_GRU: gru_bias_init != 0 is not used by the reference")
+        input_size = in_channels
+        hidden_size = latent_dim
+        self._check_sizes(input_size, hidden_size)
+        self.n_future = n_future
+        self.mixture = mixture
+        self.input_size = input_size
+        self.hidden_size = hidden_size
+        self.gru_bias_init = gru_bias_init
+        self.conv_update_1 = nn.Conv2d(input_size + hidden_size, hidden_size, kernel_size=3, bias=True, padding=1)
+        self.conv_reset_1 = nn.Conv2d(input_size + hidden_size, hidden_size, kernel_size=3, bias=True, padding=1)
+        self.conv_state_tilde_1 = nn.Conv2d(input_size + hidden_size, hidden_size, kernel_size=3, bias=True, padding=1)
+        self.conv_update_2 = nn.Conv2d(hidden_size + hidden_size, hidden_size, kernel_size=3, bias=True, padding=1)
+        self.conv_reset_2 = nn.Conv2d(hidden_size + hidden_size, hidden_size, kernel_size=3, bias=True, padding=1)
+        self.conv_state_tilde_2 = nn.Conv2d(hidden_size + hidden_size, hidden_size, kernel_size=3, bias=True, padding=1)
+        self.conv_decoder_2 = nn.Conv2d(hidden_size, hidden_size, kernel_size=3, bias=True, padding=1)
+        self.trusting_gate = nn.Sequential(
+            Bottleblock(hidden_size + hidden_size, hidden_size),
+            nn.Conv2d(hidden_size, 2, kernel_size=1, bias=False)
+        )
+
+    def _pack(self):
+        P = {}
+        P["gate1"], P["prop1"] = _gru_pack(self.conv_update_1, self.conv_reset_1, self.conv_state_tilde_1,
+                                           self.input_size, self.hidden_size)
+        P["gate2"], P["prop2"] = _gru_pack(self.conv_update_2, self.conv_reset_2, self.conv_state_tilde_2,
+                                           self.hidden_size, self.hidden_size)
+        P["dec2"] = dense.pack_conv(self.conv_decoder_2.weight.detach().float(),
+                                    self.conv_decoder_2.bias.detach().float())
+        P["trust_w"] = self.trusting_gate[1].weight.detach().float().reshape(2, self.hidden_size).contiguous()
+        return P
+
+    def forward_hl(self, x: Optional[dense.HL], state: dense.HL, out: dense.HL, out_t0: int = 0):
+        """x: HL (B, 1, H, W, >= input_size) the latent sample, or None for zeros; state: HL (B, S, H, W, 64) the
+        present states.  The n_future predicted states go to frames [out_t0, out_t0 + n_future) of out."""
+        self._require_eval()
+        if not self.mixture:
+            raise NotImplementedError("Dual_GRU: mixture=False is not built (every reference config mixes)")
+        P = self.packed()
+        B, S, H, W, _ = state.hi.shape
+        dev = state.hi.device
+        a1 = dense.HL.zeros(B, 1, H, W, 192, dev, cp=192)      # cell 1: [s1 | x | (1 - r) * s1]
+        a2 = dense.HL.zeros(B, 1, H, W, 192, dev, cp=192)      # cell 2: [h | s2 | (1 - r) * h]
+        mix = dense.HL.empty(B, 1, H, W, 128, dev, cp=128)     # [s1 | s2], the trusting gate's input
+        if x is not None:
+            dense.hl_copy(x, (a1, 64), self.input_size, T=1)
+        dense.hl_copy((state, 0, 0), a2, 64, T=1)
+        for t in range(S - 1):                                   # warm-up of gru_cell_2 over the present states
+            dense.hl_copy((state, 0, t), (a2, 64), 64, T=1)
+            _gru_step(a2, P["gate2"], P["prop2"])
+        dense.hl_copy((state, 0, S - 1), a1, 64, T=1)
+        dense.hl_copy((state, 0, S - 1), (a2, 64), 64, T=1)
+        gate_blk = self.trusting_gate[0]
+        for t in range(self.n_future):
+            _gru_step(a1, P["gate1"], P["prop1"], out2=(mix, 0))     # s1 -> a1[0:64] and mix[0:64]
+            _gru_step(a2, P["gate2"], P["prop2"])
+            dense.conv(a2, P["dec2"], out=mix, out_coff=64)          # s2 = conv_decoder_2(h) -> mix[64:128]
+            g = gate_blk.forward_hl(mix)
+            dense.trust_mix(g, P["trust_w"], (mix, 0), (mix, 64), [(a1, 0), (a2, 64), (out, 0, out_t0 + t)], 64, T=1)
+        return out
+
+    def forward(self, x, state):
+        """x (B, 1, input_size, H, W) fp32, state (B, S, hidden, H, W) fp32 -> (B, n_future, hidden, H, W) fp32."""
+        B, S, _, H, W = state.shape
+        out = dense.HL.empty(B, self.n_future, H, W, 64, state.device, cp=64)
+        self.forward_hl(dense.from_f32(x), dense.from_f32(state), out)
+        return dense.to_f32(out, 0, self.hidden_size)

@@ -7,14 +7,19 @@ Device data flow of forward():
     stp3_lift_splat_fwd      -> BEV grid directly as channels-last bf16 hi/lo planes + per-(b,t,c) spatial sums
     TemporalModel (wgmma)  -> ego-motion channels and pooling branches enter as per-image biases
     Decoder (wgmma)        -> fp32 logits in the reference's (B,S,k,X,Y) layout
-Prediction (N_FUTURE_FRAMES > 0) and planning are outside the hot path (SURVEY.md §2) and are refused loudly.
+With N_FUTURE_FRAMES > 0 (the Prediction configurations, eval mode only) the present distribution and the future
+prediction run between the temporal model and the decoder, and the decoder sees the present and future frames
+(DESIGN.md §3.16).  Planning is refused loudly.
 """
 import torch
 import torch.nn as nn
 
 from .. import dense, ops
+from ..layers.convolutions import PREDICT_EVAL_ONLY
 from ..utils import geometry as G
 from .decoder import Decoder
+from .distributions import DistributionModule
+from .future_prediction import FuturePrediction
 from .encoder import Encoder
 from .temporal_model import TemporalModel, TemporalModelIdentity
 
@@ -36,9 +41,16 @@ class STP3(nn.Module):
             assert cfg.MODEL.TEMPORAL_MODEL.NAME == 'identity'
         self.receptive_field = cfg.TIME_RECEPTIVE_FIELD
         self.n_future = cfg.N_FUTURE_FRAMES
-        if self.n_future > 0 or cfg.PLANNING.ENABLED:
-            raise NotImplementedError("stp3_b200 implements the perception hot path (N_FUTURE_FRAMES=0, PLANNING "
-                                      "disabled); prediction / planning are out of scope (SURVEY.md §2, rows 12-13)")
+        if cfg.PLANNING.ENABLED:
+            raise NotImplementedError("PLANNING.ENABLED: the planning head and its cost function (SURVEY.md row f4) are "
+                                      "not built on sm_90a")
+        if self.n_future > 0:
+            if cfg.MODEL.TEMPORAL_MODEL.NAME == 'identity':
+                raise NotImplementedError("N_FUTURE_FRAMES > 0 with the identity temporal model: the prediction stage is "
+                                          "wired behind the temporal_block model only")
+            if cfg.PROBABILISTIC.ENABLED and cfg.PROBABILISTIC.METHOD != 'GAUSSIAN':
+                raise NotImplementedError(f"PROBABILISTIC.METHOD = {cfg.PROBABILISTIC.METHOD}: only the GAUSSIAN present "
+                                          "distribution is built on sm_90a (BERNOULLI / MIXGAUSSIAN are not)")
         if self.encoder_out_channels % 64 != 0:
             raise NotImplementedError(f"MODEL.ENCODER.OUT_CHANNELS = {self.encoder_out_channels}: the tensor-core layers carry "
                                       "channels in blocks of 64 (the reference's configs use 64; the stress configuration 128)")
@@ -67,6 +79,15 @@ class STP3(nn.Module):
         else:
             raise NotImplementedError(f'Temporal module {cfg.MODEL.TEMPORAL_MODEL.NAME}.')
         self.future_pred_in_channels = self.temporal_model.out_channels
+        self.latent_dim = cfg.MODEL.DISTRIBUTION.LATENT_DIM
+        if self.n_future > 0:
+            if cfg.PROBABILISTIC.ENABLED:
+                self.present_distribution = DistributionModule(self.future_pred_in_channels, self.latent_dim,
+                                                               method=cfg.PROBABILISTIC.METHOD)
+            self.future_prediction = FuturePrediction(
+                in_channels=self.future_pred_in_channels, latent_dim=self.latent_dim, n_future=self.n_future,
+                mixture=cfg.MODEL.FUTURE_PRED.MIXTURE, n_gru_blocks=cfg.MODEL.FUTURE_PRED.N_GRU_BLOCKS,
+                n_res_layers=cfg.MODEL.FUTURE_PRED.N_RES_LAYERS)
 
         self.decoder = Decoder(
             in_channels=self.future_pred_in_channels, n_classes=len(cfg.SEMANTIC_SEG.VEHICLE.WEIGHTS),
@@ -133,6 +154,7 @@ class STP3(nn.Module):
     def forward(self, image, intrinsics, extrinsics, future_egomotion):
         """image (B,T,N,3,H,W), intrinsics (B,T,N,3,3), extrinsics (B,T,N,4,4), future_egomotion (B,T,6) -> dict with
         the reference's keys (stp3.py:132-184)."""
+        self._check_predict_eval()
         S = self.receptive_field
         image = image[:, :S].contiguous()
         if self.encoder.native:
@@ -149,6 +171,7 @@ class STP3(nn.Module):
         """forward() entering after the (third-party) EfficientNet trunk: r_lo (B,S,N,c3,H/8,W/8), r_hi
         (B,S,N,c4,H/16,W/16) -- the encoder heads (encoder.py:88-95) run on the wgmma kernels and hand their context
         features to the lift-splat channels-last."""
+        self._check_predict_eval()
         S = self.receptive_field
         dev = r_lo.device
         h = {k: v.to(dev) for k, v in self.prepare_inputs(intrinsics, extrinsics, future_egomotion).items()}
@@ -158,6 +181,7 @@ class STP3(nn.Module):
         """Device-only from images (B,S,N,3,H,W) fp32 through the native trunk: trunk -> heads -> forward_device
         (capturable in a CUDA graph, GraphedPerception(entry="images"))."""
         b, s, n = image.shape[:3]
+        self._check_predict_eval()
         self._check_encoder_train()
         self._mark("start_trunk")
         feat, depth = self.encoder.features_native(image.reshape(b * s * n, *image.shape[3:]), channels_last=True)
@@ -169,6 +193,7 @@ class STP3(nn.Module):
     def forward_heads_device(self, r_lo, r_hi, cam_M, cam_t, ego_R, ego_t, const):
         """Device-only: encoder heads -> forward_device (capturable in a CUDA graph)."""
         b, s, n = r_lo.shape[:3]
+        self._check_predict_eval()
         self._check_encoder_train()
         self._mark("start_heads")
         feat, depth = self.encoder.heads_f32(r_lo.view(b * s * n, *r_lo.shape[3:]), r_hi.view(b * s * n, *r_hi.shape[3:]),
@@ -181,6 +206,7 @@ class STP3(nn.Module):
     def forward_features(self, feat, depth_logits, intrinsics, extrinsics, future_egomotion, feat_channels_last=False):
         """Same as forward() but entering after the image encoder: feat (B,S,N,C,Hf,Wf) [or (B,S,N,Hf,Wf,C) with
         feat_channels_last], depth_logits (B,S,N,D,Hf,Wf)."""
+        self._check_predict_eval()
         S = self.receptive_field
         dev = feat.device
         h = {k: v.to(dev) for k, v in self.prepare_inputs(intrinsics, extrinsics, future_egomotion).items()}
@@ -197,6 +223,7 @@ class STP3(nn.Module):
         C = self.encoder_out_channels
         off, res, dim = self._bev_host()
         output = {'depth_prediction': depth_logits, 'cam_front': None}
+        self._check_predict_eval()
         if self._head_training() and not self.decoder.training:
             raise RuntimeError("STP3: temporal_model.final_conv is in train mode but the decoder is in eval mode, so no "
                                "gradient could reach the head -- call model.decoder.train() as well")
@@ -233,10 +260,35 @@ class STP3(nn.Module):
         else:
             states = self.temporal_model.forward_hl(x, const=const if use_ego else None, sums=sums)
         self._mark("temporal_model")
+        if self.n_future > 0:
+            states = self._predict_hl(states)
         # a train-mode head hands over fp32 (B, S, C, X, Y) with a grad_fn, for the train-mode decoder
         output.update(self.decoder(states) if torch.is_tensor(states) else self.decoder.forward_hl(states))
         self._mark("decoder")
         return output
+
+    def _predict_hl(self, states: dense.HL) -> dense.HL:
+        """Prediction stage (stp3.py:157-176): present distribution of the last present state (eval: the sample is mu,
+        broadcast over the map; zeros without PROBABILISTIC) -> future prediction.  HL (B, S, X, Y, C) present states
+        -> HL (B, S + n_future, X, Y, C)."""
+        B, S, X, Y, _ = states.hi.shape
+        self._mark("start_predict")
+        sample = None
+        if self.cfg.PROBABILISTIC.ENABLED:
+            present = dense.HL.empty(B, 1, X, Y, states.c, states.hi.device, cp=states.hi.shape[-1])
+            dense.hl_copy((states, 0, S - 1), present, states.hi.shape[-1], T=1)
+            mu_log_sigma = self.present_distribution.forward_hl(present)
+            sample = dense.HL.empty(B, 1, X, Y, self.latent_dim, states.hi.device)
+            dense.hl_broadcast(mu_log_sigma, sample, self.latent_dim)
+        self._mark("distribution")
+        y = self.future_prediction.forward_hl(sample, states)
+        self._mark("future_prediction")
+        return y
+
+    def _check_predict_eval(self):
+        """Every entry point refuses a Prediction model with a train-mode module before any work is enqueued."""
+        if self.n_future > 0 and any(m.training for m in self.modules()):
+            raise NotImplementedError(f"STP3: {PREDICT_EVAL_ONLY}")
 
     def _head_training(self) -> bool:
         return isinstance(self.temporal_model, TemporalModel) and self.temporal_model.final_conv.training
@@ -289,6 +341,9 @@ class STP3(nn.Module):
         splat of this rank's frames with the all-gather in the finalize epilogue, the two device-side barriers, discount,
         temporal model, decoder -- can be captured in ONE CUDA graph (GraphedPerception(entry="sharded"))."""
         from .. import parallel
+        if self.n_future > 0:
+            raise NotImplementedError("frame-sharded forward with N_FUTURE_FRAMES > 0: the latency mode is wired for the "
+                                      "perception configurations only")
         h = {"cam_M": cam_M, "cam_t": cam_t, "ego_R": ego_R, "ego_t": ego_t, "const": const}
         dev = feat.device
         B, S = feat.shape[:2]
