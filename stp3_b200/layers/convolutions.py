@@ -665,7 +665,12 @@ class Bottleblock(PredictModule):
     def _pack(self):
         L = self.layers
         z = lambda c: torch.zeros(c.out_channels, device=c.weight.device)
-        P = {f"c{i}": dense.pack_conv(L[i].weight.detach().float(), z(L[i])) for i in (0, 3, 6)}
+        P = {f"c{i}": dense.pack_conv(L[i].weight.detach().float(), z(L[i])) for i in (3, 6)}
+        # the 7x7 runs as one launch per 64 input channels, each adding the previous one's output as its residual: one
+        # launch over all 128 channels is a 6272-long sum in the wgmma accumulator, whose round-off grows with the
+        # length of the sum faster than round-to-nearest fp32 adds would, to 3e-5 of max (DESIGN.md section 4)
+        w0 = L[0].weight.detach().float()
+        P["c0"] = [dense.pack_conv(w0[:, c:c + dense.KB].contiguous(), z(L[0])) for c in range(0, w0.shape[1], dense.KB)]
         P.update({f"ln{i}": _ln_params(L[i]) for i in (1, 4, 7)})
         if self.projection is not None:
             P["proj"] = dense.pack_conv(self.projection[0].weight.detach().float(), z(self.projection[0]))
@@ -676,7 +681,9 @@ class Bottleblock(PredictModule):
         self._require_eval()
         P = self.packed()
         m, co = self.mid, self.out_channels
-        a = dense.conv(x, P["c0"])
+        a = None
+        for i, pc in enumerate(P["c0"]):
+            a = dense.conv(x, pc, cin_off=i * dense.KB, residual=a)
         dense.channel_norm_act(a, a, m, ln=P["ln1"], gelu=True)
         a = dense.conv(a, P["c3"])
         dense.channel_norm_act(a, a, m, ln=P["ln4"], gelu=True)

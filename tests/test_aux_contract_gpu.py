@@ -4,7 +4,8 @@ stp3_upsample2x_add) against the float64 reference of their contract (tests/aux_
 
 The launches are recorded from the model -- the dense wrappers and dense_train.to_hl replaced while it runs, each call's
 inputs cloned and what production wrote cloned too: the b4 trunk on 18 images and the b0 trunk at 224 x 480, the
-perceive forward with the fused and the unfused TemporalBlock tail, the stress shape, the encoder heads in eval, and
+perceive forward with the fused and the unfused TemporalBlock tail, the stress shape, the encoder heads in eval, the
+Prediction model (tests/test_conv_contract_gpu.py predict_model at 40 x 56, and _predict_hl at 200 x 200), and
 train steps of the decoder, the DeepLab head, the TemporalModel and the encoder heads -- and built synthetically for what
 the model never passes (stem widths and pads, channel windows inside wider strides, one-pixel maps, squeeze-excite
 projections whose last chunk is exactly 64 or 128 wide, rounding edge cases of the hi/lo split, multi-slice pooling
@@ -53,8 +54,17 @@ ULP = 2.0 ** -24
 # measured over every launch of this file on an H100 80GB HBM3 (700 W power limit; table in DESIGN.md section 4).  The
 # squeeze-excite weights are held to their exact bound instead: 2^-17 (the split) + 2^-23 (the fp32 product) of
 # |W_proj gate| with the kernel's own gate, i.e. a ratio of 1.
+# stp3_spatial_sum adds one partial per 128-pixel chunk into each sum with float atomics, in no fixed order, so its
+# round-off grows like the square root of the chunk count: its bar is BARS["spatial_sum"] up to SSUM_CHUNKS chunks per
+# image (the most of the launches it was measured on: 1.2 ulps at most), and grows with sqrt(chunks / SSUM_CHUNKS)
+# beyond (the Prediction model: 4.3 ulps at 18 chunks, bar 10.6; 7.0 at 313 chunks, bar 44).
 BARS = {"stem": 16, "dw": 10, "dw sums": 10, "se gate": 4, "se weights": 1.0, "spatial_sum": 5,
         "pool_bias": 4, "small_linear": 16, "upsample": 6}
+SSUM_CHUNKS = 4
+
+
+def ssum_bar_scale(HW):
+    return max(1.0, (-(-HW // 128) / SSUM_CHUNKS) ** 0.5)
 
 
 def _stream():
@@ -439,6 +449,7 @@ def check(case: Case) -> dict:
         ref = R.spatial_sum(a["hi"], a["lo"], a["n"], a["HW"], a["cs"])
         res["written"] = not bool(torch.isnan(win["sums"]).any())
         errs["spatial_sum"] = _ulps(win["sums"].view(a["n"], a["cs"]), ref["sums"], ref["mag"])
+        res["bar scale"] = ssum_bar_scale(a["HW"])
     elif k in ("pool", "lin"):
         if k == "pool":
             ref = R.pool_bias(a["sums"], a["n"], a["T"], a["C"], a["inv_hw"], a["temporal"], a["cv"], a["nc"], a["W1"],
@@ -463,7 +474,8 @@ def check(case: Case) -> dict:
 
 
 def passed(res):
-    return all(v for v in res.values() if isinstance(v, bool)) and all(e <= BARS[m] for m, e in res["errs"].items())
+    return all(v for v in res.values() if isinstance(v, bool)) and all(e <= BARS[m] * res.get("bar scale", 1.0)
+                                                                       for m, e in res["errs"].items())
 
 
 # ------------------------------------------------------------------------------------------------ recording
@@ -649,6 +661,23 @@ def rec_stress():
         with Recorder("stress C128 S5") as r:
             model.forward_features(inp["feat"].to(DEV), inp["depth_logits"].to(DEV), inp["intrinsics"],
                                    inp["extrinsics"], inp["future_egomotion"])
+    return r.cases
+
+
+def rec_predict_small(carla):
+    """the Prediction model's forward at 40 x 56, B = 2 (tests/test_conv_contract_gpu.py predict_model): the present
+    distribution's spatial sums on 3 x 4 maps and its small_linear with 1 / (h w) folded into the weights"""
+    from tests import test_conv_contract_gpu as CC
+    r = Recorder(f"predict {'carla' if carla else 'nuscenes'} 40x56")
+    CC.run_predict_small(carla, r)
+    return r.cases
+
+
+def rec_predict_200():
+    """STP3._predict_hl on (1, 3, 64, 200, 200) present states: the distribution's sums on 13 x 13 maps"""
+    from tests import test_conv_contract_gpu as CC
+    r = Recorder("predict 200x200")
+    CC.run_predict_200(r)
     return r.cases
 
 
@@ -842,6 +871,9 @@ SOURCES = {
     "perceive_unfused": lambda: rec_perceive("0"),
     "stress": rec_stress,
     "encoder_heads_eval": rec_encoder_heads,
+    "predict_small_nuscenes": lambda: rec_predict_small(False),
+    "predict_small_carla": lambda: rec_predict_small(True),
+    "predict_200x200": rec_predict_200,
     "train_decoder": lambda: rec_train("decoder 48x64", "rec_decoder", (2, 3, 64, 48, 64), GATES_ALL, "d"),
     "train_deeplab": lambda: rec_train("deeplab 48x64", "rec_deeplab", 64, 64, 128, 6, 48, 64, "h"),
     "train_temporal": lambda: rec_train("temporal 48x64", "rec_temporal", 70, 6, 3, 2, 48, 64, "t"),
@@ -931,8 +963,9 @@ def test_every_entry_point_and_feature_is_replayed():
         print(f"  {f:<34s} {counts[f]}")
     print("worst error per entry point (fp32 ulps of the terms' magnitudes; se weights: of the exact bound), bar")
     for m in BARS:
-        errs = [(r["res"]["errs"][m], r["tag"]) for r in rows if m in r["res"]["errs"]]
+        errs = [(r["res"]["errs"][m], r["tag"], BARS[m] * r["res"].get("bar scale", 1.0)) for r in rows
+                if m in r["res"]["errs"]]
         if errs:
-            e, tag = max(errs)
-            print(f"  {m:<14s} {e:10.3g}  bar {BARS[m]:<6g} over {len(errs):4d} launches, worst: {tag[:70]}")
+            e, tag, bar = max(errs)
+            print(f"  {m:<14s} {e:10.3g}  bar {bar:<6.3g} over {len(errs):4d} launches, worst: {tag[:70]}")
     assert all(counts.values()), [f for f, c in counts.items() if not c]

@@ -3,7 +3,11 @@ reference of the stp3_conv_fwd contract (tests/conv_reference.py).
 
 The calls are recorded from the model itself (dense.conv wrapped while the forward / backward runs), so the descriptors
 are the production ones: frame windows, trimmed K ranges, channel windows of concat tensors, split 256-column launches,
-output-size overrides of the input-gradient phases, fused heads, column sums.  Each recorded call is replayed with
+output-size overrides of the input-gradient phases, fused heads, column sums.  The Prediction model adds K windows that
+start inside a buffer (cin_off 64 of the conv-GRU cell and of the Bottleblock's second 7 x 7 launch), 49-tap layers and
+the decoder over 7 frames
+(predict_model at 40 x 56 with both gate sets, and each distinct convolution of _predict_hl at 200 x 200).  Each
+recorded call is replayed with
 tune = (0, 0) (the kernel's own heuristics: graph capture, STP3_CONV_AUTOTUNE=0) and with every candidate of
 dense.tune_candidates, into outputs pre-filled with a sentinel.  Checked per replay:
   - every written value against the exact fp64 convolution (the project's 3e-5 of max bar) and against the fp64
@@ -209,6 +213,70 @@ def rec_stress():
     return r.calls
 
 
+def predict_model(carla):
+    """The Prediction model (PROBABILISTIC on, four future frames) with the gate set of nuScenes (instance heads over
+    the 7 frames) or CARLA (pedestrian and hdmap; hdmap reads the present frame, a one-frame window at frame 2 of 7),
+    at a 40 x 56 BEV, built like tests/test_predict_gpu.py's model: the distribution goes 40 x 56 -> 20 x 28 -> 10 x 14
+    -> 5 x 7 -> 3 x 4."""
+    from oracle.make_golden_predict import build_prediction_model, predict_cfg
+    from stp3_b200.utils import synthetic as syn
+    xb, yb = [-10.0, 10.0, 0.5], [-14.0, 14.0, 0.5]
+    cfg = predict_cfg(carla)
+    cfg.merge({"LIFT": {"X_BOUND": xb, "Y_BOUND": yb, "D_BOUND": [2.0, 10.0, 1.0]}, "IMAGE": {"FINAL_DIM": (32, 48)}})
+    lcfg = syn.LiftSplatConfig(x_bound=tuple(xb), y_bound=tuple(yb), d_bound=(2.0, 10.0, 1.0), final_dim=(32, 48),
+                               out_channels=64, n_cameras=2, receptive_field=cfg.TIME_RECEPTIVE_FIELD)
+    return build_prediction_model(cfg).to(DEV), lcfg
+
+
+def run_predict_small(carla, recorder):
+    """STP3.forward_features of predict_model(carla) on B = 2 synthetic samples inside `recorder` (a context manager);
+    returns the outputs"""
+    from stp3_b200.utils import synthetic as syn
+    with torch.no_grad():
+        model, lcfg = predict_model(carla)
+        inp = syn.lift_inputs(lcfg, 2, seed=4, random_pose=True)
+        with recorder:
+            return model.forward_features(inp["feat"].to(DEV), inp["depth_logits"].to(DEV), inp["intrinsics"],
+                                          inp["extrinsics"], inp["future_egomotion"])
+
+
+def run_predict_200(recorder):
+    """STP3._predict_hl on (1, 3, 64, 200, 200) present states (the headline rig's BEV; the distribution ends 25 -> 13)
+    inside `recorder`"""
+    from oracle.make_golden_predict import build_prediction_model, predict_cfg
+    from stp3_b200.utils import synthetic as syn
+    with torch.no_grad():
+        model = build_prediction_model(predict_cfg(False)).to(DEV)
+        s = syn.exact_gauss((1, 3, 64, 200, 200), torch.Generator().manual_seed(12)).to(DEV)
+        states = dense.from_f32(s)
+        with recorder:
+            return model._predict_hl(states)
+
+
+def _distinct(calls):
+    """one call per descriptor (packed convolution, keywords and geometry): the Dual_GRU's steps repeat theirs"""
+    seen, out = set(), []
+    for c in calls:
+        key = (id(c.pc), repr(sorted((k, v) for k, v in c.kw.items() if k not in ("residual", "img_bias", "head"))),
+               c.x.hi.shape, c.kw["residual"] is not None)
+        if key not in seen:
+            seen.add(key)
+            out.append(c)
+    return out
+
+
+def rec_predict_small(carla):
+    r = Recorder(f"predict {'carla' if carla else 'nuscenes'} 40x56")
+    run_predict_small(carla, r)
+    return r.calls
+
+
+def rec_predict_200():
+    r = Recorder("predict 200x200")
+    run_predict_200(r)
+    return _distinct(r.calls)
+
+
 def rec_encoder_heads():
     """Encoder.heads_hl at the shape of test_encoder_heads_vs_reference_golden: DeepLabHead(160 -> 160, hidden 64) +
     UpsamplingConcat(216 -> 64 / 48) for the context features and the depth logits."""
@@ -388,6 +456,9 @@ SOURCES = {
     "encoder_heads": rec_encoder_heads,
     "decoder_train": rec_decoder_train,
     "decoder_full": rec_decoder_full,
+    "predict_small_nuscenes": lambda: rec_predict_small(False),
+    "predict_small_carla": lambda: rec_predict_small(True),
+    "predict_200x200": rec_predict_200,
     "synthetic": rec_synthetic,
 }
 for _m in PLANE_NAMES:
@@ -494,6 +565,13 @@ def references(call: Call):
         kw["head"] = {"w": hd["w"], "b": hd["b"], "sigmoid_mask": hd["sigmoid_mask"]}
     exact, model = R.epilogue(acc[False], call.pc, kw), R.epilogue(acc[True], call.pc, kw)
     scale = {k: max(float(v.abs().max()), 1e-20) for k, v in exact.items()}
+    if hd is not None and hd["sigmoid_mask"]:
+        # a sigmoid output moves by at most 1/4 of its logit's error: held to a quarter of the logits' max (as the
+        # instance-center head is in tests/test_predict_gpu.py), not to the max of the saturated sigmoid
+        logits = R.epilogue(acc[False], call.pc, dict(kw, head=dict(kw["head"], sigmoid_mask=0)))
+        for k in range(len(hd["outs"])):
+            if hd["sigmoid_mask"] >> k & 1:
+                scale[f"head{k}"] = max(scale[f"head{k}"], 0.25 * float(logits[f"head{k}"].abs().max()))
     if "col_sums" in exact:       # a column sum is held to the sum of the magnitudes it adds up (it may cancel to ~0)
         scale["col_sums"] = max(float(_activated(acc[False], call).abs().sum(dim=(1, 2)).max()), 1e-20)
     return exact, model, scale
@@ -588,6 +666,12 @@ def features(call: Call, cfg, t: Optional[dict] = None):
         f.add("frame window")
     if kw.get("out_hw") is not None:
         f.add("out_hw override")
+    if kw.get("cin_off", 0) > 0:
+        f.add("cin_off > 0")
+    if len(pc.taps) > 27:
+        f.add("taps > 27")
+    if Tt == 7:
+        f.add("T_total 7")
     f.add(f"res_mode {0 if kw['residual'] is None else 2 if kw.get('res_after_act') else 1}")
     for k, coff in (("out", "out_coff"), ("out2", "out2_coff")):
         if kw[k] is not None:
@@ -616,7 +700,7 @@ REQUIRED = ["width 64", "width 128", "width 256 (two launches)", "STACK", "FULLK
             "streamed (+4)", "tap group > 1", "stride 2", "causal taps at frame 0", "frame window", "out_hw override",
             "res_mode 0", "res_mode 1", "res_mode 2", "vector store", "scalar store", "vector residual",
             "scalar residual", "hi/lo output", "f32 NCHW output + sigmoid", "f32 NHWC output", "fused head", "out2",
-            "col_sums", "img_bias", "partial n_store"]
+            "col_sums", "img_bias", "partial n_store", "cin_off > 0", "taps > 27", "T_total 7"]
 
 
 # ------------------------------------------------------------------------------------------------ driver

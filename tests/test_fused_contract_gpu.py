@@ -232,9 +232,27 @@ def rec_synthetic_block():
     return calls
 
 
+def rec_predict_small(carla):
+    """the Prediction model's forward at 40 x 56, B = 2 (tests/test_conv_contract_gpu.py predict_model): the DeepLab
+    head of the last SpatialGRU over B x 7 frames"""
+    r = Recorder(f"predict {'carla' if carla else 'nuscenes'} 40x56")
+    CC.run_predict_small(carla, r)
+    return r.calls
+
+
+def rec_predict_200():
+    """STP3._predict_hl on (1, 3, 64, 200, 200) present states: the DeepLab head over 7 frames of 200 x 200"""
+    r = Recorder("predict 200x200")
+    CC.run_predict_200(r)
+    return r.calls
+
+
 SOURCES = {
     "perceive": rec_perceive,
     "headline": rec_headline,
+    "predict_small_nuscenes": lambda: rec_predict_small(False),
+    "predict_small_carla": lambda: rec_predict_small(True),
+    "predict_200x200": rec_predict_200,
     "synthetic_aspp": rec_synthetic_aspp,
     "synthetic_block": rec_synthetic_block,
 }
