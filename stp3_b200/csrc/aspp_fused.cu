@@ -10,6 +10,11 @@
 //                         acc2 += P . W_proj[:, b-th 128 input channels]   (second MMA chain, A operand = P from registers)
 //   out = hi/lo split of relu(acc2 + per-image bias)                       (the global-pool branch is that bias)
 //
+// The output tile is staged in the activation stage the last branch's last tap read, laid out as the TMA load wrote it
+// (per plane [pixel row][128 B], 128-byte swizzle), one 64-channel block at a time, and leaves by one
+// cp.async.bulk.tensor store per warpgroup, plane and block.  That stage goes back to the producer once the stores have
+// read it, early in the next tile, whose first taps load into the other two stages.
+//
 // The same kernel runs the head's tail, 3x3 conv/BN/ReLU -> 1x1 classifier (convolutions.py:272-280), as a ONE-branch
 // instance (9 taps, two input K blocks, classifier rows padded to 128, no ReLU on the output).
 //
@@ -38,6 +43,11 @@ constexpr int kAsppNA = 3, kAsppNB = 3;
 constexpr int kAStage = 2 * 8 * 16 * 128;         // hi + lo planes of 8 image rows x 16 pixels x 64 channels
 constexpr int kBStage = 2 * 128 * 128;            // hi + lo planes of the 128 weight rows
 constexpr int kAsppHidden = 128;
+// the output tile is staged in an activation stage: per plane 128 pixel rows of 128 bytes (64 channels), 1024-byte
+// aligned for the 128-byte swizzle; each warpgroup stores its 64 rows as one box of 16 x kAsppStoreRows pixels
+constexpr int kAsppStoreRows = 4;
+static_assert(kAStage / 2 == 8 * 16 * 128 && (kAStage / 2) % 1024 == 0, "an activation plane stages 128 pixels x 64 channels");
+static_assert(16 * kAsppStoreRows == 64, "one store box per warpgroup: its 64 accumulator rows");
 
 // shared memory, from the 1024-byte aligned base (the kernel carves it, the host sizes the launch from `bytes`)
 struct AsppSmem {
@@ -58,9 +68,6 @@ struct AsppParams {
   signed char tap[kAsppMaxTaps][2];               // (dy, dx)
   const float* br_bias;                           // [n_br][128]
   const float* img_bias;                          // [n_img][128]
-  __nv_bfloat16* out_hi;
-  __nv_bfloat16* out_lo;
-  int out_cstride, out_coff;
   int relu_out;                                   // ReLU on the projection output (ASPP: yes; conv3 -> classifier: no)
   int n_store;                                    // output channels stored (64 or 128): rows >= n_store of the projection are zero
 };
@@ -73,7 +80,8 @@ __device__ __forceinline__ bool aspp_tap_is_padding(const AsppParams& p, int t, 
 
 __global__ void __launch_bounds__(kAsppThreads, 1)
 aspp_fused_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ CUtensorMap tm_a_lo,
-                  const __grid_constant__ CUtensorMap tm_w, const AsppParams p) {
+                  const __grid_constant__ CUtensorMap tm_w, const __grid_constant__ CUtensorMap tm_o_hi,
+                  const __grid_constant__ CUtensorMap tm_o_lo, const AsppParams p) {
   const int cta = (int)blockIdx.x, n_cta = (int)gridDim.x;
   extern __shared__ unsigned char smem_raw[];
   unsigned char* smem = smem_raw + ((1024u - (ptx::smem_u32(smem_raw) & 1023u)) & 1023u);
@@ -88,6 +96,7 @@ aspp_fused_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (warp == 8 && lane == 0) {
     ptx::prefetch_tmap(&tm_a_hi); ptx::prefetch_tmap(&tm_a_lo); ptx::prefetch_tmap(&tm_w);
+    ptx::prefetch_tmap(&tm_o_hi); ptx::prefetch_tmap(&tm_o_lo);
     ra.init(2); rb.init(2);
     ptx::fence_mbar_init();
   }
@@ -136,6 +145,9 @@ aspp_fused_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
     const int cq = 2 * (lane & 3);                           // first of its two columns in every 8-column group
     float* wb = s_wb + wg * kAsppHidden;
     PendingSlots pend{ra.empty, rb.empty, wtid == 0};
+    int out_slot = -1;                           // activation stage holding the previous tile's output until stored
+    // acc (+)= A . B over one 64-channel K block, then commit, release the previous group's slots, and the previous
+    // tile's output stage once its stores have read it (the new group runs meanwhile)
     auto issue = [&](float* acc, uint32_t a_hi, uint32_t a_lo, uint32_t b_hi, uint32_t b_lo, uint32_t accumulate,
                      int slot_a, int slot_b) {
       const uint64_t da_hi = wg::desc_k_sw128(a_hi), da_lo = wg::desc_k_sw128(a_lo);
@@ -149,6 +161,10 @@ aspp_fused_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
       wg::commit();
       wg::wait<1>();
       pend.release_and_defer(slot_a, slot_b);
+      if (out_slot >= 0) {
+        if (wtid == 0) { ptx::bulk_wait_read0(); ptx::mbar_arrive(&ra.empty[out_slot]); }
+        out_slot = -1;
+      }
     };
     ptx::griddep_wait();
     for (int tile = cta; tile < p.n_tiles; tile += n_cta) {
@@ -159,6 +175,7 @@ aspp_fused_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
       wb[wtid] = *(reinterpret_cast<const volatile float*>(p.img_bias) + (size_t)img * kAsppHidden + wtid);
       ptx::bar_sync(1 + wg, 128);                // the output reads entries other warps of the warpgroup wrote
       float acc2[kAsppHidden / 2];
+      int stage = -1;                            // the last branch's last activation stage: the output staging area
       for (int s = 0; s < p.n_br; ++s) {
         // ---- main(s): acc1 = sum over the branch's taps
         float acc1[kAsppHidden / 2];
@@ -177,6 +194,7 @@ aspp_fused_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
           }
         }
         wg::wait<0>();                             // also: the previous branch's projection has read P's registers
+        if (s + 1 == p.n_br) { stage = pend.a; pend.a = -1; }   // the centre tap is never padding: a stage was read
         pend.release();
         // ---- P = hi/lo split of relu(acc1 + bias), kept in registers, and proj(s): acc2 (+)= P . W_proj[:, branch s],
         // one 64-column K block kb2 at a time.  Accumulator entries (4 g8 + 2 h, +1) -- row row0 + 8 h, columns
@@ -216,28 +234,46 @@ aspp_fused_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
       }
       wg::wait<0>();
       pend.release();
-      // ---- output of the projection: relu(acc2 + per-image bias) -> hi/lo planes
+      // ---- output of the projection: relu(acc2 + per-image bias) -> hi/lo planes, one 64-channel block at a time
+      // through the staging stage: row r of this warpgroup's 64 at r * 128 bytes of each plane, 16-byte chunk g at
+      // chunk g ^ (r & 7).  The second block waits until the first block's stores have read the stage
+      unsigned char* st_hi = a_ring + (size_t)stage * kAStage;
+      unsigned char* st_lo = st_hi + kAStage / 2;
+      const uint32_t src = ptx::smem_u32(st_hi) + (uint32_t)(wg * 64 * 128);
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int row = row0 + 8 * h;
-        const int oy = oy_tile + (row >> 4), ox = ox0 + (row & 15);
-        if (oy >= p.H || ox >= p.W) continue;
-        const size_t pix = ((size_t)img * p.H + oy) * p.W + ox;
+      for (int cb = 0; cb < kAsppHidden / 64; ++cb) {
+        if (cb * 64 >= p.n_store) break;
+        if (cb > 0) {
+          if (wtid == 0) ptx::bulk_wait_read0();
+          ptx::bar_sync(1 + wg, 128);
+        }
 #pragma unroll
-        for (int g8 = 0; g8 < 16; ++g8) {
-          const int c = 8 * g8 + cq;
-          if (c >= p.n_store) continue;
-          float x0 = acc2[4 * g8 + 2 * h] + wb[c];
-          float x1 = acc2[4 * g8 + 2 * h + 1] + wb[c + 1];
-          if (p.relu_out) { x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); }
-          uint32_t hw, lw;
-          ptx::split_hilo(x0, x1, hw, lw);
-          const size_t off = pix * p.out_cstride + p.out_coff + c;
-          *reinterpret_cast<uint32_t*>(p.out_hi + off) = hw;
-          *reinterpret_cast<uint32_t*>(p.out_lo + off) = lw;
+        for (int h = 0; h < 2; ++h) {
+          const int row = row0 + 8 * h;
+#pragma unroll
+          for (int g = 0; g < 8; ++g) {
+            const int g8 = 8 * cb + g, c = 8 * g8 + cq;
+            float x0 = acc2[4 * g8 + 2 * h] + wb[c];
+            float x1 = acc2[4 * g8 + 2 * h + 1] + wb[c + 1];
+            if (p.relu_out) { x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); }
+            uint32_t hw, lw;
+            ptx::split_hilo(x0, x1, hw, lw);
+            const uint32_t off = (uint32_t)(row * 128 + ((g ^ (row & 7)) << 4) + 2 * cq);
+            *reinterpret_cast<uint32_t*>(st_hi + off) = hw;
+            *reinterpret_cast<uint32_t*>(st_lo + off) = lw;
+          }
+        }
+        ptx::fence_proxy_async();                // the generic-proxy writes are visible to the TMA stores
+        ptx::bar_sync(1 + wg, 128);              // every row of this warpgroup's half is written
+        if (wtid == 0) {                         // image rows oy_tile + 4 wg .. + 3: the map clips the ragged edges
+          ptx::tma_store_4d(&tm_o_hi, src, cb * 64, ox0, oy_tile + kAsppStoreRows * wg, img);
+          ptx::tma_store_4d(&tm_o_lo, src + kAStage / 2, cb * 64, ox0, oy_tile + kAsppStoreRows * wg, img);
+          ptx::bulk_commit();
         }
       }
+      out_slot = stage;
     }
+    if (wtid == 0) ptx::bulk_wait0();            // the last tile's outputs are written before the CTA exits
   }
 }
 
@@ -277,13 +313,11 @@ extern "C" int stp3_aspp_fused_fwd(const stp3_aspp_desc* d, const void* x_hi, co
   }
   for (int b = d->n_br; b <= kAsppMaxBranches; ++b) p.br_tap0[b] = t;
   p.br_bias = br_bias; p.img_bias = img_bias;
-  p.out_hi = static_cast<__nv_bfloat16*>(y_hi); p.out_lo = static_cast<__nv_bfloat16*>(y_lo);
-  p.out_cstride = d->out_cstride; p.out_coff = d->out_coff;
   p.relu_out = d->no_relu ? 0 : 1; p.n_store = n_store;
   // every descriptor check comes before the driver lookup: a bad descriptor is reported as such without a GPU
   if (!tmap_encode_fn()) return set_error(STP3_ECUDA, "cuTensorMapEncodeTiled is not available from the driver");
 
-  CUtensorMap tm_hi, tm_lo, tm_w;
+  CUtensorMap tm_hi, tm_lo, tm_w, tm_o[2];
   {
     const CUresult r1 = encode_act_5d(&tm_hi, x_hi, d->in_cstride, d->W, d->H, d->T, d->B, 16, 8, 1);
     const CUresult r2 = encode_act_5d(&tm_lo, x_lo, d->in_cstride, d->W, d->H, d->T, d->B, 16, 8, 1);
@@ -292,12 +326,18 @@ extern "C" int stp3_aspp_fused_fwd(const stp3_aspp_desc* d, const void* x_hi, co
     const CUresult r3 = encode_rows_2d(&tm_w, w, (long long)(t * p.kblocks + 2 * d->n_br) * 256, 128);
     if (r3 != CUDA_SUCCESS) return set_error(STP3_ECUDA, "cuTensorMapEncodeTiled(weights) failed: %d", (int)r3);
   }
+  void* outs[2] = {y_hi, y_lo};
+  for (int i = 0; i < 2; ++i) {       // the n_store-channel output window; one box = one warpgroup's 4 x 16 pixels
+    const CUresult r = encode_out_4d(&tm_o[i], static_cast<__nv_bfloat16*>(outs[i]) + d->out_coff, d->out_cstride, n_store,
+                                     d->W, d->H, p.n_img, 16, kAsppStoreRows);
+    if (r != CUDA_SUCCESS) return set_error(STP3_ECUDA, "cuTensorMapEncodeTiled(output %d) failed: %d", i, (int)r);
+  }
   STP3_CUDA_OK(set_max_dynamic_smem<aspp_fused_kernel>((int)AsppSmem::bytes));
   const int n_sm = num_sms();
   // The kernel never executes griddepcontrol.launch_dependents: its dependents are released when the grid completes
   // (see block_fused.cu); it still starts early behind its predecessor.
   STP3_CUDA_OK(launch_pdl(kPdlFused, aspp_fused_kernel, dim3((unsigned)(nt < n_sm ? nt : n_sm)), dim3(kAsppThreads),
-                          AsppSmem::bytes, stream, tm_hi, tm_lo, tm_w, p));
+                          AsppSmem::bytes, stream, tm_hi, tm_lo, tm_w, tm_o[0], tm_o[1], p));
   STP3_CUDA_OK(cudaGetLastError());
   return STP3_OK;
 }

@@ -19,6 +19,11 @@
 //   proj    : acc3 = x_tile . W_projection (N = 64) when the block changes its width, on the activation stage that
 //             path 2 (the 1x1x1 chain of x, always the last chain) has loaded
 //   final   : out = relu(acc2 + per-image bias) + (acc3 + per-image bias | x), hi/lo planes, per-image column sums
+//   store   : the output tile is staged in path 2's activation stage, laid out as the TMA load wrote it (per plane
+//             [pixel row][128 B], 128-byte swizzle), and leaves by one cp.async.bulk.tensor store per warpgroup and
+//             plane; the identity residual x is read from the same bytes just before they are overwritten.  That
+//             stage goes back to the producer once the stores have read it, early in the next tile, whose first
+//             chains load into the other two stages
 //
 // Two warpgroups own rows 0..63 / 64..127 of the tile; warp 8 is the TMA producer, and its warpgroup hands its registers
 // to the MMA warpgroups (setmaxnreg 40 / 232: a chain accumulator, acc2, acc3 and the P fragments live at once do not
@@ -47,6 +52,11 @@ constexpr int kBlkAStage = 2 * kBlkBoxRows * 16 * 128;
 constexpr int kBlkMaxGroups = 16;
 constexpr int kBlkBRows = 64;                     // weight rows per plane: chains are at most 64 wide
 constexpr int kBlkBStage = 2 * kBlkBRows * 128;
+// the output tile is staged in path 2's activation stage: per plane its first 128 pixel rows of 128 bytes (64 channels),
+// 1024-byte aligned for the 128-byte swizzle; each warpgroup stores its 64 rows as one box of 16 x kBlkStoreRows pixels
+constexpr int kBlkStoreRows = 4;
+static_assert(kBlkAStage / 2 >= 8 * 16 * 128 && (kBlkAStage / 2) % 1024 == 0, "an activation plane stages 128 pixels x 64 channels");
+static_assert(16 * kBlkStoreRows == 64, "one store box per warpgroup: its 64 accumulator rows");
 
 // shared memory, from the 1024-byte aligned base (the kernel carves it, the host sizes the launch from `bytes`)
 struct BlkSmem {
@@ -92,12 +102,6 @@ struct BlkParams {
   const float* hid_bias;    // [n_img][128] bias of the hidden channels in P order
   const float* img_bias;    // [n_img][64]  aggregation bias (+ pyramid-pooling branch)
   const float* res_bias;    // [n_img][64]  projection bias (has_res_proj) or null
-  const __nv_bfloat16* res_hi;            // identity residual (x planes) when !has_res_proj
-  const __nv_bfloat16* res_lo;
-  int res_cstride;
-  __nv_bfloat16* out_hi;
-  __nv_bfloat16* out_lo;
-  int out_cstride;
   float* sum_part;          // [gridDim.x * 8][n_img][64] or null
   int wagg_blk0;            // two weight blocks (K blocks of P) of the aggregation conv
 };
@@ -118,7 +122,8 @@ template <int LAYOUT>
 __global__ void __launch_bounds__(kBlkThreads, 1)
 block_fused_kernel(const __grid_constant__ CUtensorMap tm_m_hi, const __grid_constant__ CUtensorMap tm_m_lo,
                    const __grid_constant__ CUtensorMap tm_x_hi, const __grid_constant__ CUtensorMap tm_x_lo,
-                   const __grid_constant__ CUtensorMap tm_w, const BlkParams p) {
+                   const __grid_constant__ CUtensorMap tm_w, const __grid_constant__ CUtensorMap tm_o_hi,
+                   const __grid_constant__ CUtensorMap tm_o_lo, const BlkParams p) {
   const int cta = (int)blockIdx.x, n_cta = (int)gridDim.x;
   extern __shared__ unsigned char smem_raw[];
   unsigned char* smem = smem_raw + ((1024u - (ptx::smem_u32(smem_raw) & 1023u)) & 1023u);
@@ -135,7 +140,7 @@ block_fused_kernel(const __grid_constant__ CUtensorMap tm_m_hi, const __grid_con
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (warp == 8 && lane == 0) {
     ptx::prefetch_tmap(&tm_m_hi); ptx::prefetch_tmap(&tm_m_lo); ptx::prefetch_tmap(&tm_x_hi); ptx::prefetch_tmap(&tm_x_lo);
-    ptx::prefetch_tmap(&tm_w);
+    ptx::prefetch_tmap(&tm_w); ptx::prefetch_tmap(&tm_o_hi); ptx::prefetch_tmap(&tm_o_lo);
     ra.init(2); rb.init(2);
     ptx::mbar_init(w_agg_full, 2);               // one arrive.expect_tx per aggregation block
     ptx::fence_mbar_init();
@@ -203,6 +208,7 @@ block_fused_kernel(const __grid_constant__ CUtensorMap tm_m_hi, const __grid_con
     float* wb = s_wb + wg * 128;
     const uint32_t w_agg_u32 = ptx::smem_u32(w_agg);
     PendingSlots pend{ra.empty, rb.empty, wtid == 0};
+    int out_slot = -1;                           // activation stage holding the previous tile's output until stored
     // acc (+)= A . B over KS K steps from k0 with hi*hi + hi*lo + lo*hi, then commit and release the previous group's slots
     auto issue = [&](auto n_c, auto ks_c, float* acc, uint32_t a_hi, uint32_t b_hi, int k0, uint32_t accumulate,
                      int slot_a, int slot_b) {
@@ -228,9 +234,13 @@ block_fused_kernel(const __grid_constant__ CUtensorMap tm_m_hi, const __grid_con
     uint32_t carry_hi[2] = {0u, 0u}, carry_lo[2] = {0u, 0u};   // the first half of a K step that straddles two chains
     int agg_next = 0;                           // next K step of the aggregation
 
-    // one chain of one tile: its taps (and the projection on the same activation stage), then its pieces of P into acc2
-    auto run_chain = [&](auto n_c, auto npc_c, auto odd_c, auto close_c, const BlkChain& ch, int tidx, int oy_tile, int ox0,
-                         bool with_proj) {
+    // one chain of one tile: its taps (and the projection on the same activation stage), then its pieces of P into acc2.
+    // The first chain hands the previous tile's output stage back to the producer once its stores have read it (after
+    // an issue, so the new group runs meanwhile).  The last chain (path 2, one group) keeps its activation stage as this
+    // tile's output staging area: `stage`
+    int stage = -1;
+    auto run_chain = [&](auto first_c, auto n_c, auto npc_c, auto odd_c, auto close_c, const BlkChain& ch, int tidx,
+                         int oy_tile, int ox0, bool with_proj, bool last_chain) {
       constexpr int N = decltype(n_c)::value, NPC = decltype(npc_c)::value, ODD = decltype(odd_c)::value;
       constexpr bool OPEN = ((NPC - ODD) & 1) != 0, CLOSE = decltype(close_c)::value != 0;
       float acc[N / 2];
@@ -246,16 +256,23 @@ block_fused_kernel(const __grid_constant__ CUtensorMap tm_m_hi, const __grid_con
             const uint32_t b_hi = ptx::smem_u32(b_ring + (size_t)rb.slot * kBlkBStage);
             // tap j of the group: shifted by j image rows
             issue(n_c, ks_c, acc, a_hi0 + (uint32_t)(j * 16 * 128), b_hi, ch.ks_first, accumulate,
-                  last && !with_proj ? ra.slot : -1, rb.slot);
+                  last && !with_proj && !last_chain ? ra.slot : -1, rb.slot);
             accumulate = 1;
             rb.advance();
+            if constexpr (decltype(first_c)::value != 0) {
+              if (out_slot >= 0) {
+                if (wtid == 0) { ptx::bulk_wait_read0(); ptx::mbar_arrive(&ra.empty[out_slot]); }
+                out_slot = -1;
+              }
+            }
           }
           if (with_proj) {                       // the 1x1 projection of x reads the same stage (one group, centre tap)
             rb.wait_full();
             issue(BlkC<64>{}, ks_c, acc3, a_hi0, ptx::smem_u32(b_ring + (size_t)rb.slot * kBlkBStage), p.res.ks_first, 0u,
-                  ra.slot, rb.slot);
+                  last_chain ? -1 : ra.slot, rb.slot);
             rb.advance();
           }
+          if (last_chain) stage = ra.slot;
           ra.advance();
         }
       };
@@ -340,47 +357,60 @@ block_fused_kernel(const __grid_constant__ CUtensorMap tm_m_hi, const __grid_con
       // ---------- the chains, each followed by the aggregation steps its pieces of P complete
       agg_next = 0;
       if constexpr (LAYOUT == kBlkThreePaths) {
-        run_chain(BlkC<48>{}, BlkC<5>{}, BlkC<0>{}, BlkC<0>{}, p.chain[0], tidx, oy_tile, ox0, false);
-        run_chain(BlkC<48>{}, BlkC<5>{}, BlkC<1>{}, BlkC<0>{}, p.chain[1], tidx, oy_tile, ox0, false);
-        run_chain(BlkC<48>{}, BlkC<5>{}, BlkC<0>{}, BlkC<1>{}, p.chain[2], tidx, oy_tile, ox0, p.has_res_proj != 0);
+        run_chain(BlkC<1>{}, BlkC<48>{}, BlkC<5>{}, BlkC<0>{}, BlkC<0>{}, p.chain[0], tidx, oy_tile, ox0, false, false);
+        run_chain(BlkC<0>{}, BlkC<48>{}, BlkC<5>{}, BlkC<1>{}, BlkC<0>{}, p.chain[1], tidx, oy_tile, ox0, false, false);
+        run_chain(BlkC<0>{}, BlkC<48>{}, BlkC<5>{}, BlkC<0>{}, BlkC<1>{}, p.chain[2], tidx, oy_tile, ox0, p.has_res_proj != 0, true);
       } else {
-        run_chain(BlkC<64>{}, BlkC<8>{}, BlkC<0>{}, BlkC<0>{}, p.chain[0], tidx, oy_tile, ox0, false);
-        run_chain(BlkC<32>{}, BlkC<4>{}, BlkC<0>{}, BlkC<0>{}, p.chain[1], tidx, oy_tile, ox0, p.has_res_proj != 0);
+        run_chain(BlkC<1>{}, BlkC<64>{}, BlkC<8>{}, BlkC<0>{}, BlkC<0>{}, p.chain[0], tidx, oy_tile, ox0, false, false);
+        run_chain(BlkC<0>{}, BlkC<32>{}, BlkC<4>{}, BlkC<0>{}, BlkC<0>{}, p.chain[1], tidx, oy_tile, ox0, p.has_res_proj != 0, true);
       }
       wg::wait<0>();
       pend.release();
-      // ---------- output: relu(acc2 + bias) + residual, two channels per 8-column group and row
+      // ---------- output: relu(acc2 + bias) + residual, two channels per 8-column group and row, into the staging
+      // stage: row r of this warpgroup's 64 at r * 128 bytes of each plane, 16-byte chunk g8 at chunk g8 ^ (r & 7).
+      // For the identity residual those bytes hold x (path 2's 1x1 loaded channels 0..63 of these pixels), and each
+      // thread reads exactly the words it then overwrites
+      unsigned char* st_hi = a_ring + (size_t)stage * kBlkAStage;
+      unsigned char* st_lo = st_hi + kBlkAStage / 2;
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         const int row = row0 + 8 * h;
-        const int oy = oy_tile + (row >> 4), ox = ox0 + (row & 15);
-        if (oy >= p.H || ox >= p.W) continue;
-        const size_t pix = ((size_t)img * p.H + oy) * p.W + ox;
+        const bool inside = oy_tile + (row >> 4) < p.H && ox0 + (row & 15) < p.W;
 #pragma unroll
         for (int g8 = 0; g8 < 8; ++g8) {
           const int c = 8 * g8 + cq;
+          const uint32_t off = (uint32_t)(row * 128 + ((g8 ^ (row & 7)) << 4) + 2 * cq);
+          uint32_t* w_hi = reinterpret_cast<uint32_t*>(st_hi + off);
+          uint32_t* w_lo = reinterpret_cast<uint32_t*>(st_lo + off);
           float v0 = fmaxf(acc2[4 * g8 + 2 * h] + wb[c], 0.f);
           float v1 = fmaxf(acc2[4 * g8 + 2 * h + 1] + wb[c + 1], 0.f);
           if (p.has_res_proj) {
             v0 += acc3[4 * g8 + 2 * h] + wb[64 + c];
             v1 += acc3[4 * g8 + 2 * h + 1] + wb[64 + c + 1];
           } else {                               // identity residual: the block's input planes
-            const size_t off = pix * p.res_cstride + c;
-            const float2 r = ptx::join_hilo(*reinterpret_cast<const volatile uint32_t*>(p.res_hi + off),
-                                            *reinterpret_cast<const volatile uint32_t*>(p.res_lo + off));
+            const float2 r = ptx::join_hilo(*w_hi, *w_lo);
             v0 += r.x;
             v1 += r.y;
           }
           uint32_t hw, lw;
           ptx::split_hilo(v0, v1, hw, lw);
-          const size_t off = pix * p.out_cstride + c;
-          *reinterpret_cast<uint32_t*>(p.out_hi + off) = hw;
-          *reinterpret_cast<uint32_t*>(p.out_lo + off) = lw;
-          if (p.sum_part) { sacc[2 * g8] += v0; sacc[2 * g8 + 1] += v1; }
+          *w_hi = hw;
+          *w_lo = lw;
+          if (p.sum_part && inside) { sacc[2 * g8] += v0; sacc[2 * g8 + 1] += v1; }
         }
       }
+      ptx::fence_proxy_async();                  // the generic-proxy writes are visible to the TMA stores
+      ptx::bar_sync(1 + wg, 128);                // every row of this warpgroup's half is written
+      if (wtid == 0) {                           // image rows oy_tile + 4 wg .. + 3: the map clips the ragged edges
+        const uint32_t src = ptx::smem_u32(st_hi) + (uint32_t)(wg * 64 * 128);
+        ptx::tma_store_4d(&tm_o_hi, src, 0, ox0, oy_tile + kBlkStoreRows * wg, img);
+        ptx::tma_store_4d(&tm_o_lo, src + kBlkAStage / 2, 0, ox0, oy_tile + kBlkStoreRows * wg, img);
+        ptx::bulk_commit();
+      }
+      out_slot = stage;
     }
     if (p.sum_part && sum_img >= 0) flush_sums(sum_img);
+    if (wtid == 0) ptx::bulk_wait0();            // the last tile's outputs are written before the CTA exits
   }
 }
 }  // namespace stp3
@@ -403,6 +433,12 @@ extern "C" int stp3_block_fused_fwd(const stp3_block_desc* d, const void* mid_hi
                  "channel strides: mid / x multiples of 64, out a multiple of 16 and >= 64");
   STP3_CHECK_ARG(d->n_chain >= 1 && d->n_chain <= kBlkMaxChains, "1 .. 3 path chains");
   STP3_CHECK_ARG((d->has_res_proj != 0) == (res_bias != nullptr), "res_bias is given exactly when the block has a projection");
+  {
+    const stp3_block_chain& last = d->chain[d->n_chain - 1];
+    STP3_CHECK_ARG(last.src == 1 && last.n_taps == 1 && (d->has_res_proj || last.cin_off == 0),
+                   "the last chain is the 1x1 of x (its activation stage stages the output tile and, without a projection, "
+                   "holds the identity residual: x's channels 0..63)");
+  }
   auto al32 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 31) == 0; };
   STP3_CHECK_ARG(al32(y_hi) && al32(y_lo) && al32(x_hi) && al32(x_lo), "planes must be 32-byte aligned");
 
@@ -474,11 +510,8 @@ extern "C" int stp3_block_fused_fwd(const stp3_block_desc* d, const void* mid_hi
   // every descriptor check comes before the driver lookup: a bad descriptor is reported as such without a GPU
   if (!tmap_encode_fn()) return set_error(STP3_ECUDA, "cuTensorMapEncodeTiled is not available from the driver");
   p.hid_bias = hid_bias; p.img_bias = img_bias; p.res_bias = res_bias;
-  p.res_hi = static_cast<const __nv_bfloat16*>(x_hi); p.res_lo = static_cast<const __nv_bfloat16*>(x_lo);
-  p.res_cstride = d->x_cstride;
-  p.out_hi = static_cast<__nv_bfloat16*>(y_hi); p.out_lo = static_cast<__nv_bfloat16*>(y_lo); p.out_cstride = d->out_cstride;
 
-  CUtensorMap tm[4], tm_w;
+  CUtensorMap tm[4], tm_w, tm_o[2];
   const void* planes[4] = {mid_hi, mid_lo, x_hi, x_lo};
   for (int i = 0; i < 4; ++i) {
     const CUresult r = encode_act_5d(&tm[i], planes[i], i < 2 ? d->mid_cstride : d->x_cstride, d->W, d->H, d->T, d->B,
@@ -488,6 +521,11 @@ extern "C" int stp3_block_fused_fwd(const stp3_block_desc* d, const void* mid_hi
   {
     const CUresult r = encode_rows_2d(&tm_w, w, (long long)blk * 256, 8);
     if (r != CUDA_SUCCESS) return set_error(STP3_ECUDA, "cuTensorMapEncodeTiled(weights) failed: %d", (int)r);
+  }
+  void* outs[2] = {y_hi, y_lo};
+  for (int i = 0; i < 2; ++i) {       // channels [0, 64) of the output window; one box = one warpgroup's 4 x 16 pixels
+    const CUresult r = encode_out_4d(&tm_o[i], outs[i], d->out_cstride, 64, d->W, d->H, p.n_img, 16, kBlkStoreRows);
+    if (r != CUDA_SUCCESS) return set_error(STP3_ECUDA, "cuTensorMapEncodeTiled(output %d) failed: %d", i, (int)r);
   }
   auto kern = layout == kBlkThreePaths ? block_fused_kernel<kBlkThreePaths> : block_fused_kernel<kBlkDiagPair>;
   STP3_CUDA_OK(layout == kBlkThreePaths ? set_max_dynamic_smem<block_fused_kernel<kBlkThreePaths>>((int)BlkSmem::bytes)
@@ -506,7 +544,7 @@ extern "C" int stp3_block_fused_fwd(const stp3_block_desc* d, const void* mid_hi
   // -> pool_bias -> aspp_fused be resident at once, and such a chain was seen to stop making progress.  The kernel itself
   // still starts early behind its predecessor (griddepcontrol.wait before it reads what that predecessor wrote).
   STP3_CUDA_OK(launch_pdl(kPdlFused, kern, dim3(grid), dim3(kBlkThreads), BlkSmem::bytes, stream, tm[0], tm[1], tm[2],
-                          tm[3], tm_w, p));
+                          tm[3], tm_w, tm_o[0], tm_o[1], p));
   STP3_CUDA_OK(cudaGetLastError());
   if (col_sums) return launch_col_sum_reduce(p.sum_part, (int)grid * 8, p.n_img, col_sums, stream);
   return STP3_OK;
