@@ -91,18 +91,20 @@ hilo_to_f32_kernel(const __nv_bfloat16* __restrict__ hi, const __nv_bfloat16* __
   }
 }
 
-// sums[img][c] += sum over pixels of (hi+lo); grid (pixel chunks, n_img); block = cstride threads (<= 1024)
+// sums[img][c] += sum over pixels of (hi+lo); grid (pixel chunks, n_img); block = cstride threads (<= 1024).  A chunk
+// is summed in fp64 (exact for any 128 fp32 values within 2^22 of each other) and rounded once, so a sum carries one
+// rounding per chunk plus the fp32 atomics: a serial fp32 sum of 128 same-signed values loses several ulps of the total.
 __global__ void spatial_sum_kernel(const __nv_bfloat16* __restrict__ hi, const __nv_bfloat16* __restrict__ lo,
                                    int HW, int cstride, int px_per_block, float* __restrict__ sums) {
   const int img = blockIdx.y;
   const int c = threadIdx.x;
   const int p0 = blockIdx.x * px_per_block, p1 = min(HW, p0 + px_per_block);
-  float acc = 0.f;
+  double acc = 0.0;
   for (int px = p0; px < p1; ++px) {
     const size_t i = ((size_t)img * HW + px) * cstride + c;
-    acc += join_bf16(hi[i], lo[i]);
+    acc += (double)join_bf16(hi[i], lo[i]);
   }
-  atomicAdd(sums + (size_t)img * cstride + c, acc);
+  atomicAdd(sums + (size_t)img * cstride + c, (float)acc);
 }
 
 // The spatially constant branches (PyramidSpatioTemporalPooling temporal.py:375-423, ASPPPooling convolutions.py:

@@ -6,7 +6,9 @@ The launches are recorded from the model -- the dense wrappers and dense_train.t
 inputs cloned and what production wrote cloned too: the b4 trunk on 18 images and the b0 trunk at 224 x 480, the
 perceive forward with the fused and the unfused TemporalBlock tail, the stress shape, the encoder heads in eval, the
 Prediction model (tests/test_conv_contract_gpu.py predict_model at 40 x 56, and _predict_hl at 200 x 200), and
-train steps of the decoder, the DeepLab head, the TemporalModel and the encoder heads -- and built synthetically for what
+train steps of the decoder, the DeepLab head, the TemporalModel, the encoder heads and the trainable trunk (b0 and b4 on
+3 x 35 x 51 images, b4 on 6 x 224 x 480: stp3_se_gate asked for the gate with a one-row zero projection, to_hl at the
+trunk's channel counts) -- and built synthetically for what
 the model never passes (stem widths and pads, channel windows inside wider strides, one-pixel maps, squeeze-excite
 projections whose last chunk is exactly 64 or 128 wide, rounding edge cases of the hi/lo split, multi-slice pooling
 rows, 8-mod-16 upsample windows).  stp3_f32_to_plane (the one 16-bit plane of an autocast train step) is recorded from
@@ -54,10 +56,10 @@ ULP = 2.0 ** -24
 # measured over every launch of this file on an H100 80GB HBM3 (700 W power limit; table in DESIGN.md section 4).  The
 # squeeze-excite weights are held to their exact bound instead: 2^-17 (the split) + 2^-23 (the fp32 product) of
 # |W_proj gate| with the kernel's own gate, i.e. a ratio of 1.
-# stp3_spatial_sum adds one partial per 128-pixel chunk into each sum with float atomics, in no fixed order, so its
-# round-off grows like the square root of the chunk count: its bar is BARS["spatial_sum"] up to SSUM_CHUNKS chunks per
-# image (the most of the launches it was measured on: 1.2 ulps at most), and grows with sqrt(chunks / SSUM_CHUNKS)
-# beyond (the Prediction model: 4.3 ulps at 18 chunks, bar 10.6; 7.0 at 313 chunks, bar 44).
+# stp3_spatial_sum sums each 128-pixel chunk in fp64, rounds it once and adds the chunks into each sum with float
+# atomics, in no fixed order, so its round-off grows like the square root of the chunk count: its bar is
+# BARS["spatial_sum"] up to SSUM_CHUNKS chunks per image (1.5 ulps at most measured there), and grows with
+# sqrt(chunks / SSUM_CHUNKS) beyond (the Prediction model: 3.7 ulps at 18 chunks, bar 10.6; 9.9 at 313 chunks, bar 44).
 BARS = {"stem": 16, "dw": 10, "dw sums": 10, "se gate": 4, "se weights": 1.0, "spatial_sum": 5,
         "pool_bias": 4, "small_linear": 16, "upsample": 6}
 SSUM_CHUNKS = 4
@@ -145,14 +147,14 @@ def dw_case(xh, xl, w, b, k, s, pt, pl, Ho, Wo, ocs, sums, tag):
                            ocs=ocs, sums=bool(sums)), tag, features=f)
 
 
-def se_case(sums, C, inv_hw, w_r, b_r, w_e, b_e, w_p, tag):
+def se_case(sums, C, inv_hw, w_r, b_r, w_e, b_e, w_p, tag, extra=()):
     n, ss = sums.shape
     R_, cout = w_r.shape[0], w_p.shape[0]
     if ss > C:
         sums = sums.clone()
         sums[:, C:] = NAN
     last = cout - (cout - 1) // 128 * 128
-    f = {"se", f"se last chunk {128 if last > 64 else 64}", f"se {-(-cout // 128)} chunks"}
+    f = {"se", f"se last chunk {128 if last > 64 else 64}", f"se {-(-cout // 128)} chunks"} | set(extra)
     if ss > C:
         f.add("se sums_stride > C")
     if C % 64:
@@ -189,10 +191,10 @@ def to_f32_case(hi, lo, n, H, W, c_off, C, tag):
     return Case("to_f32", dict(hi=hi, lo=lo, n=n, H=H, W=W, cs=cs, c_off=c_off, C=C), tag, features=f)
 
 
-def ssum_case(hi, lo, n, HW, tag):
+def ssum_case(hi, lo, n, HW, tag, extra=()):
     cs = hi.shape[-1]
     return Case("ssum", dict(hi=hi.reshape(n, HW, cs), lo=lo.reshape(n, HW, cs), n=n, HW=HW, cs=cs), tag,
-                features={"spatial_sum"} | ({"spatial_sum ragged chunk"} if HW % 128 else set()))
+                features={"spatial_sum"} | ({"spatial_sum ragged chunk"} if HW % 128 else set()) | set(extra))
 
 
 def pool_case(sums, T, C, inv_hw, temporal, cv, W1, b1, W2, bias, prior, acc, tag):
@@ -535,11 +537,13 @@ class Recorder:
     def _se_gate(self, orig):
         def f(sums, hw, C, w_r, b_r, w_e, b_e, w_proj, gate=None):
             sc = sums.clone()
+            # the train-mode trunk asks for the gate and passes one zero projection row it does not use
+            extra = ("se gate output, one-row projection",) if gate is not None and w_proj.shape[0] == 1 else ()
             if gate is None:
                 gate = torch.empty((sums.shape[0], C), dtype=torch.float32, device=sums.device)
             w_img = orig(sums, hw, C, w_r, b_r, w_e, b_e, w_proj, gate=gate)
             self._add(se_case(sc, C, 1.0 / hw, w_r.clone(), b_r.clone(), w_e.clone(), b_e.clone(), w_proj.clone(),
-                              f"se C{C} R{w_r.shape[0]} cout{w_proj.shape[0]} n{sums.shape[0]}"),
+                              f"se C{C} R{w_r.shape[0]} cout{w_proj.shape[0]} n{sums.shape[0]}", extra),
                       {"gate": gate.reshape(-1), "w_img": w_img.reshape(-1)})
             return w_img
         return f
@@ -564,7 +568,8 @@ class Recorder:
                 self._add(to_plane_case(xs, 1, N, C, H, W, out.hi.shape[-1], mode, f"to_hl {tuple(xs.shape)} {mode}",
                                         ("to_hl plane",)), {"plane": out.hi.reshape(-1)})
                 return out
-            self._add(to_hilo_case(xs, 1, N, C, H, W, out.hi.shape[-1], f"to_hl {tuple(xs.shape)}", ("to_hl",)),
+            extra = ("to_hl",) + (("to_hl C % 64 != 0",) if C % 64 else ()) + (("to_hl C > 512",) if C > 512 else ())
+            self._add(to_hilo_case(xs, 1, N, C, H, W, out.hi.shape[-1], f"to_hl {tuple(xs.shape)}", extra),
                       {"hi": out.hi.reshape(-1), "lo": out.lo.reshape(-1)})
             return out
         return f
@@ -701,6 +706,15 @@ def rec_amp(mode, step, *args):
     return r.cases
 
 
+def rec_train_trunk(name):
+    """a train step of the trainable trunk (tests/test_train_contract_gpu.py trunk_step): stp3_se_gate asked for the
+    gate with a one-row zero projection, and to_hl of the projections' and expand convolutions' gradients"""
+    from tests import test_train_contract_gpu as TC
+    with Recorder(f"train {name}") as r:
+        TC.trunk_step(*TC.TRUNK_STEPS[name])
+    return r.cases
+
+
 def rec_train(name, fn, *args):
     """a train step of the model of tests/test_train_contract_gpu.py (its own recorder runs too, unused)"""
     from tests import test_train_contract_gpu as TC
@@ -800,6 +814,14 @@ def synth_hilo():
     for i, (n, HW, cs) in enumerate([(3, 35, 8), (1, 1, 64), (2, 300, 1024), (4, 129, 200)]):
         hi, lo = planes_of(rnd(n, HW, 1, cs, seed=1000 + i, scale=4.0), cs)
         cases.append(ssum_case(hi, lo, n, HW, f"n{n} HW{HW} cs{cs}"))
+    # 1 at the first pixel, then 299 terms of 0.75 ulp(1) / 2: an fp32 running sum drops every one of them (95 ulps of
+    # the total in the first chunk), a chunk summed exactly loses at most one rounding
+    x = torch.full((2, 300, 1, 64), 1.5 * 2.0 ** -25, device=DEV)
+    x[:, 0] = 1.0
+    x[1] *= -1.0
+    hi, lo = planes_of(x, 64)
+    cases.append(ssum_case(hi, lo, 2, 300, "n2 HW300 cs64: small terms after a large one",
+                           ("spatial_sum small terms after a large one",)))
     return cases
 
 
@@ -885,6 +907,9 @@ SOURCES = {
     "synthetic_hilo": synth_hilo,
     "synthetic_small": synth_small,
     "synthetic_plane": synth_plane,
+    "train_trunk_b0_35x51": lambda: rec_train_trunk("trunk_b0_35x51"),
+    "train_trunk_b4_35x51": lambda: rec_train_trunk("trunk_b4_35x51"),
+    "train_trunk_b4_224x480": lambda: rec_train_trunk("trunk_b4_224x480"),
 }
 for _m, _nm in ((torch.float16, "fp16"), (torch.bfloat16, "bf16")):
     SOURCES.update({
@@ -900,6 +925,7 @@ def run_source(name):
     if name in _RUNS:
         return _RUNS[name]
     t0 = time.time()
+    torch.cuda.reset_peak_memory_stats()
     cases = SOURCES[name]()
     assert cases, f"{name}: no launch recorded"
     rows = []
@@ -908,7 +934,8 @@ def run_source(name):
         rows.append(dict(kind=c.kind, tag=c.tag, features=set(c.features), res=r, ok=passed(r)))
     del cases
     torch.cuda.empty_cache()
-    print(f"\n{name}: {len(rows)} launches in {time.time() - t0:.1f} s")
+    print(f"\n{name}: {len(rows)} launches in {time.time() - t0:.1f} s, peak "
+          f"{torch.cuda.max_memory_allocated() / 2 ** 30:.2f} GiB allocated")
     _RUNS[name] = rows
     return rows
 
@@ -930,7 +957,7 @@ def test_aux_launches_against_the_fp64_contract(name):
 
 
 REQUIRED = (["recorded"] + [f"recorded {k}" for k in ("stem", "dw", "se", "to_hilo", "to_f32", "ssum", "pool", "lin", "up")]
-            + ["to_hl", "to_hl plane", "recorded to_plane"]
+            + ["to_hl", "to_hl plane", "recorded to_plane", "to_hl C % 64 != 0", "to_hl C > 512"]
             + [f"f32_to_plane {k}" for k in ("f16", "bf16", "NCHW", "NHWC", "cp > C", "several channel tiles",
                                               "edge values")]
             + [f"stem pad ({a},{b})" for a in range(3) for b in range(3)]
@@ -942,10 +969,10 @@ REQUIRED = (["recorded"] + [f"recorded {k}" for k in ("stem", "dw", "se", "to_hi
                "dw pad_t != pad_l", "dw Ho or Wo 1", "dw ragged tiles"]
             + ["se last chunk 64", "se last chunk 128", "se 1 chunks", "se 2 chunks", "se 3 chunks",
                "se sums_stride > C", "se C % 64 != 0", "se images 1", "se images 73", "se C 8", "se C 65", "se C 4096",
-               "se R 1", "se R 1024"]
+               "se R 1", "se R 1024", "se gate output, one-row projection"]
             + ["f32_to_hilo NCHW", "f32_to_hilo NHWC", "f32_to_hilo cp > C", "f32_to_hilo ragged tiles",
                "f32_to_hilo edge values", "hilo_to_f32", "hilo_to_f32 window", "spatial_sum",
-               "spatial_sum ragged chunk"]
+               "spatial_sum ragged chunk", "spatial_sum small terms after a large one"]
             + ["pool_bias temporal", "pool_bias temporal T 1", "pool_bias n_const", "pool_bias n_const = C - 1",
                "pool_bias bias", "pool_bias bias NULL", "pool_bias accumulate", "pool_bias 4 row slices",
                "pool_bias R 1", "pool_bias C 1", "pool_bias CO % 4 != 0"]

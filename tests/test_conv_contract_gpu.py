@@ -6,7 +6,10 @@ are the production ones: frame windows, trimmed K ranges, channel windows of con
 output-size overrides of the input-gradient phases, fused heads, column sums.  The Prediction model adds K windows that
 start inside a buffer (cin_off 64 of the conv-GRU cell and of the Bottleblock's second 7 x 7 launch), 49-tap layers and
 the decoder over 7 frames
-(predict_model at 40 x 56 with both gate sets, and each distinct convolution of _predict_hl at 200 x 200).  Each
+(predict_model at 40 x 56 with both gate sets, and each distinct convolution of _predict_hl at 200 x 200).  The
+trainable trunk's train steps (tests/test_train_contract_gpu.py trunk_step) add the expand convolutions' 256-column
+chunks, the projections and their input gradients in 256-channel chunks, at channel counts that are not multiples of
+64; at 224 x 480 only one call per descriptor is replayed under every tiling, the repeats under (0, 0).  Each
 recorded call is replayed with
 tune = (0, 0) (the kernel's own heuristics: graph capture, STP3_CONV_AUTOTUNE=0) and with every candidate of
 dense.tune_candidates, into outputs pre-filled with a sentinel.  Checked per replay:
@@ -30,6 +33,7 @@ the fp32 output's guard untouched; the replay of the tiling production forced bi
 import ast
 import inspect
 import os
+import time
 from dataclasses import dataclass
 from typing import Optional
 
@@ -79,6 +83,8 @@ class Call:
     kw: dict                                  # dense.conv keywords; output tensors replaced by their specs
     tag: str = ""
     prod: Optional[tuple] = None              # one-plane calls: (tiling production forced, its out_f32)
+    chunk: Optional[tuple] = None             # trunk calls: (dense_train function, chunk index, chunks in the call)
+    all_tilings: bool = True                  # False: replayed under (0, 0) only (a repeat of a replayed descriptor)
 
     @property
     def plane(self):
@@ -320,6 +326,46 @@ def rec_decoder_full():
     return r.calls
 
 
+TRUNK_CONVS = ("conv_raw", "conv1x1_raw", "conv1x1_dgrad", "conv_dgrad")
+
+
+def rec_trunk(name):
+    """One train step of the trainable trunk (tests/test_train_contract_gpu.py trunk_step): the expand convolutions in
+    chunks of at most 256 columns (conv1x1_raw), the projections (conv_raw), their input gradients in chunks of at most
+    256 input channels (conv1x1_dgrad) and the expand convolutions' input gradients (conv_dgrad).  Each call is marked
+    with the dense_train function that made it and its chunk.  At 224 x 480 only the first call of each descriptor is
+    replayed under every tiling, the others under (0, 0)."""
+    from stp3_b200 import dense_train
+    r = Recorder(f"trunk train {name}")
+    mp = pytest.MonkeyPatch()
+
+    def marked(fn_name, fn):
+        def f(*a, **kw):
+            i0 = len(r.calls)
+            out = fn(*a, **kw)
+            new = r.calls[i0:]
+            for j, c in enumerate(new):          # the outermost function marks last: conv1x1_raw over its conv_raw
+                c.chunk = (fn_name, j, len(new))
+            return out
+        return f
+    for fn_name in TRUNK_CONVS:
+        mp.setattr(dense_train, fn_name, marked(fn_name, getattr(dense_train, fn_name)))
+    try:
+        with r:
+            TC.trunk_step(*TC.TRUNK_STEPS[name])
+    finally:
+        mp.undo()
+    assert all(c.chunk is not None for c in r.calls), "a trunk convolution outside the marked dense_train functions"
+    if name.endswith("224x480"):
+        seen = set()
+        for c in r.calls:
+            key = (tuple(c.pc.taps), c.pc.cin_p, c.pc.bn, c.pc.cout, c.pc.stride, c.pc.k_lo, c.pc.k_hi, c.x.hi.shape,
+                   c.x.c, repr(sorted((k, v) for k, v in c.kw.items() if k not in ("residual", "img_bias", "head"))))
+            c.all_tilings = key not in seen
+            seen.add(key)
+    return r.calls
+
+
 def _rnd(*shape, seed, scale=1.0):
     g = torch.Generator().manual_seed(seed)
     return ((torch.rand(*shape, generator=g) * 2 - 1) * scale).to(DEV)
@@ -461,6 +507,7 @@ SOURCES = {
     "predict_200x200": rec_predict_200,
     "synthetic": rec_synthetic,
 }
+SOURCES.update({_nm: (lambda n=_nm: rec_trunk(n)) for _nm in TC.TRUNK_STEPS})
 for _m in PLANE_NAMES:
     SOURCES.update({f"amp_{nm}_{PLANE_NAMES[_m]}": (lambda m=_m, st=st, a=a: rec_amp(m, st, *a))
                     for nm, (st, a) in AMP_STEPS.items()})
@@ -672,6 +719,14 @@ def features(call: Call, cfg, t: Optional[dict] = None):
         f.add("taps > 27")
     if Tt == 7:
         f.add("T_total 7")
+    if call.chunk is not None:
+        fn, j, n = call.chunk
+        if fn == "conv1x1_raw" and n > 1 and j == n - 1:
+            f.add("trunk: last chunk of a forward over 256 columns")
+        if fn == "conv1x1_dgrad" and n > 1:
+            f.add("trunk: input-gradient chunk of over 256 input channels")
+        if call.x.c % 64 or pc.cout % 64:
+            f.add("trunk: channels not a multiple of 64")
     f.add(f"res_mode {0 if kw['residual'] is None else 2 if kw.get('res_after_act') else 1}")
     for k, coff in (("out", "out_coff"), ("out2", "out2_coff")):
         if kw[k] is not None:
@@ -700,7 +755,9 @@ REQUIRED = ["width 64", "width 128", "width 256 (two launches)", "STACK", "FULLK
             "streamed (+4)", "tap group > 1", "stride 2", "causal taps at frame 0", "frame window", "out_hw override",
             "res_mode 0", "res_mode 1", "res_mode 2", "vector store", "scalar store", "vector residual",
             "scalar residual", "hi/lo output", "f32 NCHW output + sigmoid", "f32 NHWC output", "fused head", "out2",
-            "col_sums", "img_bias", "partial n_store", "cin_off > 0", "taps > 27", "T_total 7"]
+            "col_sums", "img_bias", "partial n_store", "cin_off > 0", "taps > 27", "T_total 7",
+            "trunk: last chunk of a forward over 256 columns", "trunk: input-gradient chunk of over 256 input channels",
+            "trunk: channels not a multiple of 64"]
 
 
 # ------------------------------------------------------------------------------------------------ driver
@@ -711,6 +768,8 @@ def run_source(name):
     """Record the source's calls, replay each under (0, 0) and every tuning candidate; cached per module."""
     if name in _RUNS:
         return _RUNS[name]
+    t0 = time.time()
+    torch.cuda.reset_peak_memory_stats()
     calls = SOURCES[name]()
     assert calls, f"{name}: no convolution recorded"
     rows = []
@@ -718,7 +777,7 @@ def run_source(name):
         exact, model, scale = references(call)
         plane = call.plane is not None
         outs = {}
-        for cfg in [(0, 0)] + dense.tune_candidates(call.pc):
+        for cfg in [(0, 0)] + (dense.tune_candidates(call.pc) if call.all_tilings else []):
             got, same, untouched, bufs = _replay(call, cfg)
             assert set(got) == set(exact), (set(got), set(exact))
             e_x = max(float((got[k] - exact[k].reshape(got[k].shape)).abs().max()) / scale[k] for k in got)
@@ -748,7 +807,10 @@ def run_source(name):
                 for r in rows[-len(outs):]:
                     r["production"] = torch.equal(bufs["out_f32"], prod)
         del exact, model, outs
+    del calls
     torch.cuda.empty_cache()
+    print(f"\n{name}: {len(rows)} replays in {time.time() - t0:.1f} s, peak "
+          f"{torch.cuda.max_memory_allocated() / 2 ** 30:.2f} GiB allocated")
     _RUNS[name] = rows
     return rows
 

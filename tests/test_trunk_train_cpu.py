@@ -188,3 +188,38 @@ def test_new_entry_points_refuse_bad_arguments():
     refused(L.stp3_se_bwd(FAKE, FAKE, FAKE, 2, 8, 0.5, FAKE, FAKE, 2, FAKE, FAKE, FAKE, None, FAKE, None), "null pointer")
     refused(L.stp3_se_bwd(FAKE, FAKE, FAKE, 2, 5000, 0.5, FAKE, FAKE, 2, FAKE, FAKE, FAKE, FAKE, FAKE, None),
             "bad dimensions")
+
+
+# rows of the three partitioned reductions around every boundary of tests/trunk_train_reference.py's partition: one
+# part, exact multiples of rows_per_part and one past them, the part cap and one past it, and the trunk's own sizes
+_ROWS = sorted({1, 2, 255, 256, 257, 425, 511, 512, 513, 1023, 1024, 1025, 1275, 40320, 65535, 65536, 65537, 131071,
+                131072, 131073, 161280, 262143, 262144, 262145, 282204, 10 ** 6})
+
+
+def test_partition_mirror_matches_the_library_scratch_queries():
+    """the scratch queries are host-only and size one fp64 partial per part, so they give the library's part counts"""
+    L = _lib_loaded()
+    for rows in _ROWS:
+        for n_img, Ho, Wo in ((1, 1, rows), (1, rows, 1)) + (((rows // 6 // 7, 7, 1), (6, rows // 6, 1))
+                                                             if rows % 42 == 0 else ()):
+            for cout in (1, 48, 64):
+                assert L.stp3_effnet_stem_wgrad_scratch_bytes(n_img, Ho, Wo, cout) == \
+                    TR.stem_wgrad_parts(n_img, Ho, Wo) * cout * 27 * 8, (rows, cout)
+            for k, C in ((3, 40), (5, 24)):
+                d = _dw(n_img=n_img, H=Ho, W=Wo, Ho=Ho, Wo=Wo, k=k, stride=1, C=C, in_cstride=C + 8, out_cstride=C)
+                assert L.stp3_dw_wgrad_scratch_bytes(d) == TR.dw_wgrad_parts(n_img, Ho, Wo) * k * k * C * 8, (rows, k)
+        for n_img, C in ((1, 8), (7, 40)):
+            assert L.stp3_image_channel_dot_scratch_bytes(n_img, rows, C) == n_img * TR.dot_parts(rows) * C * 8, rows
+
+
+def test_partitions_of_the_trunk_steps():
+    """the part counts the trunk-train contract's sources reach (stem output 17 x 25 at 35 x 51, 112 x 240 at 224 x 480)"""
+    assert TR.stem_wgrad_parts(3, 17, 25) == 2 and TR.dot_parts(17 * 25) == 2 and TR.dw_wgrad_parts(3, 17, 25) == 3
+    assert TR.part_features("dw", 3 * 17 * 25, 3, 512) == {"dw several parts"}
+    assert TR.stem_wgrad_parts(6, 112, 240) == 158
+    assert TR.part_features("stem", 6 * 112 * 240, 158, 1024) == {"stem several parts", "stem ragged last part"}
+    assert TR.dw_wgrad_parts(6, 112, 240) == 256
+    assert TR.part_features("dw", 6 * 112 * 240, 256, 512) == {"dw several parts", "dw part cap"}
+    assert TR.dw_wgrad_parts(6, 56, 120) == 79
+    assert TR.part_features("dw", 6 * 56 * 120, 79, 512) == {"dw several parts", "dw ragged last part"}
+    assert TR.part_features("dot", 282204, 256, 256) == {"dot several parts", "dot ragged last part", "dot part cap"}

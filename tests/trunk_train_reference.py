@@ -86,3 +86,42 @@ def tape_elements(net, H, W) -> int:
         n += mult * e
     return n
 
+
+
+# ------------------------------------------------------------------------------------------------ reduction partitions
+# The trunk's partitioned reductions (csrc/trunk_train.cu): the stem and depthwise weight gradients and
+# stp3_image_channel_dot split their rows into parts of ceil(rows / parts) consecutive rows, one CTA (row of CTAs) per
+# part, and add the parts' fp64 partials in part order.  parts = ceil(rows / rows_per_part), at least 1 and at most
+# TR_MAX_PARTS; at the cap the parts grow past rows_per_part, and trailing parts may be empty.
+TR_MAX_PARTS = 256
+
+
+def tr_parts(rows: int, rows_per_part: int) -> int:
+    return min(max(-(-rows // rows_per_part), 1), TR_MAX_PARTS)
+
+
+def stem_wgrad_parts(n_img: int, Ho: int, Wo: int) -> int:
+    """parts of stp3_effnet_stem_wgrad over its n_img * Ho * Wo output pixels"""
+    return tr_parts(n_img * Ho * Wo, 1024)
+
+
+def dw_wgrad_parts(n_img: int, Ho: int, Wo: int) -> int:
+    """parts of stp3_dw_wgrad over its n_img * Ho * Wo output pixels"""
+    return tr_parts(n_img * Ho * Wo, 512)
+
+
+def dot_parts(hw: int) -> int:
+    """parts of stp3_image_channel_dot over the hw pixels of each image"""
+    return tr_parts(hw, 256)
+
+
+def part_features(name: str, rows: int, parts: int, rows_per_part: int) -> set:
+    """the partition features of one launch: one part, several parts, a ragged last part (the last non-empty part
+    shorter than the others), the part cap (more than TR_MAX_PARTS * rows_per_part rows)"""
+    per = -(-rows // parts)
+    f = {f"{name} one part" if parts == 1 else f"{name} several parts"}
+    if parts > 1 and rows % per:
+        f.add(f"{name} ragged last part")
+    if rows > TR_MAX_PARTS * rows_per_part:
+        f.add(f"{name} part cap")
+    return f
