@@ -717,6 +717,65 @@ int stp3_hl_copy(const stp3_hl_slot* src, const stp3_hl_slot* dst, int B, int T,
 int stp3_hl_broadcast(const float* vec, int vstride, const stp3_hl_slot* dst, int B, int T, long long HW, int C,
                       void* stream);
 
+/* ============================================================================================================
+ * Eval-mode planning (stp3/models/planning_model.py, stp3/cost.py): the cost of every sampled trajectory at every
+ * future frame, the choice of the cheapest one within a command window, and the GRU refinement of that choice.
+ *
+ * stp3_plan_desc describes the call.  The footprints are the integer (row, col) cells of the ego rectangle that
+ * BaseCost.get_origin_points rasterises (cost.py:68-81), without and with the safety margin lambda; both are full
+ * rectangles [r0, r1] x [c0, c1] of absolute BEV cells (rows and columns >= 0).
+ *
+ * Layouts (fp32 unless noted; B samples, N candidates, T future frames, H x W BEV cells):
+ *   lane, drivable  (B, n_hd, H, W): the lane-divider and drivable-area channels of the hd map -- two logits per
+ *                   element (n_hd 2: softmax, channel 1) or the raw map (n_hd 1)
+ *   drv_map         (B, H, W): drivable probability, 0 where it is < 0.5 (the raw channel when n_hd is 1)
+ *   dang_map        (B, H, W) uint8: 1 where drv_map is 0 (Rule's dangerous area)
+ *   lane_cost       (B, H, W): LR_divider's cost at every cell, lrdivider * (L - d)^2 where the distance d to the
+ *                   nearest lane cell is <= L = lane_dist, else 0
+ *   trajs           (B, N, T, traj_c): x, y (and a third component the cost ignores) of every candidate
+ *   occupancy       (B, T, H, W) uint8 0 / 1: the predicted vehicle-or-pedestrian occupancy
+ *   cost_volume     (B, T, H, W)
+ *   target_points   (B, 2)
+ *   cost_fc         (B, N) and cost_fo (B, N, T): Cost_Function.forward's two results
+ *   windows         (B, 2) int32 device array of (first candidate, count) per sample; windows_host the same values
+ *                   on the host (checked before the launch)
+ *   h0              (B, G): the reduced front-camera features, the GRU's initial state
+ *   w_ih (3G, 6), b_ih (3G), w_hh_t (G, 3G) = GRUCell.weight_hh transposed, b_hh (3G), gate order (r, z, n);
+ *   w1_t (G, G) = decoder[0].weight transposed, b1 (G), w2 (2, G), b2 (2)
+ *   out_traj        (B, T, 3): the refined trajectory, third column 0
+ *   selected        (B) int32: index into trajs of the candidate chosen in the sample's window (lowest on ties)
+ * No atomics, and nothing is read back to the host: repeated calls are bitwise equal. */
+typedef struct stp3_plan_desc {
+  int B, N, T;                  /* N a multiple of 3; 1 <= T <= 16 */
+  int H, W;                     /* BEV rows x columns (bev_dimension[0], [1]); H == W */
+  float dx[2], bx[2];           /* BaseCost.dx, BaseCost.bx (fp32) */
+  int fp0[4];                   /* footprint at lambda 0: first row, last row, first column, last column */
+  int fp1[4];                   /* footprint at lambda: the same */
+  float safety, headway, lrdivider, comfort, progress, volume;   /* COST_FUNCTION factors */
+  float rule;                   /* Rule.factor (5) */
+  float safety_w[2];            /* SafetyCost.w */
+  float headway_dist;           /* HeadwayCost.L, metres added to y (10) */
+  float lane_dist;              /* LR_divider.L, metres (1) */
+  int n_hd;                     /* 1 or 2 channels per hd-map element */
+  int traj_c;                   /* components per trajectory point: 2 or 3 */
+  int G;                        /* GRU state size: a multiple of 32, at most 512 (stp3_plan_refine) */
+} stp3_plan_desc;
+
+/* One thread per (sample, cell): drv_map, dang_map and lane_cost */
+int stp3_plan_maps(const stp3_plan_desc* desc, const float* lane, const float* drivable, float* drv_map,
+                   uint8_t* dang_map, float* lane_cost, void* stream);
+/* One warp per (sample, candidate, frame): cost_fc and cost_fo, every term clamped as Cost_Function.forward does */
+int stp3_plan_cost(const stp3_plan_desc* desc, const float* trajs, const uint8_t* occupancy, const float* cost_volume,
+                   const float* target_points, const float* drv_map, const uint8_t* dang_map, const float* lane_cost,
+                   float* cost_fc, float* cost_fo, void* stream);
+/* One CTA per sample: argmin of cost_fc + sum_t cost_fo over the window, then T GRUCell(6, G) steps with the
+ * Linear(G, G) -> ReLU -> Linear(G, 2) decoder */
+int stp3_plan_refine(const stp3_plan_desc* desc, const int32_t* windows_host, const int32_t* windows,
+                     const float* trajs, const float* cost_fc, const float* cost_fo, const float* h0,
+                     const float* target_points, const float* w_ih, const float* b_ih, const float* w_hh_t,
+                     const float* b_hh, const float* w1_t, const float* b1, const float* w2, const float* b2,
+                     float* out_traj, int32_t* selected, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

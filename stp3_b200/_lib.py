@@ -94,6 +94,17 @@ class HlSlot(ctypes.Structure):
 
 _HS = ctypes.POINTER(HlSlot)
 
+
+class PlanDesc(ctypes.Structure):
+    """Mirror of stp3_plan_desc (include/stp3_b200.h)."""
+    _fields_ = [("B", _I), ("N", _I), ("T", _I), ("H", _I), ("W", _I), ("dx", _F * 2), ("bx", _F * 2),
+                ("fp0", _I * 4), ("fp1", _I * 4), ("safety", _F), ("headway", _F), ("lrdivider", _F), ("comfort", _F),
+                ("progress", _F), ("volume", _F), ("rule", _F), ("safety_w", _F * 2), ("headway_dist", _F), ("lane_dist", _F),
+                ("n_hd", _I), ("traj_c", _I), ("G", _I)]
+
+
+_PD = ctypes.POINTER(PlanDesc)
+
 SIGNATURES = {
     "stp3_abi_version": (_I, []),
     "stp3_conv_col_sums_scratch_bytes": (_SZ, [_I, _I]),
@@ -183,6 +194,10 @@ SIGNATURES = {
     "stp3_maxpool2_pad": (_I, [_HS, _HS, _I, _I, _I, _I, _I, _V]),
     "stp3_hl_copy": (_I, [_HS, _HS, _I, _I, _LL, _I, _V]),
     "stp3_hl_broadcast": (_I, [_V, _I, _HS, _I, _I, _LL, _I, _V]),
+    # eval-mode planning
+    "stp3_plan_maps": (_I, [_PD, _V, _V, _V, _V, _V, _V]),
+    "stp3_plan_cost": (_I, [_PD, _V, _V, _V, _V, _V, _V, _V, _V, _V, _V]),
+    "stp3_plan_refine": (_I, [_PD, _V, _V, _V, _V, _V, _V, _V, _V, _V, _V, _V, _V, _V, _V, _V, _V, _V, _V]),
 }
 
 

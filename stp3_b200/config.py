@@ -53,7 +53,10 @@ _DEFAULTS = {
     "INSTANCE_SEG": {"ENABLED": True},
     "INSTANCE_FLOW": {"ENABLED": True},
     "PROBABILISTIC": {"ENABLED": True, "METHOD": 'GAUSSIAN'},
-    "PLANNING": {"ENABLED": True, "GRU_STATE_SIZE": 256, "SAMPLE_NUM": 600},
+    "PLANNING": {"ENABLED": True, "GRU_STATE_SIZE": 256, "SAMPLE_NUM": 600, "COMMAND": ['LEFT', 'FORWARD', 'RIGHT']},
+    "EGO": {"WIDTH": 1.85, "HEIGHT": 4.084},
+    "COST_FUNCTION": {"SAFETY": 0.1, "LAMBDA": 1., "HEADWAY": 1., "LRDIVIDER": 10., "COMFORT": 0.1, "PROGRESS": 0.5,
+                      "VOLUME": 100.},
 }
 
 # stp3/configs/nuscenes/Perception.yml
@@ -77,12 +80,43 @@ PREDICTION_OVERRIDES = {
     "PROBABILISTIC": {"ENABLED": True, "METHOD": 'GAUSSIAN'}, "PLANNING": {"ENABLED": False},
 }
 
+# stp3/configs/nuscenes/Planning.yml (apply with get_cfg(PLANNING_OVERRIDES, perception=False))
+PLANNING_OVERRIDES = {
+    "TIME_RECEPTIVE_FIELD": 3, "N_FUTURE_FRAMES": 6,
+    "LIFT": {"GT_DEPTH": False},
+    "MODEL": {"ENCODER": {"NAME": 'efficientnet-b4', "USE_DEPTH_DISTRIBUTION": True},
+              "TEMPORAL_MODEL": {"NAME": 'temporal_block', "INPUT_EGOPOSE": True}, "BN_MOMENTUM": 0.05},
+    "SEMANTIC_SEG": {"PEDESTRIAN": {"ENABLED": True}, "HDMAP": {"ENABLED": True}},
+    "INSTANCE_SEG": {"ENABLED": False}, "INSTANCE_FLOW": {"ENABLED": False},
+    "PROBABILISTIC": {"ENABLED": True, "METHOD": 'GAUSSIAN'},
+    "PLANNING": {"ENABLED": True, "SAMPLE_NUM": 1800},
+    "COST_FUNCTION": {"SAFETY": 1., "HEADWAY": 1., "LRDIVIDER": 10., "COMFORT": 0.1, "PROGRESS": 0.5, "VOLUME": 100.},
+}
+
+# stp3/configs/carla/Planning.yml (apply with get_cfg(PLANNING_CARLA_OVERRIDES, perception=False))
+PLANNING_CARLA_OVERRIDES = {
+    "TIME_RECEPTIVE_FIELD": 3, "N_FUTURE_FRAMES": 4,
+    "IMAGE": {"FINAL_DIM": (256, 256)},
+    "LIFT": {"X_BOUND": [-20.0, 20.0, 0.2], "Y_BOUND": [-20.0, 20.0, 0.2], "GT_DEPTH": False},
+    "EGO": {"WIDTH": 2.12, "HEIGHT": 4.90},
+    "MODEL": {"ENCODER": {"NAME": 'efficientnet-b4', "USE_DEPTH_DISTRIBUTION": True},
+              "TEMPORAL_MODEL": {"NAME": 'temporal_block', "INPUT_EGOPOSE": True}, "BN_MOMENTUM": 0.05},
+    "SEMANTIC_SEG": {"PEDESTRIAN": {"ENABLED": True}, "HDMAP": {"ENABLED": True}},
+    "INSTANCE_SEG": {"ENABLED": False}, "INSTANCE_FLOW": {"ENABLED": False},
+    "PROBABILISTIC": {"ENABLED": True, "METHOD": 'GAUSSIAN'},
+    "PLANNING": {"ENABLED": True, "GRU_STATE_SIZE": 128, "SAMPLE_NUM": 2400},
+    "COST_FUNCTION": {"SAFETY": 1., "HEADWAY": 1., "LRDIVIDER": 10., "COMFORT": 1., "PROGRESS": 1., "VOLUME": 100.},
+}
+
 
 def get_cfg(overrides=None, perception=True):
-    """Reference defaults (+ the nuScenes perception YAML when perception=True) + overrides."""
+    """Reference defaults (+ the nuScenes perception YAML when perception=True) + overrides.  COST_FUNCTION's values
+    become floats, as the reference's get_cfg makes them (config.py:180-181)."""
     cfg = CfgNode.wrap(copy.deepcopy(_DEFAULTS))
     if perception:
         cfg.merge(PERCEPTION_OVERRIDES)
     if overrides:
         cfg.merge(overrides)
+    for k in list(cfg.COST_FUNCTION):
+        cfg.COST_FUNCTION[k] = float(cfg.COST_FUNCTION[k])
     return cfg

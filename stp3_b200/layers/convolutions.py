@@ -8,7 +8,8 @@
                    runs in train() (batch statistics, dropout, autograd; dense_train.py).
   UpsamplingConcat : bilinear x2 of the coarse map into its channel window of the concat tensor, two 3x3 conv/BN/ReLU;
                    also in train().
-  Bottleneck / LayerNorm / Block / Bottleblock : the prediction stage's blocks, eval only (DESIGN.md §3.16).
+  Bottleneck / LayerNorm / Block / Bottleblock : the prediction stage's blocks, eval only (DESIGN.md §3.16); the
+                   planner's channel reduction uses Bottleneck too (§3.17).
 """
 import os
 from collections import OrderedDict
@@ -546,33 +547,39 @@ class LayerNorm(nn.Module):
 
 
 class Bottleneck(PredictModule):
-    """The reference's Bottleneck (convolutions.py:65-170) with downsample=True, the only form the Gaussian present
-    distribution builds: 1x1 -> BN -> ReLU -> 3x3 s2 -> BN -> ReLU -> 1x1 -> BN -> ReLU, plus the skip (zero-pad an odd
-    H / W, MaxPool 2x2, 1x1 -> BN).  The skip is the up-projection's residual, added after its ReLU."""
+    """The reference's Bottleneck (convolutions.py:65-170) in the two forms the reference configurations build:
+      downsample=True (the present distribution and the planner's first three blocks): 1x1 -> BN -> ReLU -> 3x3 s2 ->
+        BN -> ReLU -> 1x1 -> BN -> ReLU, plus the skip (zero-pad an odd H / W, MaxPool 2x2, 1x1 -> BN);
+      out_channels != in_channels without resampling (the planner's last block, Bottleneck(32, 8)): the same with a
+        stride-1 3x3 and the skip 1x1 -> BN of the input, no pool.
+    The skip is the up-projection's residual, added after its ReLU."""
 
     def __init__(self, in_channels, out_channels=None, kernel_size=3, dilation=1, groups=1, upsample=False,
                  downsample=False, dropout=0.0):
         super().__init__()
-        if not downsample or upsample or kernel_size != 3 or dilation != 1 or groups != 1:
-            raise NotImplementedError("Bottleneck: only the downsampling 3x3 form (the present distribution's) is built")
+        out_channels = out_channels or in_channels
+        if upsample or kernel_size != 3 or dilation != 1 or groups != 1 or (not downsample and out_channels == in_channels):
+            raise NotImplementedError("Bottleneck: only the downsampling 3x3 form (the present distribution's) and the "
+                                      "projecting stride-1 3x3 form (the planner's last block) are built")
         self._downsample = downsample
         bottleneck_channels = int(in_channels / 2)
-        out_channels = out_channels or in_channels
         self.in_channels, self.out_channels = in_channels, out_channels
         self.layers = nn.Sequential(OrderedDict([
             ('conv_down_project', nn.Conv2d(in_channels, bottleneck_channels, kernel_size=1, bias=False)),
             ('abn_down_project', nn.Sequential(nn.BatchNorm2d(bottleneck_channels), nn.ReLU(inplace=True))),
-            ('conv', nn.Conv2d(bottleneck_channels, bottleneck_channels, kernel_size=3, bias=False, stride=2, padding=1)),
+            ('conv', nn.Conv2d(bottleneck_channels, bottleneck_channels, kernel_size=3, bias=False,
+                               stride=2 if downsample else 1, padding=1)),
             ('abn', nn.Sequential(nn.BatchNorm2d(bottleneck_channels), nn.ReLU(inplace=True))),
             ('conv_up_project', nn.Conv2d(bottleneck_channels, out_channels, kernel_size=1, bias=False)),
             ('abn_up_project', nn.Sequential(nn.BatchNorm2d(out_channels), nn.ReLU(inplace=True))),
             ('dropout', nn.Dropout2d(p=dropout)),
         ]))
-        self.projection = nn.Sequential(OrderedDict([
-            ('upsample_skip_proj', nn.MaxPool2d(kernel_size=2, stride=2)),
-            ('conv_skip_proj', nn.Conv2d(in_channels, out_channels, kernel_size=1, bias=False)),
-            ('bn_skip_proj', nn.BatchNorm2d(out_channels)),
-        ]))
+        projection = OrderedDict()
+        if downsample:
+            projection['upsample_skip_proj'] = nn.MaxPool2d(kernel_size=2, stride=2)
+        projection['conv_skip_proj'] = nn.Conv2d(in_channels, out_channels, kernel_size=1, bias=False)
+        projection['bn_skip_proj'] = nn.BatchNorm2d(out_channels)
+        self.projection = nn.Sequential(projection)
 
     def _pack(self):
         L = self.layers
@@ -585,12 +592,13 @@ class Bottleneck(PredictModule):
         return P
 
     def forward_hl(self, x: dense.HL) -> dense.HL:
-        """x: HL (B, T, H, W, >= in_channels) -> HL (B, T, ceil(H/2), ceil(W/2), 64-padded out_channels)."""
+        """x: HL (B, T, H, W, >= in_channels) -> HL (B, T, ceil(H/2), ceil(W/2), 64-padded out_channels), or
+        (B, T, H, W, ...) for the stride-1 form."""
         self._require_eval()
         P = self.packed()
         a = dense.conv(x, P["down"], relu=True)
         a = dense.conv(a, P["conv"], relu=True)
-        skip = dense.conv(dense.maxpool2_pad(x), P["skip"])
+        skip = dense.conv(dense.maxpool2_pad(x) if self._downsample else x, P["skip"])
         return dense.conv(a, P["up"], relu=True, residual=skip, res_after_act=True)
 
 

@@ -9,7 +9,9 @@ Device data flow of forward():
     Decoder (wgmma)        -> fp32 logits in the reference's (B,S,k,X,Y) layout
 With N_FUTURE_FRAMES > 0 (the Prediction configurations, eval mode only) the present distribution and the future
 prediction run between the temporal model and the decoder, and the decoder sees the present and future frames
-(DESIGN.md §3.16).  Planning is refused loudly.
+(DESIGN.md §3.16).  With PLANNING.ENABLED (the Planning configurations, eval mode only) the model also builds the
+Planning head (models/planning_model.py, DESIGN.md §3.17) and every forward entry point returns `cam_front`, the
+context features of camera 1 at the last present frame, for model.planning.
 """
 import torch
 import torch.nn as nn
@@ -20,6 +22,7 @@ from ..utils import geometry as G
 from .decoder import Decoder
 from .distributions import DistributionModule
 from .future_prediction import FuturePrediction
+from .planning_model import Planning
 from .encoder import Encoder
 from .temporal_model import TemporalModel, TemporalModelIdentity
 
@@ -42,8 +45,13 @@ class STP3(nn.Module):
         self.receptive_field = cfg.TIME_RECEPTIVE_FIELD
         self.n_future = cfg.N_FUTURE_FRAMES
         if cfg.PLANNING.ENABLED:
-            raise NotImplementedError("PLANNING.ENABLED: the planning head and its cost function (SURVEY.md row f4) are "
-                                      "not built on sm_90a")
+            if self.n_future == 0:
+                raise NotImplementedError("PLANNING.ENABLED with N_FUTURE_FRAMES = 0: the planner scores its candidates on "
+                                          "the predicted future frames, and there are none")
+            if not (cfg.SEMANTIC_SEG.HDMAP.ENABLED and cfg.SEMANTIC_SEG.PEDESTRIAN.ENABLED):
+                raise NotImplementedError("PLANNING.ENABLED needs SEMANTIC_SEG.HDMAP and SEMANTIC_SEG.PEDESTRIAN: the eval-"
+                                          "mode planner reads the model's own hdmap logits and vehicle / pedestrian "
+                                          "occupancy, as both reference Planning.yml files configure it")
         if self.n_future > 0:
             if cfg.MODEL.TEMPORAL_MODEL.NAME == 'identity':
                 raise NotImplementedError("N_FUTURE_FRAMES > 0 with the identity temporal model: the prediction stage is "
@@ -97,6 +105,8 @@ class STP3(nn.Module):
                           'predict_instance': cfg.INSTANCE_SEG.ENABLED,
                           'predict_future_flow': cfg.INSTANCE_FLOW.ENABLED,
                           'planning': cfg.PLANNING.ENABLED})
+        if cfg.PLANNING.ENABLED:
+            self.planning = Planning(cfg, self.encoder_out_channels, 6, gru_state_size=cfg.PLANNING.GRU_STATE_SIZE)
         for m in self.modules():
             if isinstance(m, (nn.BatchNorm1d, nn.BatchNorm2d, nn.BatchNorm3d)):
                 m.momentum = cfg.MODEL.BN_MOMENTUM
@@ -222,7 +232,7 @@ class STP3(nn.Module):
         X, Y = self.bev_size
         C = self.encoder_out_channels
         off, res, dim = self._bev_host()
-        output = {'depth_prediction': depth_logits, 'cam_front': None}
+        output = {'depth_prediction': depth_logits, 'cam_front': self._cam_front(feat, feat_channels_last)}
         self._check_predict_eval()
         if self._head_training() and not self.decoder.training:
             raise RuntimeError("STP3: temporal_model.final_conv is in train mode but the decoder is in eval mode, so no "
@@ -266,6 +276,17 @@ class STP3(nn.Module):
         output.update(self.decoder(states) if torch.is_tensor(states) else self.decoder.forward_hl(states))
         self._mark("decoder")
         return output
+
+    def _cam_front(self, feat, channels_last=False, cam_front_index=1):
+        """stp3.py:209-211,315: the context features of camera 1 at the last present frame, (B, C, Hf, Wf) fp32, when
+        planning is on (None otherwise).  feat is (B, S, N, C, Hf, Wf), or (B, S, N, Hf, Wf, C) when channels_last."""
+        if not self.cfg.PLANNING.ENABLED:
+            return None
+        if feat.shape[2] <= cam_front_index:
+            raise ValueError(f"planning reads the front camera (index {cam_front_index}) but the rig has {feat.shape[2]} "
+                             "camera(s)")
+        x = feat[:, -1, cam_front_index]
+        return (x.permute(0, 3, 1, 2) if channels_last else x).float().contiguous()
 
     def _predict_hl(self, states: dense.HL) -> dense.HL:
         """Prediction stage (stp3.py:157-176): present distribution of the last present state (eval: the sample is mu,
@@ -404,12 +425,14 @@ class STP3(nn.Module):
         return torch.cat([torch.zeros_like(future_egomotion[:, :1]), future_egomotion[:, :-1]], dim=1).float()
 
     def calculate_birds_eye_view_features(self, x, intrinsics, extrinsics, future_egomotion):
-        """(B,S,N,3,H,W) images -> (bev (B,S,C,X,Y) fp32, depth logits (B,S,N,D,Hf,Wf), cam_front=None) (stp3.py:303-318)."""
+        """(B,S,N,3,H,W) images -> (bev (B,S,C,X,Y) fp32, depth logits (B,S,N,D,Hf,Wf), cam_front) (stp3.py:303-318);
+        cam_front is (B,C,Hf,Wf) with planning on, else None."""
         b, s, n = x.shape[:3]
         feat, depth = self.encoder(x.view(b * s * n, *x.shape[3:]))
         feat = feat.view(b, s, n, *feat.shape[1:])
         depth = depth.view(b, s, n, *depth.shape[1:]) if depth is not None else None
-        return self.projection_to_birds_eye_view(feat, depth, intrinsics, extrinsics, future_egomotion), depth, None
+        return (self.projection_to_birds_eye_view(feat, depth, intrinsics, extrinsics, future_egomotion), depth,
+                self._cam_front(feat))
 
 
 class GraphedPerception:

@@ -248,3 +248,88 @@ def bev_discount(raw: torch.Tensor, discount: float) -> torch.Tensor:
                                             planes[1].data_ptr(), torch.cuda.current_stream(raw.device).cuda_stream)
     _lib.check(code, "stp3_bev_discount")
     return planes
+
+
+# ------------------------------------------------------------------------------------------------ planning (eval)
+def plan_desc(*, B, N, T, H, W, dx, bx, fp0, fp1, safety, headway, lrdivider, comfort, progress, volume, rule, safety_w,
+              headway_dist, lane_dist, n_hd, traj_c, G=0) -> "_lib.PlanDesc":
+    """stp3_plan_desc (include/stp3_b200.h) from host values; dx, bx, safety_w are pairs of fp32 values, fp0 / fp1 the
+    footprints as (first row, last row, first column, last column)."""
+    F2, I4 = ctypes.c_float * 2, ctypes.c_int * 4
+    return _lib.PlanDesc(B=B, N=N, T=T, H=H, W=W, dx=F2(*map(float, dx)), bx=F2(*map(float, bx)), fp0=I4(*fp0),
+                         fp1=I4(*fp1), safety=safety, headway=headway, lrdivider=lrdivider, comfort=comfort,
+                         progress=progress, volume=volume, rule=rule, safety_w=F2(*map(float, safety_w)), headway_dist=headway_dist,
+                         lane_dist=lane_dist, n_hd=n_hd, traj_c=traj_c, G=G)
+
+
+def _shape(t: torch.Tensor, shape, what: str):
+    if tuple(t.shape) != tuple(shape):
+        raise ValueError(f"{what}: expected shape {tuple(shape)}, got {tuple(t.shape)}")
+
+
+def plan_cost(desc, trajs, occupancy, cost_volume, target_points, lane, drivable):
+    """Cost_Function.forward (cost.py:25-46) on the device: trajs (B, N, T, traj_c) fp32, occupancy (B, T, H, W) bool,
+    cost_volume (B, T, H, W), target_points (B, 2), lane / drivable (B, n_hd, H, W) -> cost_fc (B, N), cost_fo (B, N, T)
+    fp32.  Two launches (stp3_plan_maps, stp3_plan_cost), no host synchronisation."""
+    _require_cuda(trajs, occupancy, cost_volume, target_points, lane, drivable)
+    B, N, T, H, W = desc.B, desc.N, desc.T, desc.H, desc.W
+    dev = trajs.device
+    if occupancy.dtype != torch.bool:
+        raise TypeError(f"semantic_pred must be a bool occupancy map (got {occupancy.dtype}): the footprint sums count "
+                        "occupied cells")
+    _shape(trajs, (B, N, T, desc.traj_c), "trajs")
+    _shape(occupancy, (B, T, H, W), "semantic_pred")
+    _shape(cost_volume, (B, T, H, W), "cost_volume")
+    _shape(target_points, (B, 2), "target_points")
+    _shape(lane, (B, desc.n_hd, H, W), "lane_divider")
+    _shape(drivable, (B, desc.n_hd, H, W), "drivable_area")
+    trajs, cost_volume, target_points, lane, drivable = (_f32c(t) for t in (trajs, cost_volume, target_points, lane,
+                                                                              drivable))
+    occ = occupancy.contiguous().view(torch.uint8)
+    drv = torch.empty((B, H, W), dtype=torch.float32, device=dev)
+    dang = torch.empty((B, H, W), dtype=torch.uint8, device=dev)
+    lane_cost = torch.empty((B, H, W), dtype=torch.float32, device=dev)
+    fc = torch.empty((B, N), dtype=torch.float32, device=dev)
+    fo = torch.empty((B, N, T), dtype=torch.float32, device=dev)
+    L = _lib.lib()
+    with torch.cuda.device(dev):
+        st = torch.cuda.current_stream(dev).cuda_stream
+        _lib.check(L.stp3_plan_maps(desc, lane.data_ptr(), drivable.data_ptr(), drv.data_ptr(), dang.data_ptr(),
+                                    lane_cost.data_ptr(), st), "stp3_plan_maps")
+        _lib.check(L.stp3_plan_cost(desc, trajs.data_ptr(), occ.data_ptr(), cost_volume.data_ptr(),
+                                    target_points.data_ptr(), drv.data_ptr(), dang.data_ptr(), lane_cost.data_ptr(),
+                                    fc.data_ptr(), fo.data_ptr(), st), "stp3_plan_cost")
+    return fc, fo
+
+
+def plan_refine(desc, windows_host, windows, trajs, cost_fc, cost_fo, h0, target_points, w_ih, b_ih, w_hh_t, b_hh,
+                w1_t, b1, w2, b2):
+    """The selection and GRU refinement of Planning.forward (planning_model.py:129-145): windows (B, 2) int32 (first
+    candidate, count) on the device and the same values on the host (windows_host, checked before the launch) ->
+    output_traj (B, T, 3) fp32 and the selected candidate index (B,) int32."""
+    _require_cuda(windows, trajs, cost_fc, cost_fo, h0)
+    B, N, T, G = desc.B, desc.N, desc.T, desc.G
+    dev = trajs.device
+    if windows_host.dtype != torch.int32 or windows.dtype != torch.int32 or windows_host.is_cuda:
+        raise TypeError("windows: int32, one copy on the host and one on the device")
+    _shape(windows_host, (B, 2), "windows_host")
+    _shape(windows, (B, 2), "windows")
+    _shape(trajs, (B, N, T, desc.traj_c), "trajs")
+    _shape(cost_fc, (B, N), "cost_fc")
+    _shape(cost_fo, (B, N, T), "cost_fo")
+    _shape(h0, (B, G), "h0")
+    _shape(w_hh_t, (G, 3 * G), "w_hh_t")
+    _shape(w1_t, (G, G), "w1_t")
+    windows_host, windows = windows_host.contiguous(), windows.contiguous()
+    trajs, cost_fc, cost_fo, h0, target_points = (_f32c(t) for t in (trajs, cost_fc, cost_fo, h0, target_points))
+    out = torch.empty((B, T, 3), dtype=torch.float32, device=dev)
+    sel = torch.empty((B,), dtype=torch.int32, device=dev)
+    with torch.cuda.device(dev):
+        code = _lib.lib().stp3_plan_refine(desc, windows_host.data_ptr(), windows.data_ptr(), trajs.data_ptr(),
+                                           cost_fc.data_ptr(), cost_fo.data_ptr(), h0.data_ptr(),
+                                           target_points.data_ptr(), w_ih.data_ptr(), b_ih.data_ptr(),
+                                           w_hh_t.data_ptr(), b_hh.data_ptr(), w1_t.data_ptr(), b1.data_ptr(),
+                                           w2.data_ptr(), b2.data_ptr(), out.data_ptr(), sel.data_ptr(),
+                                           torch.cuda.current_stream(dev).cuda_stream)
+    _lib.check(code, "stp3_plan_refine")
+    return out, sel
